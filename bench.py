@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py - headline measurement of the self-play hot path on B200 (contract: see DESIGN.md "Measurement").
+"""bench.py - headline measurement of the self-play hot path on an H100 (contract: see DESIGN.md "Measurement").
 
   python bench.py --gpus N --steps K --warmup W            # our arm (CUDA path through libkgb200's C ABI)
   python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU path timed on this box's host cores
@@ -16,6 +16,10 @@ e2e    : visits/s through the reference-facing evaluator boundary (NeuralNet::ge
          region, every step, rotating over more distinct input batches than fit in L2.
 N > 1  : one process per GPU (torchrun), games shard across ranks with no data-path collective ("weak" scaling);
          NCCL carries only the model-weight broadcast from rank 0 before the timed region (SURVEY.md §8e).
+
+--dump-outputs DIR writes, as DIR/<name>.npy, what the timed paths computed in their last step: the evaluator's outputs
+(policy, value, score_value, ownership) of the last timed NN-only step, and the self-play loop's root statistics and boards
+after its last timed wave.  Every input is seeded, so two builds run with the same arguments can be compared array by array.
 """
 import argparse
 import json
@@ -58,7 +62,17 @@ def parse_args():
     ap.add_argument("--mixed-sizes", action="store_true", help="BASELINE.json configs[3]: every game draws its board from 9x9 / 13x13 / 19x19 (equal "
                     "probabilities, like bSizes = 9,13,19) inside the 19x19 evaluator frame; a finished game's slot draws again")
     ap.add_argument("--visits", type=int, default=600, help="maxVisits per move (BASELINE.json configs[1]: 600)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps write the outputs of their last step to DIR/<name>.npy (float32 / float64)")
     return ap.parse_args()
+
+
+def dump_outputs(out_dir, arrays):
+    """float32 / float64 .npy files, one per output array (all of them at the default sizes: ~3 MB)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        np.save(os.path.join(out_dir, f"{name}.npy"), a if a.dtype in (np.float32, np.float64) else a.astype(np.float64))
 
 
 def load_peaks():
@@ -66,11 +80,12 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], tflops_burst=d["bf16_tflops"], tflops_sustained=d["bf16_tflops_sustained"], source="measured")
-    return dict(hbm_gbs=6650.0, tflops_burst=1590.0, tflops_sustained=1400.0, source="fallback")
+    # NVIDIA's data sheet for the H100 SXM (700 W): 3.35 TB/s HBM3, 989 dense fp16 TFLOP/s - not reached figures
+    return dict(hbm_gbs=3350.0, tflops_burst=989.0, tflops_sustained=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, gpu_index: int):
         self.gpu = gpu_index
@@ -278,7 +293,7 @@ def main():
     from katago_b200 import NeuralNet, SelfPlay, load_library, modelgen
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device - the B200 path has no CPU fallback (use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py: no CUDA device - the GPU path has no CPU fallback (use --impl reference for the CPU arm)")
     torch.cuda.set_device(local_rank)
     device = torch.device("cuda", local_rank)
     if world > 1:
@@ -296,7 +311,7 @@ def main():
     macs = model.desc["conv_macs_per_position"]
     flop_per_eval = 2.0 * macs * 361
 
-    # distinct input batches: 16 x 8.1 MB = 130 MB of feature rows > 126 MB L2, rotated every step
+    # distinct input batches: 16 x 8.1 MB = 130 MB of feature rows > 50 MB L2, rotated every step
     NBUF = 16
     host_sp, host_gl = [], []
     for b in range(NBUF):
@@ -388,6 +403,12 @@ def main():
     ms_dev = timed(lambda i: sp.run(1), K)
     clocks = sampler.stop() if rank == 0 else None
     after = sp.stats()
+    dumps = {}
+    if args.dump_outputs:
+        children = [sp.root_children(g) for g in range(n)]
+        dumps.update(selfplay_root_visits=sp.root_visits(), selfplay_root_child_visits=np.stack([c[0] for c in children]),
+                     selfplay_root_child_policy=np.stack([c[1] for c in children]), selfplay_root_child_utility=np.stack([c[2] for c in children]),
+                     selfplay_boards=np.stack([sp.game(g)[0] for g in range(n)]))
     # a wave delivers one evaluated leaf per game, except for games whose ladder searches are still running (stalled_waves);
     # under graph search a game can also finish extra playouts inside the wave on edges that only need to catch up
     done = after["total_visits"] - before["total_visits"]
@@ -399,6 +420,10 @@ def main():
         dist.all_reduce(visits_done, op=dist.ReduceOp.SUM)
     visits_done = float(visits_done.item())
     ms_nn = timed(step_device, K)
+    if args.dump_outputs:
+        dumps.update(nn_policy=dpol.cpu().numpy(), nn_value=dval.cpu().numpy(), nn_score_value=dsc.cpu().numpy(), nn_ownership=down.cpu().numpy())
+        if rank == 0:
+            dump_outputs(args.dump_outputs, dumps)
     s0 = sp.stats()
     ms_select, ms_backup = sp.time_tree_kernels(20)
     s1 = sp.stats()
@@ -439,9 +464,8 @@ def main():
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     barrier()
     e0.record(stream)
-    pumps = max(1, (K + PUMP - 1) // PUMP)
-    for _ in range(pumps):
-        rec.pump(PUMP)
+    for done_waves in range(0, K, PUMP):
+        rec.pump(min(PUMP, K - done_waves))
     e1.record(stream)
     handle.sync()
     barrier()
@@ -455,7 +479,6 @@ def main():
     if world > 1:
         dist.all_reduce(rec_visits, op=dist.ReduceOp.SUM)
     rec_visits = float(rec_visits.item())
-    rec_waves = pumps * PUMP + 0          # + the extra waves in which released games moved (counted from the stats below)
     rec_moves, rec_games, rec_rows = rec.moves_recorded - moves0, rec.games_written - games0, writer.row_count - rows0
     writer.flush_if_nonempty()
     rec_files = len([f for f in os.listdir(out_dir) if f.endswith(".npz")])
@@ -519,8 +542,10 @@ def main():
         achieved = conv_flop / (float(ms_conv[0]) * 1e-3) / 1e12
         whole = flop_per_eval * n * K / (ms_nn * 1e-3) / 1e12
         cpu_obj = {"value": None, "unit": UNIT, "cores": 0, "kind": "reference", "sample": "measured at N=1 only"}
-        if world == 1:      # the CPU baseline is a property of the box: measured at N=1 only
+        if world == 1 and os.path.exists(CPU_SELFPLAY):      # the CPU baseline is a property of the box: measured at N=1 only
             cpu_obj = cpu_baseline_object(cpu_selfplay(args.model, 15.0, 5.0, args.visits), args.model)
+        elif world == 1:
+            cpu_obj["sample"] = "not measured: oracle/_ref/kgref_cpu_selfplay is not built"
         out = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": K, "warmup": W,
             "ms_per_step": ms_dev / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -537,7 +562,7 @@ def main():
                        "games_per_gpu": n, "parallelism": f"games sharded over {world} GPU(s), no data-path collective",
                        "weights": "random init, real architecture (katago_b200/modelgen.py)",
                        "positions": f"every game starts from its own random legal play-out of 0..{args.opening_max} moves, then {W + args.settle_waves} untimed waves",
-                       "l2": "per-step working set (tree arrays ~1 GB + activations ~0.5 GB) far larger than the 126 MB L2; "
+                       "l2": "per-step working set (tree arrays ~1 GB + activations ~0.5 GB) far larger than the 50 MB L2; "
                              f"e2e rotates {NBUF} distinct feature batches ({NBUF * n * 22 * 361 * 4 / 1e6:.0f} MB)",
                        "avg_leaf_depth": (after["sum_leaf_depth"] - before["sum_leaf_depth"]) / max(1, after["total_visits"] - before["total_visits"]),
                        "nn_only_ms_per_step": ms_nn / K,
@@ -551,8 +576,8 @@ def main():
                                   "game_waves": n * K},
                        "weight_broadcast_ms": bcast_ms, "weight_broadcast": bcast, "gpu_competitor": competitor},
             "value_fp32_equivalent": value_fp32,
-            "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": slots.h2d / (pumps * PUMP), "d2h_bytes_per_step": slots.d2h / (pumps * PUMP),
-                    "ms_per_step": ms_rec / (pumps * PUMP),
+            "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": slots.h2d / K, "d2h_bytes_per_step": slots.d2h / K,
+                    "ms_per_step": ms_rec / K,
                     "what": "device loop in hold mode + GameRecorder.pump (per-game release every 8 waves: root readback, training targets) + TrainingDataWriter "
                             ".npz files; host work inside the timed region; a step = one playout wave (the wave in which released games move is extra)",
                     "moves_recorded": rec_moves, "games_finished": rec_games, "rows_written": rec_rows, "npz_files": rec_files, "frac_of_value": e2e_value / value,
@@ -560,10 +585,9 @@ def main():
             "e2e_nn_boundary": {"value": e2e_nn_value, "unit": UNIT, "h2d_bytes_per_step": h2d_nn, "d2h_bytes_per_step": d2h_nn, "ms_per_step": ms_e2e_nn / K,
                                 "what": "NeuralNet::getOutput -> kgb_forward with host buffers (boundary 1): one evaluated row = one visit of a host-side search"},
             "gpu_launches": launches_per_step * K,
-            "roofline": {"bound": "tensor", "kernel": f"{'kgb_conv_tc_kernel (3-term split)' if args.fp32 else 'kgb_conv_tc3_kernel'} 3x3 {mid}->{mid}, batch {n}, 4 rotating buffer sets", "achieved": achieved,
+            "roofline": {"bound": "tensor", "kernel": f"kgb_conv_wg_kernel{' (3-term split)' if args.fp32 else ''} 3x3 {mid}->{mid}, batch {n}, 4 rotating buffer sets", "achieved": achieved,
                          "peak": peaks["tflops_burst"], "unit": "TFLOP/s", "frac": achieved / peaks["tflops_burst"],
-                         "traffic": 42.4e6 if args.model == "b18c384nbt" and n == 256 and not args.fp32 else None,   # dram read 40.45 MB + write 1.93 MB per launch (profiles/r02_conv_ncu_raw.md)
-                         "peak_source": peaks["source"] + " (burst cuBLAS bf16, kernel timed alone)",
+                         "peak_source": peaks["source"] + " (kernel timed alone)",
                          "ms_per_launch": float(ms_conv[0]),
                          "whole_forward_tflops": whole, "whole_forward_frac_of_sustained": whole / peaks["tflops_sustained"]},
             # tree / board kernels: HBM-bound byte work.  Algorithmic bytes per playout (DESIGN.md §4): every node on the descent
@@ -576,7 +600,6 @@ def main():
                 "frac": (bytes_sel + bytes_bak) * n / ((ms_select + ms_backup) * 1e-3) / 1e9 / peaks["hbm_gbs"],
                 "ms_select": ms_select, "ms_backup": ms_backup, "avg_depth": tree_depth,
                 "bytes_per_playout": bytes_sel + bytes_bak,
-                "traffic": 13.2e6 if args.model == "b18c384nbt" and n == 256 and not args.mixed_sizes else None,   # DRAM bytes per wave, both kernels: ncu dram__bytes_read + write (profiles/r02_tree_kernels_ncu_summary.md)
                 "note": "latency-bound at 256 warps per launch (1.7 warps per SM); see DESIGN.md §6"})(
                     tree_depth * 362 * 20 + 362 * 20 + (22 * 361 + 19) * 4 * 2 + 128, 362 * 8 + tree_depth * 48 + 64),
             "cpu_baseline": cpu_obj,

@@ -1,4 +1,4 @@
-/* kgb200.h - C ABI of the B200-native KataGo NN-evaluator backend (libkgb200.so).
+/* kgb200.h - C ABI of the H100-native KataGo NN-evaluator backend (libkgb200.so).
  *
  * Drop-in boundary: the reference selects ONE translation unit defining `namespace NeuralNet`
  * (cpp/neuralnet/nninterface.h:32-182) at link time.  A maintainer adds `neuralnet/b200backend.cpp`
@@ -26,7 +26,7 @@ extern "C" {
 #define KGB_OK 0
 #define KGB_ERR_INVALID (-1)   /* bad argument / unsupported model */
 #define KGB_ERR_IO (-2)        /* model file could not be read / sha256 mismatch */
-#define KGB_ERR_CUDA (-3)      /* CUDA runtime or driver failure, or no sm_100 device */
+#define KGB_ERR_CUDA (-3)      /* CUDA runtime or driver failure, or no sm_90 device */
 
 typedef struct kgb_model kgb_model;     /* replaces LoadedModel     (nninterface.h:27, eigenbackend.cpp:94-107) */
 typedef struct kgb_context kgb_context; /* replaces ComputeContext  (nninterface.h:17) */

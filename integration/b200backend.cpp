@@ -1,4 +1,4 @@
-// neuralnet/b200backend.cpp - the translation unit a KataGo maintainer adds to select the B200 backend
+// neuralnet/b200backend.cpp - the translation unit a KataGo maintainer adds to select the H100 backend
 // (one TU defining `namespace NeuralNet`, cpp/neuralnet/nninterface.h:32-182; template: neuralnet/dummybackend.cpp;
 // selected like the others in cpp/CMakeLists.txt:60-172).  Everything forwards 1:1 to the C ABI of libkgb200.so
 // (include/kgb200.h); no CUDA, no torch and no weights logic lives on this side of the boundary.
@@ -16,7 +16,7 @@ using namespace std;
 
 static void kgbCheck(int rc, const char* what) {
   if(rc != KGB_OK)
-    throw StringError(string("B200 backend: ") + what + ": " + kgb_last_error());
+    throw StringError(string("H100 backend: ") + what + ": " + kgb_last_error());
 }
 
 struct LoadedModel {
@@ -108,7 +108,7 @@ ComputeHandle* NeuralNet::createComputeHandle(
   h->score.resize((size_t)maxBatchSize * 6);
   h->ownership.resize((size_t)maxBatchSize * xy);
   if(logger != NULL)
-    logger->write("B200 backend thread " + Global::intToString(serverThreadIdx) + ": Model version " + Global::intToString(h->modelVersion) +
+    logger->write("H100 backend thread " + Global::intToString(serverThreadIdx) + ": Model version " + Global::intToString(h->modelVersion) +
                   " useFP16 = " + string(kgb_handle_is_fp16(h->kh) ? "true" : "false (3-term split fp16, fp32-equivalent)"));
   return h;
 }
@@ -130,14 +130,14 @@ void NeuralNet::getOutput(
   ComputeHandle* h, InputBuffers* buffers, int numBatchEltsFilled, NNResultBuf** inputBufs, vector<NNOutput*>& outputs
 ) {
   const int n = numBatchEltsFilled;
-  if(n <= 0 || n > h->maxBatchSize || n > buffers->maxBatchSize) throw StringError("B200 backend: getOutput batch size out of range");
+  if(n <= 0 || n > h->maxBatchSize || n > buffers->maxBatchSize) throw StringError("H100 backend: getOutput batch size out of range");
   const size_t xy = (size_t)h->nnXLen * h->nnYLen;
   const size_t spElts = (size_t)h->numSpatial * xy;
   bool anyOwner = false;
   for(int i = 0; i < n; i++) {
     const NNResultBuf* rb = inputBufs[i];
-    if(rb->rowSpatialBuf.size() < spElts || rb->rowGlobalBuf.size() < (size_t)h->numGlobal) throw StringError("B200 backend: row buffers too small");
-    if(rb->hasRowMeta) throw StringError("B200 backend: SGF metadata inputs are not supported");
+    if(rb->rowSpatialBuf.size() < spElts || rb->rowGlobalBuf.size() < (size_t)h->numGlobal) throw StringError("H100 backend: row buffers too small");
+    if(rb->hasRowMeta) throw StringError("H100 backend: SGF metadata inputs are not supported");
     std::copy(rb->rowSpatialBuf.begin(), rb->rowSpatialBuf.begin() + spElts, h->spatial.begin() + i * spElts);
     std::copy(rb->rowGlobalBuf.begin(), rb->rowGlobalBuf.begin() + h->numGlobal, h->global.begin() + (size_t)i * h->numGlobal);
     h->symmetry[i] = rb->symmetry;
@@ -182,7 +182,7 @@ bool NeuralNet::testEvaluateConv(
   return true;
 }
 
-// Layer-level hooks the B200 backend does not expose (the whole-net and conv hooks are covered): report "unsupported".
+// Layer-level hooks the H100 backend does not expose (the whole-net and conv hooks are covered): report "unsupported".
 bool NeuralNet::testEvaluateBatchNorm(const BatchNormLayerDesc*, int, int, int, bool, bool, const std::vector<float>&, const std::vector<float>&, std::vector<float>&) { return false; }
 bool NeuralNet::testEvaluateResidualBlock(const ResidualBlockDesc*, int, int, int, bool, bool, const std::vector<float>&, const std::vector<float>&, std::vector<float>&) { return false; }
 bool NeuralNet::testEvaluateGlobalPoolingResidualBlock(const GlobalPoolingResidualBlockDesc*, int, int, int, bool, bool, const std::vector<float>&, const std::vector<float>&, std::vector<float>&) { return false; }

@@ -3,7 +3,7 @@
 // The engine turns a ModelDesc into a flat list of launches ("ops") at handle creation:
 //   pack-input -> initial conv(+global matmul bias) -> residual / gpool / nested-bottleneck blocks -> fused head conv
 //   -> pooling, tiny matmuls, policy / ownership / value outputs.
-// Every convolution is one launch of the tcgen05 kernel with the NEXT layer's BN+activation+mask fused into its
+// Every convolution is one launch of the wgmma kernel with the NEXT layer's BN+activation+mask fused into its
 // epilogue (kgb_conv.cuh), so a trunk layer is exactly one kernel.  Per batch size the whole list is captured once into
 // a CUDA graph (no tracing compiler: the op list is static).  Reference structure mirrored: Model/Trunk/heads
 // eigenbackend.cpp:1909-2216, getOutput :2445-2628 (and cudabackend.cpp:3649-3888 for the host<->device traffic).
@@ -93,21 +93,6 @@ static CUtensorMap makeTmap2D(const void* ptr, uint64_t rows, uint64_t cols, uin
   return m;
 }
 
-// 2-D row-major tensor of fp16 (elemBytes 2) or fp32 (4) elements, box {boxCols, boxRows} with boxCols * elemBytes = 128, 128B swizzle:
-// the epilogue tiles of kgb_conv_tc3.cu (TMA loads of the residual, TMA stores of the raw / activation outputs).
-static CUtensorMap makeTmapTile(const void* ptr, uint64_t rows, uint64_t cols, int elemBytes, uint32_t boxRows) {
-  CUtensorMap m;
-  cuuint64_t gdim[2] = {cols, rows};
-  cuuint64_t gstride[1] = {cols * (uint64_t)elemBytes};
-  cuuint32_t box[2] = {(cuuint32_t)(128 / elemBytes), boxRows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = getEncodeTiled()(&m, elemBytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(ptr),
-                                gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if(r != CUDA_SUCCESS) throw CudaFailure("cuTensorMapEncodeTiled (epilogue tile) failed with CUresult " + std::to_string((int)r));
-  return m;
-}
-
 // ------------------------------------------------------------------------------------------------------------
 // Opaque handles
 // ------------------------------------------------------------------------------------------------------------
@@ -133,13 +118,10 @@ struct ConvWeights {
   __half* w = nullptr;     // packed [taps][cout_p][cin_p * (split ? 2 : 1)]
   int ky = 0, kx = 0, cin_p = 0, cout_p = 0, n_tile = 0, num_n_tiles = 0;
   CUtensorMap tmapB;       // box {64, n_tile}
-  CUtensorMap tmapBhalf;   // box {64, n_tile/2}: each CTA of a pair loads half of the weight tile
-  bool hasIdentity = false;  // cout_p extra K columns holding the identity: the residual can enter through the tensor pipe (ConvParams::res_via_mma)
 };
 
 struct kgb_handle {
   int device = 0;
-  int numSMs = 0;
   cudaStream_t stream = nullptr;
   const ModelDesc* model = nullptr;
   Layout L{};
@@ -147,8 +129,7 @@ struct kgb_handle {
   int split = 0;          // fp32-equivalent mode
   bool nhwc = true;
   bool streamTrunkFp32 = true, streamInnerFp32 = false;
-  bool useSimt = false, useGraph = true, usePair = false, usePairTma = true;
-  int resViaMma = 1;       // 0: residuals are added in the epilogue; 1: 1x1 convs take them through the tensor pipe; 2: every conv does
+  bool useSimt = false, useGraph = true;
   std::vector<void*> allocs;
   // inputs / outputs (device, fixed addresses so graphs can be replayed)
   float *dSpatial = nullptr, *dGlobal = nullptr, *dOptimism = nullptr;
@@ -280,7 +261,7 @@ struct Builder {
   }
 
   // Pack one or more convs (concatenated along cout) as fp16 [tap][cout_p][cin_p (* 2)]
-  ConvWeights packConv(const std::vector<const ConvDesc*>& convs, bool withResidual = false) {
+  ConvWeights packConv(const std::vector<const ConvDesc*>& convs) {
     const ConvDesc& c0 = *convs[0];
     ConvWeights cw;
     cw.ky = c0.ky; cw.kx = c0.kx;
@@ -296,19 +277,13 @@ struct Builder {
     cw.num_n_tiles = nt;
     cw.n_tile = cw.cout_p / nt;
     int taps = cw.ky * cw.kx;
-    // residual through the tensor pipe (kgb_conv.cuh res_via_mma): identity columns behind the real ones
-    cw.hasIdentity = withResidual && !h.split && !h.useSimt && h.usePairTma && (h.resViaMma == 2 || (h.resViaMma == 1 && taps == 1)) &&
-                     cw.n_tile % 64 == 0;
-    int ldw = cw.cin_p * actMul + (cw.hasIdentity ? cw.cout_p : 0);
-    h.wSignature += "conv" + std::to_string(cw.ky) + "x" + std::to_string(cw.kx) + ":" + std::to_string(c0.cin) + ">" + std::to_string(cout) +
-                    (cw.hasIdentity ? "+id;" : ";");
+    int ldw = cw.cin_p * actMul;
+    h.wSignature += "conv" + std::to_string(cw.ky) + "x" + std::to_string(cw.kx) + ":" + std::to_string(c0.cin) + ">" + std::to_string(cout) + ";";
     const size_t count = (size_t)taps * cw.cout_p * ldw;
     void* hostDst = nullptr;
     cw.w = (__half*)h.walloc(count * sizeof(__half), &hostDst);
     if(h.wMode == kgb_handle::W_SIZE) return cw;
     std::vector<__half> host(count, __float2half(0.0f));
-    if(cw.hasIdentity)
-      for(int co = 0; co < cout; co++) host[(size_t)co * ldw + cw.cin_p + co] = __float2half(1.0f);
     int coBase = 0;
     for(auto c : convs) {
       for(int t = 0; t < taps; t++)
@@ -324,7 +299,6 @@ struct Builder {
     }
     memcpy(hostDst, host.data(), count * sizeof(__half));
     cw.tmapB = makeTmap2D(cw.w, (uint64_t)taps * cw.cout_p, (uint64_t)ldw, (uint32_t)cw.n_tile);
-    cw.tmapBhalf = makeTmap2D(cw.w, (uint64_t)taps * cw.cout_p, (uint64_t)ldw, (uint32_t)(cw.n_tile / 2));
     return cw;
   }
 
@@ -360,7 +334,6 @@ struct Builder {
       p.num_n_tiles = cw.num_n_tiles;
       p.split = hp->split;
       p.residual = residual; p.residual_fp32 = residualFp32 ? 1 : 0;
-      p.res_via_mma = 0;
       p.ncbias = ncbias;
       p.raw_out = rawOut; p.raw_fp32 = rawFp32 ? 1 : 0;
       p.act_out = actOut;
@@ -370,25 +343,8 @@ struct Builder {
         CK(launchConvSimt(A, cw.cin_p * actMulL, cw.w, p, s));
       }
       else {
-        CUtensorMap tmA = makeTmap2D(A, (uint64_t)p.M, (uint64_t)cw.cin_p * actMulL, (uint32_t)convTCABoxRows(cw.ky, cw.kx, p.Wp));
-        cudaError_t e = cudaErrorNotSupported;
-        if(hp->usePairTma && cw.hasIdentity && residual != nullptr && !residualFp32) {
-          ConvParams q = p;
-          q.residual = nullptr; q.res_via_mma = 1;
-          if(convTC3Supports(q)) p = q;
-        }
-        if(hp->usePairTma && convTC3Supports(p)) {
-          // epilogue tiles travel by TMA: residual in, raw / activation out (kgb_conv_tc3.cu); with res_via_mma the residual stream
-          // is a second A operand (box of 128 rows) instead
-          const CUtensorMap tmRes = p.res_via_mma ? makeTmap2D(residual, (uint64_t)p.M, (uint64_t)cw.cout_p, 128)
-                                                   : (residual ? makeTmapTile(residual, (uint64_t)p.M, (uint64_t)cw.cout_p, 2, 32) : tmA);
-          const CUtensorMap tmRaw = rawOut ? makeTmapTile(rawOut, (uint64_t)p.M, (uint64_t)cw.cout_p, rawFp32 ? 4 : 2, 32) : tmA;
-          const CUtensorMap tmAct = actOut ? makeTmapTile(actOut, (uint64_t)p.M, (uint64_t)cw.cout_p, 2, 32) : tmA;
-          e = launchConvTC3(tmA, cw.tmapBhalf, tmRes, tmRaw, tmAct, p, hp->numSMs, s);
-        }
-        if(e == cudaErrorNotSupported && hp->usePair) e = launchConvTC2(tmA, cw.tmapBhalf, p, hp->numSMs, s);
-        if(e == cudaErrorNotSupported) e = launchConvTC(tmA, cw.tmapB, p, hp->numSMs, s);
-        CK(e);
+        CUtensorMap tmA = makeTmap2D(A, (uint64_t)p.M, (uint64_t)cw.cin_p * actMulL, (uint32_t)convABoxRows(cw.ky, cw.kx, p.Wp));
+        CK(launchConvWG(tmA, cw.tmapB, p, s));
       }
     });
     h.launchesPerForward++;
@@ -405,14 +361,14 @@ struct Builder {
       void* rawOut = (last && !keepFinalRaw) ? nullptr : lv.S;
       if(b.kind == BLOCK_ORDINARY) {
         ConvWeights w1 = packConv({&b.conv1});
-        ConvWeights w2 = packConv({&b.conv2}, true);
+        ConvWeights w2 = packConv({&b.conv2});
         BNDev mid = uploadBN(b.midBN, b.midAct, w1.cout_p);
         emitConv(w1, lv.A, nullptr, false, nullptr, nullptr, false, lv.T, mid);
         emitConv(w2, lv.T, lv.S, lv.fp32, nullptr, rawOut, lv.fp32, lv.A, nextBN);
       }
       else if(b.kind == BLOCK_GPOOL) {
         ConvWeights w1 = packConv({&b.conv1, &b.gpoolConv});
-        ConvWeights w2 = packConv({&b.conv2}, true);
+        ConvWeights w2 = packConv({&b.conv2});
         const int regC = b.conv1.cout, gC = b.gpoolConv.cout;
         BNDev none;
         emitConv(w1, lv.A, nullptr, false, nullptr, lv.G, true, nullptr, none);
@@ -434,7 +390,7 @@ struct Builder {
       }
       else {
         ConvWeights wpre = packConv({&b.conv1});
-        ConvWeights wpost = packConv({&b.conv2}, true);
+        ConvWeights wpost = packConv({&b.conv2});
         Level inner = makeLevel(b.conv1.cout, h.streamInnerFp32, b.blocks);
         BNDev innerPre = uploadBN(b.blocks[0].preBN, b.blocks[0].preAct, inner.cp);
         emitConv(wpre, lv.A, nullptr, false, nullptr, inner.S, inner.fp32, inner.A, innerPre);
@@ -694,9 +650,9 @@ static void ncclCheck(ncclResult_t r, const char* what) {
 
 // The settings that decide how the graph builder lays the weights out
 static void copyBuildSettings(kgb_handle& dst, const kgb_handle& src) {
-  dst.device = src.device; dst.numSMs = src.numSMs; dst.model = src.model; dst.L = src.L; dst.maxBatch = src.maxBatch; dst.split = src.split;
+  dst.device = src.device; dst.model = src.model; dst.L = src.L; dst.maxBatch = src.maxBatch; dst.split = src.split;
   dst.nhwc = src.nhwc; dst.streamTrunkFp32 = src.streamTrunkFp32; dst.streamInnerFp32 = src.streamInnerFp32; dst.useSimt = src.useSimt;
-  dst.useGraph = src.useGraph; dst.usePair = src.usePair; dst.usePairTma = src.usePairTma; dst.resViaMma = src.resViaMma;
+  dst.useGraph = src.useGraph;
 }
 
 static void destroyHandle(kgb_handle* h) {
@@ -727,18 +683,17 @@ KGB_API int kgb_handle_create(kgb_context* ctx, const kgb_model* model, int max_
     if(dev < 0) dev = (!ctx->gpuIdxs.empty() && ctx->gpuIdxs[0] >= 0) ? ctx->gpuIdxs[0] : 0;
     int count = 0;
     if(cudaGetDeviceCount(&count) != cudaSuccess || count == 0)
-      throw CudaFailure("libkgb200: no CUDA device is visible; the B200 backend has no CPU fallback");
+      throw CudaFailure("libkgb200: no CUDA device is visible; the backend has no CPU fallback");
     if(dev >= count) throw std::invalid_argument("kgb_handle_create: gpu index " + std::to_string(dev) + " >= device count");
     CK(cudaSetDevice(dev));
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, dev));
-    if(prop.major != 10)
-      throw CudaFailure(std::string("libkgb200 is built for sm_100a (B200) only; device ") + prop.name + " is sm_" +
+    if(prop.major != 9 || prop.minor != 0)
+      throw CudaFailure(std::string("libkgb200 is built for sm_90a (H100) only; device ") + prop.name + " is sm_" +
                         std::to_string(prop.major) + std::to_string(prop.minor));
     raw = new kgb_handle();
     kgb_handle& h = *raw;
     h.device = dev;
-    h.numSMs = prop.multiProcessorCount;
     h.model = model->desc.get();
     h.maxBatch = max_batch_size;
     h.split = ctx->fp16 ? 0 : 1;
@@ -754,16 +709,10 @@ KGB_API int kgb_handle_create(kgb_context* ctx, const kgb_model* model, int max_
     h.streamInnerFp32 = streams == "all";
     env = getenv("KGB_CONV_IMPL");
     h.useSimt = env && std::string(env) == "simt";
-    h.usePair = env && std::string(env) == "tc2";        // "tc2" = round-1 CTA-pair kernel (staged epilogue)
-    h.usePairTma = !(env && (std::string(env) == "tc" || std::string(env) == "tc2"));   // default: kgb_conv_tc3.cu (CTA pair + TMA epilogue)
-    env = getenv("KGB_RES_MMA");
-    if(env) h.resViaMma = atoi(env);
     env = getenv("KGB_NO_GRAPH");
     h.useGraph = !(env && std::string(env) == "1");
     CK(cudaStreamCreateWithFlags(&h.stream, cudaStreamNonBlocking));
-    CK(convTCInit());
-    CK(convTC2Init());
-    CK(convTC3Init());
+    CK(convWGInit());
     CK(cudaStreamCreateWithFlags(&h.copyStream, cudaStreamNonBlocking));
     CK(cudaEventCreateWithFlags(&h.stagedEvent, cudaEventDisableTiming));
     CK(cudaEventCreate(&h.bcastStart));
@@ -1009,8 +958,7 @@ struct SingleConv {
     CK(cudaGetDevice(&h.device));
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, h.device));
-    if(prop.major != 10) throw CudaFailure("libkgb200 is built for sm_100a (B200) only");
-    h.numSMs = prop.multiProcessorCount;
+    if(prop.major != 9 || prop.minor != 0) throw CudaFailure("libkgb200 is built for sm_90a (H100) only");
     h.model = &dummy;
     h.maxBatch = n;
     h.split = use_fp16 ? 0 : 1;
@@ -1018,22 +966,16 @@ struct SingleConv {
     h.L.X = X; h.L.Y = Y; h.L.pad = pad; h.L.Wp = X + pad; h.L.P = (Y + pad) * (X + pad);
     const char* env = getenv("KGB_CONV_IMPL");
     h.useSimt = env && std::string(env) == "simt";
-    h.usePair = env && std::string(env) == "tc2";
-    h.usePairTma = !(env && (std::string(env) == "tc" || std::string(env) == "tc2"));
-    env = getenv("KGB_RES_MMA");
-    if(env) h.resViaMma = atoi(env);
     h.streamTrunkFp32 = h.streamInnerFp32 = h.split != 0;
     CK(cudaStreamCreateWithFlags(&h.stream, cudaStreamNonBlocking));
-    CK(convTCInit());
-    CK(convTC2Init());
-    CK(convTC3Init());
+    CK(convWGInit());
     h.wCheckSpans = false;
     h.wAllocArena((size_t)ky * kx * cpad(out_c) * ((size_t)cpad(in_c) * 2 + cpad(out_c)) * sizeof(__half) + 4 * (size_t)cpad(out_c) * sizeof(float) + 4096);
     Builder b(h);
     ConvDesc cd;
     cd.ky = ky; cd.kx = kx; cd.cin = in_c; cd.cout = out_c;
     cd.w.assign(weights, weights + (size_t)ky * kx * in_c * out_c);
-    cw = b.packConv({&cd}, actEpilogue == 2);
+    cw = b.packConv({&cd});
     M = (size_t)n * h.L.P;
     A = h.dalloc<__half>(M * cw.cin_p * b.actMul);
     h.dMask = h.dalloc<float>(M + 128);

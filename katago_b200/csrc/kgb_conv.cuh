@@ -1,4 +1,4 @@
-// Shared declarations for the B200 convolution kernels (tcgen05 implicit GEMM + SIMT debug path).
+// Shared declarations for the convolution kernels (wgmma implicit GEMM + SIMT debug path).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -9,7 +9,7 @@ namespace kgb {
 
 // One fused convolution launch:  out = conv(A, W) [+ ncbias[n]] [+ residual];  raw_out = out;
 // act_out = mask * act(out * bn_scale + bn_bias)  (the NEXT layer's BN+activation, applied by the producer so that
-// the consumer's A operand can go TMA -> smem -> tcgen05.mma untouched).
+// the consumer's A operand can go TMA -> smem -> wgmma untouched).
 //
 // Replaces, per reference call site, the sequence
 //   applyCScaleBias*Kernel (cudahelpers.cu:1370-2101) -> cudnnConvolutionForward / cublas*gemm
@@ -28,7 +28,7 @@ struct ConvParams {
   int ky, kx;       // filter size
   int cin_p;        // padded input channels (multiple of 64)
   int cout_p;       // padded output channels (multiple of 64)
-  int n_tile;       // UMMA N (cout_p / num_n_tiles), multiple of 32, <= 256
+  int n_tile;       // wgmma N (cout_p / num_n_tiles), multiple of 32, <= 256
   int num_m_tiles, num_n_tiles;
   int split;        // 0: fp16 operands; 1: 3-term split-fp16 ("fp32-equivalent") - A and W carry [hi | lo] halves
   // epilogue
@@ -42,11 +42,6 @@ struct ConvParams {
   const float* bn_bias;   // [cout_p]
   int act;                // kgb::Activation
   const float* mask;      // [M] 1.0 on-board, 0.0 pad/off-board
-  // kgb_conv_tc3.cu only: the residual enters through the tensor pipe instead of the epilogue.  The weights carry cout_p extra
-  // K columns holding the identity ([tap 0][co][cin_p + co] = 1), and after the cin_p / 64 real k-blocks the kernel runs n_tile / 64
-  // more whose A operand is the residual stream itself (fp16, exact in the fp32 accumulator): the residual rides the deep,
-  // prefetched A ring and the epilogue has no load left.  `residual` must then be null.
-  int res_via_mma;
 };
 
 // fp32 activation functions shared by every epilogue (reference: eigenbackend.cpp:780-809, cudahelpers.cu mish/silu).
@@ -162,20 +157,11 @@ __device__ __forceinline__ void epilogue_chunk(const ConvParams& p, const uint32
   }
 }
 
-// Launchers (defined in kgb_conv_tc.cu / kgb_kernels.cu)
-cudaError_t launchConvTC(const CUtensorMap& tmapA, const CUtensorMap& tmapB, const ConvParams& p, int numSMs, cudaStream_t stream);
+// Launchers (defined in kgb_conv_wg.cu / kgb_kernels.cu)
+// tmapA: [M][cin_p (* 2)] fp16, box {64, convABoxRows}; tmapB: packed weights, box {64, n_tile}; both 128B swizzle.
+cudaError_t launchConvWG(const CUtensorMap& tmapA, const CUtensorMap& tmapB, const ConvParams& p, cudaStream_t stream);
 cudaError_t launchConvSimt(const __half* A, int lda, const __half* W, const ConvParams& p, cudaStream_t stream);
-int convTCSmemBytes(int n_tile, int cout_p, int a_box_rows, int tps, int epi_warps, int* stagesOut);
-inline int convTCABoxRows(int ky, int kx, int Wp) { return 128 + 2 * ((ky / 2) * Wp + (kx / 2)); }  // TMA box rows of the A halo tile
-cudaError_t convTCInit();  // per device, before the first launch
-// CTA-pair kernel (kgb_conv_tc2.cu); tmapBhalf has box rows n_tile/2.  cudaErrorNotSupported = shape not handled, use launchConvTC.
-cudaError_t convTC2Init();
-cudaError_t launchConvTC2(const CUtensorMap& tmapA, const CUtensorMap& tmapBhalf, const ConvParams& p, int numSMs, cudaStream_t stream);
-// CTA-pair kernel with TMA epilogue and deep operand rings (kgb_conv_tc3.cu): fp16 mode's production kernel.
-// tmapRes / tmapRaw / tmapAct: [M][cout_p] tensors, box {64 fp16 | 32 fp32 columns, 32 rows}, 128B swizzle (unused ones: any valid map).
-cudaError_t convTC3Init();
-bool convTC3Supports(const ConvParams& p);
-cudaError_t launchConvTC3(const CUtensorMap& tmapA, const CUtensorMap& tmapBhalf, const CUtensorMap& tmapRes, const CUtensorMap& tmapRaw,
-                          const CUtensorMap& tmapAct, const ConvParams& p, int numSMs, cudaStream_t stream);
+inline int convABoxRows(int ky, int kx, int Wp) { return 128 + 2 * ((ky / 2) * Wp + (kx / 2)); }  // TMA box rows of the A halo tile
+cudaError_t convWGInit();  // per device, before the first launch
 
 }  // namespace kgb

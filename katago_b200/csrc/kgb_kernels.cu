@@ -1,4 +1,4 @@
-// fp32 support kernels of the NN evaluator (everything that is not the tcgen05 convolution).  HBM/latency-bound byte
+// fp32 support kernels of the NN evaluator (everything that is not the wgmma convolution).  HBM/latency-bound byte
 // shuffling and small reductions: coalesced along channels, one pass over the data each.
 #include "kgb_kernels.cuh"
 
@@ -273,7 +273,7 @@ cudaError_t launchFinalize(const float* passLogits, int ldp, int cp2, const floa
 
 // ------------------------------------------------------------------------------------------------------------
 // SIMT debug/bring-up convolution: same operands, same epilogue, no tensor cores.  Selected with KGB_CONV_IMPL=simt;
-// lets tests separate "layout/graph logic" failures from "tcgen05/TMA plumbing" failures on the GPU.
+// lets tests separate "layout/graph logic" failures from "wgmma/TMA plumbing" failures on the GPU.
 // One thread per (row, 16-column chunk).
 __global__ void convSimtKernel(const __half* __restrict__ A, int lda, const __half* __restrict__ W, const ConvParams p) {
   int chunks = p.cout_p / 16;

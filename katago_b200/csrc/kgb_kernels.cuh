@@ -1,4 +1,4 @@
-// Small fp32 kernels around the tcgen05 convolution: input packing, pooling, tiny matmuls, head outputs.
+// Small fp32 kernels around the wgmma convolution: input packing, pooling, tiny matmuls, head outputs.
 #pragma once
 #include "kgb_conv.cuh"
 

@@ -1,4 +1,4 @@
-// Model-file loader for the B200 NN evaluator.  See kgb_model.h for the reference lines this mirrors.
+// Model-file loader for the H100 NN evaluator.  See kgb_model.h for the reference lines this mirrors.
 #include "kgb_model.h"
 
 #include <zlib.h>
@@ -143,7 +143,7 @@ ConvDesc parseConv(Reader& r) {
   if(c.cin <= 0 || c.cout <= 0) throw std::runtime_error(c.name + ": number of in and out channels must be positive");
   // sane limits before the sizes are multiplied (the product below cannot wrap a size_t once these hold)
   if(c.ky > 15 || c.kx > 15 || c.cin > 16384 || c.cout > 16384) throw std::runtime_error(c.name + ": convolution of unreasonable size (" + std::to_string(c.ky) + "x" + std::to_string(c.kx) + ", " + std::to_string(c.cin) + " -> " + std::to_string(c.cout) + " channels)");
-  if(dy != 1 || dx != 1) throw std::runtime_error(c.name + ": dilated convolutions are not supported by the B200 backend");
+  if(dy != 1 || dx != 1) throw std::runtime_error(c.name + ": dilated convolutions are not supported by the H100 backend");
   r.readFloats((size_t)c.ky * c.kx * c.cin * c.cout, c.name, c.w);
   return c;
 }
@@ -240,7 +240,7 @@ BlockDesc parseBlock(Reader& r, int version, const std::string& kind) {
       throw std::runtime_error(b.name + ": nested block channel mismatch");
   }
   else
-    throw std::runtime_error("block kind '" + kind + "' is not supported by the B200 backend (transformer nets are out of scope)");
+    throw std::runtime_error("block kind '" + kind + "' is not supported by the H100 backend (transformer nets are out of scope)");
   return b;
 }
 
@@ -374,7 +374,7 @@ std::unique_ptr<ModelDesc> parseModel(const std::string& data, bool binaryFloats
   }
   if(v >= 15) {
     int metaEncoderVersion = r.readInt("metaEncoderVersion");
-    if(metaEncoderVersion != 0) throw std::runtime_error(m.name + ": SGF-metadata (humanSL) nets are not supported by the B200 backend");
+    if(metaEncoderVersion != 0) throw std::runtime_error(m.name + ": SGF-metadata (humanSL) nets are not supported by the H100 backend");
     m.preferPassAliveUnderSuicideRules = r.readInt("preferPassAliveUnderSuicideRules");
     if(m.preferPassAliveUnderSuicideRules != 0 && m.preferPassAliveUnderSuicideRules != 1)
       throw std::runtime_error(m.name + ": model preferPassAliveUnderSuicideRules unexpected value");
@@ -388,7 +388,7 @@ std::unique_ptr<ModelDesc> parseModel(const std::string& data, bool binaryFloats
   m.gpoolC = r.readInt("gpoolNumChannels");
   if(v >= 15) {
     int trunkNormKind = r.readInt("trunkNormKind");
-    if(trunkNormKind != 0) throw std::runtime_error(m.name + ": RMSNorm trunk tips are not supported by the B200 backend");
+    if(trunkNormKind != 0) throw std::runtime_error(m.name + ": RMSNorm trunk tips are not supported by the H100 backend");
     expectZeros(r, 5, "trunk option");
   }
   if(numBlocks < 1) throw std::runtime_error(m.name + ": trunk num blocks must be positive");

@@ -1,4 +1,4 @@
-// Host-side model description for the B200 NN evaluator (product code; does NOT depend on oracle/).
+// Host-side model description for the H100 NN evaluator (product code; does NOT depend on oracle/).
 //
 // Parses KataGo model files (.bin/.txt, optionally .gz) into plain structs and applies the same load-time weight
 // folding as the reference: BN merge (cpp/neuralnet/desc.cpp:282-289) and transformToReduceActivations

@@ -1,7 +1,7 @@
 """Host-side mirror of the reference's backend interface `namespace NeuralNet` (cpp/neuralnet/nninterface.h:32-182)
 over the C ABI of libkgb200.so (include/kgb200.h).  Same names, argument meaning and error behaviour as the
 reference: failures raise (StringError there, KGBError here); there is NO CPU fallback - a missing library or a
-missing sm_100 device is an error.
+missing sm_90 device is an error.
 
     model  = NeuralNet.loadModelFile(path, expectedSha256)          # nninterface.h:43
     ctx    = NeuralNet.createComputeContext([0], nnXLen, nnYLen, useFP16Mode, model)   # :50

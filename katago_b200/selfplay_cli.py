@@ -16,7 +16,7 @@ The reference randomises rules, board size and komi per game (GameInitializer); 
 keys (`koRules`, `bSizes`, ...) are drawn per game like the reference does (game_initializer.py); values the loop lacks are left out (reported).
 Under torchrun (one process per GPU) the ranks split `-max-games-total`, use LOCAL_RANK's GPU and their own seeds, and write into the
 same tdata directory (`shard_plan`); there is no collective on this path.
-There is no CPU fallback: without a B200 the command fails when it creates the evaluator."""
+There is no CPU fallback: without an H100 the command fails when it creates the evaluator."""
 import argparse
 import glob
 import os
@@ -470,7 +470,7 @@ class ModelPoller:
 
 
 def main(argv=None):
-    ap = argparse.ArgumentParser(prog="katago_b200.selfplay_cli", description="Self-play data generation on the B200 device loop", prefix_chars="-")
+    ap = argparse.ArgumentParser(prog="katago_b200.selfplay_cli", description="Self-play data generation on the H100 device loop", prefix_chars="-")
     ap.add_argument("-models-dir", required=True)
     ap.add_argument("-output-dir", required=True)
     ap.add_argument("-config", required=True)
@@ -482,8 +482,8 @@ def main(argv=None):
     ap.add_argument("-per-game-release", action="store_true", help="record and release every game as soon as its own search is finished "
                     "(GameRecorder.pump) instead of moving all games in lockstep")
     ap.add_argument("-max-playouts-per-wave", type=int, default=4, help="playouts a game may finish inside one wave without needing the evaluator (cache hits, "
-                    "graph-search catch-ups); the wave lasts as long as its slowest game, so a small bound pays with trained nets "
-                    "(profiles/r02_trained_net_playouts_per_wave_sweep.log); results do not depend on it")
+                    "graph-search catch-ups); the wave lasts as long as its slowest game, so the bound keeps one long descent from holding up "
+                    "the others; results do not depend on it")
     ap.add_argument("-model-poll-seconds", type=float, default=20.0, help="how often the models directory is checked for a newer net")
     ap.add_argument("-nccl-weights", action="store_true", help="under torchrun: rank 0 alone polls and reads new nets, the packed weights reach the other GPUs by ncclBroadcast")
     ap.add_argument("-model-poll-waves", type=int, default=64, help="with -nccl-weights: recorder iterations between two (collective) polls")
@@ -503,7 +503,7 @@ def main(argv=None):
     if report["not_built"]:
         print("[config] NOT BUILT, ignored: " + "; ".join(report["not_built"]), file=sys.stderr)
 
-    from .nn_backend import KGBError, NeuralNet, SelfPlay          # loads libkgb200; fails loudly without a B200
+    from .nn_backend import KGBError, NeuralNet, SelfPlay          # loads libkgb200; fails loudly without an H100
     from .npz_writer import RowRand, TrainingDataWriter
     from .game_recorder import GameRecorder
     model_path = newest_model(a.models_dir)

@@ -23,8 +23,8 @@ Pinning (see tests/test_oracle_nn.py): (1) the reference's own known-answer test
 embedded tiny nets, three positions, expected outputs and tolerances (tests/golden/tinymodel.json.gz + models/tiny*.bin.gz, read
 from the reference's test source by tests/golden/make_tinymodel_fixtures.py, input rows from the reference's fillRowV7); (2)
 tests/golden/torchref_*.npz: outputs of the reference's PyTorch model (python/katago/train/model_pytorch.py) on nets exported by
-the reference's exporter; (3) direct-convolution MAC counts equal to those of the reference's own loader.  The product passes
-the same known-answer test on a B200 through the unmodified reference binary (profiles/r01_reference_binary_on_b200_backend.log).
+the reference's exporter; (3) direct-convolution MAC counts equal to those of the reference's own loader.  The device path is
+held to the same known-answer test in tests/test_gpu_nn_parity.py.
 """
 from __future__ import annotations
 

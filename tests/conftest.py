@@ -9,7 +9,7 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run on the GPU box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run on a GPU machine with -m gpu)")
 
 
 def has_gpu() -> bool:
@@ -22,10 +22,10 @@ def has_gpu() -> bool:
 
 def pytest_collection_modifyitems(config, items):
     """A plain `pytest` on a machine without a GPU skips the tests marked `gpu` instead of failing in them (the product has no CPU
-    fallback, so they cannot pass there); `-m gpu` on the GPU box runs them."""
+    fallback, so they cannot pass there); `-m gpu` on a GPU machine runs them."""
     if has_gpu():
         return
-    skip = pytest.mark.skip(reason="needs a B200 (no CUDA device here)")
+    skip = pytest.mark.skip(reason="needs an H100 (no CUDA device here)")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

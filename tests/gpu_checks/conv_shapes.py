@@ -19,6 +19,7 @@ for k, cin, cout, count, name in shapes:
     flop = 2.0 * k * k * cin * cout * 361 * n
     cin_p, cout_p = (cin + 63) // 64 * 64, (cout + 63) // 64 * 64
     byts = n * 400 * (cin_p * 2 + cout_p * 2 + cout_p * 4)   # fp16 in, fp16 act out, fp32 raw out (upper bound: one of the two outputs is optional)
-    print(f"{name:24s} {k}x{k} {cin:4d}->{cout:4d} x{count:3d}: {us:7.1f} us  {flop / us / 1e6:7.1f} TFLOP/s  tensor floor {flop / 1682e12 * 1e6:5.1f} us  hbm floor {byts / 6.5e12 * 1e6:5.1f} us")
+    # floors from the H100 SXM data sheet (989 dense fp16 TFLOP/s, 3.35 TB/s HBM3), not reached rates
+    print(f"{name:24s} {k}x{k} {cin:4d}->{cout:4d} x{count:3d}: {us:7.1f} us  {flop / us / 1e6:7.1f} TFLOP/s  tensor floor {flop / 989e12 * 1e6:5.1f} us  hbm floor {byts / 3.35e12 * 1e6:5.1f} us")
     tot += us * count
 print(f"sum over b18 layers: {tot / 1e3:.2f} ms")

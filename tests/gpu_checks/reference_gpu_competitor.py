@@ -5,7 +5,7 @@ both through the reference's `katago benchmark` command (multi-threaded search o
 
 Needs oracle/_ref/katago_cuda (oracle/Makefile.cuda) and oracle/_ref/katago_b200 (oracle/Makefile.drivers), both built where the
 reference sources are and shipped with the snapshot.  Random-weight b18c384nbt (no network for real nets): policies are near
-uniform, trees wide and shallow - the same caveat as bench.py's.  Not a bench.py line: a measurement note for profiles/."""
+uniform, trees wide and shallow - the same caveat as bench.py's.  Not a bench.py line: a measurement note."""
 import json, os, re, subprocess, sys, tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -26,15 +26,15 @@ def test_library_exports_every_declared_symbol():
     assert sorted(nn_backend.ABI_SYMBOLS) == syms
 
 
-def test_library_is_sm100a_native():
-    """SASS carries tcgen05 MMA, TMA and TMEM loads (B200_PROFILING.md 'What proves a Blackwell-native kernel')."""
+def test_library_is_sm90a_native():
+    """SASS carries Hopper warpgroup MMAs (wgmma), TMA loads and ldmatrix, compiled for sm_90a."""
     import shutil, subprocess
     if shutil.which("cuobjdump") is None:
         pytest.skip("cuobjdump not on PATH")
     sass = subprocess.run(["cuobjdump", "-sass", nn_backend.library_path()], capture_output=True, text=True).stdout
-    for mnemonic in ("UTCHMMA", "UTMALDG", "LDTM"):
+    for mnemonic in ("HGMMA", "UTMALDG", "LDSM"):
         assert mnemonic in sass
-    assert "sm_100a" in sass
+    assert "sm_90a" in sass
 
 
 @pytest.mark.parametrize("key", ["tiny_reg", "tiny_nbt", "tiny_nbt_gz", "tiny_relu_v8"])

@@ -13,20 +13,15 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
-REF = "/root/reference/cpp"
-REF_LIB = os.path.join(ROOT, "oracle", "_ref", "libkgref.a")
+MOCK = {name: os.path.join(ROOT, "oracle", "_ref", f"b200_{name}_mock") for name in ("selfplay", "gatekeeper", "match")}
 
-pytestmark = pytest.mark.skipif(not (os.path.isdir(REF) and os.path.exists(REF_LIB)), reason="needs the reference sources and oracle/_ref/libkgref.a (the mock plays on the reference's Board)")
+# the hosts linked against tests/mock/kgb200_mock.cpp, which plays on the reference's Board: oracle/Makefile.mocks builds them
+pytestmark = pytest.mark.skipif(not all(os.path.exists(p) for p in MOCK.values()), reason="oracle/_ref/b200_*_mock not built (needs the reference sources at build time)")
 
 
 @pytest.fixture(scope="module")
-def host_on_mock(tmp_path_factory):
-    exe = tmp_path_factory.mktemp("cpphost_mock") / "b200_selfplay_mock"
-    subprocess.run(["g++", "-O1", "-std=c++17", "-mfpmath=sse", "-DNDEBUG", "-DNO_GIT_REVISION", "-DNO_LIBZIP", "-w", "-I" + REF, "-I" + REF + "/external",
-                    "-isystem", REF + "/external/tclap-1.2.5/include", "-isystem", REF + "/external/filesystem-1.5.8/include", "-I" + ROOT, "-o", str(exe),
-                    os.path.join(ROOT, "integration", "b200_selfplay_main.cpp"), os.path.join(ROOT, "tests", "mock", "kgb200_mock.cpp"),
-                    "-Wl,--start-group", REF_LIB, "-Wl,--end-group", "-lz", "-lpthread"], check=True, cwd=ROOT)
-    return str(exe)
+def host_on_mock():
+    return MOCK["selfplay"]
 
 
 def _replay_slots_with_limits(log, G, size, V, uneven=0):
@@ -381,7 +376,7 @@ def test_cpp_host_ranks_swap_nets_together_under_nccl_weights(tmp_path, host_on_
     """-nccl-weights, two ranks of one node (one process per GPU): rank 0 alone polls the models directory, packs the new net and announces the swap; both
     ranks join the library's broadcast of the packed weights and commit, each keeps playing its share of the games with its own seeds and file names, and a
     rank that finishes early stays until every rank has.  (On the mock the collective calls only have to line up; the broadcast itself is the library's,
-    measured on GPUs through the Python host: profiles/r02_*weight_broadcast*.)"""
+    tested on the GPU in tests/test_gpu_weight_swap.py.)"""
     import json, re
     G, V, size = 3, 20, 7
     cfg = tmp_path / "c.cfg"
@@ -419,13 +414,8 @@ def test_cpp_host_ranks_swap_nets_together_under_nccl_weights(tmp_path, host_on_
 
 
 @pytest.fixture(scope="module")
-def gatekeeper_on_mock(tmp_path_factory):
-    exe = tmp_path_factory.mktemp("cppgate_mock") / "b200_gatekeeper_mock"
-    subprocess.run(["g++", "-O1", "-std=c++17", "-mfpmath=sse", "-DNDEBUG", "-DNO_GIT_REVISION", "-DNO_LIBZIP", "-w", "-I" + REF, "-I" + REF + "/external",
-                    "-isystem", REF + "/external/tclap-1.2.5/include", "-isystem", REF + "/external/filesystem-1.5.8/include", "-I" + ROOT, "-o", str(exe),
-                    os.path.join(ROOT, "integration", "b200_gatekeeper_main.cpp"), os.path.join(ROOT, "tests", "mock", "kgb200_mock.cpp"),
-                    "-Wl,--start-group", REF_LIB, "-Wl,--end-group", "-lz", "-lpthread"], check=True, cwd=ROOT)
-    return str(exe)
+def gatekeeper_on_mock():
+    return MOCK["gatekeeper"]
 
 
 @pytest.mark.parametrize("uneven", [0, 9], ids=["instant_searches", "uneven_searches"])
@@ -487,11 +477,7 @@ def test_cpp_match_plays_two_named_bots_like_the_python_match(tmp_path, uneven):
     """`katago match` for two named bots as a C++-only host (integration/b200_match_main.cpp): per-bot search keys (maxVisits0 / maxVisits1), alternating
     colours, per-game setups - against the Python match engine on the mock loops' logs: the record file character for character, the same wins and points."""
     import re
-    exe = tmp_path / "b200_match_mock"
-    subprocess.run(["g++", "-O1", "-std=c++17", "-mfpmath=sse", "-DNDEBUG", "-DNO_GIT_REVISION", "-DNO_LIBZIP", "-w", "-I" + REF, "-I" + REF + "/external",
-                    "-isystem", REF + "/external/tclap-1.2.5/include", "-isystem", REF + "/external/filesystem-1.5.8/include", "-I" + ROOT, "-o", str(exe),
-                    os.path.join(ROOT, "integration", "b200_match_main.cpp"), os.path.join(ROOT, "tests", "mock", "kgb200_mock.cpp"),
-                    "-Wl,--start-group", REF_LIB, "-Wl,--end-group", "-lz", "-lpthread"], check=True, cwd=ROOT)
+    exe = MOCK["match"]
     from katago_b200 import match_cli as MC, selfplay_cli as C
     from katago_b200.game_initializer import GameInitializer
     from katago_b200.match_play import MatchPlay

@@ -5,6 +5,7 @@ import subprocess
 import sys
 
 import numpy as np
+import pytest
 import torch.multiprocessing as mp
 
 from conftest import ROOT
@@ -76,6 +77,8 @@ def test_weight_broadcaster_world2_protocol(tmp_path):
     assert r[0]["ms"] == r[1]["ms"] == 1.5
 
 
+@pytest.mark.skipif(not os.path.exists(os.path.join(ROOT, "oracle", "_ref", "kgref_cpu_selfplay")),
+                    reason="the reference arm runs oracle/_ref/kgref_cpu_selfplay, which build() makes only where the reference sources are")
 def test_bench_reference_arm_prints_contract_json():
     p = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--impl", "reference", "--model", "tiny_nbt", "--steps", "2",
                         "--warmup", "1"], capture_output=True, text=True, timeout=300)

@@ -1,4 +1,4 @@
-"""GPU parity tests (B200): the CUDA path THROUGH THE C ABI against the numpy oracle, the committed golden fixtures
+"""GPU parity tests (H100): the CUDA path THROUGH THE C ABI against the numpy oracle, the committed golden fixtures
 (reference PyTorch model outputs), and size-independent properties at BASELINE.json's full sizes.
 
 Tolerances (written here on purpose):
@@ -226,7 +226,7 @@ def test_full_size_b18_batch256(cfg, tmp_path):
 def test_reference_tiny_net_known_answers_on_device(golden_dir, fp16):
     """The reference's own known-answer test for the NN path (cpp/tests/tinymodel.cpp; fixture tests/golden/tinymodel.json.gz) through the
     C ABI: its two embedded nets, three positions (one 13x6 on the 19x19 frame), the symmetries it fixes, the outputs it expects and
-    its own tolerances.  (The unmodified reference binary linked to this library passes the same test: profiles/.)"""
+    its own tolerances."""
     import gzip, json
     from test_oracle_nn import _post_process
     blocks = json.loads(gzip.open(os.path.join(golden_dir, "tinymodel.json.gz"), "rb").read())

@@ -1,4 +1,4 @@
-"""GPU tests (B200) of the weight hot-swap behind the C ABI (include/kgb200.h: kgb_handle_stage_weights,
+"""GPU tests (H100) of the weight hot-swap behind the C ABI (include/kgb200.h: kgb_handle_stage_weights,
 kgb_handle_commit_weights, kgb_nccl_unique_id, kgb_handle_comm_init, kgb_handle_broadcast_staged_weights).
 
 Reference behaviour replaced: the self-play command polls its models directory and builds a fresh NNEvaluator per new net

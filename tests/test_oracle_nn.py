@@ -128,7 +128,7 @@ def test_oracle_passes_the_reference_tiny_net_known_answer_test(golden_dir):
     """The reference's own known-answer test for the NN path (cpp/tests/tinymodel.cpp): its two embedded nets (a v9 net and a v11 mish
     net), its three positions (19x19 twice, 13x6 on a 19x19 frame) under the symmetries it fixes, the outputs it expects and the
     tolerances it allows - all read from the reference's test source by tests/golden/make_tinymodel_fixtures.py, with the input rows
-    from the reference's fillRowV7.  The numpy oracle must pass it (the product passes it on a B200 through the reference binary)."""
+    from the reference's fillRowV7.  The numpy oracle must pass it (the device path is held to it in tests/test_gpu_nn_parity.py)."""
     import gzip, json
     blocks = json.loads(gzip.open(os.path.join(golden_dir, "tinymodel.json.gz"), "rb").read())
     assert [(b["model"], b["symmetry"], b["X"], b["Y"]) for b in blocks] == [("tinymodel", 6, 19, 19), ("tinymishmodel", 7, 19, 19), ("tinymishmodel", 1, 13, 6)]

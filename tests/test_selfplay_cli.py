@@ -140,7 +140,7 @@ def test_neutral_values_and_unsupported_rules():
 
 
 def test_command_fails_loudly_without_a_gpu(tmp_path, stock_cfg):
-    """No CPU fallback: on a machine without a B200 the command stops at the evaluator with the library's error."""
+    """No CPU fallback: on a machine without an H100 the command stops at the evaluator with the library's error."""
     import torch
     if torch.cuda.is_available():
         pytest.skip("a GPU is present")
@@ -153,7 +153,7 @@ def test_command_fails_loudly_without_a_gpu(tmp_path, stock_cfg):
 
 @pytest.mark.gpu
 def test_command_writes_training_files(tmp_path, stock_cfg):
-    """End to end on a B200: models dir + reference-style .cfg -> <output-dir>/<model>/tdata/<16 hex>.npz readable as training rows."""
+    """End to end on an H100: models dir + reference-style .cfg -> <output-dir>/<model>/tdata/<16 hex>.npz readable as training rows."""
     import numpy as np
     from katago_b200 import modelgen
     models = tmp_path / "models"; models.mkdir()
