@@ -422,13 +422,14 @@ KGB_API int kgb_bench_conv(int ky, int kx, int in_c, int out_c, int n, int nn_x_
                    float* ms_per_launch);
 /* The same with the epilogue chosen: epilogue_kind 0 = fp32 raw output only (heads / gpool conv), 1 = BN + mish + mask -> fp16 (first conv
  * of a residual unit), 2 = + residual stream read and rewritten in place (second conv of a unit, a nested block's post conv), 3 = raw
- * stream + activated operand (a nested block's pre conv).  `rotate` >= 1 independent input / output buffer sets are cycled through so
- * that the timed loop's working set exceeds L2. */
+ * stream + activated operand (a nested block's pre conv), 4 = kind 2 with an fp32 residual stream also in fp16 mode (the trunk's block
+ * exit with KGB_STREAM_FP32=trunk; in fp32-equivalent mode every stream is fp32).  `rotate` >= 1 independent input / output buffer
+ * sets are cycled through so that the timed loop's working set exceeds L2. */
 KGB_API int kgb_bench_conv_ex(int ky, int kx, int in_c, int out_c, int n, int nn_x_len, int nn_y_len, int use_fp16, int epilogue_kind, int rotate,
                       int warmup, int iters, float* ms_per_launch);
-/* Test hook for the fused epilogues (kinds 1-3 above) of one convolution layer: NHWC input [n][y][x][in_c], optional NHWC residual
+/* Test hook for the fused epilogues (kinds 1-4 above) of one convolution layer: NHWC input [n][y][x][in_c], optional NHWC residual
  * [n][y][x][out_c], per-channel BN scale / bias (NULL = 1 / 0), activation (0 identity, 1 relu, 2 mish); returns the raw stream after
- * the launch (kinds 2, 3) and the activated fp16 operand, both NHWC [n][y][x][out_c] as floats.  Also checks that every pad row of the
+ * the launch (kinds 2-4) and the activated fp16 operand, both NHWC [n][y][x][out_c] as floats.  Also checks that every pad row of the
  * activated operand was written as zero (reference semantics: the conv's zero padding, eigenbackend.cpp:448-701). */
 KGB_API int kgb_test_conv_epilogue(int ky, int kx, int in_c, int out_c, const float* weights, int n, int nn_x_len, int nn_y_len, int use_fp16,
                            int epilogue_kind, const float* input, const float* residual_in, const float* bn_scale, const float* bn_bias,

@@ -93,6 +93,22 @@ static CUtensorMap makeTmap2D(const void* ptr, uint64_t rows, uint64_t cols, uin
   return m;
 }
 
+// Residual stream [rows][cols], fp32 or fp16, box {32 cols, 128 rows}: the slices the convolution's epilogue reads from shared
+// memory, 128B-swizzled for fp32 (128 B rows) and 64B-swizzled for fp16 (64 B rows), zero OOB fill.
+static CUtensorMap makeTmapResidual(const void* ptr, uint64_t rows, uint64_t cols, bool fp32) {
+  CUtensorMap m;
+  const uint64_t esize = fp32 ? sizeof(float) : sizeof(__half);
+  cuuint64_t gdim[2] = {cols, rows};
+  cuuint64_t gstride[1] = {cols * esize};
+  cuuint32_t box[2] = {32, 128};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = getEncodeTiled()(&m, fp32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(ptr), gdim,
+                                gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, fp32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                                CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if(r != CUDA_SUCCESS) throw CudaFailure("cuTensorMapEncodeTiled (residual) failed with CUresult " + std::to_string((int)r));
+  return m;
+}
+
 // ------------------------------------------------------------------------------------------------------------
 // Opaque handles
 // ------------------------------------------------------------------------------------------------------------
@@ -319,6 +335,9 @@ struct Builder {
   // Emit one convolution op.  residual/rawOut may alias (in-place residual update).
   void emitConv(const ConvWeights& cw, const __half* A, const void* residual, bool residualFp32, const float* ncbias, void* rawOut,
                 bool rawFp32, __half* actOut, BNDev bn) {
+    // the kernel reads a tile's halo rows of A while the neighbouring tiles write their outputs (the scratch passes have no buffers)
+    if(h.wMode == kgb_handle::W_BUILD && ((const void*)A == (const void*)actOut || (const void*)A == rawOut))
+      throw std::logic_error("emitConv: the operand aliases an output");
     kgb_handle* hp = &h;
     const int actMulL = actMul;
     h.ops.push_back([=](int n, cudaStream_t s) {
@@ -344,7 +363,10 @@ struct Builder {
       }
       else {
         CUtensorMap tmA = makeTmap2D(A, (uint64_t)p.M, (uint64_t)cw.cin_p * actMulL, (uint32_t)convABoxRows(cw.ky, cw.kx, p.Wp));
-        CK(launchConvWG(tmA, cw.tmapB, p, s));
+        CUtensorMap tmR;
+        memset(&tmR, 0, sizeof(tmR));
+        if(residual != nullptr) tmR = makeTmapResidual(residual, (uint64_t)p.M, (uint64_t)cw.cout_p, residualFp32);
+        CK(launchConvWG(tmA, cw.tmapB, tmR, p, s));
       }
     });
     h.launchesPerForward++;
@@ -949,6 +971,7 @@ struct SingleConv {
   size_t M;
   std::vector<__half*> As, acts;
   std::vector<void*> streams;
+  bool streamF32 = false;  // the residual / raw stream of kinds 2-4 is fp32
   int rotate, next = 0;
   SingleConv(int ky, int kx, int in_c, int out_c, const float* weights, int n_, int X_, int Y_, int use_fp16, int actEpilogue = 0,
              int rotate_ = 1, const float* bnScale = nullptr, const float* bnBias = nullptr, int actKind = ACT_MISH)
@@ -983,14 +1006,16 @@ struct SingleConv {
     raw = h.dalloc<float>(M * cw.cout_p);
     // actEpilogue: 0 = fp32 raw output only; 1 = the first conv of a residual unit (BN + mish + mask -> fp16 operand of the next
     // conv); 2 = the second conv of a unit (+ fp16 residual stream, updated in place, and the next unit's BN + mish operand);
-    // 3 = a nested block's pre conv (fp16 raw stream + activated operand).  `rotate` independent buffer sets are cycled through
-    // by run() so that a timing loop does not live in L2.
+    // 3 = a nested block's pre conv (fp16 raw stream + activated operand); 4 = kind 2 with an fp32 residual stream, as the trunk
+    // runs in fp16 mode with KGB_STREAM_FP32=trunk.  In fp32-equivalent mode every stream is fp32.  `rotate` independent buffer
+    // sets are cycled through by run() so that a timing loop does not live in L2.
     BNDesc bn;
     bn.c = out_c; bn.scale.assign(out_c, 1.0f); bn.bias.assign(out_c, 0.0f);
     if(bnScale) bn.scale.assign(bnScale, bnScale + out_c);
     if(bnBias) bn.bias.assign(bnBias, bnBias + out_c);
     Builder::BNDev dev = b.uploadBN(bn, actKind, cw.cout_p);
     h.wFlushLive();
+    streamF32 = h.split != 0 || actEpilogue == 4;
     for(int r = 0; r < rotate; r++) {
       __half* Ar = r == 0 ? A : h.dalloc<__half>(M * cw.cin_p * b.actMul);
       As.push_back(Ar);
@@ -1004,10 +1029,9 @@ struct SingleConv {
         acts.push_back(actOut);
         if(actEpilogue == 1) b.emitConv(cw, Ar, nullptr, false, nullptr, nullptr, false, actOut, dev);
         else {
-          const bool f32 = h.split != 0;
-          void* S = f32 ? (void*)h.dalloc<float>(M * cw.cout_p) : (void*)h.dalloc<__half>(M * cw.cout_p);
+          void* S = streamF32 ? (void*)h.dalloc<float>(M * cw.cout_p) : (void*)h.dalloc<__half>(M * cw.cout_p);
           streams.push_back(S);
-          b.emitConv(cw, Ar, actEpilogue == 2 ? S : nullptr, f32, nullptr, S, f32, actOut, dev);
+          b.emitConv(cw, Ar, actEpilogue == 3 ? nullptr : S, streamF32, nullptr, S, streamF32, actOut, dev);
         }
       }
     }
@@ -1062,7 +1086,7 @@ KGB_API int kgb_test_conv(int ky, int kx, int in_c, int out_c, const float* weig
 
 static void benchConvImpl(int ky, int kx, int in_c, int out_c, int n, int nn_x_len, int nn_y_len, int use_fp16, int epilogue_kind, int rotate,
                           int warmup, int iters, float* ms_per_launch) {
-  if(!ms_per_launch || n < 1 || iters < 1 || epilogue_kind < 0 || epilogue_kind > 3) throw std::invalid_argument("kgb_bench_conv: bad argument");
+  if(!ms_per_launch || n < 1 || iters < 1 || epilogue_kind < 0 || epilogue_kind > 4) throw std::invalid_argument("kgb_bench_conv: bad argument");
   std::vector<float> w((size_t)ky * kx * in_c * out_c);
   uint32_t st = 12345u;
   for(auto& v : w) { st = st * 1664525u + 1013904223u; v = ((st >> 8) * (1.0f / 16777216.0f) - 0.5f) * 0.1f; }
@@ -1098,15 +1122,16 @@ KGB_API int kgb_test_conv_epilogue(int ky, int kx, int in_c, int out_c, const fl
                            int epilogue_kind, const float* input, const float* residual_in, const float* bn_scale, const float* bn_bias,
                            int activation, float* raw_out, float* act_out) {
   return guarded([&] {
-    if(!weights || !input || !act_out || n < 1 || epilogue_kind < 1 || epilogue_kind > 3) throw std::invalid_argument("kgb_test_conv_epilogue: bad argument");
-    if(epilogue_kind == 2 && !residual_in) throw std::invalid_argument("kgb_test_conv_epilogue: kind 2 needs residual_in");
-    if(epilogue_kind >= 2 && !raw_out) throw std::invalid_argument("kgb_test_conv_epilogue: kinds 2 and 3 need raw_out");
+    if(!weights || !input || !act_out || n < 1 || epilogue_kind < 1 || epilogue_kind > 4) throw std::invalid_argument("kgb_test_conv_epilogue: bad argument");
+    const bool hasResidual = epilogue_kind == 2 || epilogue_kind == 4;
+    if(hasResidual && !residual_in) throw std::invalid_argument("kgb_test_conv_epilogue: kinds 2 and 4 need residual_in");
+    if(epilogue_kind >= 2 && !raw_out) throw std::invalid_argument("kgb_test_conv_epilogue: kinds 2 to 4 need raw_out");
     SingleConv sc(ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16, epilogue_kind, 1, bn_scale, bn_bias, activation);
     sc.setInput(input);
     const int cp = sc.cw.cout_p;
-    const bool f32 = sc.h.split != 0;
+    const bool f32 = sc.streamF32;
     auto rowOf = [&](int i, int y, int x) { return (size_t)i * sc.h.L.P + (size_t)(y + sc.pad) * sc.h.L.Wp + x; };
-    if(epilogue_kind == 2) {
+    if(hasResidual) {
       std::vector<float> hf(sc.M * cp, 0.0f);
       for(int i = 0; i < n; i++) for(int y = 0; y < nn_y_len; y++) for(int x = 0; x < nn_x_len; x++) for(int c = 0; c < out_c; c++)
         hf[rowOf(i, y, x) * cp + c] = residual_in[(((size_t)i * nn_y_len + y) * nn_x_len + x) * out_c + c];
@@ -1120,7 +1145,7 @@ KGB_API int kgb_test_conv_epilogue(int ky, int kx, int in_c, int out_c, const fl
     }
     sc.run();
     CK(cudaStreamSynchronize(sc.h.stream));
-    const int am = f32 ? 2 : 1;
+    const int am = sc.h.split ? 2 : 1;
     std::vector<__half> ha(sc.M * cp * am);
     CK(cudaMemcpy(ha.data(), sc.acts[0], ha.size() * sizeof(__half), cudaMemcpyDeviceToHost));
     std::vector<float> hr;
@@ -1142,7 +1167,7 @@ KGB_API int kgb_test_conv_epilogue(int ky, int kx, int in_c, int out_c, const fl
           if(__half2float(ha[r * cp * am + c]) != 0.0f) throw std::runtime_error("kgb_test_conv_epilogue: pad row " + std::to_string(r) + " of the activation output is not zero");
     for(int i = 0; i < n; i++) for(int y = 0; y < nn_y_len; y++) for(int x = 0; x < nn_x_len; x++) for(int c = 0; c < out_c; c++) {
       const size_t row = rowOf(i, y, x), o = (((size_t)i * nn_y_len + y) * nn_x_len + x) * out_c + c;
-      act_out[o] = __half2float(ha[row * cp * am + c]) + (f32 ? __half2float(ha[row * cp * am + cp + c]) : 0.0f);
+      act_out[o] = __half2float(ha[row * cp * am + c]) + (am == 2 ? __half2float(ha[row * cp * am + cp + c]) : 0.0f);
       if(epilogue_kind >= 2) raw_out[o] = hr[row * cp + c];
     }
   });

@@ -159,7 +159,11 @@ __device__ __forceinline__ void epilogue_chunk(const ConvParams& p, const uint32
 
 // Launchers (defined in kgb_conv_wg.cu / kgb_kernels.cu)
 // tmapA: [M][cin_p (* 2)] fp16, box {64, convABoxRows}; tmapB: packed weights, box {64, n_tile}; both 128B swizzle.
-cudaError_t launchConvWG(const CUtensorMap& tmapA, const CUtensorMap& tmapB, const ConvParams& p, cudaStream_t stream);
+// tmapR (read only when p.residual is set): the residual [M][cout_p], box {32, 128}, 128B swizzle when fp32, 64B when fp16.
+// The residual may alias raw_out (each element is read and written by the CTA of its own tile); A must alias neither raw_out nor
+// act_out, since a tile's halo rows belong to the neighbouring tiles.
+cudaError_t launchConvWG(const CUtensorMap& tmapA, const CUtensorMap& tmapB, const CUtensorMap& tmapR, const ConvParams& p,
+                         cudaStream_t stream);
 cudaError_t launchConvSimt(const __half* A, int lda, const __half* W, const ConvParams& p, cudaStream_t stream);
 inline int convABoxRows(int ky, int kx, int Wp) { return 128 + 2 * ((ky / 2) * Wp + (kx / 2)); }  // TMA box rows of the A halo tile
 cudaError_t convWGInit();  // per device, before the first launch

@@ -14,9 +14,13 @@
 //   D   = fp32 in registers: warpgroup g of the two consumer warpgroups owns rows 64g..64g+63 of the 128-row tile.
 //
 // One CTA per (128-row, n_tile) tile, 384 threads:
-//   warpgroup 0   TMA producer (one lane): A halo tiles into a 2-deep ring, one weight tile per tap into a deeper ring
+//   warpgroup 0   TMA producer (one lane): A halo tiles into a 2-deep ring, one weight tile per tap into a deeper ring, and the
+//                 tile's residual in 32-column slices into a 4-slot ring (the first slices at the start, so they land during the
+//                 main loop; the rest as the epilogue frees slots)
 //   warpgroups 1-2  ldmatrix + wgmma.mma_async m64 x n_tile x 16, then the fused epilogue straight from the accumulators
-// While one consumer warpgroup loads its next A fragments the other one's wgmma keeps the tensor core busy.
+// The A fragments are double-buffered in registers: step t+1's ldmatrix runs while step t's wgmma group is still in flight,
+// and a consumer waits only for the group before the one it just issued (wait_group 1).  The epilogue reads the residual, the
+// mask and the BN constants from shared memory, so no global load sits between its stores.
 //
 // "split" mode computes a*w ~= ah*wh + al*wh + ah*wl with a = ah + al, w = wh + wl in fp16 (fp32 accumulate):
 // fp32-grade accuracy on the fp16 tensor pipe at 3x the MMA count (the backend's useFP16=false mode).
@@ -31,6 +35,8 @@ static constexpr int MAX_STAGES = 8;
 static constexpr int SMEM_LIMIT = 227 * 1024;
 static constexpr int THREADS = 384;
 static constexpr int CONSUMER_WARPS = 8;
+static constexpr int RES_COLS = 32;     // columns of one residual slice (every n_tile is a multiple of 32)
+static constexpr int RES_SLOTS = 4;     // residual ring: 4 x 16 KB for an fp32 stream, 4 x 8 KB for fp16
 
 // ------------------------------------------------------------------------------------------------------------
 // PTX wrappers
@@ -73,6 +79,8 @@ __device__ __forceinline__ void fence_acc(float (&d)[N]) {
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }   // the two consumer warpgroups
 
 // wgmma shared-memory descriptor, K-major, 128B swizzle:
 //   [0,14) start>>4 | [16,30) LBO>>4 (1, unused for swizzled K-major) | [32,46) SBO>>4 (1024 B = 8 rows x 128 B) | [62,64) 1 = 128B swizzle
@@ -91,35 +99,40 @@ struct __align__(8) Bars {
   uint64_t empty[MAX_STAGES];   // weight tile consumed by every consumer warp
   uint64_t a_full[2];           // A halo tile landed
   uint64_t a_empty[2];          // A halo tile consumed by all of its taps
+  uint64_t r_full[RES_SLOTS];   // residual slice landed
+  uint64_t r_empty[RES_SLOTS];  // residual slice consumed by every consumer warp
 };
 
-// dynamic smem: [<=1023 B slack][2 x A halo tile][stages x weight tile][Bars]
+// dynamic smem: [<=1023 B slack][2 x A halo tile][RES_SLOTS x residual slice][stages x weight tile][Bars][mask 128][BN scale N][BN bias N]
 static inline int aBufBytes(int a_box_rows) { return (a_box_rows * BLOCK_K * 2 + 1023) / 1024 * 1024; }
+// One residual slice = one TMA box of 128 rows x 32 columns.  fp32 rows are 128 B with the 128B swizzle (16-byte chunk c of row r
+// at c ^ (r & 7)), fp16 rows 64 B with the 64B swizzle (chunk c at c ^ ((r >> 1) & 3)): either way the 8 rows one warp reads per
+// fragment column fall into distinct banks.
+__host__ __device__ inline int resSlotBytes(const ConvParams& p) {
+  return p.residual != nullptr ? BLOCK_M * RES_COLS * (p.residual_fp32 ? 4 : 2) : 0;
+}
+__device__ __forceinline__ float2 load_residual(const uint8_t* slot, int r, int c, bool fp32) {
+  if(fp32) return *reinterpret_cast<const float2*>(slot + r * 128 + ((((c >> 2) ^ (r & 7)) << 4) | ((c & 3) << 2)));
+  return __half22float2(*reinterpret_cast<const __half2*>(slot + r * 64 + ((((c >> 3) ^ ((r >> 1) & 3)) << 4) | ((c & 7) << 1))));
+}
 
-// Epilogue of two adjacent columns (col, col+1) of one accumulator row.
-__device__ __forceinline__ void epilogue_pair(const ConvParams& p, int row, int col, float v0, float v1, float maskv) {
+// Epilogue of two adjacent columns (col, col+1) of one accumulator row: r = the residual (used when p.residual is set), sc / bi =
+// the BN constants of col in shared memory.
+__device__ __forceinline__ void epilogue_store(const ConvParams& p, int row, int col, float v0, float v1, float maskv, float2 r,
+                                               const float* sc, const float* bi) {
   if(p.ncbias != nullptr) {
     const float2 b = __ldg(reinterpret_cast<const float2*>(p.ncbias + (size_t)(row / p.P) * p.cout_p + col));
     v0 += b.x; v1 += b.y;
   }
   const size_t off = (size_t)row * p.cout_p + col;
-  if(p.residual != nullptr) {
-    if(p.residual_fp32) {
-      const float2 r = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(p.residual) + off);
-      v0 += r.x; v1 += r.y;
-    }
-    else {
-      const float2 r = __half22float2(*reinterpret_cast<const __half2*>(reinterpret_cast<const __half*>(p.residual) + off));
-      v0 += r.x; v1 += r.y;
-    }
-  }
+  if(p.residual != nullptr) { v0 += r.x; v1 += r.y; }
   if(p.raw_out != nullptr) {
     if(p.raw_fp32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.raw_out) + off) = make_float2(v0 * maskv, v1 * maskv);
     else *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.raw_out) + off) = __floats2half2_rn(v0 * maskv, v1 * maskv);
   }
   if(p.act_out != nullptr) {
-    float a0 = fmaf(v0, __ldg(p.bn_scale + col), __ldg(p.bn_bias + col));
-    float a1 = fmaf(v1, __ldg(p.bn_scale + col + 1), __ldg(p.bn_bias + col + 1));
+    float a0 = fmaf(v0, sc[0], bi[0]);
+    float a1 = fmaf(v1, sc[1], bi[1]);
     if(p.act == 2) {   // mish(x) = x - 2x / (e^x (e^x + 2) + 2): overflow of e gives x, underflow gives 0, no clamps needed
       const float e0 = kgb_ex2(a0 * 1.4426950408889634f), e1 = kgb_ex2(a1 * 1.4426950408889634f);
       a0 = fmaf(-2.0f, a0 * kgb_rcp(fmaf(e0, e0 + 2.0f, 2.0f)), a0);
@@ -144,15 +157,22 @@ __device__ __forceinline__ void epilogue_pair(const ConvParams& p, int row, int 
 template <int N>
 __global__ void __launch_bounds__(THREADS, 1)
 kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapB,
-                   const __grid_constant__ ConvParams p, int stages) {
+                   const __grid_constant__ CUtensorMap tmapR, const __grid_constant__ ConvParams p, int stages) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr int b_tile_bytes = N * BLOCK_K * 2;               // one tap's weight tile
   const int halo = (p.ky / 2) * p.Wp + (p.kx / 2);            // rows of A above / below the tile that the taps reach
   const int a_tx_bytes = (BLOCK_M + 2 * halo) * BLOCK_K * 2;
   const int a_buf_bytes = (a_tx_bytes + 1023) / 1024 * 1024;
-  const uint32_t smem_b = smem_base + 2 * a_buf_bytes;
-  Bars* bars = reinterpret_cast<Bars*>(smem_raw + (smem_base - smem_u32(smem_raw)) + 2 * (size_t)a_buf_bytes + (size_t)stages * b_tile_bytes);
+  constexpr int slices = N / RES_COLS;
+  const int r_slot_bytes = resSlotBytes(p);
+  const uint32_t smem_r = smem_base + 2 * a_buf_bytes;
+  const uint32_t smem_b = smem_r + RES_SLOTS * r_slot_bytes;
+  uint8_t* const smem = smem_raw + (smem_base - smem_u32(smem_raw));
+  Bars* bars = reinterpret_cast<Bars*>(smem + (smem_b - smem_base) + (size_t)stages * b_tile_bytes);
+  float* const s_mask = reinterpret_cast<float*>(bars + 1);
+  float* const s_scale = s_mask + BLOCK_M;
+  float* const s_bias = s_scale + N;
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
@@ -165,6 +185,7 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
   if(threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapB) : "memory");
+    if(p.residual != nullptr) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapR) : "memory");
     for(int s = 0; s < stages; s++) {
       mbar_init(smem_u32(&bars->full[s]), 1);
       mbar_init(smem_u32(&bars->empty[s]), CONSUMER_WARPS);
@@ -172,6 +193,10 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
     for(int s = 0; s < 2; s++) {
       mbar_init(smem_u32(&bars->a_full[s]), 1);
       mbar_init(smem_u32(&bars->a_empty[s]), CONSUMER_WARPS);
+    }
+    for(int s = 0; s < RES_SLOTS; s++) {
+      mbar_init(smem_u32(&bars->r_full[s]), 1);
+      mbar_init(smem_u32(&bars->r_empty[s]), CONSUMER_WARPS);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -181,6 +206,13 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
     // ===================== TMA producer =====================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if(warp == 0 && lane == 0) {
+      auto load_residual_slice = [&](int s) {
+        const uint32_t rfull = smem_u32(&bars->r_full[s % RES_SLOTS]);
+        mbar_arrive_expect_tx(rfull, (uint32_t)r_slot_bytes);
+        tma_load_2d(smem_r + (s % RES_SLOTS) * r_slot_bytes, &tmapR, rfull, n0 + s * RES_COLS, m0);
+      };
+      if(p.residual != nullptr)
+        for(int s = 0; s < slices && s < RES_SLOTS; s++) load_residual_slice(s);
       int stage = 0; uint32_t phase = 0;
       for(int ph = 0; ph < phases; ph++) {
         const int kb = ph / parts, part = ph - kb * parts;
@@ -199,6 +231,12 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
           if(++stage == stages) { stage = 0; phase ^= 1; }
         }
       }
+      // slice s reuses the slot of slice s - RES_SLOTS once every consumer warp has read that one
+      if(p.residual != nullptr)
+        for(int s = RES_SLOTS; s < slices; s++) {
+          mbar_wait(smem_u32(&bars->r_empty[s % RES_SLOTS]), (uint32_t)(s / RES_SLOTS - 1) & 1);
+          load_residual_slice(s);
+        }
     }
     return;
   }
@@ -210,50 +248,86 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
   // ldmatrix.x4 lane roles: matrix j = lane / 8 supplies (rows +0 / +8) x (k 0-7 / 8-15) of a 16 x 16 A fragment
   const int lrow = g * 64 + q * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
   const uint32_t lchunk = (uint32_t)(lane >> 4);
+  // the tile's mask and BN constants into shared memory; the epilogue reads them after the consumer barrier below
+  {
+    const int ct = threadIdx.x - 128;
+    if(ct < BLOCK_M) s_mask[ct] = m0 + ct < p.M ? __ldg(p.mask + m0 + ct) : 0.0f;
+    if(p.act_out != nullptr)
+      for(int i = ct; i < N; i += 32 * CONSUMER_WARPS) { s_scale[i] = __ldg(p.bn_scale + n0 + i); s_bias[i] = __ldg(p.bn_bias + n0 + i); }
+  }
   float acc[N / 2];
 #pragma unroll
   for(int i = 0; i < N / 2; i++) acc[i] = 0.0f;
-  int stage = 0; uint32_t phase = 0;
-  for(int ph = 0; ph < phases; ph++) {
+  fence_acc(acc);
+  // One step = one (k-block, tap): ldmatrix the tap's A fragments into `af` and issue its 4 wgmma as one group.  Steps alternate
+  // between two fragment buffers; wait_group 1 after issuing step i means step i-1's group has finished, so its weight stage can be
+  // released and its fragment buffer is free for step i+1.  The MMAs reach the accumulators in k-block, tap, k16 order as before.
+  int stage = 0, prev_stage = -1, ph = 0, t = 0, dy = -ry, dx = -rx;
+  uint32_t phase = 0;
+  auto step = [&](uint32_t (&af)[4][4]) {
     const int abuf = ph & 1;
-    mbar_wait(smem_u32(&bars->a_full[abuf]), (ph >> 1) & 1);
+    if(t == 0) mbar_wait(smem_u32(&bars->a_full[abuf]), (ph >> 1) & 1);
     const uint32_t a_base = smem_base + abuf * a_buf_bytes;
-    int dy = -ry, dx = -rx;
-    for(int t = 0; t < taps; t++) {
-      // tap (dy,dx) = the tile's rows shifted by `halo + dy*Wp + dx`; the 128B swizzle puts 16-byte chunk c of row r at c ^ (r & 7)
-      const uint32_t r = (uint32_t)(lrow + halo + dy * p.Wp + dx);
-      uint32_t af[4][4];
+    // tap (dy,dx) = the tile's rows shifted by `halo + dy*Wp + dx`; the 128B swizzle puts 16-byte chunk c of row r at c ^ (r & 7)
+    const uint32_t r = (uint32_t)(lrow + halo + dy * p.Wp + dx);
 #pragma unroll
-      for(int k = 0; k < 4; k++) ldmatrix_x4(a_base + r * 128u + (((2u * k + lchunk) ^ (r & 7u)) << 4), af[k]);
-      mbar_wait(smem_u32(&bars->full[stage]), phase);
-      const uint64_t db = make_smem_desc(smem_b + stage * b_tile_bytes);
-      fence_acc(acc);
-      wgmma_fence();
+    for(int k = 0; k < 4; k++) ldmatrix_x4(a_base + r * 128u + (((2u * k + lchunk) ^ (r & 7u)) << 4), af[k]);
+    mbar_wait(smem_u32(&bars->full[stage]), phase);
+    const uint64_t db = make_smem_desc(smem_b + stage * b_tile_bytes);
+    wgmma_fence();
 #pragma unroll
-      for(int k = 0; k < 4; k++) Wgmma<N>::mma(acc, af[k], db + 2 * k);
-      wgmma_commit();
-      wgmma_wait0();
-      fence_acc(acc);
+    for(int k = 0; k < 4; k++) Wgmma<N>::mma(acc, af[k], db + 2 * k);
+    wgmma_commit();
+    // the wgmma issue above consumed the fragments of the k-block's last tap, so its A halo tile may be refilled
+    if(t == taps - 1) {
       __syncwarp();
-      if(lane == 0) mbar_arrive(smem_u32(&bars->empty[stage]));
-      if(++stage == stages) { stage = 0; phase ^= 1; }
-      if(++dx > rx) { dx = -rx; dy++; }
+      if(lane == 0) mbar_arrive(smem_u32(&bars->a_empty[abuf]));
     }
-    __syncwarp();
-    if(lane == 0) mbar_arrive(smem_u32(&bars->a_empty[abuf]));
+    wgmma_wait1();
+    if(prev_stage >= 0) {
+      __syncwarp();
+      if(lane == 0) mbar_arrive(smem_u32(&bars->empty[prev_stage]));
+    }
+    prev_stage = stage;
+    if(++stage == stages) { stage = 0; phase ^= 1; }
+    if(++dx > rx) { dx = -rx; dy++; }
+    if(++t == taps) { t = 0; dy = -ry; ph++; }
+  };
+  const int steps = phases * taps;
+  uint32_t af0[4][4], af1[4][4];
+  for(int i = 0; i + 1 < steps; i += 2) {
+    step(af0);
+    step(af1);
   }
+  if(steps & 1) step(af0);
+  wgmma_wait0();   // the last group; the producer loads no further weight tile, so its stage is not released
+  fence_acc(acc);
+  consumer_sync();   // s_mask / s_scale / s_bias written
 
-  // ===================== epilogue straight from the accumulator fragments =====================
+  // ===================== epilogue straight from the accumulator fragments, one 32-column residual slice at a time =====================
   // acc[4j + 2h + e]: row 16q + lane/4 + 8h of the warpgroup's 64, column 8j + 2*(lane%4) + e
-  const int rowA = m0 + g * 64 + q * 16 + (lane >> 2);
+  const int rloc = g * 64 + q * 16 + (lane >> 2);
+  const uint8_t* const ring = smem + (smem_r - smem_base);
 #pragma unroll
-  for(int h = 0; h < 2; h++) {
-    const int row = rowA + 8 * h;
-    if(row >= p.M) continue;
-    const float maskv = __ldg(p.mask + row);
+  for(int s = 0; s < slices; s++) {
+    const uint8_t* const slot = ring + (s % RES_SLOTS) * r_slot_bytes;
+    if(p.residual != nullptr) mbar_wait(smem_u32(&bars->r_full[s % RES_SLOTS]), (uint32_t)(s / RES_SLOTS) & 1);
 #pragma unroll
-    for(int j = 0; j < N / 8; j++)
-      epilogue_pair(p, row, n0 + 8 * j + 2 * (lane & 3), acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], maskv);
+    for(int h = 0; h < 2; h++) {
+      const int rl = rloc + 8 * h, row = m0 + rl;
+      if(row >= p.M) continue;
+      const float maskv = s_mask[rl];
+#pragma unroll
+      for(int jj = 0; jj < RES_COLS / 8; jj++) {
+        const int j = s * (RES_COLS / 8) + jj, lc = 8 * j + 2 * (lane & 3);
+        const float2 r = p.residual != nullptr ? load_residual(slot, rl, lc - s * RES_COLS, p.residual_fp32 != 0) : make_float2(0.0f, 0.0f);
+        epilogue_store(p, row, n0 + lc, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], maskv, r, s_scale + lc, s_bias + lc);
+      }
+    }
+    if(p.residual != nullptr && s + RES_SLOTS < slices) {
+      __syncwarp();
+      if(lane == 0) mbar_arrive(smem_u32(&bars->r_empty[s % RES_SLOTS]));
+    }
   }
 }
 
@@ -271,30 +345,34 @@ cudaError_t convWGInit() {
 }
 
 template <int N>
-static cudaError_t launchN(const CUtensorMap& tmapA, const CUtensorMap& tmapB, const ConvParams& p, int stages, int smem,
-                           cudaStream_t stream) {
-  kgb_conv_wg_kernel<N><<<p.num_m_tiles * p.num_n_tiles, THREADS, smem, stream>>>(tmapA, tmapB, p, stages);
+static cudaError_t launchN(const CUtensorMap& tmapA, const CUtensorMap& tmapB, const CUtensorMap& tmapR, const ConvParams& p, int stages,
+                           int smem, cudaStream_t stream) {
+  kgb_conv_wg_kernel<N><<<p.num_m_tiles * p.num_n_tiles, THREADS, smem, stream>>>(tmapA, tmapB, tmapR, p, stages);
   return cudaGetLastError();
 }
 
-cudaError_t launchConvWG(const CUtensorMap& tmapA, const CUtensorMap& tmapB, const ConvParams& p, cudaStream_t stream) {
+cudaError_t launchConvWG(const CUtensorMap& tmapA, const CUtensorMap& tmapB, const CUtensorMap& tmapR, const ConvParams& p,
+                         cudaStream_t stream) {
   const int halo = (p.ky / 2) * p.Wp + (p.kx / 2);
   if(BLOCK_M + 2 * halo > 256) return cudaErrorInvalidValue;  // TMA box limit
+  if(p.n_tile % RES_COLS != 0) return cudaErrorInvalidValue;
   const int bTile = p.n_tile * BLOCK_K * 2;
-  const int fixed = 1024 + 2 * aBufBytes(BLOCK_M + 2 * halo) + (int)sizeof(Bars);
+  // the residual ring and the epilogue's mask / BN copies come first; the weight ring gets what is left
+  const int fixed = 1024 + 2 * aBufBytes(BLOCK_M + 2 * halo) + RES_SLOTS * resSlotBytes(p) + (int)sizeof(Bars) +
+                    (BLOCK_M + 2 * p.n_tile) * (int)sizeof(float);
   int stages = (SMEM_LIMIT - fixed) / bTile;
   if(stages > MAX_STAGES) stages = MAX_STAGES;
   if(stages < 2) return cudaErrorInvalidValue;
   const int smem = fixed + stages * bTile;
   switch(p.n_tile) {
-    case 32: return launchN<32>(tmapA, tmapB, p, stages, smem, stream);
-    case 64: return launchN<64>(tmapA, tmapB, p, stages, smem, stream);
-    case 96: return launchN<96>(tmapA, tmapB, p, stages, smem, stream);
-    case 128: return launchN<128>(tmapA, tmapB, p, stages, smem, stream);
-    case 160: return launchN<160>(tmapA, tmapB, p, stages, smem, stream);
-    case 192: return launchN<192>(tmapA, tmapB, p, stages, smem, stream);
-    case 224: return launchN<224>(tmapA, tmapB, p, stages, smem, stream);
-    case 256: return launchN<256>(tmapA, tmapB, p, stages, smem, stream);
+    case 32: return launchN<32>(tmapA, tmapB, tmapR, p, stages, smem, stream);
+    case 64: return launchN<64>(tmapA, tmapB, tmapR, p, stages, smem, stream);
+    case 96: return launchN<96>(tmapA, tmapB, tmapR, p, stages, smem, stream);
+    case 128: return launchN<128>(tmapA, tmapB, tmapR, p, stages, smem, stream);
+    case 160: return launchN<160>(tmapA, tmapB, tmapR, p, stages, smem, stream);
+    case 192: return launchN<192>(tmapA, tmapB, tmapR, p, stages, smem, stream);
+    case 224: return launchN<224>(tmapA, tmapB, tmapR, p, stages, smem, stream);
+    case 256: return launchN<256>(tmapA, tmapB, tmapR, p, stages, smem, stream);
     default: return cudaErrorInvalidValue;
   }
 }

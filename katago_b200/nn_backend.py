@@ -403,7 +403,10 @@ class NeuralNet:
 def test_conv_epilogue(ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16, kind, x, residual=None, bn_scale=None, bn_bias=None,
                        activation=2):
     """One convolution launch with a production epilogue (include/kgb200.h kgb_test_conv_epilogue): kind 1 = BN + act + mask -> fp16
-    operand, 2 = + residual stream updated in place, 3 = raw stream + operand.  Returns (raw or None, act), NHWC."""
+    operand, 2 = + residual stream updated in place, 3 = raw stream + operand, 4 = kind 2 with an fp32 residual stream in fp16 mode
+    too.  Returns (raw or None, act), NHWC."""
+    if kind not in (1, 2, 3, 4):
+        raise ValueError(f"test_conv_epilogue: epilogue kind {kind} is not 1-4")
     lib = load_library()
     w, xx = _f32(weights), _f32(x)
     raw = np.zeros((n, nn_y_len, nn_x_len, out_c), np.float32)
