@@ -416,15 +416,13 @@ KGB_API int kgb_zobrist_tables(int x_size, int y_size, uint64_t* board_hash, uin
 KGB_API int kgb_test_board_replay(int x_size, int y_size, int num_boards, int num_moves, int multi_stone_suicide_legal, const int8_t* moves,
                           uint8_t* colors, int8_t* ko, int16_t* caps, uint8_t* lib_class, uint8_t* legal_next, uint64_t* pos_hash, uint8_t* area);
 
-/* Kernel-level timing hook for bench.py's roofline object: runs ONE convolution layer (random weights/inputs resident in
- * HBM, the production epilogue of a residual unit's first conv: BN + mish + mask -> fp16) `iters` times on a stream and returns the CUDA-event average per launch. */
-KGB_API int kgb_bench_conv(int ky, int kx, int in_c, int out_c, int n, int nn_x_len, int nn_y_len, int use_fp16, int warmup, int iters,
-                   float* ms_per_launch);
-/* The same with the epilogue chosen: epilogue_kind 0 = fp32 raw output only (heads / gpool conv), 1 = BN + mish + mask -> fp16 (first conv
- * of a residual unit), 2 = + residual stream read and rewritten in place (second conv of a unit, a nested block's post conv), 3 = raw
- * stream + activated operand (a nested block's pre conv), 4 = kind 2 with an fp32 residual stream also in fp16 mode (the trunk's block
- * exit with KGB_STREAM_FP32=trunk; in fp32-equivalent mode every stream is fp32).  `rotate` >= 1 independent input / output buffer
- * sets are cycled through so that the timed loop's working set exceeds L2. */
+/* Kernel-level timing hook for bench.py's roofline object: runs ONE convolution layer (random weights / inputs resident in HBM)
+ * `iters` times on a stream after `warmup` launches and returns the CUDA-event average per launch.  epilogue_kind chooses the
+ * production epilogue: 0 = fp32 raw output only (heads / gpool conv), 1 = BN + mish + mask -> fp16 (first conv of a residual unit),
+ * 2 = + residual stream read and rewritten in place (second conv of a unit, a nested block's post conv), 3 = raw stream + activated
+ * operand (a nested block's pre conv), 4 = kind 2 with an fp32 residual stream also in fp16 mode (the trunk's block exit with
+ * KGB_STREAM_FP32=trunk; in fp32-equivalent mode every stream is fp32).  `rotate` >= 1 independent input / output buffer sets are
+ * cycled through so that the timed loop's working set exceeds L2. */
 KGB_API int kgb_bench_conv_ex(int ky, int kx, int in_c, int out_c, int n, int nn_x_len, int nn_y_len, int use_fp16, int epilogue_kind, int rotate,
                       int warmup, int iters, float* ms_per_launch);
 /* Test hook for the fused epilogues (kinds 1-4 above) of one convolution layer: NHWC input [n][y][x][in_c], optional NHWC residual

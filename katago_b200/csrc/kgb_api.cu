@@ -145,7 +145,6 @@ struct kgb_handle {
   int split = 0;          // fp32-equivalent mode
   bool nhwc = true;
   bool streamTrunkFp32 = true, streamInnerFp32 = false;
-  bool useSimt = false, useGraph = true;
   std::vector<void*> allocs;
   // inputs / outputs (device, fixed addresses so graphs can be replayed)
   float *dSpatial = nullptr, *dGlobal = nullptr, *dOptimism = nullptr;
@@ -175,7 +174,6 @@ struct kgb_handle {
   cudaStream_t copyStream = nullptr;
   cudaEvent_t stagedEvent = nullptr, bcastStart = nullptr, bcastStop = nullptr;
   bool staged = false;
-  bool wCheckSpans = true;        // false: free-form arena of a given size (the single-convolution test / bench objects)
   void* ncclComm = nullptr;
   int ncclRank = 0, ncclRanks = 0;
 
@@ -198,7 +196,7 @@ struct kgb_handle {
       *host = nullptr;
       return (void*)(uintptr_t)(256 + o);
     }
-    if((wCheckSpans && (wIndex >= wSizes.size() || wSizes[wIndex] != b)) || o + b > wBytes)
+    if(wIndex >= wSizes.size() || wSizes[wIndex] != b || o + b > wBytes)
       throw std::invalid_argument("the model's weights do not have the layout this handle was built for (different architecture)");
     wIndex++;
     *host = wHost + o;
@@ -232,10 +230,6 @@ struct kgb_handle {
 // Graph builder
 // ------------------------------------------------------------------------------------------------------------
 namespace {
-
-struct ConvSource {
-  const ConvDesc* conv;
-};
 
 struct Builder {
   kgb_handle& h;
@@ -358,16 +352,11 @@ struct Builder {
       p.act_out = actOut;
       p.bn_scale = bn.scale; p.bn_bias = bn.bias; p.act = bn.act;
       p.mask = hp->dMask;
-      if(hp->useSimt) {
-        CK(launchConvSimt(A, cw.cin_p * actMulL, cw.w, p, s));
-      }
-      else {
-        CUtensorMap tmA = makeTmap2D(A, (uint64_t)p.M, (uint64_t)cw.cin_p * actMulL, (uint32_t)convABoxRows(cw.ky, cw.kx, p.Wp));
-        CUtensorMap tmR;
-        memset(&tmR, 0, sizeof(tmR));
-        if(residual != nullptr) tmR = makeTmapResidual(residual, (uint64_t)p.M, (uint64_t)cw.cout_p, residualFp32);
-        CK(launchConvWG(tmA, cw.tmapB, tmR, p, s));
-      }
+      CUtensorMap tmA = makeTmap2D(A, (uint64_t)p.M, (uint64_t)cw.cin_p * actMulL, (uint32_t)convABoxRows(cw.ky, cw.kx, p.Wp));
+      CUtensorMap tmR;
+      memset(&tmR, 0, sizeof(tmR));
+      if(residual != nullptr) tmR = makeTmapResidual(residual, (uint64_t)p.M, (uint64_t)cw.cout_p, residualFp32);
+      CK(launchConvWG(tmA, cw.tmapB, tmR, p, s));
     });
     h.launchesPerForward++;
   }
@@ -524,10 +513,6 @@ struct Builder {
 };
 
 void runOps(kgb_handle* h, int n) {
-  if(!h->useGraph) {
-    for(auto& op : h->ops) op(n, h->stream);
-    return;
-  }
   auto it = h->graphs.find(n);
   if(it == h->graphs.end()) {
     cudaGraph_t graph = nullptr;
@@ -673,8 +658,41 @@ static void ncclCheck(ncclResult_t r, const char* what) {
 // The settings that decide how the graph builder lays the weights out
 static void copyBuildSettings(kgb_handle& dst, const kgb_handle& src) {
   dst.device = src.device; dst.model = src.model; dst.L = src.L; dst.maxBatch = src.maxBatch; dst.split = src.split;
-  dst.nhwc = src.nhwc; dst.streamTrunkFp32 = src.streamTrunkFp32; dst.streamInnerFp32 = src.streamInnerFp32; dst.useSimt = src.useSimt;
-  dst.useGraph = src.useGraph;
+  dst.nhwc = src.nhwc; dst.streamTrunkFp32 = src.streamTrunkFp32; dst.streamInnerFp32 = src.streamInnerFp32;
+}
+
+// Makes device `dev` (-1: the current device) current, after checking that it exists and is the sm_90a device the kernels are
+// built for.  Returns its index.
+static int selectDevice(int dev) {
+  int count = 0;
+  if(cudaGetDeviceCount(&count) != cudaSuccess || count == 0)
+    throw CudaFailure("libkgb200: no CUDA device is visible; the backend has no CPU fallback");
+  if(dev < 0) CK(cudaGetDevice(&dev));
+  if(dev >= count) throw std::invalid_argument("libkgb200: gpu index " + std::to_string(dev) + " >= device count");
+  CK(cudaSetDevice(dev));
+  cudaDeviceProp prop;
+  CK(cudaGetDeviceProperties(&prop, dev));
+  if(prop.major != 9 || prop.minor != 0)
+    throw CudaFailure(std::string("libkgb200 is built for sm_90a (H100) only; device ") + prop.name + " is sm_" +
+                      std::to_string(prop.major) + std::to_string(prop.minor));
+  return dev;
+}
+
+// Padded rows of an X x Y board with `pad` zero rows on top and `pad` zero columns at the right (kgb_conv.cuh)
+static Layout boardLayout(int X, int Y, int pad) { return Layout{X, Y, pad, X + pad, (Y + pad) * (X + pad)}; }
+
+// The weight arena is laid out by two passes over the same code: pack(handle) runs on a scratch handle that only adds up the
+// spans, then on h for real, where walloc checks every span against that list.  The packed bytes reach the device in one copy.
+static void buildWeights(kgb_handle& h, const std::function<void(kgb_handle&)>& pack) {
+  kgb_handle sizing;
+  copyBuildSettings(sizing, h);
+  sizing.wMode = kgb_handle::W_SIZE;
+  pack(sizing);
+  h.wSizes = sizing.wSizes;
+  h.wAllocArena(sizing.wCursor);
+  pack(h);
+  if(h.wCursor != h.wBytes || h.wSignature != sizing.wSignature) throw std::logic_error("libkgb200: the two builder passes disagree");
+  h.wFlushLive();
 }
 
 static void destroyHandle(kgb_handle* h) {
@@ -703,16 +721,7 @@ KGB_API int kgb_handle_create(kgb_context* ctx, const kgb_model* model, int max_
     if(max_batch_size < 1 || max_batch_size > 65536) throw std::invalid_argument("kgb_handle_create: maxBatchSize out of range");
     int dev = gpu_idx;
     if(dev < 0) dev = (!ctx->gpuIdxs.empty() && ctx->gpuIdxs[0] >= 0) ? ctx->gpuIdxs[0] : 0;
-    int count = 0;
-    if(cudaGetDeviceCount(&count) != cudaSuccess || count == 0)
-      throw CudaFailure("libkgb200: no CUDA device is visible; the backend has no CPU fallback");
-    if(dev >= count) throw std::invalid_argument("kgb_handle_create: gpu index " + std::to_string(dev) + " >= device count");
-    CK(cudaSetDevice(dev));
-    cudaDeviceProp prop;
-    CK(cudaGetDeviceProperties(&prop, dev));
-    if(prop.major != 9 || prop.minor != 0)
-      throw CudaFailure(std::string("libkgb200 is built for sm_90a (H100) only; device ") + prop.name + " is sm_" +
-                        std::to_string(prop.major) + std::to_string(prop.minor));
+    dev = selectDevice(dev);
     raw = new kgb_handle();
     kgb_handle& h = *raw;
     h.device = dev;
@@ -720,40 +729,21 @@ KGB_API int kgb_handle_create(kgb_context* ctx, const kgb_model* model, int max_
     h.maxBatch = max_batch_size;
     h.split = ctx->fp16 ? 0 : 1;
     h.nhwc = inputs_nhwc != 0;
-    int pad = h.model->maxConvRadius();
-    h.L.X = ctx->X; h.L.Y = ctx->Y; h.L.pad = pad; h.L.Wp = ctx->X + pad; h.L.P = (ctx->Y + pad) * (ctx->X + pad);
+    h.L = boardLayout(ctx->X, ctx->Y, h.model->maxConvRadius());
     // Residual streams: fp32-equivalent mode keeps all of them in fp32; fp16 mode keeps all of them in fp16, like the reference's
     // FP16 CUDA path keeps its trunk in half (cudabackend.cpp: useFP16 buffers).  KGB_STREAM_FP32 = all | trunk | none overrides
-    // fp16 mode only (measured: trunk 10.15 ms, none 9.59 ms per b18 forward at batch 256).
+    // fp16 mode only.
     const char* env = getenv("KGB_STREAM_FP32");
     std::string streams = h.split ? "all" : (env ? env : "none");
     h.streamTrunkFp32 = streams != "none";
     h.streamInnerFp32 = streams == "all";
-    env = getenv("KGB_CONV_IMPL");
-    h.useSimt = env && std::string(env) == "simt";
-    env = getenv("KGB_NO_GRAPH");
-    h.useGraph = !(env && std::string(env) == "1");
     CK(cudaStreamCreateWithFlags(&h.stream, cudaStreamNonBlocking));
     CK(convWGInit());
     CK(cudaStreamCreateWithFlags(&h.copyStream, cudaStreamNonBlocking));
     CK(cudaEventCreateWithFlags(&h.stagedEvent, cudaEventDisableTiming));
     CK(cudaEventCreate(&h.bcastStart));
     CK(cudaEventCreate(&h.bcastStop));
-    {
-      kgb_handle sizing;                       // pass 1: how large is the weight arena, and in which spans
-      copyBuildSettings(sizing, h);
-      sizing.wMode = kgb_handle::W_SIZE;
-      Builder(sizing).build();
-      h.wSizes = sizing.wSizes;
-      h.wSignature = sizing.wSignature;
-      h.wAllocArena(sizing.wCursor);
-    }
-    const std::string signature = h.wSignature;
-    h.wSignature.clear();
-    Builder b(h);
-    b.build();
-    if(h.wCursor != h.wBytes || h.wSignature != signature) throw std::logic_error("kgb_handle_create: the two builder passes disagree");
-    h.wFlushLive();
+    buildWeights(h, [](kgb_handle& hh) { Builder(hh).build(); });
     const int XY = h.L.X * h.L.Y;
     const ModelDesc& m = *h.model;
     CK(cudaMallocHost((void**)&h.hSpatial, (size_t)h.maxBatch * m.numInputChannels * XY * sizeof(float)));
@@ -965,75 +955,55 @@ struct SingleConv {
   kgb_handle h;
   ModelDesc dummy;
   ConvWeights cw;
-  __half* A = nullptr;
-  float* raw = nullptr;
-  int n, X, Y, cin, cout, pad;
+  int n, X, Y, cin, cout;
   size_t M;
+  // one entry per buffer set: the operand, the activated output (kinds 1-4) and the raw output (kind 0) or raw stream (kinds 2-4)
   std::vector<__half*> As, acts;
-  std::vector<void*> streams;
-  bool streamF32 = false;  // the residual / raw stream of kinds 2-4 is fp32
+  std::vector<void*> raws;
+  bool rawF32 = true;   // the raw output of kind 0 is fp32; the stream of kinds 2-4 is fp32 for kind 4 and in fp32-equivalent mode
   int rotate, next = 0;
-  SingleConv(int ky, int kx, int in_c, int out_c, const float* weights, int n_, int X_, int Y_, int use_fp16, int actEpilogue = 0,
-             int rotate_ = 1, const float* bnScale = nullptr, const float* bnBias = nullptr, int actKind = ACT_MISH)
+  // kind: 0 = fp32 raw output only; 1 = the first conv of a residual unit (BN + mish + mask -> fp16 operand of the next conv);
+  // 2 = the second conv of a unit (+ fp16 residual stream, updated in place, and the next unit's BN + mish operand); 3 = a nested
+  // block's pre conv (fp16 raw stream + activated operand); 4 = kind 2 with an fp32 residual stream, as the trunk runs in fp16 mode
+  // with KGB_STREAM_FP32=trunk.  In fp32-equivalent mode every stream is fp32.  `rotate` independent buffer sets are cycled through
+  // by run() so that a timing loop does not live in L2.
+  SingleConv(int ky, int kx, int in_c, int out_c, const float* weights, int n_, int X_, int Y_, int use_fp16, int kind, int rotate_ = 1,
+             const float* bnScale = nullptr, const float* bnBias = nullptr, int actKind = ACT_MISH)
       : n(n_), X(X_), Y(Y_), cin(in_c), cout(out_c), rotate(rotate_ < 1 ? 1 : rotate_) {
-    int count = 0;
-    if(cudaGetDeviceCount(&count) != cudaSuccess || count == 0) throw CudaFailure("libkgb200: no CUDA device is visible");
-    CK(cudaGetDevice(&h.device));
-    cudaDeviceProp prop;
-    CK(cudaGetDeviceProperties(&prop, h.device));
-    if(prop.major != 9 || prop.minor != 0) throw CudaFailure("libkgb200 is built for sm_90a (H100) only");
+    h.device = selectDevice(-1);
     h.model = &dummy;
     h.maxBatch = n;
     h.split = use_fp16 ? 0 : 1;
-    pad = std::max(1, std::max(ky / 2, kx / 2));
-    h.L.X = X; h.L.Y = Y; h.L.pad = pad; h.L.Wp = X + pad; h.L.P = (Y + pad) * (X + pad);
-    const char* env = getenv("KGB_CONV_IMPL");
-    h.useSimt = env && std::string(env) == "simt";
+    h.L = boardLayout(X, Y, std::max(1, std::max(ky / 2, kx / 2)));
     h.streamTrunkFp32 = h.streamInnerFp32 = h.split != 0;
     CK(cudaStreamCreateWithFlags(&h.stream, cudaStreamNonBlocking));
     CK(convWGInit());
-    h.wCheckSpans = false;
-    h.wAllocArena((size_t)ky * kx * cpad(out_c) * ((size_t)cpad(in_c) * 2 + cpad(out_c)) * sizeof(__half) + 4 * (size_t)cpad(out_c) * sizeof(float) + 4096);
-    Builder b(h);
     ConvDesc cd;
     cd.ky = ky; cd.kx = kx; cd.cin = in_c; cd.cout = out_c;
     cd.w.assign(weights, weights + (size_t)ky * kx * in_c * out_c);
-    cw = b.packConv({&cd});
-    M = (size_t)n * h.L.P;
-    A = h.dalloc<__half>(M * cw.cin_p * b.actMul);
-    h.dMask = h.dalloc<float>(M + 128);
-    h.dMaskSum = h.dalloc<float>(n);
-    raw = h.dalloc<float>(M * cw.cout_p);
-    // actEpilogue: 0 = fp32 raw output only; 1 = the first conv of a residual unit (BN + mish + mask -> fp16 operand of the next
-    // conv); 2 = the second conv of a unit (+ fp16 residual stream, updated in place, and the next unit's BN + mish operand);
-    // 3 = a nested block's pre conv (fp16 raw stream + activated operand); 4 = kind 2 with an fp32 residual stream, as the trunk
-    // runs in fp16 mode with KGB_STREAM_FP32=trunk.  In fp32-equivalent mode every stream is fp32.  `rotate` independent buffer
-    // sets are cycled through by run() so that a timing loop does not live in L2.
     BNDesc bn;
     bn.c = out_c; bn.scale.assign(out_c, 1.0f); bn.bias.assign(out_c, 0.0f);
     if(bnScale) bn.scale.assign(bnScale, bnScale + out_c);
     if(bnBias) bn.bias.assign(bnBias, bnBias + out_c);
-    Builder::BNDev dev = b.uploadBN(bn, actKind, cw.cout_p);
-    h.wFlushLive();
-    streamF32 = h.split != 0 || actEpilogue == 4;
+    Builder::BNDev dev;
+    buildWeights(h, [&](kgb_handle& hh) {
+      Builder b(hh);
+      cw = b.packConv({&cd});
+      dev = b.uploadBN(bn, actKind, cw.cout_p);
+    });
+    Builder b(h);
+    M = (size_t)n * h.L.P;
+    h.dMask = h.dalloc<float>(M + 128);
+    h.dMaskSum = h.dalloc<float>(n);
+    rawF32 = kind == 0 || kind == 4 || h.split != 0;
     for(int r = 0; r < rotate; r++) {
-      __half* Ar = r == 0 ? A : h.dalloc<__half>(M * cw.cin_p * b.actMul);
-      As.push_back(Ar);
-      if(actEpilogue == 0) {
-        Builder::BNDev none;
-        float* rawr = r == 0 ? raw : h.dalloc<float>(M * cw.cout_p);
-        b.emitConv(cw, Ar, nullptr, false, nullptr, rawr, true, nullptr, none);
-      }
-      else {
-        __half* actOut = h.dalloc<__half>(M * cw.cout_p * b.actMul);
-        acts.push_back(actOut);
-        if(actEpilogue == 1) b.emitConv(cw, Ar, nullptr, false, nullptr, nullptr, false, actOut, dev);
-        else {
-          void* S = streamF32 ? (void*)h.dalloc<float>(M * cw.cout_p) : (void*)h.dalloc<__half>(M * cw.cout_p);
-          streams.push_back(S);
-          b.emitConv(cw, Ar, actEpilogue == 3 ? nullptr : S, streamF32, nullptr, S, streamF32, actOut, dev);
-        }
-      }
+      __half* A = h.dalloc<__half>(M * cw.cin_p * b.actMul);
+      __half* act = kind == 0 ? nullptr : h.dalloc<__half>(M * cw.cout_p * b.actMul);
+      void* raw = kind == 1 ? nullptr : rawF32 ? (void*)h.dalloc<float>(M * cw.cout_p) : (void*)h.dalloc<__half>(M * cw.cout_p);
+      As.push_back(A);
+      if(act) acts.push_back(act);
+      if(raw) raws.push_back(raw);
+      b.emitConv(cw, A, kind == 2 || kind == 4 ? raw : nullptr, rawF32, nullptr, raw, rawF32, act, kind == 0 ? Builder::BNDev() : dev);
     }
   }
   ~SingleConv() {
@@ -1045,15 +1015,14 @@ struct SingleConv {
     float* dIn = h.dalloc<float>((size_t)n * X * Y * cin);
     CK(cudaMemcpy(dIn, input, (size_t)n * X * Y * cin * sizeof(float), cudaMemcpyHostToDevice));
     CK(cudaDeviceSynchronize());   // see below: the pack kernel runs on a non-blocking stream
-    Builder b(h);
-    CK(launchPackInput(dIn, n, cin, true, nullptr, h.L, A, cw.cin_p, h.split, h.dMask, h.dMaskSum, h.stream));
+    CK(launchPackInput(dIn, n, cin, true, nullptr, h.L, As[0], cw.cin_p, h.split, h.dMask, h.dMaskSum, h.stream));
     CK(cudaStreamSynchronize(h.stream));
-    for(size_t r = 1; r < As.size(); r++) CK(cudaMemcpy(As[r], A, M * cw.cin_p * (h.split ? 2 : 1) * sizeof(__half), cudaMemcpyDeviceToDevice));
+    for(size_t r = 1; r < As.size(); r++) CK(cudaMemcpy(As[r], As[0], M * cw.cin_p * (h.split ? 2 : 1) * sizeof(__half), cudaMemcpyDeviceToDevice));
     // the mask of a bare convolution is "every board point", not input channel 0
     std::vector<float> hm(M, 0.0f);
     for(int i = 0; i < n; i++)
       for(int y = 0; y < Y; y++)
-        for(int x = 0; x < X; x++) hm[(size_t)i * h.L.P + (size_t)(y + pad) * h.L.Wp + x] = 1.0f;
+        for(int x = 0; x < X; x++) hm[(size_t)i * h.L.P + (size_t)(y + h.L.pad) * h.L.Wp + x] = 1.0f;
     CK(cudaMemcpy(h.dMask, hm.data(), M * sizeof(float), cudaMemcpyHostToDevice));
     // cudaMemcpy from pageable memory may return before the DMA has landed, and h.stream is non-blocking:
     // nothing else orders these uploads before the kernels launched on it.
@@ -1061,6 +1030,65 @@ struct SingleConv {
   }
   void run() { h.ops[next](n, h.stream); next = (next + 1) % rotate; }
 };
+
+// kgb_test_conv (kind 0) and kgb_test_conv_epilogue (kinds 1-4): one launch, NHWC in and out
+void testConv(const char* fn, int ky, int kx, int in_c, int out_c, const float* weights, int n, int nn_x_len, int nn_y_len, int use_fp16, int kind,
+              const float* input, const float* residual_in, const float* bn_scale, const float* bn_bias, int activation, float* raw_out,
+              float* act_out) {
+  const bool hasResidual = kind == 2 || kind == 4;
+  if(!weights || !input || n < 1 || (kind == 0 ? !raw_out : !act_out)) throw std::invalid_argument(std::string(fn) + ": bad argument");
+  if(hasResidual && !residual_in) throw std::invalid_argument(std::string(fn) + ": kinds 2 and 4 need residual_in");
+  if(kind >= 2 && !raw_out) throw std::invalid_argument(std::string(fn) + ": kinds 2 to 4 need raw_out");
+  SingleConv sc(ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16, kind, 1, bn_scale, bn_bias, activation);
+  sc.setInput(input);
+  const int cp = sc.cw.cout_p;
+  const bool f32 = sc.rawF32;
+  auto rowOf = [&](int i, int y, int x) { return (size_t)i * sc.h.L.P + (size_t)(y + sc.h.L.pad) * sc.h.L.Wp + x; };
+  if(hasResidual) {
+    std::vector<float> hf(sc.M * cp, 0.0f);
+    for(int i = 0; i < n; i++) for(int y = 0; y < nn_y_len; y++) for(int x = 0; x < nn_x_len; x++) for(int c = 0; c < out_c; c++)
+      hf[rowOf(i, y, x) * cp + c] = residual_in[(((size_t)i * nn_y_len + y) * nn_x_len + x) * out_c + c];
+    if(f32) CK(cudaMemcpy(sc.raws[0], hf.data(), hf.size() * sizeof(float), cudaMemcpyHostToDevice));
+    else {
+      std::vector<__half> hh(hf.size());
+      for(size_t k = 0; k < hf.size(); k++) hh[k] = __float2half_rn(hf[k]);
+      CK(cudaMemcpy(sc.raws[0], hh.data(), hh.size() * sizeof(__half), cudaMemcpyHostToDevice));
+    }
+    CK(cudaDeviceSynchronize());
+  }
+  sc.run();
+  CK(cudaStreamSynchronize(sc.h.stream));
+  const int am = sc.h.split ? 2 : 1;
+  std::vector<__half> ha;
+  if(!sc.acts.empty()) {
+    ha.resize(sc.M * cp * am);
+    CK(cudaMemcpy(ha.data(), sc.acts[0], ha.size() * sizeof(__half), cudaMemcpyDeviceToHost));
+  }
+  std::vector<float> hr;
+  if(!sc.raws.empty()) {
+    hr.resize(sc.M * cp);
+    if(f32) CK(cudaMemcpy(hr.data(), sc.raws[0], hr.size() * sizeof(float), cudaMemcpyDeviceToHost));
+    else {
+      std::vector<__half> hh(hr.size());
+      CK(cudaMemcpy(hh.data(), sc.raws[0], hh.size() * sizeof(__half), cudaMemcpyDeviceToHost));
+      for(size_t k = 0; k < hr.size(); k++) hr[k] = __half2float(hh[k]);
+    }
+  }
+  if(!ha.empty()) {
+    // every row that is not a board point (pad rows / columns) must have been written as zero: the next conv's halo reads them
+    std::vector<char> onBoard(sc.M, 0);
+    for(int i = 0; i < n; i++) for(int y = 0; y < nn_y_len; y++) for(int x = 0; x < nn_x_len; x++) onBoard[rowOf(i, y, x)] = 1;
+    for(size_t r = 0; r < sc.M; r++)
+      if(!onBoard[r])
+        for(int c = 0; c < cp * am; c++)
+          if(__half2float(ha[r * cp * am + c]) != 0.0f) throw std::runtime_error(std::string(fn) + ": pad row " + std::to_string(r) + " of the activation output is not zero");
+  }
+  for(int i = 0; i < n; i++) for(int y = 0; y < nn_y_len; y++) for(int x = 0; x < nn_x_len; x++) for(int c = 0; c < out_c; c++) {
+    const size_t row = rowOf(i, y, x), o = (((size_t)i * nn_y_len + y) * nn_x_len + x) * out_c + c;
+    if(!ha.empty()) act_out[o] = __half2float(ha[row * cp * am + c]) + (am == 2 ? __half2float(ha[row * cp * am + cp + c]) : 0.0f);
+    if(!hr.empty()) raw_out[o] = hr[row * cp + c];
+  }
+}
 }  // namespace
 
 extern "C" {
@@ -1068,108 +1096,44 @@ extern "C" {
 KGB_API int kgb_test_conv(int ky, int kx, int in_c, int out_c, const float* weights, int n, int nn_x_len, int nn_y_len, int use_fp16,
                   const float* input, float* output) {
   return guarded([&] {
-    if(!weights || !input || !output || n < 1) throw std::invalid_argument("kgb_test_conv: bad argument");
-    SingleConv sc(ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16);
-    sc.setInput(input);
-    sc.run();
-    CK(cudaStreamSynchronize(sc.h.stream));
-    std::vector<float> hr(sc.M * sc.cw.cout_p);
-    CK(cudaMemcpy(hr.data(), sc.raw, hr.size() * sizeof(float), cudaMemcpyDeviceToHost));
-    for(int i = 0; i < n; i++)
-      for(int y = 0; y < nn_y_len; y++)
-        for(int x = 0; x < nn_x_len; x++) {
-          size_t row = (size_t)i * sc.h.L.P + (size_t)(y + sc.pad) * sc.h.L.Wp + x;
-          for(int c = 0; c < out_c; c++) output[(((size_t)i * nn_y_len + y) * nn_x_len + x) * out_c + c] = hr[row * sc.cw.cout_p + c];
-        }
+    testConv("kgb_test_conv", ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16, 0, input, nullptr, nullptr, nullptr, ACT_IDENTITY, output,
+             nullptr);
   });
-}
-
-static void benchConvImpl(int ky, int kx, int in_c, int out_c, int n, int nn_x_len, int nn_y_len, int use_fp16, int epilogue_kind, int rotate,
-                          int warmup, int iters, float* ms_per_launch) {
-  if(!ms_per_launch || n < 1 || iters < 1 || epilogue_kind < 0 || epilogue_kind > 4) throw std::invalid_argument("kgb_bench_conv: bad argument");
-  std::vector<float> w((size_t)ky * kx * in_c * out_c);
-  uint32_t st = 12345u;
-  for(auto& v : w) { st = st * 1664525u + 1013904223u; v = ((st >> 8) * (1.0f / 16777216.0f) - 0.5f) * 0.1f; }
-  SingleConv sc(ky, kx, in_c, out_c, w.data(), n, nn_x_len, nn_y_len, use_fp16, epilogue_kind, rotate);
-  std::vector<float> in((size_t)n * nn_x_len * nn_y_len * in_c);
-  for(auto& v : in) { st = st * 1664525u + 1013904223u; v = (st >> 8) * (1.0f / 16777216.0f); }
-  sc.setInput(in.data());
-  for(int i = 0; i < warmup; i++) sc.run();
-  cudaEvent_t e0, e1;
-  CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
-  CK(cudaStreamSynchronize(sc.h.stream));
-  CK(cudaEventRecord(e0, sc.h.stream));
-  for(int i = 0; i < iters; i++) sc.run();
-  CK(cudaEventRecord(e1, sc.h.stream));
-  CK(cudaStreamSynchronize(sc.h.stream));
-  float ms = 0.0f;
-  CK(cudaEventElapsedTime(&ms, e0, e1));
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
-  *ms_per_launch = ms / iters;
-}
-
-KGB_API int kgb_bench_conv(int ky, int kx, int in_c, int out_c, int n, int nn_x_len, int nn_y_len, int use_fp16, int warmup, int iters,
-                   float* ms_per_launch) {
-  return guarded([&] { benchConvImpl(ky, kx, in_c, out_c, n, nn_x_len, nn_y_len, use_fp16, 1, 1, warmup, iters, ms_per_launch); });
-}
-
-KGB_API int kgb_bench_conv_ex(int ky, int kx, int in_c, int out_c, int n, int nn_x_len, int nn_y_len, int use_fp16, int epilogue_kind, int rotate,
-                      int warmup, int iters, float* ms_per_launch) {
-  return guarded([&] { benchConvImpl(ky, kx, in_c, out_c, n, nn_x_len, nn_y_len, use_fp16, epilogue_kind, rotate, warmup, iters, ms_per_launch); });
 }
 
 KGB_API int kgb_test_conv_epilogue(int ky, int kx, int in_c, int out_c, const float* weights, int n, int nn_x_len, int nn_y_len, int use_fp16,
                            int epilogue_kind, const float* input, const float* residual_in, const float* bn_scale, const float* bn_bias,
                            int activation, float* raw_out, float* act_out) {
   return guarded([&] {
-    if(!weights || !input || !act_out || n < 1 || epilogue_kind < 1 || epilogue_kind > 4) throw std::invalid_argument("kgb_test_conv_epilogue: bad argument");
-    const bool hasResidual = epilogue_kind == 2 || epilogue_kind == 4;
-    if(hasResidual && !residual_in) throw std::invalid_argument("kgb_test_conv_epilogue: kinds 2 and 4 need residual_in");
-    if(epilogue_kind >= 2 && !raw_out) throw std::invalid_argument("kgb_test_conv_epilogue: kinds 2 to 4 need raw_out");
-    SingleConv sc(ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16, epilogue_kind, 1, bn_scale, bn_bias, activation);
-    sc.setInput(input);
-    const int cp = sc.cw.cout_p;
-    const bool f32 = sc.streamF32;
-    auto rowOf = [&](int i, int y, int x) { return (size_t)i * sc.h.L.P + (size_t)(y + sc.pad) * sc.h.L.Wp + x; };
-    if(hasResidual) {
-      std::vector<float> hf(sc.M * cp, 0.0f);
-      for(int i = 0; i < n; i++) for(int y = 0; y < nn_y_len; y++) for(int x = 0; x < nn_x_len; x++) for(int c = 0; c < out_c; c++)
-        hf[rowOf(i, y, x) * cp + c] = residual_in[(((size_t)i * nn_y_len + y) * nn_x_len + x) * out_c + c];
-      if(f32) CK(cudaMemcpy(sc.streams[0], hf.data(), hf.size() * sizeof(float), cudaMemcpyHostToDevice));
-      else {
-        std::vector<__half> hh(hf.size());
-        for(size_t k = 0; k < hf.size(); k++) hh[k] = __float2half_rn(hf[k]);
-        CK(cudaMemcpy(sc.streams[0], hh.data(), hh.size() * sizeof(__half), cudaMemcpyHostToDevice));
-      }
-      CK(cudaDeviceSynchronize());
-    }
-    sc.run();
+    if(epilogue_kind < 1 || epilogue_kind > 4) throw std::invalid_argument("kgb_test_conv_epilogue: bad argument");
+    testConv("kgb_test_conv_epilogue", ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16, epilogue_kind, input, residual_in, bn_scale,
+             bn_bias, activation, raw_out, act_out);
+  });
+}
+
+KGB_API int kgb_bench_conv_ex(int ky, int kx, int in_c, int out_c, int n, int nn_x_len, int nn_y_len, int use_fp16, int epilogue_kind, int rotate,
+                      int warmup, int iters, float* ms_per_launch) {
+  return guarded([&] {
+    if(!ms_per_launch || n < 1 || iters < 1 || epilogue_kind < 0 || epilogue_kind > 4) throw std::invalid_argument("kgb_bench_conv_ex: bad argument");
+    std::vector<float> w((size_t)ky * kx * in_c * out_c);
+    uint32_t st = 12345u;
+    for(auto& v : w) { st = st * 1664525u + 1013904223u; v = ((st >> 8) * (1.0f / 16777216.0f) - 0.5f) * 0.1f; }
+    SingleConv sc(ky, kx, in_c, out_c, w.data(), n, nn_x_len, nn_y_len, use_fp16, epilogue_kind, rotate);
+    std::vector<float> in((size_t)n * nn_x_len * nn_y_len * in_c);
+    for(auto& v : in) { st = st * 1664525u + 1013904223u; v = (st >> 8) * (1.0f / 16777216.0f); }
+    sc.setInput(in.data());
+    for(int i = 0; i < warmup; i++) sc.run();
+    cudaEvent_t e0, e1;
+    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
     CK(cudaStreamSynchronize(sc.h.stream));
-    const int am = sc.h.split ? 2 : 1;
-    std::vector<__half> ha(sc.M * cp * am);
-    CK(cudaMemcpy(ha.data(), sc.acts[0], ha.size() * sizeof(__half), cudaMemcpyDeviceToHost));
-    std::vector<float> hr;
-    if(epilogue_kind >= 2) {
-      hr.resize(sc.M * cp);
-      if(f32) CK(cudaMemcpy(hr.data(), sc.streams[0], hr.size() * sizeof(float), cudaMemcpyDeviceToHost));
-      else {
-        std::vector<__half> hh(hr.size());
-        CK(cudaMemcpy(hh.data(), sc.streams[0], hh.size() * sizeof(__half), cudaMemcpyDeviceToHost));
-        for(size_t k = 0; k < hr.size(); k++) hr[k] = __half2float(hh[k]);
-      }
-    }
-    // every row that is not a board point (pad rows / columns) must have been written as zero: the next conv's halo reads them
-    std::vector<char> onBoard(sc.M, 0);
-    for(int i = 0; i < n; i++) for(int y = 0; y < nn_y_len; y++) for(int x = 0; x < nn_x_len; x++) onBoard[rowOf(i, y, x)] = 1;
-    for(size_t r = 0; r < sc.M; r++)
-      if(!onBoard[r])
-        for(int c = 0; c < cp * am; c++)
-          if(__half2float(ha[r * cp * am + c]) != 0.0f) throw std::runtime_error("kgb_test_conv_epilogue: pad row " + std::to_string(r) + " of the activation output is not zero");
-    for(int i = 0; i < n; i++) for(int y = 0; y < nn_y_len; y++) for(int x = 0; x < nn_x_len; x++) for(int c = 0; c < out_c; c++) {
-      const size_t row = rowOf(i, y, x), o = (((size_t)i * nn_y_len + y) * nn_x_len + x) * out_c + c;
-      act_out[o] = __half2float(ha[row * cp * am + c]) + (am == 2 ? __half2float(ha[row * cp * am + cp + c]) : 0.0f);
-      if(epilogue_kind >= 2) raw_out[o] = hr[row * cp + c];
-    }
+    CK(cudaEventRecord(e0, sc.h.stream));
+    for(int i = 0; i < iters; i++) sc.run();
+    CK(cudaEventRecord(e1, sc.h.stream));
+    CK(cudaStreamSynchronize(sc.h.stream));
+    float ms = 0.0f;
+    CK(cudaEventElapsedTime(&ms, e0, e1));
+    cudaEventDestroy(e0); cudaEventDestroy(e1);
+    *ms_per_launch = ms / iters;
   });
 }
 
@@ -1288,10 +1252,6 @@ KGB_API int kgb_selfplay_run(kgb_selfplay* sp, int steps) {
     if(!sp || steps < 0) throw std::invalid_argument("kgb_selfplay_run: bad argument");
     kgb_handle* h = sp->h;
     CK(cudaSetDevice(h->device));
-    if(!h->useGraph) {
-      for(int i = 0; i < steps; i++) selfplayStepLaunches(sp, h->stream);
-      return;
-    }
     if(!sp->stepGraph) {
       cudaGraph_t graph = nullptr;
       CK(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));

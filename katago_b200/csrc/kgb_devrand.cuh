@@ -59,9 +59,9 @@ struct DevRand {
     s.hasGaussian = 1;
     return v1 * multiplier;
   }
-  // The part of nextGamma that consumes the generator: the Marsaglia-Tsang draw and, for shape <= 1, the uniform whose power scales it.
-  // Returns the unscaled draw; boostU >= 0 means the result still has to be multiplied by pow(boostU, inva) - a pure function that a caller
-  // holding many draws can evaluate in parallel (the stream of random numbers is consumed in exactly the reference's order either way).
+  // A gamma draw without its final scaling: the Marsaglia-Tsang draw and, for shape a <= 1 (drawn with shape a + 1 and scaled by
+  // U^(1/a)), the uniform U.  Returns the unscaled draw; boostU >= 0 means the result still has to be multiplied by pow(boostU, inva) - a pure function
+  // that a caller holding many draws can evaluate in parallel (the stream of random numbers is consumed in exactly the reference's order).
   __device__ double nextGammaCore(double a, double& boostU, double& inva) {
     bool small = false;
     inva = 0.0; boostU = -1.0;
@@ -81,28 +81,6 @@ struct DevRand {
     }
     if(small && inva != 0.0) boostU = nextDouble();   // drawn AFTER the inner gamma, like the recursion in the reference
     return r;
-  }
-  __device__ double nextGamma(double a) {
-    // shape <= 1: draw with shape + 1 and scale by U^(1/a)
-    double boost = 1.0;
-    bool small = false;
-    double inva = 0.0;
-    if(a <= 1.0) { small = true; inva = 1.0 / a; a = a + 1.0; }
-    const double dd = a - 1.0 / 3.0;
-    const double c = (1.0 / 3.0) / sqrt(dd);
-    double r;
-    while(true) {
-      const double x = nextGaussian();
-      const double vtmp = 1.0 + c * x;
-      if(vtmp <= 0.0) continue;
-      const double v = vtmp * vtmp * vtmp;
-      const double u = nextDouble();
-      const double xx = x * x;
-      if(u < 1.0 - 0.0331 * xx * xx) { r = dd * v; break; }
-      if(u == 0.0 || log(u) < 0.5 * xx + dd * (1.0 - v + log(v))) { r = dd * v; break; }
-    }
-    if(small) boost = inva == 0.0 ? 1.0 : pow(nextDouble(), inva);   // drawn AFTER the inner gamma, like the recursion in the reference
-    return r * boost;
   }
 };
 

@@ -271,50 +271,4 @@ cudaError_t launchFinalize(const float* passLogits, int ldp, int cp2, const floa
   return cudaGetLastError();
 }
 
-// ------------------------------------------------------------------------------------------------------------
-// SIMT debug/bring-up convolution: same operands, same epilogue, no tensor cores.  Selected with KGB_CONV_IMPL=simt;
-// lets tests separate "layout/graph logic" failures from "wgmma/TMA plumbing" failures on the GPU.
-// One thread per (row, 16-column chunk).
-__global__ void convSimtKernel(const __half* __restrict__ A, int lda, const __half* __restrict__ W, const ConvParams p) {
-  int chunks = p.cout_p / 16;
-  size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if(idx >= (size_t)p.M * chunks) return;
-  int row = (int)(idx / chunks);
-  int col = (int)(idx % chunks) * 16;
-  float acc[16];
-#pragma unroll
-  for(int j = 0; j < 16; j++) acc[j] = 0.0f;
-  int ry = p.ky / 2, rx = p.kx / 2;
-  int ldw = p.split ? 2 * p.cin_p : p.cin_p;
-  for(int tap = 0; tap < p.ky * p.kx; tap++) {
-    int dy = tap / p.kx - ry, dx = tap % p.kx - rx;
-    long r = (long)row + dy * p.Wp + dx;
-    if(r < 0 || r >= p.M) continue;
-    const __half* a = A + (size_t)r * lda;
-    for(int ci = 0; ci < p.cin_p; ci++) {
-      float av = __half2float(a[ci]);
-      if(p.split) av += __half2float(a[p.cin_p + ci]);
-      if(av == 0.0f) continue;
-#pragma unroll
-      for(int j = 0; j < 16; j++) {
-        const __half* w = W + ((size_t)tap * p.cout_p + col + j) * ldw;
-        float wv = __half2float(w[ci]);
-        if(p.split) wv += __half2float(w[p.cin_p + ci]);
-        acc[j] = fmaf(av, wv, acc[j]);
-      }
-    }
-  }
-  uint32_t accu[16];
-#pragma unroll
-  for(int j = 0; j < 16; j++) accu[j] = __float_as_uint(acc[j]);
-  epilogue_chunk(p, accu, row, col, p.mask[row], row / p.P, p.bn_scale ? p.bn_scale + col : nullptr,
-                 p.bn_bias ? p.bn_bias + col : nullptr);
-}
-
-cudaError_t launchConvSimt(const __half* A, int lda, const __half* W, const ConvParams& p, cudaStream_t stream) {
-  size_t total = (size_t)p.M * (p.cout_p / 16);
-  convSimtKernel<<<(unsigned)((total + 127) / 128), 128, 0, stream>>>(A, lda, W, p);
-  return cudaGetLastError();
-}
-
 }  // namespace kgb

@@ -1312,54 +1312,11 @@ __global__ void __launch_bounds__(SP_LADDER_WARPS * 32, 2) spSelectKernel(const 
 
 // Search::maybeAddPolicyNoiseAndTemp (searchhelpers.cpp:150-215) on the root's post-processed policy: temperature
 // (interpolateEarly :541-545), then Dirichlet noise (addDirichletNoise / computeDirichletAlphaDistribution :78-147).
-// One thread; every sum runs over the policy in position order like the reference's loops.
-__device__ void rootPolicyTemperatureAndNoise(float* pol, int policySize, int X, int Y, int turnNumber, bool noise, double concentration,
-                                              double weight, double temperature, double temperatureEarly, double halflife, DevRandState* randState,
-                                              double* r) {
-  if(temperature != 1.0 || temperatureEarly != 1.0) {
-    const double rawHalflives = (double)turnNumber / halflife;
-    const double halflives = rawHalflives * 19.0 / sqrt((double)(X * Y));
-    const double temp = temperature + (temperatureEarly - temperature) * pow(0.5, halflives);
-    double maxValue = 0.0;
-    for(int i = 0; i < policySize; i++) { const double prob = pol[i]; if(prob > maxValue) maxValue = prob; }
-    const double logMaxValue = log(maxValue), invTemp = 1.0 / temp;
-    double sum = 0.0;
-    for(int i = 0; i < policySize; i++)
-      if(pol[i] > 0) { const float p = (float)exp((log((double)pol[i]) - logMaxValue) * invTemp); pol[i] = p; sum += p; }
-    for(int i = 0; i < policySize; i++)
-      if(pol[i] >= 0) pol[i] = (float)(pol[i] / sum);
-  }
-  if(!noise) return;
-  int legalCount = 0;
-  for(int i = 0; i < policySize; i++) if(pol[i] >= 0) legalCount++;
-  // half of the alpha mass uniform, half shaped by the log policy (clipped at 0.01) above its mean
-  double logPolicySum = 0.0;
-  for(int i = 0; i < policySize; i++)
-    if(pol[i] >= 0) { r[i] = log(fmin(0.01, (double)pol[i]) + 1e-20); logPolicySum += r[i]; }
-  const double logPolicyMean = logPolicySum / legalCount;
-  double alphaPropSum = 0.0;
-  for(int i = 0; i < policySize; i++)
-    if(pol[i] >= 0) { r[i] = fmax(0.0, r[i] - logPolicyMean); alphaPropSum += r[i]; }
-  const double uniformProb = 1.0 / legalCount;
-  for(int i = 0; i < policySize; i++)
-    if(pol[i] >= 0) r[i] = alphaPropSum <= 0.0 ? uniformProb : 0.5 * (r[i] / alphaPropSum + uniformProb);
-  DevRand rand;
-  rand.s = *randState;
-  double rSum = 0.0;
-  for(int i = 0; i < policySize; i++) {
-    if(pol[i] >= 0) { r[i] = rand.nextGamma(r[i] * concentration); rSum += r[i]; }
-    else r[i] = 0.0;
-  }
-  *randState = rand.s;
-  for(int i = 0; i < policySize; i++) r[i] /= rSum;
-  for(int i = 0; i < policySize; i++)
-    if(pol[i] >= 0) pol[i] = (float)(r[i] * weight + pol[i] * (1.0 - weight));
-}
-
-// The same computation by a whole warp: every per-element expression (log / exp / pow, the divisions) is evaluated by the lanes in parallel, every
-// sum is still added in position order (all lanes run the short loop over the staged values), and the gamma draws - one sequential stream of the
-// reference's generator - are made by lane 0 without their final pow, which the lanes then apply in parallel.  Bit-identical to the function
-// above (tests/test_gpu_board_selfplay.py::test_root_dirichlet_noise_matches_reference runs this one).  r: [policySize], r2: [2 * policySize] doubles.
+// One warp: every per-element expression (log / exp / pow, the divisions) is evaluated by the lanes in parallel, every sum is
+// added in position order like the reference's loops (all lanes run the short loop over the staged values), and the gamma
+// draws - one sequential stream of the reference's generator - are made by lane 0 without their final pow, which the lanes
+// then apply in parallel (tests/test_gpu_board_selfplay.py::test_root_dirichlet_noise_matches_reference checks it against the
+// reference's output).  r: [policySize], r2: [2 * policySize] doubles.
 __device__ void rootPolicyTemperatureAndNoiseWarp(float* pol, int policySize, int X, int Y, int turnNumber, bool noise, double concentration,
                                                   double weight, double temperature, double temperatureEarly, double halflife, DevRandState* randState,
                                                   double* r, double* r2, int lane) {
@@ -1386,6 +1343,7 @@ __device__ void rootPolicyTemperatureAndNoiseWarp(float* pol, int policySize, in
   int legalCount = 0;
   for(int i = lane; i < policySize; i += 32) if(pol[i] >= 0) legalCount++;
   legalCount = __reduce_add_sync(KGB_FULL, legalCount);
+  // half of the alpha mass uniform, half shaped by the log policy (clipped at 0.01) above its mean
   for(int i = lane; i < policySize; i += 32)
     if(pol[i] >= 0) r[i] = log(fmin(0.01, (double)pol[i]) + 1e-20);
   __syncwarp();

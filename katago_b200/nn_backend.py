@@ -77,7 +77,7 @@ ABI_SYMBOLS = [
     "kgb_global_init", "kgb_global_cleanup", "kgb_last_error", "kgb_device_count", "kgb_device_name",
     "kgb_model_load_file", "kgb_model_free", "kgb_model_get_info", "kgb_context_create", "kgb_context_free",
     "kgb_handle_create", "kgb_handle_free", "kgb_handle_is_fp16", "kgb_forward", "kgb_forward_device", "kgb_handle_sync",
-    "kgb_handle_stream", "kgb_handle_launches_per_forward", "kgb_test_conv", "kgb_bench_conv", "kgb_bench_conv_ex", "kgb_test_conv_epilogue",
+    "kgb_handle_stream", "kgb_handle_launches_per_forward", "kgb_test_conv", "kgb_bench_conv_ex", "kgb_test_conv_epilogue",
     "kgb_selfplay_create", "kgb_selfplay_free", "kgb_selfplay_run", "kgb_selfplay_get_stats", "kgb_selfplay_get_game",
     "kgb_selfplay_get_root_children", "kgb_selfplay_launches_per_step", "kgb_selfplay_play_moves", "kgb_selfplay_time_tree_kernels", "kgb_zobrist_tables", "kgb_selfplay_get_nn_row", "kgb_selfplay_get_root_row", "kgb_test_board_replay", "kgb_selfplay_get_leaf_path", "kgb_expected_white_score_value", "kgb_value_weight_cdf_table", "kgb_rand_uint32_stream", "kgb_test_root_policy_noise", "kgb_test_history_replay", "kgb_test_repetition_bound", "kgb_selfplay_get_play_selection_values", "kgb_selfplay_random_openings", "kgb_selfplay_set_search_rand", "kgb_selfplay_get_root_value_stats", "kgb_test_choose_index_with_temperature",
     "kgb_handle_weights_bytes", "kgb_handle_stage_weights", "kgb_handle_commit_weights", "kgb_handle_wait_staged", "kgb_nccl_unique_id", "kgb_handle_comm_init",
@@ -147,7 +147,6 @@ def load_library():
     lib.kgb_handle_stream.restype = C.c_uint64
     lib.kgb_handle_launches_per_forward.argtypes = [P]
     lib.kgb_test_conv.argtypes = [I, I, I, I, P, I, I, I, I, P, P]
-    lib.kgb_bench_conv.argtypes = [I, I, I, I, I, I, I, I, I, I, F]
     lib.kgb_bench_conv_ex.argtypes = [I, I, I, I, I, I, I, I, I, I, I, I, F]
     lib.kgb_test_conv_epilogue.argtypes = [I, I, I, I, P, I, I, I, I, I, P, P, P, P, I, P, P]
     lib.kgb_selfplay_create.argtypes = [P, C.POINTER(SelfplayConfig), C.POINTER(P)]

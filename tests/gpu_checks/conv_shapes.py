@@ -13,7 +13,7 @@ shapes = [(3, 192, 192, 72, "b18 inner 3x3"), (1, 384, 192, 18, "b18 block entry
 tot = 0.0
 for k, cin, cout, count, name in shapes:
     ms = np.zeros(1, np.float32)
-    rc = lib.kgb_bench_conv(k, k, cin, cout, n, 19, 19, 1, 5, 40, ms.ctypes.data_as(C.POINTER(C.c_float)))
+    rc = lib.kgb_bench_conv_ex(k, k, cin, cout, n, 19, 19, 1, 1, 1, 5, 40, ms.ctypes.data_as(C.POINTER(C.c_float)))
     assert rc == 0, lib.kgb_last_error()
     us = float(ms[0]) * 1e3
     flop = 2.0 * k * k * cin * cout * 361 * n
