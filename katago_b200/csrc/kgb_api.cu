@@ -93,19 +93,20 @@ static CUtensorMap makeTmap2D(const void* ptr, uint64_t rows, uint64_t cols, uin
   return m;
 }
 
-// Residual stream [rows][cols], fp32 or fp16, box {32 cols, 128 rows}: the slices the convolution's epilogue reads from shared
-// memory, 128B-swizzled for fp32 (128 B rows) and 64B-swizzled for fp16 (64 B rows), zero OOB fill.
-static CUtensorMap makeTmapResidual(const void* ptr, uint64_t rows, uint64_t cols, bool fp32) {
+// Epilogue slices of a stream or operand [rows][cols], fp32 or fp16, box {32 cols, convSliceBoxRows() rows}: the residual the
+// convolution's epilogue reads into shared memory and the raw and activated outputs it stores from there, 128B-swizzled for fp32
+// (128 B rows) and 64B-swizzled for fp16 (64 B rows), zero OOB fill (rows past the end are clipped on store).
+static CUtensorMap makeTmapSlices(const void* ptr, uint64_t rows, uint64_t cols, bool fp32) {
   CUtensorMap m;
   const uint64_t esize = fp32 ? sizeof(float) : sizeof(__half);
   cuuint64_t gdim[2] = {cols, rows};
   cuuint64_t gstride[1] = {cols * esize};
-  cuuint32_t box[2] = {32, 128};
+  cuuint32_t box[2] = {32, (cuuint32_t)convSliceBoxRows()};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = getEncodeTiled()(&m, fp32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(ptr), gdim,
                                 gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, fp32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
                                 CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if(r != CUDA_SUCCESS) throw CudaFailure("cuTensorMapEncodeTiled (residual) failed with CUresult " + std::to_string((int)r));
+  if(r != CUDA_SUCCESS) throw CudaFailure("cuTensorMapEncodeTiled (slices) failed with CUresult " + std::to_string((int)r));
   return m;
 }
 
@@ -332,6 +333,9 @@ struct Builder {
     // the kernel reads a tile's halo rows of A while the neighbouring tiles write their outputs (the scratch passes have no buffers)
     if(h.wMode == kgb_handle::W_BUILD && ((const void*)A == (const void*)actOut || (const void*)A == rawOut))
       throw std::logic_error("emitConv: the operand aliases an output");
+    // the epilogue writes the raw output over the residual slice it read
+    if(residual != nullptr && rawOut != nullptr && residualFp32 != rawFp32)
+      throw std::logic_error("emitConv: the residual and the raw output differ in dtype");
     kgb_handle* hp = &h;
     const int actMulL = actMul;
     h.ops.push_back([=](int n, cudaStream_t s) {
@@ -352,11 +356,14 @@ struct Builder {
       p.act_out = actOut;
       p.bn_scale = bn.scale; p.bn_bias = bn.bias; p.act = bn.act;
       p.mask = hp->dMask;
-      CUtensorMap tmA = makeTmap2D(A, (uint64_t)p.M, (uint64_t)cw.cin_p * actMulL, (uint32_t)convABoxRows(cw.ky, cw.kx, p.Wp));
-      CUtensorMap tmR;
-      memset(&tmR, 0, sizeof(tmR));
-      if(residual != nullptr) tmR = makeTmapResidual(residual, (uint64_t)p.M, (uint64_t)cw.cout_p, residualFp32);
-      CK(launchConvWG(tmA, cw.tmapB, tmR, p, s));
+      ConvTmaps tm;
+      memset(&tm, 0, sizeof(tm));
+      tm.A = makeTmap2D(A, (uint64_t)p.M, (uint64_t)cw.cin_p * actMulL, (uint32_t)convABoxRows(cw.ky, cw.kx, p.Wp));
+      tm.B = cw.tmapB;
+      if(residual != nullptr) tm.residual = makeTmapSlices(residual, (uint64_t)p.M, (uint64_t)cw.cout_p, residualFp32);
+      if(rawOut != nullptr) tm.raw = makeTmapSlices(rawOut, (uint64_t)p.M, (uint64_t)cw.cout_p, rawFp32);
+      if(actOut != nullptr) tm.act = makeTmapSlices(actOut, (uint64_t)p.M, (uint64_t)cw.cout_p * actMulL, false);
+      CK(launchConvWG(tm, p, s));
     });
     h.launchesPerForward++;
   }

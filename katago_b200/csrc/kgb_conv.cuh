@@ -61,14 +61,22 @@ __device__ __forceinline__ float kgb_activate(float x, int act) {
   return x;
 }
 
-// Launcher (defined in kgb_conv_wg.cu)
-// tmapA: [M][cin_p (* 2)] fp16, box {64, convABoxRows}; tmapB: packed weights, box {64, n_tile}; both 128B swizzle.
-// tmapR (read only when p.residual is set): the residual [M][cout_p], box {32, 128}, 128B swizzle when fp32, 64B when fp16.
-// The residual may alias raw_out (each element is read and written by the CTA of its own tile); A must alias neither raw_out nor
-// act_out, since a tile's halo rows belong to the neighbouring tiles.
-cudaError_t launchConvWG(const CUtensorMap& tmapA, const CUtensorMap& tmapB, const CUtensorMap& tmapR, const ConvParams& p,
-                         cudaStream_t stream);
+// Tensor maps of one launch.  A: [M][cin_p (* 2)] fp16, box {64, convABoxRows}; B: packed weights, box {64, n_tile}; both 128B
+// swizzle.  residual, raw, act: box {32, 64} (convSliceBoxRows), 128B swizzle when fp32 and 64B when fp16.  residual = the
+// residual [M][cout_p] (read only when p.residual is set), raw = raw_out [M][cout_p] and act = act_out [M][cout_p * (split ? 2 : 1)]
+// (written only when set).
+struct ConvTmaps {
+  CUtensorMap A, B, residual, raw, act;
+};
+
+// Launcher (defined in kgb_conv_wg.cu).  A persistent grid of at most one CTA per SM walks the output tiles; the epilogue stages
+// its outputs in shared memory and writes them with TMA stores.  When both the residual and raw_out are set they must have the
+// same dtype: the raw output is written back over the residual slice in shared memory.  The residual may alias raw_out (each
+// element is read and written by the CTA of its own tile); A must alias neither raw_out nor act_out, since a tile's halo rows
+// belong to the neighbouring tiles.
+cudaError_t launchConvWG(const ConvTmaps& tm, const ConvParams& p, cudaStream_t stream);
 inline int convABoxRows(int ky, int kx, int Wp) { return 128 + 2 * ((ky / 2) * Wp + (kx / 2)); }  // TMA box rows of the A halo tile
-cudaError_t convWGInit();  // per device, before the first launch
+inline int convSliceBoxRows() { return 64; }  // TMA box rows of the epilogue's slices: one consumer warpgroup's half of a tile
+cudaError_t convWGInit();  // per device, before the first launch (sets the kernels' shared-memory limit, reads the SM count)
 
 }  // namespace kgb

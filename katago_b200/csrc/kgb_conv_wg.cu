@@ -13,17 +13,24 @@
 //         through a shared-memory descriptor.
 //   D   = fp32 in registers: warpgroup g of the two consumer warpgroups owns rows 64g..64g+63 of the 128-row tile.
 //
-// One CTA per (128-row, n_tile) tile, 384 threads:
-//   warpgroup 0   TMA producer (one lane): A halo tiles into a 2-deep ring, one weight tile per tap into a deeper ring, and the
-//                 tile's residual in 32-column slices into a 4-slot ring (the first slices at the start, so they land during the
-//                 main loop; the rest as the epilogue frees slots)
-//   warpgroups 1-2  ldmatrix + wgmma.mma_async m64 x n_tile x 16, then the fused epilogue straight from the accumulators
+// Persistent CTAs, 384 threads: min(tiles, SMs) CTAs (rounded down to a multiple of num_n_tiles, so that a CTA keeps one n0)
+// walk the (128-row, n_tile) tiles blockIdx.x, blockIdx.x + gridDim.x, ... in m-major order.
+//   warpgroup 0   TMA producers.  Lane 0 of warp 0: A halo tiles into a 2-deep ring and one weight tile per tap into a deeper
+//                 ring.  Lane 0 of warp 1: the residual in 32-column slices into a ring of up to 4 slots.  Every ring keeps its
+//                 stage and phase across tiles, so tile i+1's A halo, first weight stages and first residual slices land while
+//                 the consumers are still in tile i's epilogue.
+//   warpgroups 1-2  ldmatrix + wgmma.mma_async m64 x n_tile x 16, then the fused epilogue from the accumulators into shared
+//                 memory, written out by TMA stores that overlap the next tile's main loop.
 // The A fragments are double-buffered in registers: step t+1's ldmatrix runs while step t's wgmma group is still in flight,
-// and a consumer waits only for the group before the one it just issued (wait_group 1).  The epilogue reads the residual, the
-// mask and the BN constants from shared memory, so no global load sits between its stores.
+// and a consumer waits only for the group before the one it just issued (wait_group 1).  The epilogue reads the residual and the
+// BN constants from shared memory and the tile's mask from registers, so no global load sits in it.  It writes the raw stream back
+// into the residual slice it read (a staging slot when there is no residual) and the activated operand into a 2-slot ring of
+// 128 x 32 fp16 slices; each warpgroup stores its 64-row half of a slice with one TMA store per output.
 //
 // "split" mode computes a*w ~= ah*wh + al*wh + ah*wl with a = ah + al, w = wh + wl in fp16 (fp32 accumulate):
 // fp32-grade accuracy on the fp16 tensor pipe at 3x the MMA count (the backend's useFP16=false mode).
+#include <algorithm>
+
 #include "kgb_conv.cuh"
 #include "kgb_wgmma.cuh"
 
@@ -35,8 +42,11 @@ static constexpr int MAX_STAGES = 8;
 static constexpr int SMEM_LIMIT = 227 * 1024;
 static constexpr int THREADS = 384;
 static constexpr int CONSUMER_WARPS = 8;
-static constexpr int RES_COLS = 32;     // columns of one residual slice (every n_tile is a multiple of 32)
-static constexpr int RES_SLOTS = 4;     // residual ring: 4 x 16 KB for an fp32 stream, 4 x 8 KB for fp16
+static constexpr int RES_COLS = 32;     // columns of one epilogue slice (every n_tile is a multiple of 32)
+static constexpr int RES_SLOTS = 4;     // stream ring with a residual: 4 x 16 KB for an fp32 stream, 4 x 8 KB for fp16
+static constexpr int STAGE_SLOTS = 2;   // stream ring without one (raw output staging only)
+static constexpr int ACT_SLOTS = 2;     // activated-operand ring: 128 x 32 fp16 slices (hi and lo in split mode)
+static constexpr int ACT_SLICE_BYTES = BLOCK_M * RES_COLS * 2;
 
 // ------------------------------------------------------------------------------------------------------------
 // PTX wrappers
@@ -81,6 +91,16 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 __device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }   // the two consumer warpgroups
+__device__ __forceinline__ void warpgroup_sync(int g) { asm volatile("bar.sync %0, 128;" ::"r"(2 + g) : "memory"); }
+// TMA stores: the generic-proxy writes of every thread are made visible to the async proxy before the barrier that precedes the store
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(map), "r"(src), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // wgmma shared-memory descriptor, K-major, 128B swizzle:
 //   [0,14) start>>4 | [16,30) LBO>>4 (1, unused for swizzled K-major) | [32,46) SBO>>4 (1024 B = 8 rows x 128 B) | [62,64) 1 = 128B swizzle
@@ -100,35 +120,44 @@ struct __align__(8) Bars {
   uint64_t a_full[2];           // A halo tile landed
   uint64_t a_empty[2];          // A halo tile consumed by all of its taps
   uint64_t r_full[RES_SLOTS];   // residual slice landed
-  uint64_t r_empty[RES_SLOTS];  // residual slice consumed by every consumer warp
+  uint64_t r_empty[RES_SLOTS];  // residual slice read, and the raw stream written over it stored, by both consumer warpgroups
 };
 
-// dynamic smem: [<=1023 B slack][2 x A halo tile][RES_SLOTS x residual slice][stages x weight tile][Bars][mask 128][BN scale N][BN bias N]
+// dynamic smem: [<=1023 B slack][2 x A halo tile][stream ring][ACT_SLOTS x act slice (x 2 split)][stages x weight tile][Bars]
+//               [BN scale N][BN bias N]
 static inline int aBufBytes(int a_box_rows) { return (a_box_rows * BLOCK_K * 2 + 1023) / 1024 * 1024; }
-// One residual slice = one TMA box of 128 rows x 32 columns.  fp32 rows are 128 B with the 128B swizzle (16-byte chunk c of row r
-// at c ^ (r & 7)), fp16 rows 64 B with the 64B swizzle (chunk c at c ^ ((r >> 1) & 3)): either way the 8 rows one warp reads per
-// fragment column fall into distinct banks.
-__host__ __device__ inline int resSlotBytes(const ConvParams& p) {
-  return p.residual != nullptr ? BLOCK_M * RES_COLS * (p.residual_fp32 ? 4 : 2) : 0;
+// The stream ring holds the residual, and the raw output written back over it; without a residual it only stages the raw output.
+// When both exist they have the same dtype (the launcher checks it).
+__host__ __device__ inline bool streamFp32(const ConvParams& p) { return p.residual != nullptr ? p.residual_fp32 != 0 : p.raw_fp32 != 0; }
+__host__ __device__ inline int streamSlots(const ConvParams& p) {
+  return p.residual != nullptr ? RES_SLOTS : p.raw_out != nullptr ? STAGE_SLOTS : 0;
 }
-__device__ __forceinline__ float2 load_residual(const uint8_t* slot, int r, int c, bool fp32) {
-  if(fp32) return *reinterpret_cast<const float2*>(slot + r * 128 + ((((c >> 2) ^ (r & 7)) << 4) | ((c & 3) << 2)));
-  return __half22float2(*reinterpret_cast<const __half2*>(slot + r * 64 + ((((c >> 3) ^ ((r >> 1) & 3)) << 4) | ((c & 7) << 1))));
+__host__ __device__ inline int streamSlotBytes(const ConvParams& p) { return BLOCK_M * RES_COLS * (streamFp32(p) ? 4 : 2); }
+__host__ __device__ inline int actSlotBytes(const ConvParams& p) {
+  return p.act_out != nullptr ? ACT_SLICE_BYTES * (p.split ? 2 : 1) : 0;
+}
+// One slice = 128 rows x 32 columns, moved as two TMA boxes of 64 rows (one per consumer warpgroup).  fp32 rows are 128 B with the
+// 128B swizzle (16-byte chunk c of row r at c ^ (r & 7)), fp16 rows 64 B with the 64B swizzle (chunk c at c ^ ((r >> 1) & 3)):
+// either way the 8 rows one warp touches per fragment column fall into distinct banks.
+__device__ __forceinline__ int slice_offset(int r, int c, bool fp32) {
+  if(fp32) return r * 128 + ((((c >> 2) ^ (r & 7)) << 4) | ((c & 3) << 2));
+  return r * 64 + ((((c >> 3) ^ ((r >> 1) & 3)) << 4) | ((c & 7) << 1));
 }
 
 // Epilogue of two adjacent columns (col, col+1) of one accumulator row: r = the residual (used when p.residual is set), sc / bi =
-// the BN constants of col in shared memory.
+// the BN constants of col in shared memory.  raw goes to `raw_dst` in the stream slice, the activated operand to `act_dst` (and
+// its lo half to `act_lo_dst` in split mode).
 __device__ __forceinline__ void epilogue_store(const ConvParams& p, int row, int col, float v0, float v1, float maskv, float2 r,
-                                               const float* sc, const float* bi) {
+                                               const float* sc, const float* bi, uint8_t* raw_dst, uint8_t* act_dst,
+                                               uint8_t* act_lo_dst) {
   if(p.ncbias != nullptr) {
     const float2 b = __ldg(reinterpret_cast<const float2*>(p.ncbias + (size_t)(row / p.P) * p.cout_p + col));
     v0 += b.x; v1 += b.y;
   }
-  const size_t off = (size_t)row * p.cout_p + col;
   if(p.residual != nullptr) { v0 += r.x; v1 += r.y; }
   if(p.raw_out != nullptr) {
-    if(p.raw_fp32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.raw_out) + off) = make_float2(v0 * maskv, v1 * maskv);
-    else *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.raw_out) + off) = __floats2half2_rn(v0 * maskv, v1 * maskv);
+    if(p.raw_fp32) *reinterpret_cast<float2*>(raw_dst) = make_float2(v0 * maskv, v1 * maskv);
+    else *reinterpret_cast<__half2*>(raw_dst) = __floats2half2_rn(v0 * maskv, v1 * maskv);
   }
   if(p.act_out != nullptr) {
     float a0 = fmaf(v0, sc[0], bi[0]);
@@ -143,13 +172,11 @@ __device__ __forceinline__ void epilogue_store(const ConvParams& p, int row, int
       a1 = kgb_activate(a1, p.act);
     }
     if(maskv == 0.0f) { a0 = 0.0f; a1 = 0.0f; }   // pad and off-board rows (also guards NaN/inf garbage there)
-    const int ldo = p.split ? 2 * p.cout_p : p.cout_p;
-    __half* dst = p.act_out + (size_t)row * ldo + col;
     const __half2 h = __floats2half2_rn(a0, a1);
-    *reinterpret_cast<__half2*>(dst) = h;
+    *reinterpret_cast<__half2*>(act_dst) = h;
     if(p.split) {
       const float2 hf = __half22float2(h);
-      *reinterpret_cast<__half2*>(dst + p.cout_p) = __floats2half2_rn(a0 - hf.x, a1 - hf.y);
+      *reinterpret_cast<__half2*>(act_lo_dst) = __floats2half2_rn(a0 - hf.x, a1 - hf.y);
     }
   }
 }
@@ -157,7 +184,8 @@ __device__ __forceinline__ void epilogue_store(const ConvParams& p, int row, int
 template <int N>
 __global__ void __launch_bounds__(THREADS, 1)
 kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapB,
-                   const __grid_constant__ CUtensorMap tmapR, const __grid_constant__ ConvParams p, int stages) {
+                   const __grid_constant__ CUtensorMap tmapR, const __grid_constant__ CUtensorMap tmapRaw,
+                   const __grid_constant__ CUtensorMap tmapAct, const __grid_constant__ ConvParams p, int stages) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr int b_tile_bytes = N * BLOCK_K * 2;               // one tap's weight tile
@@ -165,19 +193,20 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
   const int a_tx_bytes = (BLOCK_M + 2 * halo) * BLOCK_K * 2;
   const int a_buf_bytes = (a_tx_bytes + 1023) / 1024 * 1024;
   constexpr int slices = N / RES_COLS;
-  const int r_slot_bytes = resSlotBytes(p);
+  const int r_slots = streamSlots(p), r_slot_bytes = streamSlotBytes(p), act_slot_bytes = actSlotBytes(p);
+  const bool s_fp32 = streamFp32(p);
   const uint32_t smem_r = smem_base + 2 * a_buf_bytes;
-  const uint32_t smem_b = smem_r + RES_SLOTS * r_slot_bytes;
+  const uint32_t smem_act = smem_r + r_slots * r_slot_bytes;
+  const uint32_t smem_b = smem_act + ACT_SLOTS * act_slot_bytes;
   uint8_t* const smem = smem_raw + (smem_base - smem_u32(smem_raw));
   Bars* bars = reinterpret_cast<Bars*>(smem + (smem_b - smem_base) + (size_t)stages * b_tile_bytes);
-  float* const s_mask = reinterpret_cast<float*>(bars + 1);
-  float* const s_scale = s_mask + BLOCK_M;
+  float* const s_scale = reinterpret_cast<float*>(bars + 1);
   float* const s_bias = s_scale + N;
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
-  const int m0 = (blockIdx.x / p.num_n_tiles) * BLOCK_M;
-  const int n0 = (blockIdx.x % p.num_n_tiles) * N;
+  const int tiles = p.num_m_tiles * p.num_n_tiles;
+  const int n0 = (blockIdx.x % p.num_n_tiles) * N;            // gridDim.x is a multiple of num_n_tiles: one n0 per CTA
   const int taps = p.ky * p.kx;
   const int parts = p.split ? 3 : 1;
   const int phases = (p.cin_p / BLOCK_K) * parts;             // one A halo tile per (k-block, split part)
@@ -186,6 +215,8 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapB) : "memory");
     if(p.residual != nullptr) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapR) : "memory");
+    if(p.raw_out != nullptr) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapRaw) : "memory");
+    if(p.act_out != nullptr) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapAct) : "memory");
     for(int s = 0; s < stages; s++) {
       mbar_init(smem_u32(&bars->full[s]), 1);
       mbar_init(smem_u32(&bars->empty[s]), CONSUMER_WARPS);
@@ -196,47 +227,55 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
     }
     for(int s = 0; s < RES_SLOTS; s++) {
       mbar_init(smem_u32(&bars->r_full[s]), 1);
-      mbar_init(smem_u32(&bars->r_empty[s]), CONSUMER_WARPS);
+      mbar_init(smem_u32(&bars->r_empty[s]), 2);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
 
   if(warp < 4) {
-    // ===================== TMA producer =====================
+    // ===================== TMA producers =====================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if(warp == 0 && lane == 0) {
-      auto load_residual_slice = [&](int s) {
-        const uint32_t rfull = smem_u32(&bars->r_full[s % RES_SLOTS]);
-        mbar_arrive_expect_tx(rfull, (uint32_t)r_slot_bytes);
-        tma_load_2d(smem_r + (s % RES_SLOTS) * r_slot_bytes, &tmapR, rfull, n0 + s * RES_COLS, m0);
-      };
-      if(p.residual != nullptr)
-        for(int s = 0; s < slices && s < RES_SLOTS; s++) load_residual_slice(s);
-      int stage = 0; uint32_t phase = 0;
-      for(int ph = 0; ph < phases; ph++) {
-        const int kb = ph / parts, part = ph - kb * parts;
-        const int colA = kb * BLOCK_K + (part == 1 ? p.cin_p : 0);
-        const int colB = kb * BLOCK_K + (part == 2 ? p.cin_p : 0);
-        const int abuf = ph & 1;
-        mbar_wait(smem_u32(&bars->a_empty[abuf]), ((ph >> 1) & 1) ^ 1);
-        const uint32_t afull = smem_u32(&bars->a_full[abuf]);
-        mbar_arrive_expect_tx(afull, (uint32_t)a_tx_bytes);
-        tma_load_2d(smem_base + abuf * a_buf_bytes, &tmapA, afull, colA, m0 - halo);
-        for(int t = 0; t < taps; t++) {
-          mbar_wait(smem_u32(&bars->empty[stage]), phase ^ 1);
-          const uint32_t full = smem_u32(&bars->full[stage]);
-          mbar_arrive_expect_tx(full, (uint32_t)b_tile_bytes);
-          tma_load_2d(smem_b + stage * b_tile_bytes, &tmapB, full, colB, t * p.cout_p + n0);
-          if(++stage == stages) { stage = 0; phase ^= 1; }
+      // A halo tiles and weight tiles, running ahead across tiles as far as the two rings allow
+      int stage = 0, ac = 0;
+      uint32_t phase = 0;
+      for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        const int m0 = (tile / p.num_n_tiles) * BLOCK_M;
+        for(int ph = 0; ph < phases; ph++, ac++) {
+          const int kb = ph / parts, part = ph - kb * parts;
+          const int colA = kb * BLOCK_K + (part == 1 ? p.cin_p : 0);
+          const int colB = kb * BLOCK_K + (part == 2 ? p.cin_p : 0);
+          const int abuf = ac & 1;
+          mbar_wait(smem_u32(&bars->a_empty[abuf]), ((ac >> 1) & 1) ^ 1);
+          const uint32_t afull = smem_u32(&bars->a_full[abuf]);
+          mbar_arrive_expect_tx(afull, (uint32_t)a_tx_bytes);
+          tma_load_2d(smem_base + abuf * a_buf_bytes, &tmapA, afull, colA, m0 - halo);
+          for(int t = 0; t < taps; t++) {
+            mbar_wait(smem_u32(&bars->empty[stage]), phase ^ 1);
+            const uint32_t full = smem_u32(&bars->full[stage]);
+            mbar_arrive_expect_tx(full, (uint32_t)b_tile_bytes);
+            tma_load_2d(smem_b + stage * b_tile_bytes, &tmapB, full, colB, t * p.cout_p + n0);
+            if(++stage == stages) { stage = 0; phase ^= 1; }
+          }
         }
       }
-      // slice s reuses the slot of slice s - RES_SLOTS once every consumer warp has read that one
-      if(p.residual != nullptr)
-        for(int s = RES_SLOTS; s < slices; s++) {
-          mbar_wait(smem_u32(&bars->r_empty[s % RES_SLOTS]), (uint32_t)(s / RES_SLOTS - 1) & 1);
-          load_residual_slice(s);
+    }
+    else if(warp == 1 && lane == 0 && p.residual != nullptr) {
+      // residual slices, in their own lane so that one waiting on a slot does not hold up the next tile's A
+      int rs = 0;
+      uint32_t rphase = 0;
+      for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        const int m0 = (tile / p.num_n_tiles) * BLOCK_M;
+        for(int s = 0; s < slices; s++) {
+          mbar_wait(smem_u32(&bars->r_empty[rs]), rphase ^ 1);
+          const uint32_t rfull = smem_u32(&bars->r_full[rs]), dst = smem_r + rs * r_slot_bytes;
+          mbar_arrive_expect_tx(rfull, (uint32_t)r_slot_bytes);
+          tma_load_2d(dst, &tmapR, rfull, n0 + s * RES_COLS, m0);
+          tma_load_2d(dst + r_slot_bytes / 2, &tmapR, rfull, n0 + s * RES_COLS, m0 + BLOCK_M / 2);
+          if(++rs == RES_SLOTS) { rs = 0; rphase ^= 1; }
         }
+      }
     }
     return;
   }
@@ -244,94 +283,135 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
   // ===================== consumers: warpgroup g owns tile rows 64g..64g+63, warp q of it rows 16q..16q+15 =====================
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
   const int g = (warp - 4) >> 2, q = warp & 3;
+  const bool leader = q == 0 && lane == 0;    // issues the warpgroup's TMA stores
   const int ry = p.ky / 2, rx = p.kx / 2;
   // ldmatrix.x4 lane roles: matrix j = lane / 8 supplies (rows +0 / +8) x (k 0-7 / 8-15) of a 16 x 16 A fragment
   const int lrow = g * 64 + q * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
   const uint32_t lchunk = (uint32_t)(lane >> 4);
-  // the tile's mask and BN constants into shared memory; the epilogue reads them after the consumer barrier below
-  {
-    const int ct = threadIdx.x - 128;
-    if(ct < BLOCK_M) s_mask[ct] = m0 + ct < p.M ? __ldg(p.mask + m0 + ct) : 0.0f;
-    if(p.act_out != nullptr)
-      for(int i = ct; i < N; i += 32 * CONSUMER_WARPS) { s_scale[i] = __ldg(p.bn_scale + n0 + i); s_bias[i] = __ldg(p.bn_bias + n0 + i); }
-  }
-  float acc[N / 2];
-#pragma unroll
-  for(int i = 0; i < N / 2; i++) acc[i] = 0.0f;
-  fence_acc(acc);
-  // One step = one (k-block, tap): ldmatrix the tap's A fragments into `af` and issue its 4 wgmma as one group.  Steps alternate
-  // between two fragment buffers; wait_group 1 after issuing step i means step i-1's group has finished, so its weight stage can be
-  // released and its fragment buffer is free for step i+1.  The MMAs reach the accumulators in k-block, tap, k16 order as before.
-  int stage = 0, prev_stage = -1, ph = 0, t = 0, dy = -ry, dx = -rx;
-  uint32_t phase = 0;
-  auto step = [&](uint32_t (&af)[4][4]) {
-    const int abuf = ph & 1;
-    if(t == 0) mbar_wait(smem_u32(&bars->a_full[abuf]), (ph >> 1) & 1);
-    const uint32_t a_base = smem_base + abuf * a_buf_bytes;
-    // tap (dy,dx) = the tile's rows shifted by `halo + dy*Wp + dx`; the 128B swizzle puts 16-byte chunk c of row r at c ^ (r & 7)
-    const uint32_t r = (uint32_t)(lrow + halo + dy * p.Wp + dx);
-#pragma unroll
-    for(int k = 0; k < 4; k++) ldmatrix_x4(a_base + r * 128u + (((2u * k + lchunk) ^ (r & 7u)) << 4), af[k]);
-    mbar_wait(smem_u32(&bars->full[stage]), phase);
-    const uint64_t db = make_smem_desc(smem_b + stage * b_tile_bytes);
-    wgmma_fence();
-#pragma unroll
-    for(int k = 0; k < 4; k++) Wgmma<N>::mma(acc, af[k], db + 2 * k);
-    wgmma_commit();
-    // the wgmma issue above consumed the fragments of the k-block's last tap, so its A halo tile may be refilled
-    if(t == taps - 1) {
-      __syncwarp();
-      if(lane == 0) mbar_arrive(smem_u32(&bars->a_empty[abuf]));
-    }
-    wgmma_wait1();
-    if(prev_stage >= 0) {
-      __syncwarp();
-      if(lane == 0) mbar_arrive(smem_u32(&bars->empty[prev_stage]));
-    }
-    prev_stage = stage;
-    if(++stage == stages) { stage = 0; phase ^= 1; }
-    if(++dx > rx) { dx = -rx; dy++; }
-    if(++t == taps) { t = 0; dy = -ry; ph++; }
-  };
-  const int steps = phases * taps;
-  uint32_t af0[4][4], af1[4][4];
-  for(int i = 0; i + 1 < steps; i += 2) {
-    step(af0);
-    step(af1);
-  }
-  if(steps & 1) step(af0);
-  wgmma_wait0();   // the last group; the producer loads no further weight tile, so its stage is not released
-  fence_acc(acc);
-  consumer_sync();   // s_mask / s_scale / s_bias written
-
-  // ===================== epilogue straight from the accumulator fragments, one 32-column residual slice at a time =====================
   // acc[4j + 2h + e]: row 16q + lane/4 + 8h of the warpgroup's 64, column 8j + 2*(lane%4) + e
   const int rloc = g * 64 + q * 16 + (lane >> 2);
-  const uint8_t* const ring = smem + (smem_r - smem_base);
+  // the CTA's BN constants into shared memory, once: every tile of the CTA has the same n0
+  if(p.act_out != nullptr)
+    for(int i = threadIdx.x - 128; i < N; i += 32 * CONSUMER_WARPS) { s_scale[i] = __ldg(p.bn_scale + n0 + i); s_bias[i] = __ldg(p.bn_bias + n0 + i); }
+  consumer_sync();
+
+  // ring positions, carried across tiles like the producers'
+  int stage = 0, ph = 0;
+  uint32_t phase = 0;
+  int rs = 0, prev_rs = -1, as = 0;
+  uint32_t rphase = 0;
+  uint8_t* const ring = smem + (smem_r - smem_base);
+  uint8_t* const act_ring = smem + (smem_act - smem_base);
+  for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int m0 = (tile / p.num_n_tiles) * BLOCK_M;
+    // this thread's two epilogue rows' mask values; the loads complete during the main loop
+    const float mask0 = m0 + rloc < p.M ? __ldg(p.mask + m0 + rloc) : 0.0f;
+    const float mask1 = m0 + rloc + 8 < p.M ? __ldg(p.mask + m0 + rloc + 8) : 0.0f;
+    float acc[N / 2];
 #pragma unroll
-  for(int s = 0; s < slices; s++) {
-    const uint8_t* const slot = ring + (s % RES_SLOTS) * r_slot_bytes;
-    if(p.residual != nullptr) mbar_wait(smem_u32(&bars->r_full[s % RES_SLOTS]), (uint32_t)(s / RES_SLOTS) & 1);
+    for(int i = 0; i < N / 2; i++) acc[i] = 0.0f;
+    fence_acc(acc);
+    // One step = one (k-block, tap): ldmatrix the tap's A fragments into `af` and issue its 4 wgmma as one group.  Steps alternate
+    // between two fragment buffers; wait_group 1 after issuing step i means step i-1's group has finished, so its weight stage can
+    // be released and its fragment buffer is free for step i+1.  The MMAs reach the accumulators in k-block, tap, k16 order.
+    int prev_stage = -1, t = 0, dy = -ry, dx = -rx;
+    auto step = [&](uint32_t (&af)[4][4]) {
+      const int abuf = ph & 1;
+      if(t == 0) mbar_wait(smem_u32(&bars->a_full[abuf]), (ph >> 1) & 1);
+      const uint32_t a_base = smem_base + abuf * a_buf_bytes;
+      // tap (dy,dx) = the tile's rows shifted by `halo + dy*Wp + dx`; the 128B swizzle puts 16-byte chunk c of row r at c ^ (r & 7)
+      const uint32_t r = (uint32_t)(lrow + halo + dy * p.Wp + dx);
 #pragma unroll
-    for(int h = 0; h < 2; h++) {
-      const int rl = rloc + 8 * h, row = m0 + rl;
-      if(row >= p.M) continue;
-      const float maskv = s_mask[rl];
+      for(int k = 0; k < 4; k++) ldmatrix_x4(a_base + r * 128u + (((2u * k + lchunk) ^ (r & 7u)) << 4), af[k]);
+      mbar_wait(smem_u32(&bars->full[stage]), phase);
+      const uint64_t db = make_smem_desc(smem_b + stage * b_tile_bytes);
+      wgmma_fence();
 #pragma unroll
-      for(int jj = 0; jj < RES_COLS / 8; jj++) {
-        const int j = s * (RES_COLS / 8) + jj, lc = 8 * j + 2 * (lane & 3);
-        const float2 r = p.residual != nullptr ? load_residual(slot, rl, lc - s * RES_COLS, p.residual_fp32 != 0) : make_float2(0.0f, 0.0f);
-        epilogue_store(p, row, n0 + lc, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], maskv, r, s_scale + lc, s_bias + lc);
+      for(int k = 0; k < 4; k++) Wgmma<N>::mma(acc, af[k], db + 2 * k);
+      wgmma_commit();
+      // the wgmma issue above consumed the fragments of the k-block's last tap, so its A halo tile may be refilled
+      if(t == taps - 1) {
+        __syncwarp();
+        if(lane == 0) mbar_arrive(smem_u32(&bars->a_empty[abuf]));
       }
+      wgmma_wait1();
+      if(prev_stage >= 0) {
+        __syncwarp();
+        if(lane == 0) mbar_arrive(smem_u32(&bars->empty[prev_stage]));
+      }
+      prev_stage = stage;
+      if(++stage == stages) { stage = 0; phase ^= 1; }
+      if(++dx > rx) { dx = -rx; dy++; }
+      if(++t == taps) { t = 0; dy = -ry; ph++; }
+    };
+    const int steps = phases * taps;
+    uint32_t af0[4][4], af1[4][4];
+    for(int i = 0; i + 1 < steps; i += 2) {
+      step(af0);
+      step(af1);
     }
-    if(p.residual != nullptr && s + RES_SLOTS < slices) {
-      __syncwarp();
-      if(lane == 0) mbar_arrive(smem_u32(&bars->r_empty[s % RES_SLOTS]));
+    if(steps & 1) step(af0);
+    wgmma_wait0();
+    fence_acc(acc);
+    __syncwarp();
+    if(lane == 0) mbar_arrive(smem_u32(&bars->empty[prev_stage]));   // the tile's last stage: the producer is already on the next tile
+
+    // ===================== epilogue: one 32-column slice at a time, into shared memory, out by TMA stores =====================
+#pragma unroll
+    for(int s = 0; s < slices; s++) {
+      uint8_t* const slot = ring + rs * r_slot_bytes;
+      uint8_t* const aslot = act_ring + as * act_slot_bytes;
+      if(p.residual != nullptr) mbar_wait(smem_u32(&bars->r_full[rs]), rphase);
+#pragma unroll
+      for(int h = 0; h < 2; h++) {
+        const int rl = rloc + 8 * h, row = m0 + rl;
+        if(row >= p.M) continue;   // no ncbias entry for rows past the batch; the TMA stores clip them
+        const float maskv = h ? mask1 : mask0;
+#pragma unroll
+        for(int jj = 0; jj < RES_COLS / 8; jj++) {
+          const int j = s * (RES_COLS / 8) + jj, lc = 8 * j + 2 * (lane & 3), c = lc - s * RES_COLS;
+          uint8_t* const rp = slot + slice_offset(rl, c, s_fp32);
+          uint8_t* const ap = aslot + slice_offset(rl, c, false);
+          const float2 r = p.residual != nullptr ? (s_fp32 ? *reinterpret_cast<const float2*>(rp)
+                                                           : __half22float2(*reinterpret_cast<const __half2*>(rp)))
+                                                 : make_float2(0.0f, 0.0f);
+          epilogue_store(p, row, n0 + lc, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], maskv, r, s_scale + lc, s_bias + lc, rp, ap,
+                         ap + ACT_SLICE_BYTES);
+        }
+      }
+      fence_proxy_async();
+      if(leader) {
+        // the previous slice's stores have read their slots: its act slot (the next slice's) and its stream slot are free again
+        bulk_wait_read0();
+        if(p.residual != nullptr && prev_rs >= 0) mbar_arrive(smem_u32(&bars->r_empty[prev_rs]));
+      }
+      warpgroup_sync(g);
+      if(leader) {
+        const int c0 = n0 + s * RES_COLS, r0 = m0 + g * (BLOCK_M / 2);
+        if(p.raw_out != nullptr) tma_store_2d(&tmapRaw, smem_u32(slot + g * (r_slot_bytes / 2)), c0, r0);
+        if(p.act_out != nullptr) {
+          tma_store_2d(&tmapAct, smem_u32(aslot + g * (ACT_SLICE_BYTES / 2)), c0, r0);
+          if(p.split) tma_store_2d(&tmapAct, smem_u32(aslot + ACT_SLICE_BYTES + g * (ACT_SLICE_BYTES / 2)), p.cout_p + c0, r0);
+        }
+        bulk_commit();
+      }
+      prev_rs = rs;
+      if(++rs >= r_slots) { rs = 0; rphase ^= 1; }   // r_slots is 0 when there is no stream
+      as ^= 1;
     }
   }
+  if(leader) bulk_wait0();
 }
 
+static int g_smCount[64];   // per device ordinal, read by convWGInit
+
 cudaError_t convWGInit() {
+  int dev = 0;
+  cudaError_t e0 = cudaGetDevice(&dev);
+  if(e0 != cudaSuccess) return e0;
+  if(dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
+  e0 = cudaDeviceGetAttribute(&g_smCount[dev], cudaDevAttrMultiProcessorCount, dev);
+  if(e0 != cudaSuccess) return e0;
   for(cudaError_t e : {cudaFuncSetAttribute(kgb_conv_wg_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
                        cudaFuncSetAttribute(kgb_conv_wg_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
                        cudaFuncSetAttribute(kgb_conv_wg_kernel<96>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
@@ -345,34 +425,42 @@ cudaError_t convWGInit() {
 }
 
 template <int N>
-static cudaError_t launchN(const CUtensorMap& tmapA, const CUtensorMap& tmapB, const CUtensorMap& tmapR, const ConvParams& p, int stages,
-                           int smem, cudaStream_t stream) {
-  kgb_conv_wg_kernel<N><<<p.num_m_tiles * p.num_n_tiles, THREADS, smem, stream>>>(tmapA, tmapB, tmapR, p, stages);
+static cudaError_t launchN(const ConvTmaps& tm, const ConvParams& p, int grid, int stages, int smem, cudaStream_t stream) {
+  kgb_conv_wg_kernel<N><<<grid, THREADS, smem, stream>>>(tm.A, tm.B, tm.residual, tm.raw, tm.act, p, stages);
   return cudaGetLastError();
 }
 
-cudaError_t launchConvWG(const CUtensorMap& tmapA, const CUtensorMap& tmapB, const CUtensorMap& tmapR, const ConvParams& p,
-                         cudaStream_t stream) {
+cudaError_t launchConvWG(const ConvTmaps& tm, const ConvParams& p, cudaStream_t stream) {
   const int halo = (p.ky / 2) * p.Wp + (p.kx / 2);
   if(BLOCK_M + 2 * halo > 256) return cudaErrorInvalidValue;  // TMA box limit
   if(p.n_tile % RES_COLS != 0) return cudaErrorInvalidValue;
+  // the raw output is written over the residual slice it was read from
+  if(p.residual != nullptr && p.raw_out != nullptr && (p.residual_fp32 != 0) != (p.raw_fp32 != 0)) return cudaErrorInvalidValue;
+  int dev = 0;
+  const cudaError_t e = cudaGetDevice(&dev);
+  if(e != cudaSuccess) return e;
+  if(dev < 0 || dev >= 64 || g_smCount[dev] < 1) return cudaErrorInitializationError;   // convWGInit not run on this device
   const int bTile = p.n_tile * BLOCK_K * 2;
-  // the residual ring and the epilogue's mask / BN copies come first; the weight ring gets what is left
-  const int fixed = 1024 + 2 * aBufBytes(BLOCK_M + 2 * halo) + RES_SLOTS * resSlotBytes(p) + (int)sizeof(Bars) +
-                    (BLOCK_M + 2 * p.n_tile) * (int)sizeof(float);
+  // the stream and act rings and the BN copies come first; the weight ring gets what is left
+  const int fixed = 1024 + 2 * aBufBytes(BLOCK_M + 2 * halo) + streamSlots(p) * streamSlotBytes(p) + ACT_SLOTS * actSlotBytes(p) +
+                    (int)sizeof(Bars) + 2 * p.n_tile * (int)sizeof(float);
   int stages = (SMEM_LIMIT - fixed) / bTile;
   if(stages > MAX_STAGES) stages = MAX_STAGES;
   if(stages < 2) return cudaErrorInvalidValue;
   const int smem = fixed + stages * bTile;
+  // persistent grid: at most one CTA per SM (the rings take all of shared memory), a multiple of num_n_tiles
+  const int tiles = p.num_m_tiles * p.num_n_tiles;
+  int grid = std::min(tiles, g_smCount[dev]) / p.num_n_tiles * p.num_n_tiles;
+  if(grid < p.num_n_tiles) grid = p.num_n_tiles;
   switch(p.n_tile) {
-    case 32: return launchN<32>(tmapA, tmapB, tmapR, p, stages, smem, stream);
-    case 64: return launchN<64>(tmapA, tmapB, tmapR, p, stages, smem, stream);
-    case 96: return launchN<96>(tmapA, tmapB, tmapR, p, stages, smem, stream);
-    case 128: return launchN<128>(tmapA, tmapB, tmapR, p, stages, smem, stream);
-    case 160: return launchN<160>(tmapA, tmapB, tmapR, p, stages, smem, stream);
-    case 192: return launchN<192>(tmapA, tmapB, tmapR, p, stages, smem, stream);
-    case 224: return launchN<224>(tmapA, tmapB, tmapR, p, stages, smem, stream);
-    case 256: return launchN<256>(tmapA, tmapB, tmapR, p, stages, smem, stream);
+    case 32: return launchN<32>(tm, p, grid, stages, smem, stream);
+    case 64: return launchN<64>(tm, p, grid, stages, smem, stream);
+    case 96: return launchN<96>(tm, p, grid, stages, smem, stream);
+    case 128: return launchN<128>(tm, p, grid, stages, smem, stream);
+    case 160: return launchN<160>(tm, p, grid, stages, smem, stream);
+    case 192: return launchN<192>(tm, p, grid, stages, smem, stream);
+    case 224: return launchN<224>(tm, p, grid, stages, smem, stream);
+    case 256: return launchN<256>(tm, p, grid, stages, smem, stream);
     default: return cudaErrorInvalidValue;
   }
 }
