@@ -426,12 +426,26 @@ KGB_API int kgb_test_board_replay(int x_size, int y_size, int num_boards, int nu
 KGB_API int kgb_bench_conv_ex(int ky, int kx, int in_c, int out_c, int n, int nn_x_len, int nn_y_len, int use_fp16, int epilogue_kind, int rotate,
                       int warmup, int iters, float* ms_per_launch);
 /* Test hook for the fused epilogues (kinds 1-4 above) of one convolution layer: NHWC input [n][y][x][in_c], optional NHWC residual
- * [n][y][x][out_c], per-channel BN scale / bias (NULL = 1 / 0), activation (0 identity, 1 relu, 2 mish); returns the raw stream after
+ * [n][y][x][out_c], per-channel BN scale / bias (NULL = 1 / 0), activation (0 identity, 1 relu, 2 mish, 3 silu); returns the raw stream after
  * the launch (kinds 2-4) and the activated fp16 operand, both NHWC [n][y][x][out_c] as floats.  Also checks that every pad row of the
  * activated operand was written as zero (reference semantics: the conv's zero padding, eigenbackend.cpp:448-701). */
 KGB_API int kgb_test_conv_epilogue(int ky, int kx, int in_c, int out_c, const float* weights, int n, int nn_x_len, int nn_y_len, int use_fp16,
                            int epilogue_kind, const float* input, const float* residual_in, const float* bn_scale, const float* bn_bias,
                            int activation, float* raw_out, float* act_out);
+/* Test hook that reaches every input of the fused epilogue (kinds 0-4 above; kgb_test_conv and kgb_test_conv_epilogue are its
+ * narrower forms).  Beyond kgb_test_conv_epilogue's arguments:
+ *   board_xy [n][2] {X_i, Y_i}, or NULL for the whole frame: the mask is 1 on image i's top-left X_i x Y_i board and 0 elsewhere, as
+ *     the self-play loop places smaller boards.  The input may be nonzero off the board; only the mask zeroes those outputs.
+ *   ncbias [n][out_c] or NULL: a per-image bias added before the residual, as the initial conv adds the global-input bias.  The
+ *     kernel applies it in every kind; tests/test_gpu_conv_fp64.py checks it in kind 3, the initial conv's, only.
+ *   residual_in is fp32; an fp16 stream holds it rounded to nearest.  activation 0 identity, 1 relu, 2 mish, 3 silu.
+ * Outputs, NHWC [n][y][x][out_c] as floats: raw_out (kind 0 and kinds 2-4), act_hi_out (kinds 1-4) and, in split mode, act_lo_out
+ * (kinds 1-4), the activated operand's two fp16 halves as the next layer reads them.  The hook fails if any output is nonzero in a
+ * row the mask zeroes, or in the padded channels out_c..cout_p of any row. */
+KGB_API int kgb_test_conv_ex(int ky, int kx, int in_c, int out_c, const float* weights, int n, int nn_x_len, int nn_y_len, int use_fp16,
+                             int epilogue_kind, const float* input, const int32_t* board_xy, const float* ncbias, const float* residual_in,
+                             const float* bn_scale, const float* bn_bias, int activation, float* raw_out, float* act_hi_out,
+                             float* act_lo_out);
 
 #ifdef __cplusplus
 }

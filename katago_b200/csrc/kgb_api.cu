@@ -967,6 +967,8 @@ struct SingleConv {
   // one entry per buffer set: the operand, the activated output (kinds 1-4) and the raw output (kind 0) or raw stream (kinds 2-4)
   std::vector<__half*> As, acts;
   std::vector<void*> raws;
+  float* ncbias = nullptr;   // [n][cout_p], the initial conv's per-image bias, when asked for
+  std::vector<float> mask;   // [M], as setInput uploaded it
   bool rawF32 = true;   // the raw output of kind 0 is fp32; the stream of kinds 2-4 is fp32 for kind 4 and in fp32-equivalent mode
   int rotate, next = 0;
   // kind: 0 = fp32 raw output only; 1 = the first conv of a residual unit (BN + mish + mask -> fp16 operand of the next conv);
@@ -975,7 +977,7 @@ struct SingleConv {
   // with KGB_STREAM_FP32=trunk.  In fp32-equivalent mode every stream is fp32.  `rotate` independent buffer sets are cycled through
   // by run() so that a timing loop does not live in L2.
   SingleConv(int ky, int kx, int in_c, int out_c, const float* weights, int n_, int X_, int Y_, int use_fp16, int kind, int rotate_ = 1,
-             const float* bnScale = nullptr, const float* bnBias = nullptr, int actKind = ACT_MISH)
+             const float* bnScale = nullptr, const float* bnBias = nullptr, int actKind = ACT_MISH, bool withNcbias = false)
       : n(n_), X(X_), Y(Y_), cin(in_c), cout(out_c), rotate(rotate_ < 1 ? 1 : rotate_) {
     h.device = selectDevice(-1);
     h.model = &dummy;
@@ -1003,6 +1005,7 @@ struct SingleConv {
     h.dMask = h.dalloc<float>(M + 128);
     h.dMaskSum = h.dalloc<float>(n);
     rawF32 = kind == 0 || kind == 4 || h.split != 0;
+    if(withNcbias) ncbias = h.dalloc<float>((size_t)n * cw.cout_p);
     for(int r = 0; r < rotate; r++) {
       __half* A = h.dalloc<__half>(M * cw.cin_p * b.actMul);
       __half* act = kind == 0 ? nullptr : h.dalloc<__half>(M * cw.cout_p * b.actMul);
@@ -1010,7 +1013,7 @@ struct SingleConv {
       As.push_back(A);
       if(act) acts.push_back(act);
       if(raw) raws.push_back(raw);
-      b.emitConv(cw, A, kind == 2 || kind == 4 ? raw : nullptr, rawF32, nullptr, raw, rawF32, act, kind == 0 ? Builder::BNDev() : dev);
+      b.emitConv(cw, A, kind == 2 || kind == 4 ? raw : nullptr, rawF32, ncbias, raw, rawF32, act, kind == 0 ? Builder::BNDev() : dev);
     }
   }
   ~SingleConv() {
@@ -1018,18 +1021,22 @@ struct SingleConv {
     if(h.wHost) cudaFreeHost(h.wHost);
     if(h.stream) cudaStreamDestroy(h.stream);
   }
-  void setInput(const float* input /* NHWC */) {
+  // boardXY [n][2] (or null = the whole frame): image i's board is its top-left X_i x Y_i, as the self-play loop places boards
+  void setInput(const float* input /* NHWC */, const int32_t* boardXY = nullptr) {
     float* dIn = h.dalloc<float>((size_t)n * X * Y * cin);
     CK(cudaMemcpy(dIn, input, (size_t)n * X * Y * cin * sizeof(float), cudaMemcpyHostToDevice));
     CK(cudaDeviceSynchronize());   // see below: the pack kernel runs on a non-blocking stream
     CK(launchPackInput(dIn, n, cin, true, nullptr, h.L, As[0], cw.cin_p, h.split, h.dMask, h.dMaskSum, h.stream));
     CK(cudaStreamSynchronize(h.stream));
     for(size_t r = 1; r < As.size(); r++) CK(cudaMemcpy(As[r], As[0], M * cw.cin_p * (h.split ? 2 : 1) * sizeof(__half), cudaMemcpyDeviceToDevice));
-    // the mask of a bare convolution is "every board point", not input channel 0
+    // the mask of a bare convolution is "every point of the image's board", not input channel 0
     std::vector<float> hm(M, 0.0f);
-    for(int i = 0; i < n; i++)
-      for(int y = 0; y < Y; y++)
-        for(int x = 0; x < X; x++) hm[(size_t)i * h.L.P + (size_t)(y + h.L.pad) * h.L.Wp + x] = 1.0f;
+    for(int i = 0; i < n; i++) {
+      const int bx = boardXY ? boardXY[2 * i] : X, by = boardXY ? boardXY[2 * i + 1] : Y;
+      for(int y = 0; y < by; y++)
+        for(int x = 0; x < bx; x++) hm[(size_t)i * h.L.P + (size_t)(y + h.L.pad) * h.L.Wp + x] = 1.0f;
+    }
+    mask = hm;
     CK(cudaMemcpy(h.dMask, hm.data(), M * sizeof(float), cudaMemcpyHostToDevice));
     // cudaMemcpy from pageable memory may return before the DMA has landed, and h.stream is non-blocking:
     // nothing else orders these uploads before the kernels launched on it.
@@ -1038,20 +1045,35 @@ struct SingleConv {
   void run() { h.ops[next](n, h.stream); next = (next + 1) % rotate; }
 };
 
-// kgb_test_conv (kind 0) and kgb_test_conv_epilogue (kinds 1-4): one launch, NHWC in and out
+// kgb_test_conv_ex and its two narrower forms kgb_test_conv (kind 0) and kgb_test_conv_epilogue (kinds 1-4): one launch, NHWC in
+// and out.  act_lo_out is written in split mode only.
 void testConv(const char* fn, int ky, int kx, int in_c, int out_c, const float* weights, int n, int nn_x_len, int nn_y_len, int use_fp16, int kind,
-              const float* input, const float* residual_in, const float* bn_scale, const float* bn_bias, int activation, float* raw_out,
-              float* act_out) {
+              const float* input, const int32_t* board_xy, const float* ncbias, const float* residual_in, const float* bn_scale,
+              const float* bn_bias, int activation, float* raw_out, float* act_hi_out, float* act_lo_out) {
   const bool hasResidual = kind == 2 || kind == 4;
-  if(!weights || !input || n < 1 || (kind == 0 ? !raw_out : !act_out)) throw std::invalid_argument(std::string(fn) + ": bad argument");
+  if(!weights || !input || n < 1 || kind < 0 || kind > 4 || activation < ACT_IDENTITY || activation > ACT_SILU ||
+     (kind == 0 ? !raw_out : !act_hi_out))
+    throw std::invalid_argument(std::string(fn) + ": bad argument");
   if(hasResidual && !residual_in) throw std::invalid_argument(std::string(fn) + ": kinds 2 and 4 need residual_in");
   if(kind >= 2 && !raw_out) throw std::invalid_argument(std::string(fn) + ": kinds 2 to 4 need raw_out");
-  SingleConv sc(ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16, kind, 1, bn_scale, bn_bias, activation);
-  sc.setInput(input);
+  if(board_xy)
+    for(int i = 0; i < n; i++)
+      if(board_xy[2 * i] < 1 || board_xy[2 * i] > nn_x_len || board_xy[2 * i + 1] < 1 || board_xy[2 * i + 1] > nn_y_len)
+        throw std::invalid_argument(std::string(fn) + ": board size of image " + std::to_string(i) + " not in the frame");
+  SingleConv sc(ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16, kind, 1, bn_scale, bn_bias, activation, ncbias != nullptr);
+  sc.setInput(input, board_xy);
   const int cp = sc.cw.cout_p;
   const bool f32 = sc.rawF32;
+  const bool split = sc.h.split != 0;
+  if(split && kind != 0 && !act_lo_out) throw std::invalid_argument(std::string(fn) + ": split mode needs act_lo_out");
   auto rowOf = [&](int i, int y, int x) { return (size_t)i * sc.h.L.P + (size_t)(y + sc.h.L.pad) * sc.h.L.Wp + x; };
+  if(ncbias) {
+    std::vector<float> hb((size_t)n * cp, 0.0f);
+    for(int i = 0; i < n; i++) for(int c = 0; c < out_c; c++) hb[(size_t)i * cp + c] = ncbias[(size_t)i * out_c + c];
+    CK(cudaMemcpy(sc.ncbias, hb.data(), hb.size() * sizeof(float), cudaMemcpyHostToDevice));
+  }
   if(hasResidual) {
+    // given as fp32; an fp16 stream holds it rounded to nearest
     std::vector<float> hf(sc.M * cp, 0.0f);
     for(int i = 0; i < n; i++) for(int y = 0; y < nn_y_len; y++) for(int x = 0; x < nn_x_len; x++) for(int c = 0; c < out_c; c++)
       hf[rowOf(i, y, x) * cp + c] = residual_in[(((size_t)i * nn_y_len + y) * nn_x_len + x) * out_c + c];
@@ -1061,11 +1083,11 @@ void testConv(const char* fn, int ky, int kx, int in_c, int out_c, const float* 
       for(size_t k = 0; k < hf.size(); k++) hh[k] = __float2half_rn(hf[k]);
       CK(cudaMemcpy(sc.raws[0], hh.data(), hh.size() * sizeof(__half), cudaMemcpyHostToDevice));
     }
-    CK(cudaDeviceSynchronize());
   }
+  CK(cudaDeviceSynchronize());   // pageable uploads, then a launch on a non-blocking stream
   sc.run();
   CK(cudaStreamSynchronize(sc.h.stream));
-  const int am = sc.h.split ? 2 : 1;
+  const int am = split ? 2 : 1;
   std::vector<__half> ha;
   if(!sc.acts.empty()) {
     ha.resize(sc.M * cp * am);
@@ -1081,18 +1103,29 @@ void testConv(const char* fn, int ky, int kx, int in_c, int out_c, const float* 
       for(size_t k = 0; k < hr.size(); k++) hr[k] = __half2float(hh[k]);
     }
   }
+  // Exact zeros where the next layer relies on them: every column of a row the mask zeroes (pad rows and columns, and points off
+  // a smaller board), which the next conv's halo reads as its zero padding; and the padded channels cout..cout_p of every row, which
+  // the next conv reads as part of K (0 x NaN is not 0).  The raw output is checked too, and in split mode the lo half.
+  auto check = [&](const char* what, int ld, int col0, auto value) {
+    for(size_t r = 0; r < sc.M; r++) {
+      const bool off = sc.mask[r] == 0.0f;
+      for(int c = off ? 0 : out_c; c < cp; c++)
+        if(value(r * ld + col0 + c) != 0.0f)
+          throw std::runtime_error(std::string(fn) + ": " + what + " is not zero at row " + std::to_string(r) + (off ? " (masked)" : "") +
+                                   ", channel " + std::to_string(c));
+    }
+  };
+  if(!hr.empty()) check("the raw output", cp, 0, [&](size_t k) { return hr[k]; });
   if(!ha.empty()) {
-    // every row that is not a board point (pad rows / columns) must have been written as zero: the next conv's halo reads them
-    std::vector<char> onBoard(sc.M, 0);
-    for(int i = 0; i < n; i++) for(int y = 0; y < nn_y_len; y++) for(int x = 0; x < nn_x_len; x++) onBoard[rowOf(i, y, x)] = 1;
-    for(size_t r = 0; r < sc.M; r++)
-      if(!onBoard[r])
-        for(int c = 0; c < cp * am; c++)
-          if(__half2float(ha[r * cp * am + c]) != 0.0f) throw std::runtime_error(std::string(fn) + ": pad row " + std::to_string(r) + " of the activation output is not zero");
+    check("the activated operand", cp * am, 0, [&](size_t k) { return __half2float(ha[k]); });
+    if(split) check("the activated operand's lo half", cp * am, cp, [&](size_t k) { return __half2float(ha[k]); });
   }
   for(int i = 0; i < n; i++) for(int y = 0; y < nn_y_len; y++) for(int x = 0; x < nn_x_len; x++) for(int c = 0; c < out_c; c++) {
     const size_t row = rowOf(i, y, x), o = (((size_t)i * nn_y_len + y) * nn_x_len + x) * out_c + c;
-    if(!ha.empty()) act_out[o] = __half2float(ha[row * cp * am + c]) + (am == 2 ? __half2float(ha[row * cp * am + cp + c]) : 0.0f);
+    if(!ha.empty()) {
+      act_hi_out[o] = __half2float(ha[row * cp * am + c]);
+      if(split) act_lo_out[o] = __half2float(ha[row * cp * am + cp + c]);
+    }
     if(!hr.empty()) raw_out[o] = hr[row * cp + c];
   }
 }
@@ -1103,8 +1136,8 @@ extern "C" {
 KGB_API int kgb_test_conv(int ky, int kx, int in_c, int out_c, const float* weights, int n, int nn_x_len, int nn_y_len, int use_fp16,
                   const float* input, float* output) {
   return guarded([&] {
-    testConv("kgb_test_conv", ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16, 0, input, nullptr, nullptr, nullptr, ACT_IDENTITY, output,
-             nullptr);
+    testConv("kgb_test_conv", ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16, 0, input, nullptr, nullptr, nullptr, nullptr, nullptr,
+             ACT_IDENTITY, output, nullptr, nullptr);
   });
 }
 
@@ -1113,8 +1146,21 @@ KGB_API int kgb_test_conv_epilogue(int ky, int kx, int in_c, int out_c, const fl
                            int activation, float* raw_out, float* act_out) {
   return guarded([&] {
     if(epilogue_kind < 1 || epilogue_kind > 4) throw std::invalid_argument("kgb_test_conv_epilogue: bad argument");
-    testConv("kgb_test_conv_epilogue", ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16, epilogue_kind, input, residual_in, bn_scale,
-             bn_bias, activation, raw_out, act_out);
+    // the activated operand as the next layer sees it: hi + lo in split mode
+    std::vector<float> lo(use_fp16 || !act_out ? 0 : (size_t)n * nn_x_len * nn_y_len * out_c);
+    testConv("kgb_test_conv_epilogue", ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16, epilogue_kind, input, nullptr, nullptr,
+             residual_in, bn_scale, bn_bias, activation, raw_out, act_out, lo.empty() ? nullptr : lo.data());
+    for(size_t k = 0; k < lo.size(); k++) act_out[k] += lo[k];
+  });
+}
+
+KGB_API int kgb_test_conv_ex(int ky, int kx, int in_c, int out_c, const float* weights, int n, int nn_x_len, int nn_y_len, int use_fp16,
+                             int epilogue_kind, const float* input, const int32_t* board_xy, const float* ncbias, const float* residual_in,
+                             const float* bn_scale, const float* bn_bias, int activation, float* raw_out, float* act_hi_out,
+                             float* act_lo_out) {
+  return guarded([&] {
+    testConv("kgb_test_conv_ex", ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16, epilogue_kind, input, board_xy, ncbias,
+             residual_in, bn_scale, bn_bias, activation, raw_out, act_hi_out, act_lo_out);
   });
 }
 

@@ -78,6 +78,7 @@ ABI_SYMBOLS = [
     "kgb_model_load_file", "kgb_model_free", "kgb_model_get_info", "kgb_context_create", "kgb_context_free",
     "kgb_handle_create", "kgb_handle_free", "kgb_handle_is_fp16", "kgb_forward", "kgb_forward_device", "kgb_handle_sync",
     "kgb_handle_stream", "kgb_handle_launches_per_forward", "kgb_test_conv", "kgb_bench_conv_ex", "kgb_test_conv_epilogue",
+    "kgb_test_conv_ex",
     "kgb_selfplay_create", "kgb_selfplay_free", "kgb_selfplay_run", "kgb_selfplay_get_stats", "kgb_selfplay_get_game",
     "kgb_selfplay_get_root_children", "kgb_selfplay_launches_per_step", "kgb_selfplay_play_moves", "kgb_selfplay_time_tree_kernels", "kgb_zobrist_tables", "kgb_selfplay_get_nn_row", "kgb_selfplay_get_root_row", "kgb_test_board_replay", "kgb_selfplay_get_leaf_path", "kgb_expected_white_score_value", "kgb_value_weight_cdf_table", "kgb_rand_uint32_stream", "kgb_test_root_policy_noise", "kgb_test_history_replay", "kgb_test_repetition_bound", "kgb_selfplay_get_play_selection_values", "kgb_selfplay_random_openings", "kgb_selfplay_set_search_rand", "kgb_selfplay_get_root_value_stats", "kgb_test_choose_index_with_temperature",
     "kgb_handle_weights_bytes", "kgb_handle_stage_weights", "kgb_handle_commit_weights", "kgb_handle_wait_staged", "kgb_nccl_unique_id", "kgb_handle_comm_init",
@@ -149,6 +150,7 @@ def load_library():
     lib.kgb_test_conv.argtypes = [I, I, I, I, P, I, I, I, I, P, P]
     lib.kgb_bench_conv_ex.argtypes = [I, I, I, I, I, I, I, I, I, I, I, I, F]
     lib.kgb_test_conv_epilogue.argtypes = [I, I, I, I, P, I, I, I, I, I, P, P, P, P, I, P, P]
+    lib.kgb_test_conv_ex.argtypes = [I, I, I, I, P, I, I, I, I, I, P, P, P, P, P, P, I, P, P, P]
     lib.kgb_selfplay_create.argtypes = [P, C.POINTER(SelfplayConfig), C.POINTER(P)]
     lib.kgb_selfplay_free.argtypes = [P]
     lib.kgb_selfplay_free.restype = None
@@ -417,6 +419,27 @@ def test_conv_epilogue(ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_
                                       res.ctypes.data if res is not None else None, sc.ctypes.data if sc is not None else None,
                                       bi.ctypes.data if bi is not None else None, activation, raw.ctypes.data, act.ctypes.data))
     return (raw if kind >= 2 else None), act
+
+
+def test_conv_ex(ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16, kind, x, board_xy=None, ncbias=None, residual=None,
+                 bn_scale=None, bn_bias=None, activation=2):
+    """One convolution launch with every epilogue input (include/kgb200.h kgb_test_conv_ex): kinds 0-4 as in test_conv_epilogue,
+    board_xy [n][2] = (X_i, Y_i) boards in the top-left of the frame (None = the whole frame), ncbias [n][out_c], residual in fp32,
+    activation 0-3.  Returns (raw or None, act hi or None, act lo or None), NHWC; lo only in split mode."""
+    if kind not in (0, 1, 2, 3, 4):
+        raise ValueError(f"test_conv_ex: epilogue kind {kind} is not 0-4")
+    lib = load_library()
+    shape = (n, nn_y_len, nn_x_len, out_c)
+    w, xx = _f32(weights), _f32(x)
+    raw = np.zeros(shape, np.float32) if kind != 1 else None
+    hi = np.zeros(shape, np.float32) if kind != 0 else None
+    lo = np.zeros(shape, np.float32) if kind != 0 and not use_fp16 else None
+    bxy = np.ascontiguousarray(board_xy, dtype=np.int32) if board_xy is not None else None
+    opt = [_f32(a) if a is not None else None for a in (ncbias, residual, bn_scale, bn_bias)]
+    ptr = lambda a: a.ctypes.data if a is not None else None
+    _check(lib.kgb_test_conv_ex(ky, kx, in_c, out_c, w.ctypes.data, n, nn_x_len, nn_y_len, int(bool(use_fp16)), kind, xx.ctypes.data,
+                                ptr(bxy), *[ptr(a) for a in opt], activation, ptr(raw), ptr(hi), ptr(lo)))
+    return raw, hi, lo
 
 
 def zobrist_tables(x_size: int, y_size: int):

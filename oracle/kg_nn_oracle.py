@@ -471,14 +471,20 @@ def load_model(path: str, apply_transform: bool = True) -> Model:
 
 
 # --------------------------------------------------------------------------------------------------------------
-# Forward pass (fp32, NHWC)
+# Forward pass (NHWC; fp32 by default, or float64)
 # --------------------------------------------------------------------------------------------------------------
 
 def _f32(x):
     return np.asarray(x, dtype=np.float32)
 
 
-def act_fn(x: np.ndarray, act: int) -> np.ndarray:
+# The forward pass runs in fp32 by default, as the reference does; dt=np.float64 gives a high-precision reference of the same
+# function (same weights, same constants) to measure fp32 implementations against.
+def _as(dt, x):
+    return np.asarray(x, dtype=dt)
+
+
+def act_fn(x: np.ndarray, act: int, dt=np.float32) -> np.ndarray:
     """eigenbackend.cpp:780-809."""
     if act == ACT_IDENTITY:
         return x
@@ -486,28 +492,28 @@ def act_fn(x: np.ndarray, act: int) -> np.ndarray:
         return np.maximum(x, np.float32(0))
     if act == ACT_MISH:
         sp = np.log1p(np.exp(np.minimum(x, np.float32(20)))) + (np.maximum(x, np.float32(20)) - np.float32(20))
-        return _f32(x * np.tanh(sp))
+        return _as(dt, x * np.tanh(sp))
     if act == ACT_SILU:
-        return _f32(x / (np.exp(-x) + np.float32(1)))
+        return _as(dt, x / (np.exp(-x) + np.float32(1)))
     raise ValueError(act)
 
 
-def bn_act_mask(x: np.ndarray, bn: BN, act: int, mask: np.ndarray) -> np.ndarray:
+def bn_act_mask(x: np.ndarray, bn: BN, act: int, mask: np.ndarray, dt=np.float32) -> np.ndarray:
     """eigenbackend.cpp:739-762: mask==1 ? act(x*s+b) : 0.   x [N,H,W,C], mask [N,H,W]."""
-    y = act_fn(_f32(x * bn.scale + bn.bias), act)
-    return _f32(np.where(mask[..., None] == 1.0, y, np.float32(0)))
+    y = act_fn(_as(dt, x * bn.scale + bn.bias), act, dt)
+    return _as(dt, np.where(mask[..., None] == 1.0, y, np.float32(0)))
 
 
-def conv2d(x: np.ndarray, c: Conv) -> np.ndarray:
+def conv2d(x: np.ndarray, c: Conv, dt=np.float32) -> np.ndarray:
     """Zero-padded 'same' cross-correlation, NHWC (eigenbackend.cpp:448-701 computes the same function)."""
     n, h, w, cin = x.shape
     assert cin == c.cin, (c.name, cin, c.cin)
     py, px = c.ky // 2, c.kx // 2
     if c.ky == 1 and c.kx == 1:
-        return _f32(x.reshape(-1, cin) @ c.w.reshape(cin, c.cout)).reshape(n, h, w, c.cout)
-    xp = np.zeros((n, h + 2 * py, w + 2 * px, cin), np.float32)
+        return _as(dt, x.reshape(-1, cin) @ c.w.reshape(cin, c.cout)).reshape(n, h, w, c.cout)
+    xp = np.zeros((n, h + 2 * py, w + 2 * px, cin), dt)
     xp[:, py:py + h, px:px + w, :] = x
-    out = np.zeros((n * h * w, c.cout), np.float32)
+    out = np.zeros((n * h * w, c.cout), dt)
     for dy in range(c.ky):
         for dx in range(c.kx):
             patch = xp[:, dy:dy + h, dx:dx + w, :].reshape(-1, cin)
@@ -515,84 +521,86 @@ def conv2d(x: np.ndarray, c: Conv) -> np.ndarray:
     return out.reshape(n, h, w, c.cout)
 
 
-def gpool(x: np.ndarray, mask: np.ndarray, mask_sum: np.ndarray) -> np.ndarray:
+def gpool(x: np.ndarray, mask: np.ndarray, mask_sum: np.ndarray, dt=np.float32) -> np.ndarray:
     """eigenbackend.cpp:152-177 -> [N, 3C]."""
     n, h, w, c = x.shape
-    s = x.reshape(n, -1, c).sum(axis=1, dtype=np.float32)
+    s = x.reshape(n, -1, c).sum(axis=1, dtype=dt)
     mx = np.maximum((x + (mask[..., None] - np.float32(1))).reshape(n, -1, c).max(axis=1), np.float32(-1.0))
     div = mask_sum.reshape(n, 1)
     sq = np.sqrt(div)
-    mean = _f32(s / div)
-    return _f32(np.concatenate([mean, mean * (sq - np.float32(14)) * np.float32(0.1), mx], axis=1))
+    mean = _as(dt, s / div)
+    return _as(dt, np.concatenate([mean, mean * (sq - np.float32(14)) * np.float32(0.1), mx], axis=1))
 
 
-def vpool(x: np.ndarray, mask_sum: np.ndarray) -> np.ndarray:
+def vpool(x: np.ndarray, mask_sum: np.ndarray, dt=np.float32) -> np.ndarray:
     """eigenbackend.cpp:179-197 -> [N, 3C]."""
     n, h, w, c = x.shape
-    s = x.reshape(n, -1, c).sum(axis=1, dtype=np.float32)
+    s = x.reshape(n, -1, c).sum(axis=1, dtype=dt)
     div = mask_sum.reshape(n, 1)
     sq = np.sqrt(div)
-    mean = _f32(s / div)
+    mean = _as(dt, s / div)
     a = (sq - np.float32(14))
-    return _f32(np.concatenate([mean, mean * a * np.float32(0.1),
+    return _as(dt, np.concatenate([mean, mean * a * np.float32(0.1),
                                 mean * (a * a * np.float32(0.01) - np.float32(0.1))], axis=1))
 
 
-def _apply_blocks(blocks: list, x: np.ndarray, mask, mask_sum) -> np.ndarray:
+def _apply_blocks(blocks: list, x: np.ndarray, mask, mask_sum, dt=np.float32) -> np.ndarray:
     for b in blocks:
         if isinstance(b, ResBlock):       # eigenbackend.cpp:1127-1145
-            mid = conv2d(bn_act_mask(x, b.pre_bn, b.pre_act, mask), b.conv1)
-            x = _f32(x + conv2d(bn_act_mask(mid, b.mid_bn, b.mid_act, mask), b.conv2))
+            mid = conv2d(bn_act_mask(x, b.pre_bn, b.pre_act, mask, dt), b.conv1, dt)
+            x = _as(dt, x + conv2d(bn_act_mask(mid, b.mid_bn, b.mid_act, mask, dt), b.conv2, dt))
         elif isinstance(b, GPoolBlock):   # eigenbackend.cpp:1183-1229
-            a = bn_act_mask(x, b.pre_bn, b.pre_act, mask)
-            reg = conv2d(a, b.regular_conv)
-            g = bn_act_mask(conv2d(a, b.gpool_conv), b.gpool_bn, b.gpool_act, mask)
-            bias = _f32(gpool(g, mask, mask_sum) @ b.gpool_to_bias.w)
-            reg = _f32(reg + bias[:, None, None, :])
-            x = _f32(x + conv2d(bn_act_mask(reg, b.mid_bn, b.mid_act, mask), b.conv2))
+            a = bn_act_mask(x, b.pre_bn, b.pre_act, mask, dt)
+            reg = conv2d(a, b.regular_conv, dt)
+            g = bn_act_mask(conv2d(a, b.gpool_conv, dt), b.gpool_bn, b.gpool_act, mask, dt)
+            bias = _as(dt, gpool(g, mask, mask_sum, dt) @ b.gpool_to_bias.w)
+            reg = _as(dt, reg + bias[:, None, None, :])
+            x = _as(dt, x + conv2d(bn_act_mask(reg, b.mid_bn, b.mid_act, mask, dt), b.conv2, dt))
         elif isinstance(b, NestedBlock):  # eigenbackend.cpp:1295-1314
-            mid = conv2d(bn_act_mask(x, b.pre_bn, b.pre_act, mask), b.pre_conv)
-            mid = _apply_blocks(b.blocks, mid, mask, mask_sum)
-            x = _f32(x + conv2d(bn_act_mask(mid, b.post_bn, b.post_act, mask), b.post_conv))
+            mid = conv2d(bn_act_mask(x, b.pre_bn, b.pre_act, mask, dt), b.pre_conv, dt)
+            mid = _apply_blocks(b.blocks, mid, mask, mask_sum, dt)
+            x = _as(dt, x + conv2d(bn_act_mask(mid, b.post_bn, b.post_act, mask, dt), b.post_conv, dt))
         else:
             raise TypeError(b)
     return x
 
 
-def forward_raw(m: Model, spatial: np.ndarray, glob: np.ndarray, return_trunk: bool = False) -> dict:
-    """Model::apply (eigenbackend.cpp:2162-2216).  spatial [N,H,W,Cin] fp32 NHWC, glob [N,G].
+def forward_raw(m: Model, spatial: np.ndarray, glob: np.ndarray, return_trunk: bool = False, dtype=np.float32) -> dict:
+    """Model::apply (eigenbackend.cpp:2162-2216).  spatial [N,H,W,Cin] NHWC, glob [N,G]; computed in `dtype` (fp32 by default,
+    np.float64 for a high-precision reference).
 
     Returns raw head outputs: policy [N,H,W,Cp], policy_pass [N,Cp], value [N,3], score_value [N,S],
     ownership [N,H,W]."""
-    x_in = _f32(spatial)
-    g_in = _f32(glob)
+    dt = dtype
+    x_in = _as(dt, spatial)
+    g_in = _as(dt, glob)
     mask = x_in[..., 0].copy()                                   # :2181
-    mask_sum = mask.reshape(mask.shape[0], -1).sum(axis=1, dtype=np.float32)
+    mask_sum = mask.reshape(mask.shape[0], -1).sum(axis=1, dtype=dt)
     # Trunk::apply :1909-1947
-    x = conv2d(x_in, m.initial_conv)
-    x = _f32(x + _f32(g_in @ m.initial_matmul.w)[:, None, None, :])
-    x = _apply_blocks(m.blocks, x, mask, mask_sum)
-    trunk = bn_act_mask(x, m.tip_bn, m.tip_act, mask)
+    x = conv2d(x_in, m.initial_conv, dt)
+    x = _as(dt, x + _as(dt, g_in @ m.initial_matmul.w)[:, None, None, :])
+    x = _apply_blocks(m.blocks, x, mask, mask_sum, dt)
+    trunk = bn_act_mask(x, m.tip_bn, m.tip_act, mask, dt)
     # PolicyHead::apply :1992-2036
-    p1 = conv2d(trunk, m.p1_conv)
-    g1 = bn_act_mask(conv2d(trunk, m.g1_conv), m.g1_bn, m.g1_act, mask)
-    g1c = gpool(g1, mask, mask_sum)
-    p1 = _f32(p1 + _f32(g1c @ m.gpool_to_bias.w)[:, None, None, :])
-    p1 = bn_act_mask(p1, m.p1_bn, m.p1_act, mask)
-    policy = conv2d(p1, m.p2_conv)
+    p1 = conv2d(trunk, m.p1_conv, dt)
+    g1 = bn_act_mask(conv2d(trunk, m.g1_conv, dt), m.g1_bn, m.g1_act, mask, dt)
+    g1c = gpool(g1, mask, mask_sum, dt)
+    p1 = _as(dt, p1 + _as(dt, g1c @ m.gpool_to_bias.w)[:, None, None, :])
+    p1 = bn_act_mask(p1, m.p1_bn, m.p1_act, mask, dt)
+    policy = conv2d(p1, m.p2_conv, dt)
     if m.version >= 15:
-        pp = _f32(g1c @ m.gpool_to_pass.w) + m.gpool_to_pass_bias.w
-        pp = act_fn(_f32(pp), m.pass_act)
-        policy_pass = _f32(pp @ m.gpool_to_pass2.w)
+        pp = _as(dt, g1c @ m.gpool_to_pass.w) + m.gpool_to_pass_bias.w
+        pp = act_fn(_as(dt, pp), m.pass_act, dt)
+        policy_pass = _as(dt, pp @ m.gpool_to_pass2.w)
     else:
-        policy_pass = _f32(g1c @ m.gpool_to_pass.w)
+        policy_pass = _as(dt, g1c @ m.gpool_to_pass.w)
     # ValueHead::apply :2079-2114
-    v1 = bn_act_mask(conv2d(trunk, m.v1_conv), m.v1_bn, m.v1_act, mask)
-    v1m = vpool(v1, mask_sum)
-    v2 = act_fn(_f32(_f32(v1m @ m.v2_mul.w) + m.v2_bias.w), m.v2_act)
-    value = _f32(_f32(v2 @ m.v3_mul.w) + m.v3_bias.w)
-    score_value = _f32(_f32(v2 @ m.sv3_mul.w) + m.sv3_bias.w)
-    ownership = conv2d(v1, m.ownership_conv)[..., 0]
+    v1 = bn_act_mask(conv2d(trunk, m.v1_conv, dt), m.v1_bn, m.v1_act, mask, dt)
+    v1m = vpool(v1, mask_sum, dt)
+    v2 = act_fn(_as(dt, _as(dt, v1m @ m.v2_mul.w) + m.v2_bias.w), m.v2_act, dt)
+    value = _as(dt, _as(dt, v2 @ m.v3_mul.w) + m.v3_bias.w)
+    score_value = _as(dt, _as(dt, v2 @ m.sv3_mul.w) + m.sv3_bias.w)
+    ownership = conv2d(v1, m.ownership_conv, dt)[..., 0]
     out = dict(policy=policy, policy_pass=policy_pass, value=value, score_value=score_value, ownership=ownership)
     if return_trunk:
         out["trunk"] = trunk
@@ -635,28 +643,29 @@ def apply_symmetry_nhwc(x: np.ndarray, symmetry: int, reverse: bool = False) -> 
     return out.reshape(x.shape)
 
 
-def get_output(m: Model, spatial: np.ndarray, glob: np.ndarray, symmetries=None, policy_optimism=None) -> dict:
+def get_output(m: Model, spatial: np.ndarray, glob: np.ndarray, symmetries=None, policy_optimism=None, dtype=np.float32) -> dict:
     """NeuralNet::getOutput (eigenbackend.cpp:2445-2628): rows given un-symmetrised (as fillRowV7 wrote them, NHWC);
     returns logits with the symmetry already inverted.
 
     policy [N, H*W+1] (pass last), value [N,3], score_value [N,6-padded: mean, meansq, lead, vartime, stwl, stscore],
     ownership [N,H*W]."""
+    dt = dtype
     n, h, w, _ = spatial.shape
     symmetries = [0] * n if symmetries is None else list(symmetries)
     policy_optimism = [0.0] * n if policy_optimism is None else list(policy_optimism)
-    sp = np.stack([apply_symmetry_nhwc(_f32(spatial[i]), symmetries[i], False) for i in range(n)])
-    raw = forward_raw(m, sp, glob)
+    sp = np.stack([apply_symmetry_nhwc(_as(dt, spatial[i]), symmetries[i], False) for i in range(n)])
+    raw = forward_raw(m, sp, glob, dtype=dt)
     cp = m.policy_out_channels
-    policy = np.zeros((n, h * w + 1), np.float32)
-    own = np.zeros((n, h * w), np.float32)
+    policy = np.zeros((n, h * w + 1), dt)
+    own = np.zeros((n, h * w), dt)
     for i in range(n):
-        po = np.float32(policy_optimism[i])
+        po = dt(policy_optimism[i])
         if cp == 2 or (cp == 4 and m.version >= 16):
             p = raw["policy"][i, :, :, 0]
             popt = raw["policy"][i, :, :, 1]
-            pt = _f32(p + (popt - p) * po)
+            pt = _as(dt, p + (popt - p) * po)
             pp = raw["policy_pass"][i]
-            ppass = np.float32(pp[0] + (pp[1] - pp[0]) * po)
+            ppass = dt(pp[0] + (pp[1] - pp[0]) * po)
         else:
             pt = raw["policy"][i, :, :, 0]
             ppass = raw["policy_pass"][i, 0]
@@ -664,7 +673,7 @@ def get_output(m: Model, spatial: np.ndarray, glob: np.ndarray, symmetries=None,
         policy[i, h * w] = ppass
         own[i] = apply_symmetry_nhwc(raw["ownership"][i], symmetries[i], True).reshape(-1)
     sv = raw["score_value"]
-    sv6 = np.zeros((n, 6), np.float32)
+    sv6 = np.zeros((n, 6), dt)
     if m.version >= 9:
         sv6[:] = sv[:, :6]
     elif m.version >= 8:

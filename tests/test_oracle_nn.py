@@ -78,6 +78,25 @@ def test_symmetric_evaluation_is_equivariant(tmp_models):
         assert np.abs(a["value"] - b["value"]).max() < 1e-6
 
 
+@pytest.mark.parametrize("key", ["tiny_reg", "tiny_nbt", "tiny_relu_v8"])
+def test_forward_dtype_defaults_to_fp32_and_float64_stays_float64(tmp_models, key):
+    """get_output's dtype: the default is the fp32 forward pass, bit for bit, with every intermediate in fp32; float64 keeps every
+    output in float64 and agrees with fp32 to fp32 accuracy."""
+    m = orc.load_model(tmp_models[key])
+    sp, gl = modelgen.synthetic_inputs(3, 9, 9, seed=8, board_sizes=[(9, 9), (7, 5), (9, 9)])
+    sym, opt = [0, 3, 6], [0.0, 0.5, 1.0]
+    a = orc.get_output(m, sp, gl, sym, opt)
+    b = orc.get_output(m, sp, gl, sym, opt, dtype=np.float32)
+    c = orc.get_output(m, sp, gl, sym, opt, dtype=np.float64)
+    raw = orc.forward_raw(m, sp, gl, return_trunk=True)
+    assert all(v.dtype == np.float32 for v in raw.values())
+    assert all(v.dtype == np.float64 for v in orc.forward_raw(m, sp, gl, return_trunk=True, dtype=np.float64).values())
+    for k in a:
+        assert a[k].dtype == np.float32 and np.array_equal(a[k], b[k]), k
+        assert c[k].dtype == np.float64, k
+        assert np.abs(c[k] - a[k]).max() <= 1e-4 * max(1.0, np.abs(c[k]).max()), k
+
+
 def test_masked_rows_do_not_depend_on_offboard_garbage(tmp_models):
     m = orc.load_model(tmp_models["tiny_nbt"])
     sp, gl = modelgen.synthetic_inputs(2, 19, 19, seed=8, board_sizes=[(9, 9), (13, 7)])
