@@ -62,9 +62,9 @@ Z_ROUND = 2.0 ** -22   # the fma's rounding of z is at most 2^-24 |z|: 4x, so th
 REHEARSAL_MAX_N = 24
 
 
-def _case(cid, ky, cin, cout, n, X, Y, kind, fp16, act, boards=None, ncbias=False, bias=1.0):
+def _case(cid, ky, cin, cout, n, X, Y, kind, fp16, act, boards=None, ncbias=False, bias=1.0, check_images=None):
     return pytest.param(dict(ky=ky, cin=cin, cout=cout, n=n, X=X, Y=Y, kind=kind, fp16=fp16, act=act, boards=boards, ncbias=ncbias,
-                             bias=bias), id=cid)
+                             bias=bias, check_images=check_images), id=cid)
 
 
 MIXED = ((19, 19), (9, 9), (13, 13), (7, 11))   # repeated over the batch
@@ -101,10 +101,35 @@ CASES = [
     _case("exit1x1-k2-split-b256-two-n-tiles", 1, 192, 384, 256, 19, 19, 2, False, 2, bias=12.0),
     _case("n160-five-slices-k2-split", 1, 128, 320, 100, 19, 19, 2, False, 3, bias=12.0),
     _case("n224-seven-slices-k4-split", 1, 128, 448, 100, 19, 19, 4, False, 1),
+    # b28c512nbt (trunk 512, mid 256, gpool 64) as the evaluator emits its layers, in both modes (fp16 mode keeps every stream in fp16):
+    # the entry 1x1 (8 k-blocks), the mid 3x3, the exit 1x1 and the 3x3 initial conv (two 256-wide n-tiles), and the gpool unit's first
+    # conv with its 3x3 256 -> 64 gpool conv packed in as channels 256-319
+    _case("b28-entry1x1-512-k3-split-mish", 1, 512, 256, 24, 19, 19, 3, False, 2, bias=12.0),
+    _case("b28-entry1x1-512-k3-fp16-mish-mixed", 1, 512, 256, 24, 19, 19, 3, True, 2, boards=MIXED, bias=12.0),
+    _case("b28-3x3-256-k1-fp16-mish-b64-mixed", 3, 256, 256, 64, 19, 19, 1, True, 2, boards=MIXED, bias=12.0),
+    _case("b28-3x3-256-k2-fp16-mish-b64-mixed", 3, 256, 256, 64, 19, 19, 2, True, 2, boards=MIXED, bias=12.0),
+    _case("b28-exit1x1-512-k2-split-mish", 1, 256, 512, 24, 19, 19, 2, False, 2, bias=12.0),
+    _case("b28-exit1x1-512-k2-fp16-mish-mixed", 1, 256, 512, 24, 19, 19, 2, True, 2, boards=MIXED, bias=12.0),
+    _case("b28-initial3x3-512-k3-split-mish-mixed", 3, 22, 512, 16, 19, 19, 3, False, 2, boards=MIXED, ncbias=True, bias=12.0),
+    _case("b28-initial3x3-512-k3-fp16-mish-mixed", 3, 22, 512, 16, 19, 19, 3, True, 2, boards=MIXED, ncbias=True, bias=12.0),
+    _case("b28-gpool3x3-256-320-k0-split-mixed", 3, 256, 320, 24, 19, 19, 0, False, 0, boards=MIXED),
+    _case("b28-gpool3x3-256-320-k0-fp16-mixed", 3, 256, 320, 24, 19, 19, 0, True, 0, boards=MIXED),
+    # b28's batch: 1024 images of 400 rows are 3200 whole 128-row tiles, about 24 per CTA; at 1021 image 1020 holds the partial last tile.
+    # Checked on the first images, both sides of 511 / 512 and the last ones (the padding rows between images are zero, so they are
+    # independent)
+    _case("b28-3x3-256-k2-split-mish-b1024", 3, 256, 256, 1024, 19, 19, 2, False, 2, bias=12.0,
+          check_images=(0, 1, 510, 511, 512, 513, 1022, 1023)),
+    _case("b28-3x3-256-k2-split-silu-b1021", 3, 256, 256, 1021, 19, 19, 2, False, 3, bias=12.0,
+          check_images=(0, 1, 510, 511, 512, 513, 1019, 1020)),
 ]
 
 
 # ---- data -------------------------------------------------------------------------------------------------------------------------
+
+def select_images(d, idx):
+    """The per-image inputs of the images idx (weights and BN are shared by all images)."""
+    return {k: v[idx] if k in ("x", "res", "ncb", "board_xy", "mask") and v is not None else v for k, v in d.items()}
+
 
 def make_data(c, n=None):
     """Seeded inputs of one case; nothing is fp16-exact, and the input is nonzero off the board."""
@@ -417,6 +442,10 @@ def test_conv_against_fp64(c):
                                           d["x"], board_xy=d["board_xy"], ncbias=d["ncb"], residual=d["res"], bn_scale=d["sc"],
                                           bn_bias=d["bi"], activation=c["act"])
     assert (hi is None) == (c["kind"] == 0) and (lo is None) == (c["fp16"] or c["kind"] == 0)
+    if c["check_images"] is not None:
+        idx = np.array(c["check_images"])
+        d = select_images(d, idx)
+        raw, hi, lo = (a[idx] if a is not None else None for a in (raw, hi, lo))
     r = check(c, d, reference(c, d), raw, hi, lo)
     print("worst error / bound:", {k: f"{v:.3g}" for k, v in r.items()})
     assert max(r.values()) <= 1.0, r
