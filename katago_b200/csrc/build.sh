@@ -15,7 +15,7 @@ fi
 mkdir -p ../_build
 for f in kgb_conv_wg.cu kgb_kernels.cu kgb_api.cu kgb_selfplay.cu; do
   o=../_build/${f%.cu}.o
-  if [ ! -f $o ] || [ $f -nt $o ] || [ kgb_conv.cuh -nt $o ] || [ kgb_wgmma.cuh -nt $o ] || [ kgb_kernels.cuh -nt $o ] || [ kgb_model.h -nt $o ] || [ kgb_board.cuh -nt $o ] || [ kgb_ladder.cuh -nt $o ] || [ kgb_history.cuh -nt $o ] || [ kgb_devrand.cuh -nt $o ] || [ kgb_scorevalue.h -nt $o ] || [ kgb_selfplay.h -nt $o ] || [ kgb_rand.h -nt $o ] || [ ../../include/kgb200.h -nt $o ]; then
+  if [ ! -f $o ] || [ $f -nt $o ] || [ kgb_conv.cuh -nt $o ] || [ kgb_wgmma.cuh -nt $o ] || [ kgb_kernels.cuh -nt $o ] || [ kgb_model.h -nt $o ] || [ kgb_board.cuh -nt $o ] || [ kgb_ladder.cuh -nt $o ] || [ kgb_history.cuh -nt $o ] || [ kgb_devrand.cuh -nt $o ] || [ kgb_scorevalue.h -nt $o ] || [ kgb_handle.h -nt $o ] || [ kgb_rand.h -nt $o ] || [ ../../include/kgb200.h -nt $o ]; then
     X=""
     # the search arithmetic follows the reference's doubles operation by operation: no FMA contraction there
     if [ $f = kgb_selfplay.cu ]; then X="-fmad=false"; fi

@@ -25,41 +25,13 @@
 
 #include "../../include/kgb200.h"
 #include "kgb_conv.cuh"
+#include "kgb_handle.h"
 #include "kgb_kernels.cuh"
 #include "kgb_model.h"
-#include "kgb_selfplay.h"
 #include "kgb_scorevalue.h"
 #include "kgb_rand.h"
 
 using namespace kgb;
-
-// ------------------------------------------------------------------------------------------------------------
-// Error plumbing
-// ------------------------------------------------------------------------------------------------------------
-static thread_local std::string g_lastError;
-
-struct CudaFailure : std::runtime_error {
-  using std::runtime_error::runtime_error;
-};
-
-#define CK(expr)                                                                                                       \
-  do {                                                                                                                 \
-    cudaError_t _e = (expr);                                                                                           \
-    if(_e != cudaSuccess)                                                                                              \
-      throw CudaFailure(std::string("CUDA error ") + cudaGetErrorName(_e) + " (" + cudaGetErrorString(_e) + ") at " + \
-                        __FILE__ + ":" + std::to_string(__LINE__) + ": " #expr);                                       \
-  } while(0)
-
-template <class F>
-static int guarded(F&& f) {
-  try {
-    f();
-    return KGB_OK;
-  }
-  catch(const CudaFailure& e) { g_lastError = e.what(); return KGB_ERR_CUDA; }
-  catch(const std::invalid_argument& e) { g_lastError = e.what(); return KGB_ERR_INVALID; }
-  catch(const std::exception& e) { g_lastError = e.what(); return KGB_ERR_IO; }
-}
 
 // ------------------------------------------------------------------------------------------------------------
 // Driver entry point for cuTensorMapEncodeTiled (no link-time dependency on libcuda)
@@ -135,96 +107,6 @@ struct ConvWeights {
   __half* w = nullptr;     // packed [taps][cout_p][cin_p * (split ? 2 : 1)]
   int ky = 0, kx = 0, cin_p = 0, cout_p = 0, n_tile = 0, num_n_tiles = 0;
   CUtensorMap tmapB;       // box {64, n_tile}
-};
-
-struct kgb_handle {
-  int device = 0;
-  cudaStream_t stream = nullptr;
-  const ModelDesc* model = nullptr;
-  Layout L{};
-  int maxBatch = 0;
-  int split = 0;          // fp32-equivalent mode
-  bool nhwc = true;
-  bool streamTrunkFp32 = true, streamInnerFp32 = false;
-  std::vector<void*> allocs;
-  // inputs / outputs (device, fixed addresses so graphs can be replayed)
-  float *dSpatial = nullptr, *dGlobal = nullptr, *dOptimism = nullptr;
-  int* dSymmetry = nullptr;
-  float *dPolicy = nullptr, *dValue = nullptr, *dScore = nullptr, *dOwnership = nullptr;
-  // pinned staging
-  float *hSpatial = nullptr, *hGlobal = nullptr, *hOptimism = nullptr, *hPolicy = nullptr, *hValue = nullptr, *hScore = nullptr,
-        *hOwnership = nullptr;
-  int* hSymmetry = nullptr;
-  float *dMask = nullptr, *dMaskSum = nullptr;
-  std::vector<std::function<void(int, cudaStream_t)>> ops;
-  int launchesPerForward = 0;
-  std::map<int, cudaGraphExec_t> graphs;
-
-  // Weights live in ONE arena: a net of the same architecture is swapped in between two waves by one device copy
-  // (kgb_handle_stage_weights / kgb_handle_commit_weights) and travels between the GPUs of a node as one ncclBroadcast
-  // (kgb_handle_broadcast_staged_weights).  The graph builder runs in three modes over the same code:
-  //   W_SIZE   on a scratch handle: only adds up the arena (nothing is allocated, no op is kept)
-  //   W_BUILD  the real build: device addresses from wLive, bytes packed into the pinned mirror wHost, one H2D copy at the end
-  //   W_REPACK on a scratch handle: packs ANOTHER model's weights into wHost at the same offsets, destined for wShadow
-  enum { W_BUILD = 0, W_SIZE = 1, W_REPACK = 2 };
-  int wMode = W_BUILD;
-  char *wLive = nullptr, *wShadow = nullptr, *wHost = nullptr;
-  size_t wBytes = 0, wCursor = 0, wIndex = 0;
-  std::vector<size_t> wSizes;     // the arena's spans in build order: a staged model must produce the same sequence
-  std::string wSignature;         // shapes, activations and head constants that ops capture by value (must match as well)
-  cudaStream_t copyStream = nullptr;
-  cudaEvent_t stagedEvent = nullptr, bcastStart = nullptr, bcastStop = nullptr;
-  bool staged = false;
-  void* ncclComm = nullptr;
-  int ncclRank = 0, ncclRanks = 0;
-
-  template <class T>
-  T* dalloc(size_t count) {
-    if(wMode != W_BUILD) return (T*)(uintptr_t)256;      // scratch pass: activations are never touched
-    void* p = nullptr;
-    CK(cudaMalloc(&p, count * sizeof(T)));
-    CK(cudaMemset(p, 0, count * sizeof(T)));
-    allocs.push_back(p);
-    return (T*)p;
-  }
-  // One span of the weight arena: returns its device address and (except in W_SIZE) where to pack its bytes on the host
-  void* walloc(size_t bytes, void** host) {
-    const size_t b = (bytes + 255) & ~(size_t)255;
-    const size_t o = wCursor;
-    wCursor += b;
-    if(wMode == W_SIZE) {
-      wSizes.push_back(b);
-      *host = nullptr;
-      return (void*)(uintptr_t)(256 + o);
-    }
-    if(wIndex >= wSizes.size() || wSizes[wIndex] != b || o + b > wBytes)
-      throw std::invalid_argument("the model's weights do not have the layout this handle was built for (different architecture)");
-    wIndex++;
-    *host = wHost + o;
-    return (wMode == W_BUILD ? wLive : wShadow) + o;
-  }
-  void wAllocArena(size_t bytes) {
-    wBytes = bytes;
-    CK(cudaMalloc((void**)&wLive, std::max<size_t>(bytes, 256)));
-    CK(cudaMemset(wLive, 0, std::max<size_t>(bytes, 256)));
-    allocs.push_back(wLive);
-    CK(cudaMallocHost((void**)&wHost, std::max<size_t>(bytes, 256)));
-    memset(wHost, 0, std::max<size_t>(bytes, 256));
-  }
-  void wFlushLive() {       // the packed bytes reach the device in one copy
-    CK(cudaMemcpy(wLive, wHost, wCursor, cudaMemcpyHostToDevice));
-    CK(cudaDeviceSynchronize());
-  }
-  float* upload(const std::vector<float>& v, size_t padTo = 0) {
-    size_t n = std::max(v.size(), padTo);
-    void* hp = nullptr;
-    float* d = (float*)walloc(n * sizeof(float), &hp);
-    if(hp) {
-      memset(hp, 0, n * sizeof(float));
-      if(!v.empty()) memcpy(hp, v.data(), v.size() * sizeof(float));
-    }
-    return d;
-  }
 };
 
 // ------------------------------------------------------------------------------------------------------------
@@ -521,27 +403,31 @@ struct Builder {
 
 void runOps(kgb_handle* h, int n) {
   auto it = h->graphs.find(n);
-  if(it == h->graphs.end()) {
-    cudaGraph_t graph = nullptr;
-    CK(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
-    try {
-      for(auto& op : h->ops) op(n, h->stream);
-    }
-    catch(...) {
-      cudaStreamEndCapture(h->stream, &graph);
-      if(graph) cudaGraphDestroy(graph);
-      throw;
-    }
-    CK(cudaStreamEndCapture(h->stream, &graph));
-    cudaGraphExec_t exec = nullptr;
-    CK(cudaGraphInstantiate(&exec, graph, 0));
-    CK(cudaGraphDestroy(graph));
-    it = h->graphs.emplace(n, exec).first;
-  }
+  if(it == h->graphs.end())
+    it = h->graphs.emplace(n, captureGraph(h->stream, [&] { for(auto& op : h->ops) op(n, h->stream); })).first;
   CK(cudaGraphLaunch(it->second, h->stream));
 }
 
 }  // namespace
+
+cudaGraphExec_t captureGraph(cudaStream_t s, const std::function<void()>& launches) {
+  cudaGraph_t graph = nullptr;
+  CK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+  try {
+    launches();
+  }
+  catch(...) {
+    cudaStreamEndCapture(s, &graph);
+    if(graph) cudaGraphDestroy(graph);
+    throw;
+  }
+  CK(cudaStreamEndCapture(s, &graph));
+  cudaGraphExec_t exec = nullptr;
+  const cudaError_t e = cudaGraphInstantiate(&exec, graph, 0);
+  cudaGraphDestroy(graph);
+  CK(e);
+  return exec;
+}
 
 // ------------------------------------------------------------------------------------------------------------
 // C ABI
@@ -761,7 +647,7 @@ KGB_API int kgb_handle_create(kgb_context* ctx, const kgb_model* model, int max_
     CK(cudaMallocHost((void**)&h.hValue, (size_t)h.maxBatch * 3 * sizeof(float)));
     CK(cudaMallocHost((void**)&h.hScore, (size_t)h.maxBatch * 6 * sizeof(float)));
     CK(cudaMallocHost((void**)&h.hOwnership, (size_t)h.maxBatch * XY * sizeof(float)));
-    CK(cudaDeviceSynchronize());
+    CK(cudaStreamSynchronize(h.stream));
     *out = raw;
     raw = nullptr;
   });
@@ -783,7 +669,7 @@ KGB_API int kgb_handle_weights_bytes(const kgb_handle* handle, uint64_t* bytes) 
 static void ensureShadow(kgb_handle* h) {
   if(h->wShadow) return;
   CK(cudaMalloc((void**)&h->wShadow, std::max<size_t>(h->wBytes, 256)));
-  CK(cudaMemset(h->wShadow, 0, std::max<size_t>(h->wBytes, 256)));
+  CK(cudaMemsetAsync(h->wShadow, 0, std::max<size_t>(h->wBytes, 256), h->copyStream));
 }
 
 KGB_API int kgb_handle_stage_weights(kgb_handle* handle, const kgb_model* model) {
@@ -1024,11 +910,10 @@ struct SingleConv {
   // boardXY [n][2] (or null = the whole frame): image i's board is its top-left X_i x Y_i, as the self-play loop places boards
   void setInput(const float* input /* NHWC */, const int32_t* boardXY = nullptr) {
     float* dIn = h.dalloc<float>((size_t)n * X * Y * cin);
-    CK(cudaMemcpy(dIn, input, (size_t)n * X * Y * cin * sizeof(float), cudaMemcpyHostToDevice));
-    CK(cudaDeviceSynchronize());   // see below: the pack kernel runs on a non-blocking stream
+    CK(cudaMemcpyAsync(dIn, input, (size_t)n * X * Y * cin * sizeof(float), cudaMemcpyHostToDevice, h.stream));
     CK(launchPackInput(dIn, n, cin, true, nullptr, h.L, As[0], cw.cin_p, h.split, h.dMask, h.dMaskSum, h.stream));
-    CK(cudaStreamSynchronize(h.stream));
-    for(size_t r = 1; r < As.size(); r++) CK(cudaMemcpy(As[r], As[0], M * cw.cin_p * (h.split ? 2 : 1) * sizeof(__half), cudaMemcpyDeviceToDevice));
+    for(size_t r = 1; r < As.size(); r++)
+      CK(cudaMemcpyAsync(As[r], As[0], M * cw.cin_p * (h.split ? 2 : 1) * sizeof(__half), cudaMemcpyDeviceToDevice, h.stream));
     // the mask of a bare convolution is "every point of the image's board", not input channel 0
     std::vector<float> hm(M, 0.0f);
     for(int i = 0; i < n; i++) {
@@ -1037,10 +922,7 @@ struct SingleConv {
         for(int x = 0; x < bx; x++) hm[(size_t)i * h.L.P + (size_t)(y + h.L.pad) * h.L.Wp + x] = 1.0f;
     }
     mask = hm;
-    CK(cudaMemcpy(h.dMask, hm.data(), M * sizeof(float), cudaMemcpyHostToDevice));
-    // cudaMemcpy from pageable memory may return before the DMA has landed, and h.stream is non-blocking:
-    // nothing else orders these uploads before the kernels launched on it.
-    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpyAsync(h.dMask, hm.data(), M * sizeof(float), cudaMemcpyHostToDevice, h.stream));
   }
   void run() { h.ops[next](n, h.stream); next = (next + 1) % rotate; }
 };
@@ -1065,41 +947,44 @@ void testConv(const char* fn, int ky, int kx, int in_c, int out_c, const float* 
   const int cp = sc.cw.cout_p;
   const bool f32 = sc.rawF32;
   const bool split = sc.h.split != 0;
+  const cudaStream_t s = sc.h.stream;
   if(split && kind != 0 && !act_lo_out) throw std::invalid_argument(std::string(fn) + ": split mode needs act_lo_out");
   auto rowOf = [&](int i, int y, int x) { return (size_t)i * sc.h.L.P + (size_t)(y + sc.h.L.pad) * sc.h.L.Wp + x; };
   if(ncbias) {
     std::vector<float> hb((size_t)n * cp, 0.0f);
     for(int i = 0; i < n; i++) for(int c = 0; c < out_c; c++) hb[(size_t)i * cp + c] = ncbias[(size_t)i * out_c + c];
-    CK(cudaMemcpy(sc.ncbias, hb.data(), hb.size() * sizeof(float), cudaMemcpyHostToDevice));
+    CK(cudaMemcpyAsync(sc.ncbias, hb.data(), hb.size() * sizeof(float), cudaMemcpyHostToDevice, s));
   }
   if(hasResidual) {
     // given as fp32; an fp16 stream holds it rounded to nearest
     std::vector<float> hf(sc.M * cp, 0.0f);
     for(int i = 0; i < n; i++) for(int y = 0; y < nn_y_len; y++) for(int x = 0; x < nn_x_len; x++) for(int c = 0; c < out_c; c++)
       hf[rowOf(i, y, x) * cp + c] = residual_in[(((size_t)i * nn_y_len + y) * nn_x_len + x) * out_c + c];
-    if(f32) CK(cudaMemcpy(sc.raws[0], hf.data(), hf.size() * sizeof(float), cudaMemcpyHostToDevice));
+    if(f32) CK(cudaMemcpyAsync(sc.raws[0], hf.data(), hf.size() * sizeof(float), cudaMemcpyHostToDevice, s));
     else {
       std::vector<__half> hh(hf.size());
       for(size_t k = 0; k < hf.size(); k++) hh[k] = __float2half_rn(hf[k]);
-      CK(cudaMemcpy(sc.raws[0], hh.data(), hh.size() * sizeof(__half), cudaMemcpyHostToDevice));
+      CK(cudaMemcpyAsync(sc.raws[0], hh.data(), hh.size() * sizeof(__half), cudaMemcpyHostToDevice, s));
     }
   }
-  CK(cudaDeviceSynchronize());   // pageable uploads, then a launch on a non-blocking stream
   sc.run();
-  CK(cudaStreamSynchronize(sc.h.stream));
+  auto download = [&](void* dst, const void* src, size_t bytes) {
+    CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+  };
   const int am = split ? 2 : 1;
   std::vector<__half> ha;
   if(!sc.acts.empty()) {
     ha.resize(sc.M * cp * am);
-    CK(cudaMemcpy(ha.data(), sc.acts[0], ha.size() * sizeof(__half), cudaMemcpyDeviceToHost));
+    download(ha.data(), sc.acts[0], ha.size() * sizeof(__half));
   }
   std::vector<float> hr;
   if(!sc.raws.empty()) {
     hr.resize(sc.M * cp);
-    if(f32) CK(cudaMemcpy(hr.data(), sc.raws[0], hr.size() * sizeof(float), cudaMemcpyDeviceToHost));
+    if(f32) download(hr.data(), sc.raws[0], hr.size() * sizeof(float));
     else {
       std::vector<__half> hh(hr.size());
-      CK(cudaMemcpy(hh.data(), sc.raws[0], hh.size() * sizeof(__half), cudaMemcpyDeviceToHost));
+      download(hh.data(), sc.raws[0], hh.size() * sizeof(__half));
       for(size_t k = 0; k < hr.size(); k++) hr[k] = __half2float(hh[k]);
     }
   }
@@ -1190,22 +1075,7 @@ KGB_API int kgb_bench_conv_ex(int ky, int kx, int in_c, int out_c, int n, int nn
   });
 }
 
-// ---- Boundary 2: device-resident self-play ------------------------------------------------------------------
-struct kgb_selfplay {
-  kgb_handle* h = nullptr;
-  SelfplayImpl* impl = nullptr;
-  int n = 0;
-  bool fakeNN = false;
-  cudaGraphExec_t stepGraph = nullptr;
-};
-
-static void selfplayStepLaunches(kgb_selfplay* sp, cudaStream_t s) {
-  selfplayLaunchSelect(sp->impl, s);
-  if(sp->fakeNN) selfplayLaunchFakeNN(sp->impl, sp->h->dPolicy, sp->h->dValue, sp->h->dScore, sp->h->dOwnership, s);
-  else for(auto& op : sp->h->ops) op(sp->n, s);
-  selfplayLaunchBackup(sp->impl, s);
-}
-
+// ---- Host-side tables and generators of the self-play loop (the loop itself is in kgb_selfplay.cu) ----------------------
 KGB_API int kgb_expected_white_score_value(int n, const double* mean, const double* stdev, const double* center, const double* scale,
                                            const double* sqrt_board_area, double* out) {
   return guarded([&] {
@@ -1231,374 +1101,6 @@ KGB_API int kgb_value_weight_cdf_table(double* out, int n) {
   });
 }
 
-KGB_API int kgb_selfplay_get_play_selection_values(kgb_selfplay* sp, int game, double* values) {
-  return guarded([&] {
-    if(!sp || !values) throw std::invalid_argument("kgb_selfplay_get_play_selection_values: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplayReadPlaySelection(sp->impl, game, values);
-  });
-}
-
-KGB_API int kgb_test_choose_index_with_temperature(const char* seed_string, const double* relative_probs, int n, double temperature,
-                                                   double only_below_prob, int count, int32_t* chosen) {
-  return guarded([&] {
-    if(!seed_string || !relative_probs || !chosen || n < 1 || count < 1) throw std::invalid_argument("kgb_test_choose_index_with_temperature: bad argument");
-    chooseIndexTest(seed_string, relative_probs, n, temperature, only_below_prob, count, chosen);
-  });
-}
-
-KGB_API int kgb_test_history_replay(int x_len, int y_len, int ko_rule, int multi_stone_suicide_legal, int num_games, int max_moves, const int8_t* moves_xy,
-                                    uint8_t* flags, uint8_t* legal_next, uint8_t* super_ko_banned) {
-  return guarded([&] {
-    if(!moves_xy || !flags || !legal_next || !super_ko_banned || num_games < 1 || max_moves < 1 || ko_rule < 0 || ko_rule > 3)
-      throw std::invalid_argument("kgb_test_history_replay: bad argument");
-    historyReplay(x_len, y_len, ko_rule, multi_stone_suicide_legal, num_games, max_moves, moves_xy, flags, legal_next, super_ko_banned);
-  });
-}
-
-KGB_API int kgb_test_repetition_bound(int x_len, int y_len, int num_moves, int bound, const int8_t* moves_xyp, uint8_t* out) {
-  return guarded([&] {
-    if(!moves_xyp || !out || num_moves < 1) throw std::invalid_argument("kgb_test_repetition_bound: bad argument");
-    repBoundTest(x_len, y_len, num_moves, bound, moves_xyp, out);
-  });
-}
-
-KGB_API int kgb_test_root_policy_noise(const char* seed_string, int x_len, int y_len, int policy_size, int turn_number, int noise_enabled,
-                                       double concentration, double weight, double temperature, double temperature_early, double halflife,
-                                       const float* policy_in, float* policy_out) {
-  return guarded([&] {
-    if(!seed_string || !policy_in || !policy_out || policy_size < 1 || policy_size > 362) throw std::invalid_argument("kgb_test_root_policy_noise: bad argument");
-    rootNoiseTest(seed_string, x_len, y_len, policy_size, turn_number, noise_enabled, concentration, weight, temperature, temperature_early, halflife,
-                  policy_in, policy_out);
-  });
-}
-
-KGB_API int kgb_selfplay_create(kgb_handle* handle, const kgb_selfplay_config* config, kgb_selfplay** out) {
-  return guarded([&] {
-    if(!handle || !config || !out) throw std::invalid_argument("kgb_selfplay_create: NULL argument");
-    if(config->num_games > handle->maxBatch) throw std::invalid_argument("kgb_selfplay_create: num_games exceeds the handle's max_batch_size");
-    if(!handle->nhwc) throw std::invalid_argument("kgb_selfplay_create: the handle must be created with inputs_nhwc = 1");
-    if(handle->model->numInputChannels != 22 || handle->model->numInputGlobalChannels != 19)
-      throw std::invalid_argument("kgb_selfplay_create: the device loop writes V7 features (22 spatial, 19 global)");
-    CK(cudaSetDevice(handle->device));
-    std::unique_ptr<kgb_selfplay> sp(new kgb_selfplay());
-    sp->h = handle;
-    sp->n = config->num_games;
-    sp->fakeNN = config->debug_fake_nn != 0;
-    SelfplayNNBuffers nn{handle->dSpatial, handle->dGlobal, handle->dOptimism, handle->dSymmetry, handle->dPolicy, handle->dValue, handle->dScore, handle->dOwnership,
-                         (double)handle->model->scoreMeanMultiplier, (double)handle->model->scoreStdevMultiplier, (double)handle->model->leadMultiplier};
-    sp->impl = selfplayCreate(*config, handle->L.X, handle->L.Y, nn, handle->stream);
-    *out = sp.release();
-  });
-}
-
-KGB_API void kgb_selfplay_free(kgb_selfplay* sp) {
-  if(!sp) return;
-  if(sp->stepGraph) cudaGraphExecDestroy(sp->stepGraph);
-  selfplayDestroy(sp->impl);
-  delete sp;
-}
-
-KGB_API int kgb_selfplay_run(kgb_selfplay* sp, int steps) {
-  return guarded([&] {
-    if(!sp || steps < 0) throw std::invalid_argument("kgb_selfplay_run: bad argument");
-    kgb_handle* h = sp->h;
-    CK(cudaSetDevice(h->device));
-    if(!sp->stepGraph) {
-      cudaGraph_t graph = nullptr;
-      CK(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
-      try { selfplayStepLaunches(sp, h->stream); }
-      catch(...) { cudaStreamEndCapture(h->stream, &graph); if(graph) cudaGraphDestroy(graph); throw; }
-      CK(cudaStreamEndCapture(h->stream, &graph));
-      CK(cudaGraphInstantiate(&sp->stepGraph, graph, 0));
-      CK(cudaGraphDestroy(graph));
-    }
-    for(int i = 0; i < steps; i++) CK(cudaGraphLaunch(sp->stepGraph, h->stream));
-  });
-}
-
-KGB_API int kgb_selfplay_set_search_rand(kgb_selfplay* sp, const char* seed_string) {
-  return guarded([&] {
-    if(!sp || !seed_string) throw std::invalid_argument("kgb_selfplay_set_search_rand: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplaySetSearchRand(sp->impl, seed_string);
-  });
-}
-
-KGB_API int kgb_selfplay_random_openings(kgb_selfplay* sp, int max_moves) {
-  return guarded([&] {
-    if(!sp || max_moves < 0) throw std::invalid_argument("kgb_selfplay_random_openings: bad argument");
-    CK(cudaSetDevice(sp->h->device));
-    selfplayRandomOpenings(sp->impl, max_moves, sp->h->stream);
-  });
-}
-
-KGB_API int kgb_selfplay_get_stats(kgb_selfplay* sp, kgb_selfplay_stats* out) {
-  return guarded([&] {
-    if(!sp || !out) throw std::invalid_argument("kgb_selfplay_get_stats: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplayReadStats(sp->impl, out);
-  });
-}
-
-KGB_API int kgb_selfplay_get_game(kgb_selfplay* sp, int game, uint8_t* colors, int32_t* info) {
-  return guarded([&] {
-    if(!sp || !colors || !info) throw std::invalid_argument("kgb_selfplay_get_game: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplayReadGame(sp->impl, game, colors, info);
-  });
-}
-
-KGB_API int kgb_selfplay_get_root_children(kgb_selfplay* sp, int game, int32_t* visits, float* policy, double* util_sum) {
-  return guarded([&] {
-    if(!sp || !visits || !policy || !util_sum) throw std::invalid_argument("kgb_selfplay_get_root_children: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplayReadRootChildren(sp->impl, game, visits, policy, util_sum);
-  });
-}
-
-KGB_API int kgb_selfplay_get_root_value_stats(kgb_selfplay* sp, int game, double* child_stats, double* root_stats) {
-  return guarded([&] {
-    if(!sp || !child_stats || !root_stats) throw std::invalid_argument("kgb_selfplay_get_root_value_stats: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplayReadRootMoments(sp->impl, game, child_stats, root_stats);
-  });
-}
-
-KGB_API int kgb_selfplay_set_komi(kgb_selfplay* sp, const float* komi, int also_current_games) {
-  return guarded([&] {
-    if(!sp || !komi) throw std::invalid_argument("kgb_selfplay_set_komi: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplaySetKomi(sp->impl, komi, also_current_games != 0);
-  });
-}
-
-KGB_API int kgb_selfplay_set_game_setup(kgb_selfplay* sp, const int32_t* setup, int also_current_games) {
-  return guarded([&] {
-    if(!sp || !setup) throw std::invalid_argument("kgb_selfplay_set_game_setup: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplaySetGameSetup(sp->impl, setup, also_current_games != 0, sp->h->stream);
-  });
-}
-
-KGB_API int kgb_selfplay_set_next_search_limits(kgb_selfplay* sp, const int32_t* visits, const uint8_t* plain_root, int also_current_roots) {
-  return guarded([&] {
-    if(!sp || !visits) throw std::invalid_argument("kgb_selfplay_set_next_search_limits: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplaySetNextSearchLimits(sp->impl, visits, plain_root, also_current_roots != 0, sp->h->stream);
-  });
-}
-
-KGB_API int kgb_selfplay_get_search_limits(kgb_selfplay* sp, int32_t* visits, uint8_t* plain_root) {
-  return guarded([&] {
-    if(!sp) throw std::invalid_argument("kgb_selfplay_get_search_limits: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplayReadSearchLimits(sp->impl, visits, plain_root);
-  });
-}
-
-KGB_API int kgb_selfplay_set_policy_init(kgb_selfplay* sp, const int32_t* num_moves, double temperature, int also_current_games) {
-  return guarded([&] {
-    if(!sp || !num_moves) throw std::invalid_argument("kgb_selfplay_set_policy_init: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplaySetPolicyInit(sp->impl, num_moves, temperature, also_current_games != 0, sp->h->stream);
-  });
-}
-
-KGB_API int kgb_selfplay_get_policy_init(kgb_selfplay* sp, int32_t* moves_left, int32_t* count, int16_t* moves, int max_moves) {
-  return guarded([&] {
-    if(!sp) throw std::invalid_argument("kgb_selfplay_get_policy_init: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplayReadPolicyInit(sp->impl, moves_left, count, moves, max_moves);
-  });
-}
-
-KGB_API int kgb_selfplay_get_nn_symmetries(kgb_selfplay* sp, int32_t* symmetries) {
-  return guarded([&] {
-    if(!sp || !symmetries) throw std::invalid_argument("kgb_selfplay_get_nn_symmetries: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplayReadSymmetries(sp->impl, symmetries);
-  });
-}
-
-KGB_API int kgb_selfplay_get_root_raw_policy_entropy(kgb_selfplay* sp, double* entropy) {
-  return guarded([&] {
-    if(!sp || !entropy) throw std::invalid_argument("kgb_selfplay_get_root_raw_policy_entropy: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplayReadRootRawEntropy(sp->impl, entropy);
-  });
-}
-
-KGB_API int kgb_selfplay_get_game_setup(kgb_selfplay* sp, int32_t* current, int32_t* last_finished) {
-  return guarded([&] {
-    if(!sp) throw std::invalid_argument("kgb_selfplay_get_game_setup: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplayReadGameSetup(sp->impl, current, last_finished);
-  });
-}
-
-KGB_API int kgb_selfplay_get_komi(kgb_selfplay* sp, float* current, float* last_finished) {
-  return guarded([&] {
-    if(!sp) throw std::invalid_argument("kgb_selfplay_get_komi: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplayReadKomi(sp->impl, current, last_finished);
-  });
-}
-
-KGB_API int kgb_selfplay_get_leaf_cache_key(kgb_selfplay* sp, int game, uint64_t* key2) {
-  return guarded([&] {
-    if(!sp || !key2) throw std::invalid_argument("kgb_selfplay_get_leaf_cache_key: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    unsigned long long k[2];
-    selfplayReadLeafKey(sp->impl, game, k);
-    key2[0] = k[0]; key2[1] = k[1];
-  });
-}
-
-KGB_API int kgb_selfplay_clear_nn_cache(kgb_selfplay* sp) {
-  return guarded([&] {
-    if(!sp) throw std::invalid_argument("kgb_selfplay_clear_nn_cache: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    selfplayClearNNCache(sp->impl, sp->h->stream);
-  });
-}
-
-KGB_API int kgb_selfplay_release(kgb_selfplay* sp, const uint8_t* games_mask) {
-  return guarded([&] {
-    if(!sp) throw std::invalid_argument("kgb_selfplay_release: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplayRelease(sp->impl, games_mask);
-  });
-}
-
-KGB_API int kgb_selfplay_get_root_visits(kgb_selfplay* sp, int32_t* visits) {
-  return guarded([&] {
-    if(!sp || !visits) throw std::invalid_argument("kgb_selfplay_get_root_visits: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplayReadRootVisitsAll(sp->impl, visits);
-  });
-}
-
-KGB_API int kgb_selfplay_get_root_extra(kgb_selfplay* sp, int game, int32_t* child_node_visits, double* root_nn_stats) {
-  return guarded([&] {
-    if(!sp || !child_node_visits || !root_nn_stats) throw std::invalid_argument("kgb_selfplay_get_root_extra: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplayReadRootExtra(sp->impl, game, child_node_visits, root_nn_stats);
-  });
-}
-
-KGB_API int kgb_selfplay_get_last_move(kgb_selfplay* sp, int game, int32_t* info, float* final_score, uint8_t* final_colors, uint8_t* final_area) {
-  return guarded([&] {
-    if(!sp || !info || !final_score || !final_colors || !final_area) throw std::invalid_argument("kgb_selfplay_get_last_move: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplayReadLastMove(sp->impl, game, info, final_score, final_colors, final_area);
-  });
-}
-
-KGB_API int kgb_selfplay_get_nn_row(kgb_selfplay* sp, int game, float* spatial, float* global) {
-  return guarded([&] {
-    if(!sp || !spatial || !global || game < 0 || game >= sp->n) throw std::invalid_argument("kgb_selfplay_get_nn_row: bad argument");
-    kgb_handle* h = sp->h;
-    CK(cudaSetDevice(h->device));
-    CK(cudaStreamSynchronize(h->stream));
-    const size_t XY = (size_t)h->L.X * h->L.Y;
-    CK(cudaMemcpy(spatial, h->dSpatial + (size_t)game * XY * 22, XY * 22 * sizeof(float), cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(global, h->dGlobal + (size_t)game * 19, 19 * sizeof(float), cudaMemcpyDeviceToHost));
-  });
-}
-
-KGB_API int kgb_selfplay_get_root_row(kgb_selfplay* sp, int game, float* spatial, float* global) {
-  return guarded([&] {
-    if(!sp || !spatial || !global || game < 0 || game >= sp->n) throw std::invalid_argument("kgb_selfplay_get_root_row: bad argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplayReadRootRow(sp->impl, game, spatial, global);
-  });
-}
-
-KGB_API int kgb_selfplay_get_leaf_path(kgb_selfplay* sp, int game, int32_t* moves_xy, int32_t max_len, int32_t* len_out, int32_t* valid_out) {
-  return guarded([&] {
-    if(!sp || !moves_xy || !len_out || !valid_out || max_len < 0) throw std::invalid_argument("kgb_selfplay_get_leaf_path: bad argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    *len_out = selfplayReadLeafPath(sp->impl, game, moves_xy, max_len, valid_out);
-  });
-}
-
-KGB_API int kgb_selfplay_play_moves(kgb_selfplay* sp, const int8_t* moves_xy, int num_moves) {
-  return guarded([&] {
-    if(!sp || (!moves_xy && num_moves > 0) || num_moves < 0) throw std::invalid_argument("kgb_selfplay_play_moves: bad argument");
-    CK(cudaSetDevice(sp->h->device));
-    selfplayPlayMoves(sp->impl, moves_xy, num_moves, sp->h->stream);
-  });
-}
-
-KGB_API int kgb_selfplay_play_moves_game(kgb_selfplay* sp, int game, const int8_t* moves_xy, int num_moves) {
-  return guarded([&] {
-    if(!sp || game < 0 || (!moves_xy && num_moves > 0) || num_moves < 0) throw std::invalid_argument("kgb_selfplay_play_moves_game: bad argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplayPlayMoves(sp->impl, moves_xy, num_moves, sp->h->stream, game);
-  });
-}
-
-KGB_API int kgb_selfplay_time_tree_kernels(kgb_selfplay* sp, int iters, float* ms_select, float* ms_backup) {
-  return guarded([&] {
-    if(!sp || iters < 1 || !ms_select || !ms_backup) throw std::invalid_argument("kgb_selfplay_time_tree_kernels: bad argument");
-    kgb_handle* h = sp->h;
-    CK(cudaSetDevice(h->device));
-    cudaEvent_t e0, e1, e2;
-    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1)); CK(cudaEventCreate(&e2));
-    float accS = 0.f, accB = 0.f;
-    CK(cudaStreamSynchronize(h->stream));
-    for(int i = 0; i < iters; i++) {   // the evaluator outputs of the last wave are reused: the trees keep growing normally
-      CK(cudaEventRecord(e0, h->stream));
-      selfplayLaunchSelect(sp->impl, h->stream);
-      CK(cudaEventRecord(e1, h->stream));
-      selfplayLaunchBackup(sp->impl, h->stream);
-      CK(cudaEventRecord(e2, h->stream));
-      CK(cudaStreamSynchronize(h->stream));
-      float a = 0.f, b = 0.f;
-      CK(cudaEventElapsedTime(&a, e0, e1)); CK(cudaEventElapsedTime(&b, e1, e2));
-      accS += a; accB += b;
-    }
-    cudaEventDestroy(e0); cudaEventDestroy(e1); cudaEventDestroy(e2);
-    *ms_select = accS / iters; *ms_backup = accB / iters;
-  });
-}
-
-KGB_API int kgb_selfplay_debug_cycles(kgb_selfplay* sp, int64_t* cycles, int clear) {
-  return guarded([&] {
-    if(!sp || !cycles) throw std::invalid_argument("kgb_selfplay_debug_cycles: NULL argument");
-    CK(cudaSetDevice(sp->h->device));
-    CK(cudaStreamSynchronize(sp->h->stream));
-    selfplayReadDebugCycles(sp->impl, (long long*)cycles, clear != 0);
-  });
-}
-
-KGB_API int kgb_selfplay_launches_per_step(const kgb_selfplay* sp) { return sp ? sp->h->launchesPerForward + 2 : 0; }
-
 KGB_API int kgb_zobrist_tables(int x_size, int y_size, uint64_t* board_hash, uint64_t* size_hash) {
   return guarded([&] {
     if(!board_hash || !size_hash || x_size < 2 || y_size < 2 || x_size > 19 || y_size > 19) throw std::invalid_argument("kgb_zobrist_tables: bad argument");
@@ -1611,17 +1113,6 @@ KGB_API int kgb_zobrist_tables(int x_size, int y_size, uint64_t* board_hash, uin
           o[0] = h.h0; o[1] = h.h1;
         }
     size_hash[0] = z.sizeHash.h0; size_hash[1] = z.sizeHash.h1;
-  });
-}
-
-KGB_API int kgb_test_board_replay(int x_size, int y_size, int num_boards, int num_moves, int multi_stone_suicide_legal, const int8_t* moves,
-                          uint8_t* colors, int8_t* ko, int16_t* caps, uint8_t* lib_class, uint8_t* legal_next, uint64_t* pos_hash, uint8_t* area) {
-  return guarded([&] {
-    if(!moves || !colors || !ko || !caps || !lib_class || !legal_next || !pos_hash || !area || num_boards < 1 || num_moves < 1)
-      throw std::invalid_argument("kgb_test_board_replay: bad argument");
-    int count = 0;
-    if(cudaGetDeviceCount(&count) != cudaSuccess || count == 0) throw CudaFailure("libkgb200: no CUDA device is visible");
-    boardReplay(x_size, y_size, num_boards, num_moves, multi_stone_suicide_legal, moves, colors, ko, caps, lib_class, legal_next, pos_hash, area);
   });
 }
 

@@ -37,10 +37,10 @@
 #include "../../include/kgb200.h"
 #include "kgb_board.cuh"
 #include "kgb_devrand.cuh"
+#include "kgb_handle.h"
 #include "kgb_history.cuh"
 #include "kgb_ladder.cuh"
 #include "kgb_scorevalue.h"
-#include "kgb_selfplay.h"
 #include "kgb_rand.h"
 
 namespace kgb {
@@ -2242,34 +2242,181 @@ __global__ void historyReplayKernel(int X, int Y, int koRule, int multiSuicide, 
   }
 }
 
+// Board size and ko / suicide rules per game (GameInitializer::createGameSharedUnsynchronized, program/play.cpp:330-650: bSizes /
+// bSizeRelProbs, koRules, multiStoneSuicideLegals drawn per game).  setup[numGames][4] = X, Y, ko rule, multi-stone suicide: taken by each slot's
+// NEXT game; with alsoCurrent also by the game in progress, which must not have started (no move played, root not searched) - its history
+// restarts under the new rules.  Ko rules other than the loop's own need full_history_rules (BoardHistory's lists are per game already).
+__global__ void spApplySetupKernel(const SPDev d, int* refused) {
+  const int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if(g >= d.numGames) return;
+  const size_t gb = (size_t)g * d.maxNodes;
+  if(d.moveNum[g] != 0 || d.nodeVisits[gb] != 0 || d.rootSymCount[g] != 0 || d.ladPending[g] != 0) { if(lane == 0) atomicAdd(refused, 1); return; }
+  __syncwarp();
+  if(lane == 0) { d.gX[g] = d.nextSetup[g * 4 + 0]; d.gY[g] = d.nextSetup[g * 4 + 1]; d.gKoRule[g] = d.nextSetup[g * 4 + 2]; d.gMultiSuicide[g] = d.nextSetup[g * 4 + 3]; }
+  __syncwarp();
+  gameHistReset(d, g, lane);
+  __syncwarp();
+  rootHashesInit(d, g, lane);
+}
+
+// Search limits of the roots to come (getSearchLimitsThisMove, program/play.cpp:1093-1223: cheap searches, reduced visits).  visits[numGames][2],
+// plain[numGames][2] (may be NULL = all 0): index 0 applies to the root after the slot's next move when the game goes on, index 1 when that
+// move ends the game (first root of the slot's next game).  alsoCurrent: index 0 also replaces the limits of the current roots, which
+// must not have been searched yet.
+__global__ void spApplyLimitsKernel(const SPDev d, int* refused) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if(g >= d.numGames) return;
+  if(d.nodeVisits[(size_t)g * d.maxNodes] != 0 || d.rootSymCount[g] != 0) { atomicAdd(refused, 1); return; }
+  d.visitBudget[g] = d.nextBudget[g * 2]; d.plainRoot[g] = d.nextPlain[g * 2];
+}
+
+// Policy-initialised openings (PlaySettings::initGamesWithPolicy / policyInitAreaProp / policyInitAreaTemperature; playutils.cpp:232-266): moves[numGames] =
+// how many opening moves each slot's NEXT game draws from the raw policy before its first searched move (the host draws the count: floor of an
+// exponential with mean area * policyInitAreaProp).  alsoCurrent: the games in progress take them too; they must not have started.
+__global__ void spApplyPolicyInitKernel(const SPDev d, int* refused) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if(g >= d.numGames) return;
+  if(d.moveNum[g] != 0 || d.nodeVisits[(size_t)g * d.maxNodes] != 0 || d.rootSymCount[g] != 0) { atomicAdd(refused, 1); return; }
+  d.initMovesLeft[g] = d.nextInitMoves[g]; d.initMoveCount[g] = 0;
+  if(d.initMovesLeft[g] > 0) { d.visitBudget[g] = 1; d.plainRoot[g] = 1; }
+}
+
+}  // namespace kgb
+
 // ------------------------------------------------------------------------------------------------------------
 // Host side
 // ------------------------------------------------------------------------------------------------------------
-#define SPCK(expr)                                                                                               \
-  do {                                                                                                           \
-    cudaError_t _e = (expr);                                                                                     \
-    if(_e != cudaSuccess) throw std::runtime_error(std::string("CUDA error ") + cudaGetErrorString(_e) + " at " #expr); \
-  } while(0)
+using namespace kgb;
 
-struct SelfplayImpl {
-  SPDev d;
-  std::vector<void*> allocs;
-  cudaStream_t stream;
-  template <class T> T* alloc(size_t n) {
-    void* p = nullptr;
-    SPCK(cudaMalloc(&p, n * sizeof(T)));
-    SPCK(cudaMemset(p, 0, n * sizeof(T)));
-    allocs.push_back(p);
-    return (T*)p;
-  }
-  ~SelfplayImpl() { for(void* p : allocs) cudaFree(p); }
+namespace {
+
+// Device scratch of one call, freed on every way out of it
+template <class T>
+struct Scratch {
+  T* p = nullptr;
+  explicit Scratch(size_t count) { CK(cudaMalloc(&p, count * sizeof(T))); }
+  ~Scratch() { cudaFree(p); }
+  Scratch(const Scratch&) = delete;
+  Scratch& operator=(const Scratch&) = delete;
 };
 
-SelfplayImpl* selfplayCreate(const kgb_selfplay_config& c, int X, int Y, const SelfplayNNBuffers& nn, cudaStream_t stream) {
+// The device twin of the reference's Rand seeded from `seed`
+DevRandState devRandState(const std::string& seed) {
+  RefRand rr(seed);
+  DevRandState st;
+  memset(&st, 0, sizeof(st));
+  uint64_t a[16], idx, pcg;
+  rr.exportState(a, idx, pcg);
+  for(int i = 0; i < 16; i++) st.a[i] = a[i];
+  st.aIdx = idx; st.pcg = pcg;
+  return st;
+}
+
+}  // namespace
+
+// One device loop on an evaluator handle.  Every transfer and launch of the loop goes on the handle's stream, which orders it
+// against the waves (the stream is non-blocking: the legacy default stream would not).
+struct kgb_selfplay {
+  kgb_handle* h = nullptr;
+  SPDev d;
+  std::vector<void*> allocs;
+  int* refused = nullptr;      // games an apply kernel had to leave unchanged
+  cudaGraphExec_t stepGraph = nullptr;
+
+  ~kgb_selfplay() {
+    if(stepGraph) cudaGraphExecDestroy(stepGraph);
+    for(void* p : allocs) cudaFree(p);
+  }
+  template <class T> T* alloc(size_t count) {
+    void* p = nullptr;
+    CK(cudaMalloc(&p, count * sizeof(T)));
+    allocs.push_back(p);
+    fill((T*)p, 0, count);
+    return (T*)p;
+  }
+  // counts are in elements of the device array
+  template <class T> void upload(T* dst, const void* src, size_t count) {
+    CK(cudaMemcpyAsync(dst, src, count * sizeof(T), cudaMemcpyHostToDevice, h->stream));
+  }
+  template <class T> void download(void* dst, const T* src, size_t count) {
+    CK(cudaMemcpyAsync(dst, src, count * sizeof(T), cudaMemcpyDeviceToHost, h->stream));
+    sync();
+  }
+  template <class T> void fill(T* dst, int byte, size_t count) { CK(cudaMemsetAsync(dst, byte, count * sizeof(T), h->stream)); }
+  void sync() { CK(cudaStreamSynchronize(h->stream)); }
+  // What every entry point does first: make the loop's device current and, with `drain`, wait for the waves queued on its stream
+  void enter(bool drain = true) {
+    CK(cudaSetDevice(h->device));
+    if(drain) sync();
+  }
+  void checkGame(int g) const {
+    if(g < 0 || g >= d.numGames) throw std::invalid_argument("selfplay: game index out of range");
+  }
+
+  void launchSelect() {
+    spSelectKernel<<<d.numGames, SP_LADDER_WARPS * 32, 0, h->stream>>>(d);
+    CK(cudaGetLastError());
+  }
+  void launchBackup() {
+    int threads = 128, warpsPerBlock = threads / 32;
+    spBackupKernel<<<(d.numGames + warpsPerBlock - 1) / warpsPerBlock, threads, 0, h->stream>>>(d);
+    CK(cudaGetLastError());
+  }
+  // One wave: select a leaf per game, evaluate the leaves (debug_fake_nn: a stand-in for the net), back up
+  void stepLaunches() {
+    launchSelect();
+    if(d.fakeNN) {
+      int threads = 128, warpsPerBlock = threads / 32;
+      spFakeNNKernel<<<(d.numGames + warpsPerBlock - 1) / warpsPerBlock, threads, 0, h->stream>>>(d, h->dPolicy, h->dValue, h->dScore, h->dOwnership);
+      CK(cudaGetLastError());
+    }
+    else for(auto& op : h->ops) op(d.numGames, h->stream);
+    launchBackup();
+  }
+
+  // The values of each slot's NEXT game have been uploaded; with alsoCurrent `kernel` also gives them to the games in progress.
+  // Games that have already started are left unchanged and reported as "selfplay: <count><refusal>".  threadsPerGame: 32 for a
+  // kernel that runs a warp per game, 1 for a thread per game.
+  void applyNext(bool alsoCurrent, void (*kernel)(const SPDev, int*), int threadsPerGame, const char* refusal) {
+    if(alsoCurrent) {
+      fill(refused, 0, 1);
+      kernel<<<(d.numGames * threadsPerGame + 127) / 128, 128, 0, h->stream>>>(d, refused);
+      CK(cudaGetLastError());
+      int n = 0;
+      download(&n, refused, 1);
+      if(n != 0) throw std::invalid_argument("selfplay: " + std::to_string(n) + refusal);
+    }
+    sync();
+  }
+
+  void playMoves(const int8_t* movesXY, int numMoves, int onlyGame) {
+    if(onlyGame >= d.numGames) throw std::invalid_argument("selfplay: game index out of range");
+    {   // every move must lie on the board of every game it is played on (a game's board can be smaller than the evaluator's frame)
+      std::vector<int> gx((size_t)d.numGames), gy((size_t)d.numGames);
+      download(gx.data(), d.gX, gx.size());
+      download(gy.data(), d.gY, gy.size());
+      for(int g = 0; g < d.numGames; g++) {
+        if(onlyGame >= 0 && g != onlyGame) continue;
+        for(int m = 0; m < numMoves; m++)
+          if(movesXY[2 * m] >= 0 && (movesXY[2 * m] >= gx[g] || movesXY[2 * m + 1] < 0 || movesXY[2 * m + 1] >= gy[g]))
+            throw std::invalid_argument("selfplay: move " + std::to_string(m) + " is off the board of game " + std::to_string(g));
+      }
+    }
+    Scratch<int8_t> dm((size_t)numMoves * 2);
+    upload(dm.p, movesXY, (size_t)numMoves * 2);
+    int threads = 128, warpsPerBlock = threads / 32;
+    spPlayMovesKernel<<<(d.numGames + warpsPerBlock - 1) / warpsPerBlock, threads, 0, h->stream>>>(d, dm.p, numMoves, onlyGame, onlyGame >= 0 ? 1 : 0);
+    CK(cudaGetLastError());
+    sync();
+  }
+};
+
+static void initLoop(kgb_selfplay* sp, const kgb_selfplay_config& c) {
+  const kgb_handle& hd = *sp->h;
+  const int X = hd.L.X, Y = hd.L.Y;
   if(X > 19 || Y > 19 || X < 2 || Y < 2) throw std::invalid_argument("selfplay: board sizes 2..19 only");
   if(c.num_games < 1 || c.max_visits < 2) throw std::invalid_argument("selfplay: num_games >= 1 and max_visits >= 2 required");
-  std::unique_ptr<SelfplayImpl> sp(new SelfplayImpl());
-  sp->stream = stream;
   SPDev& d = sp->d;
   memset(&d, 0, sizeof(d));
   d.X = X; d.Y = Y; d.XY = X * Y; d.policySize = X * Y + 1;
@@ -2282,7 +2429,7 @@ SelfplayImpl* selfplayCreate(const kgb_selfplay_config& c, int X, int Y, const S
   {
     std::vector<float> k((size_t)c.num_games, (float)c.komi);
     d.komiG = sp->alloc<float>(c.num_games); d.nextKomi = sp->alloc<float>(c.num_games); d.lastKomi = sp->alloc<float>(c.num_games);
-    for(float* dst : {d.komiG, d.nextKomi, d.lastKomi}) SPCK(cudaMemcpy(dst, k.data(), k.size() * sizeof(float), cudaMemcpyHostToDevice));
+    for(float* dst : {d.komiG, d.nextKomi, d.lastKomi}) sp->upload(dst, k.data(), k.size());
   }
   {   // every game starts with the frame as its board and the configuration's rules (kgb_selfplay_set_game_setup changes that per game)
     if(c.ko_rule < 0 || c.ko_rule > 3) throw std::invalid_argument("selfplay: ko_rule must be 0 (simple), 1 (positional), 2 (situational) or 3 (spight)");
@@ -2294,11 +2441,11 @@ SelfplayImpl* selfplayCreate(const kgb_selfplay_config& c, int X, int Y, const S
     std::vector<int> one((size_t)G), four((size_t)G * 4);
     for(int k = 0; k < 4; k++) {
       std::fill(one.begin(), one.end(), vals[k]);
-      SPCK(cudaMemcpy(dst[k], one.data(), one.size() * sizeof(int), cudaMemcpyHostToDevice));
+      sp->upload(dst[k], one.data(), one.size());
       for(int g = 0; g < G; g++) four[(size_t)g * 4 + k] = vals[k];
     }
-    SPCK(cudaMemcpy(d.nextSetup, four.data(), four.size() * sizeof(int), cudaMemcpyHostToDevice));
-    SPCK(cudaMemcpy(d.lastSetup, four.data(), four.size() * sizeof(int), cudaMemcpyHostToDevice));
+    sp->upload(d.nextSetup, four.data(), four.size());
+    sp->upload(d.lastSetup, four.data(), four.size());
     // every root gets the full budget and its root parameters unless the host says otherwise (kgb_selfplay_set_next_search_limits)
     d.visitBudget = sp->alloc<int>(G); d.nextBudget = sp->alloc<int>((size_t)G * 2);
     d.plainRoot = sp->alloc<uint8_t>(G); d.nextPlain = sp->alloc<uint8_t>((size_t)G * 2);
@@ -2306,10 +2453,10 @@ SelfplayImpl* selfplayCreate(const kgb_selfplay_config& c, int X, int Y, const S
     d.initMovesLeft = sp->alloc<int>(G); d.nextInitMoves = sp->alloc<int>(G); d.initMoveCount = sp->alloc<int>(G);
     d.initMoves = sp->alloc<int16_t>((size_t)G * SP_MAX_INIT_MOVES);
     d.policyInitTemperature = sp->alloc<double>(1);
-    { const double one = 1.0; SPCK(cudaMemcpy(d.policyInitTemperature, &one, sizeof(double), cudaMemcpyHostToDevice)); }
+    { const double one = 1.0; sp->upload(d.policyInitTemperature, &one, 1); }
     std::vector<int> full((size_t)G * 2, c.max_visits);
-    SPCK(cudaMemcpy(d.visitBudget, full.data(), (size_t)G * sizeof(int), cudaMemcpyHostToDevice));
-    SPCK(cudaMemcpy(d.nextBudget, full.data(), (size_t)G * 2 * sizeof(int), cudaMemcpyHostToDevice));
+    sp->upload(d.visitBudget, full.data(), G);
+    sp->upload(d.nextBudget, full.data(), (size_t)G * 2);
   }
   d.cpuctExploration = c.cpuct_exploration; d.cpuctExplorationLog = c.cpuct_exploration_log; d.cpuctExplorationBase = c.cpuct_exploration_base;
   d.fpuReductionMax = c.fpu_reduction_max; d.rootFpuReductionMax = c.root_fpu_reduction_max;
@@ -2327,7 +2474,7 @@ SelfplayImpl* selfplayCreate(const kgb_selfplay_config& c, int X, int Y, const S
   d.dynamicScoreCenterZeroWeight = c.dynamic_score_center_zero_weight; d.dynamicScoreCenterScale = c.dynamic_score_center_scale;
   d.drawEquivalentWinsForWhite = c.draw_equivalent_wins_for_white;
   if(d.dynamicScoreUtilityFactor != 0.0 && !(d.dynamicScoreCenterScale > 0.0)) throw std::invalid_argument("selfplay: dynamic_score_center_scale must be > 0");
-  d.scoreMeanMultiplier = nn.scoreMeanMultiplier; d.scoreStdevMultiplier = nn.scoreStdevMultiplier; d.leadMultiplier = nn.leadMultiplier;
+  d.scoreMeanMultiplier = hd.model->scoreMeanMultiplier; d.scoreStdevMultiplier = hd.model->scoreStdevMultiplier; d.leadMultiplier = hd.model->leadMultiplier;
   d.seed = c.seed;
   const size_t G = d.numGames, N = d.maxNodes, PS = d.policySize;
   d.rootB = sp->alloc<uint32_t>(G * 32); d.rootW = sp->alloc<uint32_t>(G * 32);
@@ -2345,7 +2492,7 @@ SelfplayImpl* selfplayCreate(const kgb_selfplay_config& c, int X, int Y, const S
   d.ladderNodesPerWave = c.ladder_nodes_per_wave > 0 ? c.ladder_nodes_per_wave : 0;
   d.fixedSymmetryPlusOne = (c.debug_fixed_symmetry_plus_one >= 1 && c.debug_fixed_symmetry_plus_one <= 8) ? c.debug_fixed_symmetry_plus_one : 0;
   d.maxPlayoutsPerWave = c.max_playouts_per_wave > 0 ? c.max_playouts_per_wave : SP_MAX_PLAYOUTS_PER_WAVE;
-  { std::vector<int> kos2(2 * G, -1); SPCK(cudaMemcpy(d.prevKo, kos2.data(), 2 * G * sizeof(int), cudaMemcpyHostToDevice)); }
+  { std::vector<int> kos2(2 * G, -1); sp->upload(d.prevKo, kos2.data(), 2 * G); }
   d.nodeCount = sp->alloc<int>(G); d.nodeVisits = sp->alloc<int>(G * N); 
   d.nodeWeightSum = sp->alloc<double>(G * N); d.nodeWeightSqSum = sp->alloc<double>(G * N); d.nodeUtilAvg = sp->alloc<double>(G * N);
   d.nodeUtilSqAvg = sp->alloc<double>(G * N); d.nodeNNUtil = sp->alloc<double>(G * N); d.nodeNumChildren = sp->alloc<int>(G * N);
@@ -2380,26 +2527,13 @@ SelfplayImpl* selfplayCreate(const kgb_selfplay_config& c, int X, int Y, const S
     // one generator per game, seeded like the reference's Rand from a string (the reference reseeds its search thread's
     // generator for every search from strings the device cannot hash; here the stream simply continues from move to move)
     std::vector<DevRandState> st(G);
-    for(size_t g2 = 0; g2 < G; g2++) {
-      RefRand rr("kgb200$seed" + std::to_string(c.seed) + "$game" + std::to_string(g2) + "$searchThread");
-      memset(&st[g2], 0, sizeof(DevRandState));
-      uint64_t a[16], idx, pcg;
-      rr.exportState(a, idx, pcg);
-      for(int i = 0; i < 16; i++) st[g2].a[i] = a[i];
-      st[g2].aIdx = idx; st[g2].pcg = pcg;
-    }
+    const std::string prefix = "kgb200$seed" + std::to_string(c.seed) + "$game";
+    for(size_t g2 = 0; g2 < G; g2++) st[g2] = devRandState(prefix + std::to_string(g2) + "$searchThread");
     d.searchRand = sp->alloc<DevRandState>(G);
-    SPCK(cudaMemcpy(d.searchRand, st.data(), G * sizeof(DevRandState), cudaMemcpyHostToDevice));
-    for(size_t g2 = 0; g2 < G; g2++) {
-      RefRand rr("kgb200$seed" + std::to_string(c.seed) + "$game" + std::to_string(g2) + "$nonSearchRand");
-      memset(&st[g2], 0, sizeof(DevRandState));
-      uint64_t a[16], idx, pcg;
-      rr.exportState(a, idx, pcg);
-      for(int i = 0; i < 16; i++) st[g2].a[i] = a[i];
-      st[g2].aIdx = idx; st[g2].pcg = pcg;
-    }
+    sp->upload(d.searchRand, st.data(), G);
+    for(size_t g2 = 0; g2 < G; g2++) st[g2] = devRandState(prefix + std::to_string(g2) + "$nonSearchRand");
     d.nonSearchRand = sp->alloc<DevRandState>(G);
-    SPCK(cudaMemcpy(d.nonSearchRand, st.data(), G * sizeof(DevRandState), cudaMemcpyHostToDevice));
+    sp->upload(d.nonSearchRand, st.data(), G);
   }
   d.cacheSize = 0;
   if(c.nn_cache_size_power_of_two > 0) {
@@ -2423,7 +2557,7 @@ SelfplayImpl* selfplayCreate(const kgb_selfplay_config& c, int X, int Y, const S
     const ZobristTables zt = makeZobristTables(X, Y);
     static_assert(sizeof(ZobEntry) == sizeof(Hash128), "layout");
     ZobEntry* dz = sp->alloc<ZobEntry>(zt.board.size());
-    SPCK(cudaMemcpy(dz, zt.board.data(), zt.board.size() * sizeof(ZobEntry), cudaMemcpyHostToDevice));
+    sp->upload(dz, zt.board.data(), zt.board.size());
     d.zob = dz;
   }
   d.biasTableSize = 64;
@@ -2439,492 +2573,581 @@ SelfplayImpl* selfplayCreate(const kgb_selfplay_config& c, int X, int Y, const S
   unsigned long long* stats = sp->alloc<unsigned long long>(16);
   d.totalVisits = stats; d.totalMoves = stats + 1; d.gamesFinished = stats + 2; d.blackWins = stats + 3; d.nodesAllocated = stats + 4;
   d.rootEndingBonusPoints = c.root_ending_bonus_points; d.rootPruneUselessMoves = c.root_prune_useless_moves != 0 ? 1 : 0;
-  d.nnOwnership = nn.ownership;
+  d.nnOwnership = hd.dOwnership;
   d.rootOwnAcc = sp->alloc<float>(G * (size_t)X * Y); d.rootEndBonus = sp->alloc<double>(G * PS); d.rootAllowed = sp->alloc<uint32_t>(G * 32);
   d.passStreak = sp->alloc<int>(G * 2);
-  SPCK(cudaMemset(d.rootAllowed, 0xff, G * 32 * sizeof(uint32_t)));
+  sp->fill(d.rootAllowed, 0xff, G * 32);
   d.dbgCycles = sp->alloc<long long>(G * 8);
   d.rootRow = sp->alloc<float>(G * ((size_t)X * Y * 22 + 19));
   d.sumDepth = stats + 5; d.ladderCounters = stats + 6; d.stalledWaves = stats + 8; d.instantPlayouts = stats + 9; d.cacheHits = stats + 10; d.cacheStores = stats + 11;
-  d.nnSpatial = nn.spatial; d.nnGlobal = nn.global; d.nnOptimism = nn.optimism; d.nnSymmetry = nn.symmetry;
-  d.nnPolicy = nn.policy; d.nnValue = nn.value; d.nnScore = nn.score;
+  d.nnSpatial = hd.dSpatial; d.nnGlobal = hd.dGlobal; d.nnOptimism = hd.dOptimism; d.nnSymmetry = hd.dSymmetry;
+  d.nnPolicy = hd.dPolicy; d.nnValue = hd.dValue; d.nnScore = hd.dScore;
   {
     const std::vector<double> table = makeExpectedSVTable();
     double* dt = sp->alloc<double>(table.size());
-    SPCK(cudaMemcpy(dt, table.data(), table.size() * sizeof(double), cudaMemcpyHostToDevice));
+    sp->upload(dt, table.data(), table.size());
     d.svTable = dt;
     const std::vector<double> cdf = makeValueWeightCdfTable();
     double* dc = sp->alloc<double>(cdf.size());
-    SPCK(cudaMemcpy(dc, cdf.data(), cdf.size() * sizeof(double), cudaMemcpyHostToDevice));
+    sp->upload(dc, cdf.data(), cdf.size());
     d.vwCdfTable = dc;
   }
   d.recentScoreCenter = sp->alloc<double>(G); d.leafTerminalScore = sp->alloc<float>(G);
+  sp->refused = sp->alloc<int>(1);
   // initial state: empty boards, black to move, history empty, one unevaluated root node per game
   std::vector<int> ones(G, 1), minus(G * 5, -1), kos(G, -1);
-  SPCK(cudaMemcpy(d.rootBlackToMove, ones.data(), G * sizeof(int), cudaMemcpyHostToDevice));
-  SPCK(cudaMemcpy(d.nodeCount, ones.data(), G * sizeof(int), cudaMemcpyHostToDevice));
-  SPCK(cudaMemcpy(d.hist, minus.data(), G * 5 * sizeof(int), cudaMemcpyHostToDevice));
-  SPCK(cudaMemcpy(d.rootKo, kos.data(), G * sizeof(int), cudaMemcpyHostToDevice));
-  SPCK(cudaMemset(d.childNode, 0xff, G * N * PS * sizeof(int)));
-  SPCK(cudaDeviceSynchronize());
-  spInitRootsKernel<<<(unsigned)((G * 32 + 127) / 128), 128>>>(d);
-  SPCK(cudaGetLastError());
-  SPCK(cudaDeviceSynchronize());   // the uploads above are not ordered against the (non-blocking) stream the loop runs on
-  return sp.release();
+  sp->upload(d.rootBlackToMove, ones.data(), G);
+  sp->upload(d.nodeCount, ones.data(), G);
+  sp->upload(d.hist, minus.data(), G * 5);
+  sp->upload(d.rootKo, kos.data(), G);
+  sp->fill(d.childNode, 0xff, G * N * PS);
+  spInitRootsKernel<<<(unsigned)((G * 32 + 127) / 128), 128, 0, hd.stream>>>(d);
+  CK(cudaGetLastError());
+  sp->sync();
 }
 
-void selfplayDestroy(SelfplayImpl* sp) { delete sp; }
+// ------------------------------------------------------------------------------------------------------------
+// C ABI of the loop
+// ------------------------------------------------------------------------------------------------------------
+extern "C" {
 
-// After a weight swap (kgb_handle_commit_weights) the cached outputs belong to the previous net: the reference gets the same effect by
-// giving every NNEvaluator its own NNCacheTable (nneval.cpp:129-130).  Ordered on the wave stream.
-void selfplayClearNNCache(SelfplayImpl* sp, cudaStream_t s) {
-  SPDev& d = sp->d;
-  if(d.cacheSize <= 0) return;
-  SPCK(cudaMemsetAsync(d.cacheKey0, 0, (size_t)d.cacheSize * sizeof(unsigned long long), s));
-  SPCK(cudaMemsetAsync(d.cacheKey1, 0, (size_t)d.cacheSize * sizeof(unsigned long long), s));
+KGB_API int kgb_selfplay_create(kgb_handle* handle, const kgb_selfplay_config* config, kgb_selfplay** out) {
+  return guarded([&] {
+    if(!handle || !config || !out) throw std::invalid_argument("kgb_selfplay_create: NULL argument");
+    if(config->num_games > handle->maxBatch) throw std::invalid_argument("kgb_selfplay_create: num_games exceeds the handle's max_batch_size");
+    if(!handle->nhwc) throw std::invalid_argument("kgb_selfplay_create: the handle must be created with inputs_nhwc = 1");
+    if(handle->model->numInputChannels != 22 || handle->model->numInputGlobalChannels != 19)
+      throw std::invalid_argument("kgb_selfplay_create: the device loop writes V7 features (22 spatial, 19 global)");
+    CK(cudaSetDevice(handle->device));
+    std::unique_ptr<kgb_selfplay> sp(new kgb_selfplay());
+    sp->h = handle;
+    initLoop(sp.get(), *config);
+    *out = sp.release();
+  });
 }
 
-void selfplayLaunchSelect(SelfplayImpl* sp, cudaStream_t s) {
-  spSelectKernel<<<sp->d.numGames, SP_LADDER_WARPS * 32, 0, s>>>(sp->d);
-  SPCK(cudaGetLastError());
-}
-void selfplayLaunchBackup(SelfplayImpl* sp, cudaStream_t s) {
-  int threads = 128, warpsPerBlock = threads / 32;
-  spBackupKernel<<<(sp->d.numGames + warpsPerBlock - 1) / warpsPerBlock, threads, 0, s>>>(sp->d);
-  SPCK(cudaGetLastError());
+KGB_API void kgb_selfplay_free(kgb_selfplay* sp) { delete sp; }
+
+KGB_API int kgb_selfplay_run(kgb_selfplay* sp, int steps) {
+  return guarded([&] {
+    if(!sp || steps < 0) throw std::invalid_argument("kgb_selfplay_run: bad argument");
+    sp->enter(false);
+    if(!sp->stepGraph) sp->stepGraph = captureGraph(sp->h->stream, [&] { sp->stepLaunches(); });
+    for(int i = 0; i < steps; i++) CK(cudaGraphLaunch(sp->stepGraph, sp->h->stream));
+  });
 }
 
-void selfplayLaunchFakeNN(SelfplayImpl* sp, float* policyOut, float* valueOut, float* scoreOut, float* ownershipOut, cudaStream_t s) {
-  int threads = 128, warpsPerBlock = threads / 32;
-  spFakeNNKernel<<<(sp->d.numGames + warpsPerBlock - 1) / warpsPerBlock, threads, 0, s>>>(sp->d, policyOut, valueOut, scoreOut, ownershipOut);
-  SPCK(cudaGetLastError());
+KGB_API int kgb_selfplay_set_search_rand(kgb_selfplay* sp, const char* seed_string) {
+  return guarded([&] {
+    if(!sp || !seed_string) throw std::invalid_argument("kgb_selfplay_set_search_rand: NULL argument");
+    sp->enter();
+    const std::vector<DevRandState> all(sp->d.numGames, devRandState(seed_string));
+    sp->upload(sp->d.searchRand, all.data(), all.size());
+    sp->sync();
+  });
 }
 
-void selfplayPlayMoves(SelfplayImpl* sp, const int8_t* movesXY, int numMoves, cudaStream_t s, int onlyGame) {
-  if(onlyGame >= sp->d.numGames) throw std::invalid_argument("selfplay: game index out of range");
-  {   // every move must lie on the board of every game it is played on (a game's board can be smaller than the evaluator's frame)
-    std::vector<int> gx((size_t)sp->d.numGames), gy((size_t)sp->d.numGames);
-    SPCK(cudaMemcpy(gx.data(), sp->d.gX, gx.size() * sizeof(int), cudaMemcpyDeviceToHost));
-    SPCK(cudaMemcpy(gy.data(), sp->d.gY, gy.size() * sizeof(int), cudaMemcpyDeviceToHost));
-    for(int g = 0; g < sp->d.numGames; g++) {
-      if(onlyGame >= 0 && g != onlyGame) continue;
-      for(int m = 0; m < numMoves; m++)
-        if(movesXY[2 * m] >= 0 && (movesXY[2 * m] >= gx[g] || movesXY[2 * m + 1] < 0 || movesXY[2 * m + 1] >= gy[g]))
-          throw std::invalid_argument("selfplay: move " + std::to_string(m) + " is off the board of game " + std::to_string(g));
-    }
-  }
-  int8_t* dm = nullptr;
-  SPCK(cudaMalloc(&dm, (size_t)numMoves * 2));
-  SPCK(cudaMemcpyAsync(dm, movesXY, (size_t)numMoves * 2, cudaMemcpyHostToDevice, s));
-  int threads = 128, warpsPerBlock = threads / 32;
-  spPlayMovesKernel<<<(sp->d.numGames + warpsPerBlock - 1) / warpsPerBlock, threads, 0, s>>>(sp->d, dm, numMoves, onlyGame, onlyGame >= 0 ? 1 : 0);
-  cudaError_t e = cudaStreamSynchronize(s);
-  cudaFree(dm);
-  SPCK(e);
+KGB_API int kgb_selfplay_random_openings(kgb_selfplay* sp, int max_moves) {
+  return guarded([&] {
+    if(!sp || max_moves < 0) throw std::invalid_argument("kgb_selfplay_random_openings: bad argument");
+    sp->enter(false);
+    spRandomOpeningsKernel<<<(sp->d.numGames * 32 + 127) / 128, 128, 0, sp->h->stream>>>(sp->d, max_moves);
+    CK(cudaGetLastError());
+    sp->sync();
+  });
 }
 
-void selfplaySetSearchRand(SelfplayImpl* sp, const char* seedString) {
-  RefRand rr(seedString);
-  DevRandState st;
-  memset(&st, 0, sizeof(st));
-  uint64_t a[16], idx, pcg;
-  rr.exportState(a, idx, pcg);
-  for(int i = 0; i < 16; i++) st.a[i] = a[i];
-  st.aIdx = idx; st.pcg = pcg;
-  std::vector<DevRandState> all(sp->d.numGames, st);
-  SPCK(cudaMemcpy(sp->d.searchRand, all.data(), all.size() * sizeof(DevRandState), cudaMemcpyHostToDevice));
-  SPCK(cudaDeviceSynchronize());
+KGB_API int kgb_selfplay_get_stats(kgb_selfplay* sp, kgb_selfplay_stats* out) {
+  return guarded([&] {
+    if(!sp || !out) throw std::invalid_argument("kgb_selfplay_get_stats: NULL argument");
+    sp->enter();
+    unsigned long long h[16];
+    sp->download(h, sp->d.totalVisits, 16);
+    out->total_visits = h[0]; out->total_moves = h[1]; out->games_finished = h[2]; out->black_wins = h[3];
+    out->nodes_allocated = h[4]; out->sum_leaf_depth = h[5]; out->ladder_searches = h[6]; out->ladder_nodes = h[7];
+    out->stalled_waves = h[8]; out->instant_playouts = h[9]; out->nn_cache_hits = h[10]; out->nn_cache_stores = h[11];
+  });
 }
 
-void selfplayRandomOpenings(SelfplayImpl* sp, int maxLen, cudaStream_t s) {
-  spRandomOpeningsKernel<<<(sp->d.numGames * 32 + 127) / 128, 128, 0, s>>>(sp->d, maxLen);
-  SPCK(cudaGetLastError());
-  SPCK(cudaStreamSynchronize(s));
+KGB_API int kgb_selfplay_get_game(kgb_selfplay* sp, int game, uint8_t* colors, int32_t* info) {
+  return guarded([&] {
+    if(!sp || !colors || !info) throw std::invalid_argument("kgb_selfplay_get_game: NULL argument");
+    sp->enter();
+    const SPDev& d = sp->d;
+    const int g = game;
+    sp->checkGame(g);
+    uint32_t b[32], w[32];
+    sp->download(b, d.rootB + (size_t)g * 32, 32);
+    sp->download(w, d.rootW + (size_t)g * 32, 32);
+    for(int y = 0; y < d.Y; y++)
+      for(int x = 0; x < d.X; x++) colors[y * d.X + x] = (b[y] >> x) & 1 ? 1 : (w[y] >> x) & 1 ? 2 : 0;
+    sp->download(&info[0], d.moveNum + g, 1);
+    sp->download(&info[1], d.rootBlackToMove + g, 1);
+    sp->download(&info[2], d.rootKo + g, 1);
+    sp->download(&info[3], d.rootCapB + g, 1);
+    sp->download(&info[4], d.rootCapW + g, 1);
+    sp->download(&info[5], d.nodeVisits + (size_t)g * d.maxNodes, 1);
+  });
+}
+
+KGB_API int kgb_selfplay_get_root_children(kgb_selfplay* sp, int game, int32_t* visits, float* policy, double* util_sum) {
+  return guarded([&] {
+    if(!sp || !visits || !policy || !util_sum) throw std::invalid_argument("kgb_selfplay_get_root_children: NULL argument");
+    sp->enter();
+    const SPDev& d = sp->d;
+    sp->checkGame(game);
+    const size_t nb = (size_t)game * d.maxNodes * d.policySize;
+    sp->download(visits, d.childVisits + nb, d.policySize);
+    sp->download(policy, d.policy + nb, d.policySize);
+    std::vector<int> child(d.policySize);
+    std::vector<double> avg(d.maxNodes);
+    sp->download(child.data(), d.childNode + nb, d.policySize);
+    sp->download(avg.data(), d.nodeUtilAvg + (size_t)game * d.maxNodes, d.maxNodes);
+    for(int i = 0; i < d.policySize; i++) util_sum[i] = child[i] >= 0 ? avg[child[i]] : 0.0;
+  });
+}
+
+KGB_API int kgb_selfplay_get_root_value_stats(kgb_selfplay* sp, int game, double* child_stats, double* root_stats) {
+  return guarded([&] {
+    if(!sp || !child_stats || !root_stats) throw std::invalid_argument("kgb_selfplay_get_root_value_stats: NULL argument");
+    sp->enter();
+    const SPDev& d = sp->d;
+    sp->checkGame(game);
+    std::vector<int> child(d.policySize);
+    std::vector<double> mom((size_t)d.maxNodes * 5);
+    sp->download(child.data(), d.childNode + (size_t)game * d.maxNodes * d.policySize, d.policySize);
+    sp->download(mom.data(), d.nodeMoments + (size_t)game * d.maxNodes * 5, mom.size());
+    for(int i = 0; i < d.policySize; i++)
+      for(int k = 0; k < 5; k++) child_stats[i * 5 + k] = child[i] >= 0 ? mom[(size_t)child[i] * 5 + k] : 0.0;
+    for(int k = 0; k < 5; k++) root_stats[k] = mom[k];
+  });
 }
 
 // Komi per game (GameInitializer draws one per game: program/play.cpp:330-420 komiMean / komiStdev / ...).  `komi[numGames]` becomes
-// the komi of each slot's NEXT game; with alsoCurrent it also replaces the komi of the game in progress (meant for games that have
-// not started searching).  The host must have synchronised the wave stream.
-void selfplaySetKomi(SelfplayImpl* sp, const float* komi, bool alsoCurrent) {
-  const SPDev& d = sp->d;
-  for(int g = 0; g < d.numGames; g++)
-    if(!(komi[g] >= -150.0f && komi[g] <= 150.0f) || komi[g] * 2.0f != floorf(komi[g] * 2.0f))
-      throw std::invalid_argument("selfplay: komi must be a multiple of 0.5 in [-150, 150] (Rules::komiIsIntOrHalfInt)");
-  SPCK(cudaMemcpy(d.nextKomi, komi, (size_t)d.numGames * sizeof(float), cudaMemcpyHostToDevice));
-  if(alsoCurrent) SPCK(cudaMemcpy(d.komiG, komi, (size_t)d.numGames * sizeof(float), cudaMemcpyHostToDevice));
-}
-void selfplayReadLeafKey(SelfplayImpl* sp, int g, unsigned long long* key2) {
-  const SPDev& d = sp->d;
-  if(g < 0 || g >= d.numGames) throw std::invalid_argument("selfplay: game index out of range");
-  SPCK(cudaMemcpy(key2, d.leafKey + (size_t)g * 2, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-}
-void selfplayReadKomi(SelfplayImpl* sp, float* current, float* lastFinished) {
-  const SPDev& d = sp->d;
-  if(current) SPCK(cudaMemcpy(current, d.komiG, (size_t)d.numGames * sizeof(float), cudaMemcpyDeviceToHost));
-  if(lastFinished) SPCK(cudaMemcpy(lastFinished, d.lastKomi, (size_t)d.numGames * sizeof(float), cudaMemcpyDeviceToHost));
+// the komi of each slot's NEXT game; with also_current_games it also replaces the komi of the game in progress (meant for games that
+// have not started searching).
+KGB_API int kgb_selfplay_set_komi(kgb_selfplay* sp, const float* komi, int also_current_games) {
+  return guarded([&] {
+    if(!sp || !komi) throw std::invalid_argument("kgb_selfplay_set_komi: NULL argument");
+    sp->enter();
+    const SPDev& d = sp->d;
+    for(int g = 0; g < d.numGames; g++)
+      if(!(komi[g] >= -150.0f && komi[g] <= 150.0f) || komi[g] * 2.0f != floorf(komi[g] * 2.0f))
+        throw std::invalid_argument("selfplay: komi must be a multiple of 0.5 in [-150, 150] (Rules::komiIsIntOrHalfInt)");
+    sp->upload(d.nextKomi, komi, d.numGames);
+    if(also_current_games) sp->upload(d.komiG, komi, d.numGames);
+    sp->sync();
+  });
 }
 
-// Board size and ko / suicide rules per game (GameInitializer::createGameSharedUnsynchronized, program/play.cpp:330-650: bSizes /
-// bSizeRelProbs, koRules, multiStoneSuicideLegals drawn per game).  setup[numGames][4] = X, Y, ko rule, multi-stone suicide: taken by each slot's
-// NEXT game; with alsoCurrent also by the game in progress, which must not have started (no move played, root not searched) - its history
-// restarts under the new rules.  Ko rules other than the loop's own need full_history_rules (BoardHistory's lists are per game already).
-__global__ void spApplySetupKernel(const SPDev d, int* refused) {
-  const int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if(g >= d.numGames) return;
-  const size_t gb = (size_t)g * d.maxNodes;
-  if(d.moveNum[g] != 0 || d.nodeVisits[gb] != 0 || d.rootSymCount[g] != 0 || d.ladPending[g] != 0) { if(lane == 0) atomicAdd(refused, 1); return; }
-  __syncwarp();
-  if(lane == 0) { d.gX[g] = d.nextSetup[g * 4 + 0]; d.gY[g] = d.nextSetup[g * 4 + 1]; d.gKoRule[g] = d.nextSetup[g * 4 + 2]; d.gMultiSuicide[g] = d.nextSetup[g * 4 + 3]; }
-  __syncwarp();
-  gameHistReset(d, g, lane);
-  __syncwarp();
-  rootHashesInit(d, g, lane);
-}
-void selfplaySetGameSetup(SelfplayImpl* sp, const int* setup, bool alsoCurrent, cudaStream_t s) {
-  const SPDev& d = sp->d;
-  for(int g = 0; g < d.numGames; g++) {
-    const int* q = setup + (size_t)g * 4;
-    if(q[0] < 2 || q[0] > d.X || q[1] < 2 || q[1] > d.Y) throw std::invalid_argument("selfplay: a game's board must be at least 2x2 and fit the evaluator's frame");
-    if(q[2] < 0 || q[2] > 3) throw std::invalid_argument("selfplay: ko_rule must be 0 (simple), 1 (positional), 2 (situational) or 3 (spight)");
-    if(q[2] != d.koRule && !d.histRules) throw std::invalid_argument("selfplay: per-game ko rules need full_history_rules = 1 (or a superko rule) in the loop's configuration");
-    if(q[3] != 0 && q[3] != 1) throw std::invalid_argument("selfplay: multi_stone_suicide_legal must be 0 or 1");
-  }
-  SPCK(cudaMemcpy(d.nextSetup, setup, (size_t)d.numGames * 4 * sizeof(int), cudaMemcpyHostToDevice));
-  if(!alsoCurrent) return;
-  int* refused = nullptr;
-  SPCK(cudaMalloc(&refused, sizeof(int)));
-  SPCK(cudaMemsetAsync(refused, 0, sizeof(int), s));
-  spApplySetupKernel<<<(d.numGames * 32 + 127) / 128, 128, 0, s>>>(d, refused);
-  int h = 0;
-  cudaError_t e = cudaMemcpyAsync(&h, refused, sizeof(int), cudaMemcpyDeviceToHost, s);
-  if(e == cudaSuccess) e = cudaStreamSynchronize(s);
-  cudaFree(refused);
-  SPCK(e);
-  if(h != 0) throw std::invalid_argument("selfplay: " + std::to_string(h) + " game(s) in progress have already started; their setup was left unchanged");
-}
-// Search limits of the roots to come (getSearchLimitsThisMove, program/play.cpp:1093-1223: cheap searches, reduced visits).  visits[numGames][2],
-// plain[numGames][2] (may be NULL = all 0): index 0 applies to the root after the slot's next move when the game goes on, index 1 when that
-// move ends the game (first root of the slot's next game).  alsoCurrent: index 0 also replaces the limits of the current roots, which
-// must not have been searched yet.
-__global__ void spApplyLimitsKernel(const SPDev d, int* refused) {
-  const int g = blockIdx.x * blockDim.x + threadIdx.x;
-  if(g >= d.numGames) return;
-  if(d.nodeVisits[(size_t)g * d.maxNodes] != 0 || d.rootSymCount[g] != 0) { atomicAdd(refused, 1); return; }
-  d.visitBudget[g] = d.nextBudget[g * 2]; d.plainRoot[g] = d.nextPlain[g * 2];
-}
-void selfplaySetNextSearchLimits(SelfplayImpl* sp, const int* visits, const uint8_t* plain, bool alsoCurrent, cudaStream_t s) {
-  const SPDev& d = sp->d;
-  for(int i = 0; i < d.numGames * 2; i++)
-    if(visits[i] < 2 || visits[i] > d.maxVisits) throw std::invalid_argument("selfplay: a visit budget must lie between 2 and max_visits");
-  SPCK(cudaMemcpy(d.nextBudget, visits, (size_t)d.numGames * 2 * sizeof(int), cudaMemcpyHostToDevice));
-  if(plain) SPCK(cudaMemcpy(d.nextPlain, plain, (size_t)d.numGames * 2, cudaMemcpyHostToDevice));
-  else SPCK(cudaMemset(d.nextPlain, 0, (size_t)d.numGames * 2));
-  if(!alsoCurrent) return;
-  int* refused = nullptr;
-  SPCK(cudaMalloc(&refused, sizeof(int)));
-  SPCK(cudaMemsetAsync(refused, 0, sizeof(int), s));
-  spApplyLimitsKernel<<<(d.numGames + 127) / 128, 128, 0, s>>>(d, refused);
-  int h = 0;
-  cudaError_t e = cudaMemcpyAsync(&h, refused, sizeof(int), cudaMemcpyDeviceToHost, s);
-  if(e == cudaSuccess) e = cudaStreamSynchronize(s);
-  cudaFree(refused);
-  SPCK(e);
-  if(h != 0) throw std::invalid_argument("selfplay: " + std::to_string(h) + " root(s) have already been searched; their limits were left unchanged");
-}
-// Policy-initialised openings (PlaySettings::initGamesWithPolicy / policyInitAreaProp / policyInitAreaTemperature; playutils.cpp:232-266): moves[numGames] =
-// how many opening moves each slot's NEXT game draws from the raw policy before its first searched move (the host draws the count: floor of an
-// exponential with mean area * policyInitAreaProp).  alsoCurrent: the games in progress take them too; they must not have started.
-__global__ void spApplyPolicyInitKernel(const SPDev d, int* refused) {
-  const int g = blockIdx.x * blockDim.x + threadIdx.x;
-  if(g >= d.numGames) return;
-  if(d.moveNum[g] != 0 || d.nodeVisits[(size_t)g * d.maxNodes] != 0 || d.rootSymCount[g] != 0) { atomicAdd(refused, 1); return; }
-  d.initMovesLeft[g] = d.nextInitMoves[g]; d.initMoveCount[g] = 0;
-  if(d.initMovesLeft[g] > 0) { d.visitBudget[g] = 1; d.plainRoot[g] = 1; }
-}
-void selfplaySetPolicyInit(SelfplayImpl* sp, const int* moves, double temperature, bool alsoCurrent, cudaStream_t s) {
-  const SPDev& d = sp->d;
-  if(!(temperature > 0.0 && temperature < 10.0)) throw std::invalid_argument("selfplay: policy init temperature must lie in (0, 10)");
-  for(int g = 0; g < d.numGames; g++)
-    if(moves[g] < 0) throw std::invalid_argument("selfplay: negative number of opening moves");
-  SPCK(cudaMemcpy(d.policyInitTemperature, &temperature, sizeof(double), cudaMemcpyHostToDevice));
-  SPCK(cudaMemcpy(d.nextInitMoves, moves, (size_t)d.numGames * sizeof(int), cudaMemcpyHostToDevice));
-  if(!alsoCurrent) return;
-  int* refused = nullptr;
-  SPCK(cudaMalloc(&refused, sizeof(int)));
-  SPCK(cudaMemsetAsync(refused, 0, sizeof(int), s));
-  spApplyPolicyInitKernel<<<(d.numGames + 127) / 128, 128, 0, s>>>(d, refused);
-  int h = 0;
-  cudaError_t e = cudaMemcpyAsync(&h, refused, sizeof(int), cudaMemcpyDeviceToHost, s);
-  if(e == cudaSuccess) e = cudaStreamSynchronize(s);
-  cudaFree(refused);
-  SPCK(e);
-  if(h != 0) throw std::invalid_argument("selfplay: " + std::to_string(h) + " game(s) in progress have already started; their openings were left unchanged");
-}
-// movesLeft[numGames]: opening moves still to be drawn (> 0 = the slot is not a recorded turn yet); count / moves[numGames][maxMoves]: the opening played so far
-// in the current game (move positions, pass = policy size - 1).  Any pointer may be NULL.
-void selfplayReadPolicyInit(SelfplayImpl* sp, int* movesLeft, int* count, int16_t* moves, int maxMoves) {
-  const SPDev& d = sp->d;
-  if(movesLeft) SPCK(cudaMemcpy(movesLeft, d.initMovesLeft, (size_t)d.numGames * sizeof(int), cudaMemcpyDeviceToHost));
-  if(count) SPCK(cudaMemcpy(count, d.initMoveCount, (size_t)d.numGames * sizeof(int), cudaMemcpyDeviceToHost));
-  if(moves) {
-    if(maxMoves < 1 || maxMoves > SP_MAX_INIT_MOVES) throw std::invalid_argument("selfplay: max_moves must lie in 1..512");
-    SPCK(cudaMemcpy2D(moves, (size_t)maxMoves * sizeof(int16_t), d.initMoves, (size_t)SP_MAX_INIT_MOVES * sizeof(int16_t), (size_t)maxMoves * sizeof(int16_t),
-                      (size_t)d.numGames, cudaMemcpyDeviceToHost));
-  }
-}
-
-void selfplayReadSymmetries(SelfplayImpl* sp, int* out) {
-  SPCK(cudaMemcpy(out, sp->d.nnSymmetry, (size_t)sp->d.numGames * sizeof(int), cudaMemcpyDeviceToHost));
-}
-void selfplayReadRootRawEntropy(SelfplayImpl* sp, double* out) {
-  SPCK(cudaMemcpy(out, sp->d.rootRawEntropy, (size_t)sp->d.numGames * sizeof(double), cudaMemcpyDeviceToHost));
-}
-void selfplayReadSearchLimits(SelfplayImpl* sp, int* visits, uint8_t* plain) {
-  const SPDev& d = sp->d;
-  if(visits) SPCK(cudaMemcpy(visits, d.visitBudget, (size_t)d.numGames * sizeof(int), cudaMemcpyDeviceToHost));
-  if(plain) SPCK(cudaMemcpy(plain, d.plainRoot, (size_t)d.numGames, cudaMemcpyDeviceToHost));
-}
-
-void selfplayReadGameSetup(SelfplayImpl* sp, int* current, int* lastFinished) {
-  const SPDev& d = sp->d;
-  if(current) {
-    std::vector<int> a((size_t)d.numGames);
-    int* const src[4] = {d.gX, d.gY, d.gKoRule, d.gMultiSuicide};
-    for(int k = 0; k < 4; k++) {
-      SPCK(cudaMemcpy(a.data(), src[k], a.size() * sizeof(int), cudaMemcpyDeviceToHost));
-      for(int g = 0; g < d.numGames; g++) current[(size_t)g * 4 + k] = a[g];
+KGB_API int kgb_selfplay_set_game_setup(kgb_selfplay* sp, const int32_t* setup, int also_current_games) {
+  return guarded([&] {
+    if(!sp || !setup) throw std::invalid_argument("kgb_selfplay_set_game_setup: NULL argument");
+    sp->enter();
+    const SPDev& d = sp->d;
+    for(int g = 0; g < d.numGames; g++) {
+      const int* q = setup + (size_t)g * 4;
+      if(q[0] < 2 || q[0] > d.X || q[1] < 2 || q[1] > d.Y) throw std::invalid_argument("selfplay: a game's board must be at least 2x2 and fit the evaluator's frame");
+      if(q[2] < 0 || q[2] > 3) throw std::invalid_argument("selfplay: ko_rule must be 0 (simple), 1 (positional), 2 (situational) or 3 (spight)");
+      if(q[2] != d.koRule && !d.histRules) throw std::invalid_argument("selfplay: per-game ko rules need full_history_rules = 1 (or a superko rule) in the loop's configuration");
+      if(q[3] != 0 && q[3] != 1) throw std::invalid_argument("selfplay: multi_stone_suicide_legal must be 0 or 1");
     }
-  }
-  if(lastFinished) SPCK(cudaMemcpy(lastFinished, d.lastSetup, (size_t)d.numGames * 4 * sizeof(int), cudaMemcpyDeviceToHost));
+    sp->upload(d.nextSetup, setup, (size_t)d.numGames * 4);
+    sp->applyNext(also_current_games != 0, spApplySetupKernel, 32, " game(s) in progress have already started; their setup was left unchanged");
+  });
 }
 
-void selfplayReadRootRow(SelfplayImpl* sp, int g, float* spatial, float* global) {
-  const size_t n = (size_t)sp->d.XY * 22;
-  SPCK(cudaMemcpy(spatial, sp->d.rootRow + (size_t)g * (n + 19), n * sizeof(float), cudaMemcpyDeviceToHost));
-  SPCK(cudaMemcpy(global, sp->d.rootRow + (size_t)g * (n + 19) + n, 19 * sizeof(float), cudaMemcpyDeviceToHost));
+KGB_API int kgb_selfplay_set_next_search_limits(kgb_selfplay* sp, const int32_t* visits, const uint8_t* plain_root, int also_current_roots) {
+  return guarded([&] {
+    if(!sp || !visits) throw std::invalid_argument("kgb_selfplay_set_next_search_limits: NULL argument");
+    sp->enter();
+    const SPDev& d = sp->d;
+    for(int i = 0; i < d.numGames * 2; i++)
+      if(visits[i] < 2 || visits[i] > d.maxVisits) throw std::invalid_argument("selfplay: a visit budget must lie between 2 and max_visits");
+    sp->upload(d.nextBudget, visits, (size_t)d.numGames * 2);
+    if(plain_root) sp->upload(d.nextPlain, plain_root, (size_t)d.numGames * 2);
+    else sp->fill(d.nextPlain, 0, (size_t)d.numGames * 2);
+    sp->applyNext(also_current_roots != 0, spApplyLimitsKernel, 1, " root(s) have already been searched; their limits were left unchanged");
+  });
 }
 
-void selfplayReadDebugCycles(SelfplayImpl* sp, long long* out /*[numGames][8]*/, bool clear) {
-  SPCK(cudaMemcpy(out, sp->d.dbgCycles, (size_t)sp->d.numGames * 8 * sizeof(long long), cudaMemcpyDeviceToHost));
-  if(clear) SPCK(cudaMemset(sp->d.dbgCycles, 0, (size_t)sp->d.numGames * 8 * sizeof(long long)));
+KGB_API int kgb_selfplay_get_search_limits(kgb_selfplay* sp, int32_t* visits, uint8_t* plain_root) {
+  return guarded([&] {
+    if(!sp) throw std::invalid_argument("kgb_selfplay_get_search_limits: NULL argument");
+    sp->enter();
+    if(visits) sp->download(visits, sp->d.visitBudget, sp->d.numGames);
+    if(plain_root) sp->download(plain_root, sp->d.plainRoot, sp->d.numGames);
+  });
 }
 
-void selfplayReadStats(SelfplayImpl* sp, kgb_selfplay_stats* out) {
-  unsigned long long h[16];
-  SPCK(cudaMemcpy(h, sp->d.totalVisits, sizeof(h), cudaMemcpyDeviceToHost));
-  out->total_visits = h[0]; out->total_moves = h[1]; out->games_finished = h[2]; out->black_wins = h[3];
-  out->nodes_allocated = h[4]; out->sum_leaf_depth = h[5]; out->ladder_searches = h[6]; out->ladder_nodes = h[7];
-  out->stalled_waves = h[8]; out->instant_playouts = h[9]; out->nn_cache_hits = h[10]; out->nn_cache_stores = h[11];
+KGB_API int kgb_selfplay_set_policy_init(kgb_selfplay* sp, const int32_t* num_moves, double temperature, int also_current_games) {
+  return guarded([&] {
+    if(!sp || !num_moves) throw std::invalid_argument("kgb_selfplay_set_policy_init: NULL argument");
+    sp->enter();
+    const SPDev& d = sp->d;
+    if(!(temperature > 0.0 && temperature < 10.0)) throw std::invalid_argument("selfplay: policy init temperature must lie in (0, 10)");
+    for(int g = 0; g < d.numGames; g++)
+      if(num_moves[g] < 0) throw std::invalid_argument("selfplay: negative number of opening moves");
+    sp->upload(d.policyInitTemperature, &temperature, 1);
+    sp->upload(d.nextInitMoves, num_moves, d.numGames);
+    sp->applyNext(also_current_games != 0, spApplyPolicyInitKernel, 1, " game(s) in progress have already started; their openings were left unchanged");
+  });
 }
 
-void selfplayReadRootMoments(SelfplayImpl* sp, int g, double* childMoments /*[policySize][5]*/, double* rootMoments /*[5]*/) {
-  const SPDev& d = sp->d;
-  if(g < 0 || g >= d.numGames) throw std::invalid_argument("selfplay: game index out of range");
-  std::vector<int> child(d.policySize);
-  std::vector<double> mom((size_t)d.maxNodes * 5);
-  SPCK(cudaMemcpy(child.data(), d.childNode + (size_t)g * d.maxNodes * d.policySize, d.policySize * sizeof(int), cudaMemcpyDeviceToHost));
-  SPCK(cudaMemcpy(mom.data(), d.nodeMoments + (size_t)g * d.maxNodes * 5, mom.size() * sizeof(double), cudaMemcpyDeviceToHost));
-  for(int i = 0; i < d.policySize; i++)
-    for(int k = 0; k < 5; k++) childMoments[i * 5 + k] = child[i] >= 0 ? mom[(size_t)child[i] * 5 + k] : 0.0;
-  for(int k = 0; k < 5; k++) rootMoments[k] = mom[k];
+// moves_left[numGames]: opening moves still to be drawn (> 0 = the slot is not a recorded turn yet); count / moves[numGames][max_moves]: the
+// opening played so far in the current game (move positions, pass = policy size - 1).  Any pointer may be NULL.
+KGB_API int kgb_selfplay_get_policy_init(kgb_selfplay* sp, int32_t* moves_left, int32_t* count, int16_t* moves, int max_moves) {
+  return guarded([&] {
+    if(!sp) throw std::invalid_argument("kgb_selfplay_get_policy_init: NULL argument");
+    sp->enter();
+    const SPDev& d = sp->d;
+    if(moves_left) sp->download(moves_left, d.initMovesLeft, d.numGames);
+    if(count) sp->download(count, d.initMoveCount, d.numGames);
+    if(moves) {
+      if(max_moves < 1 || max_moves > SP_MAX_INIT_MOVES) throw std::invalid_argument("selfplay: max_moves must lie in 1..512");
+      CK(cudaMemcpy2DAsync(moves, (size_t)max_moves * sizeof(int16_t), d.initMoves, (size_t)SP_MAX_INIT_MOVES * sizeof(int16_t),
+                           (size_t)max_moves * sizeof(int16_t), (size_t)d.numGames, cudaMemcpyDeviceToHost, sp->h->stream));
+      sp->sync();
+    }
+  });
+}
+
+KGB_API int kgb_selfplay_get_nn_symmetries(kgb_selfplay* sp, int32_t* symmetries) {
+  return guarded([&] {
+    if(!sp || !symmetries) throw std::invalid_argument("kgb_selfplay_get_nn_symmetries: NULL argument");
+    sp->enter();
+    sp->download(symmetries, sp->d.nnSymmetry, sp->d.numGames);
+  });
+}
+
+KGB_API int kgb_selfplay_get_root_raw_policy_entropy(kgb_selfplay* sp, double* entropy) {
+  return guarded([&] {
+    if(!sp || !entropy) throw std::invalid_argument("kgb_selfplay_get_root_raw_policy_entropy: NULL argument");
+    sp->enter();
+    sp->download(entropy, sp->d.rootRawEntropy, sp->d.numGames);
+  });
+}
+
+KGB_API int kgb_selfplay_get_game_setup(kgb_selfplay* sp, int32_t* current, int32_t* last_finished) {
+  return guarded([&] {
+    if(!sp) throw std::invalid_argument("kgb_selfplay_get_game_setup: NULL argument");
+    sp->enter();
+    const SPDev& d = sp->d;
+    if(current) {
+      std::vector<int> a((size_t)d.numGames);
+      int* const src[4] = {d.gX, d.gY, d.gKoRule, d.gMultiSuicide};
+      for(int k = 0; k < 4; k++) {
+        sp->download(a.data(), src[k], a.size());
+        for(int g = 0; g < d.numGames; g++) current[(size_t)g * 4 + k] = a[g];
+      }
+    }
+    if(last_finished) sp->download(last_finished, d.lastSetup, (size_t)d.numGames * 4);
+  });
+}
+
+KGB_API int kgb_selfplay_get_komi(kgb_selfplay* sp, float* current, float* last_finished) {
+  return guarded([&] {
+    if(!sp) throw std::invalid_argument("kgb_selfplay_get_komi: NULL argument");
+    sp->enter();
+    if(current) sp->download(current, sp->d.komiG, sp->d.numGames);
+    if(last_finished) sp->download(last_finished, sp->d.lastKomi, sp->d.numGames);
+  });
+}
+
+KGB_API int kgb_selfplay_get_leaf_cache_key(kgb_selfplay* sp, int game, uint64_t* key2) {
+  return guarded([&] {
+    if(!sp || !key2) throw std::invalid_argument("kgb_selfplay_get_leaf_cache_key: NULL argument");
+    sp->enter();
+    sp->checkGame(game);
+    sp->download(key2, sp->d.leafKey + (size_t)game * 2, 2);
+  });
+}
+
+// After a weight swap (kgb_handle_commit_weights) the cached outputs belong to the previous net: the reference gets the same effect by
+// giving every NNEvaluator its own NNCacheTable (nneval.cpp:129-130).  Ordered on the wave stream.
+KGB_API int kgb_selfplay_clear_nn_cache(kgb_selfplay* sp) {
+  return guarded([&] {
+    if(!sp) throw std::invalid_argument("kgb_selfplay_clear_nn_cache: NULL argument");
+    sp->enter(false);
+    if(sp->d.cacheSize <= 0) return;
+    sp->fill(sp->d.cacheKey0, 0, sp->d.cacheSize);
+    sp->fill(sp->d.cacheKey1, 0, sp->d.cacheSize);
+  });
 }
 
 // ---- game recording support (hold mode) ------------------------------------------------------------------------------------------
-void selfplayRelease(SelfplayImpl* sp, const uint8_t* mask /*[numGames] or NULL = all*/) {
-  const SPDev& d = sp->d;
-  if(mask) SPCK(cudaMemcpy(d.releaseFlag, mask, d.numGames, cudaMemcpyHostToDevice));
-  else SPCK(cudaMemset(d.releaseFlag, 1, d.numGames));
-  SPCK(cudaDeviceSynchronize());   // the loop's stream does not synchronise with the default stream these ran on
+KGB_API int kgb_selfplay_release(kgb_selfplay* sp, const uint8_t* games_mask /*[numGames] or NULL = all*/) {
+  return guarded([&] {
+    if(!sp) throw std::invalid_argument("kgb_selfplay_release: NULL argument");
+    sp->enter();
+    if(games_mask) sp->upload(sp->d.releaseFlag, games_mask, sp->d.numGames);
+    else sp->fill(sp->d.releaseFlag, 1, sp->d.numGames);
+    sp->sync();
+  });
 }
 
-void selfplayReadRootVisitsAll(SelfplayImpl* sp, int* out /*[numGames]*/) {
-  const SPDev& d = sp->d;
-  SPCK(cudaMemcpy2D(out, sizeof(int), d.nodeVisits, (size_t)d.maxNodes * sizeof(int), sizeof(int), d.numGames, cudaMemcpyDeviceToHost));
+KGB_API int kgb_selfplay_get_root_visits(kgb_selfplay* sp, int32_t* visits /*[numGames]*/) {
+  return guarded([&] {
+    if(!sp || !visits) throw std::invalid_argument("kgb_selfplay_get_root_visits: NULL argument");
+    sp->enter();
+    const SPDev& d = sp->d;
+    CK(cudaMemcpy2DAsync(visits, sizeof(int), d.nodeVisits, (size_t)d.maxNodes * sizeof(int), sizeof(int), d.numGames, cudaMemcpyDeviceToHost,
+                         sp->h->stream));
+    sp->sync();
+  });
 }
 
 // Visits of the root's child NODES by move position (0 where there is no child; under graph search a node's visits can exceed its
 // edge's) and the root's own evaluation: winLoss, noResult, scoreMean, scoreMeanSq, lead (white's perspective).
-void selfplayReadRootExtra(SelfplayImpl* sp, int g, int* childNodeVisits, double* rootNN) {
-  const SPDev& d = sp->d;
-  if(g < 0 || g >= d.numGames) throw std::invalid_argument("selfplay: game index out of range");
-  std::vector<int> child(d.policySize), nv(d.maxNodes);
-  SPCK(cudaMemcpy(child.data(), d.childNode + (size_t)g * d.maxNodes * d.policySize, d.policySize * sizeof(int), cudaMemcpyDeviceToHost));
-  SPCK(cudaMemcpy(nv.data(), d.nodeVisits + (size_t)g * d.maxNodes, d.maxNodes * sizeof(int), cudaMemcpyDeviceToHost));
-  for(int i = 0; i < d.policySize; i++) childNodeVisits[i] = child[i] >= 0 ? nv[child[i]] : 0;
-  SPCK(cudaMemcpy(rootNN, d.nodeNNMoments + (size_t)g * d.maxNodes * 5, 5 * sizeof(double), cudaMemcpyDeviceToHost));
+KGB_API int kgb_selfplay_get_root_extra(kgb_selfplay* sp, int game, int32_t* child_node_visits, double* root_nn_stats) {
+  return guarded([&] {
+    if(!sp || !child_node_visits || !root_nn_stats) throw std::invalid_argument("kgb_selfplay_get_root_extra: NULL argument");
+    sp->enter();
+    const SPDev& d = sp->d;
+    sp->checkGame(game);
+    std::vector<int> child(d.policySize), nv(d.maxNodes);
+    sp->download(child.data(), d.childNode + (size_t)game * d.maxNodes * d.policySize, d.policySize);
+    sp->download(nv.data(), d.nodeVisits + (size_t)game * d.maxNodes, d.maxNodes);
+    for(int i = 0; i < d.policySize; i++) child_node_visits[i] = child[i] >= 0 ? nv[child[i]] : 0;
+    sp->download(root_nn_stats, d.nodeNNMoments + (size_t)game * d.maxNodes * 5, 5);
+  });
 }
 
 // The last root move of game slot g: info[4] = move position (X*Y = pass), flags (1 it ended the game | 2 without result | 4 by the
 // move limit), the move number it was played at, the slot's game index; when it ended the game also the final score (white minus
 // black, komi included), the final position and its area (0 none, 1 black, 2 white).
-void selfplayReadLastMove(SelfplayImpl* sp, int g, int* info, float* score, uint8_t* finalColors, uint8_t* finalArea) {
-  const SPDev& d = sp->d;
-  if(g < 0 || g >= d.numGames) throw std::invalid_argument("selfplay: game index out of range");
-  SPCK(cudaMemcpy(info, d.lastMove + (size_t)g * 4, 4 * sizeof(int), cudaMemcpyDeviceToHost));
-  SPCK(cudaMemcpy(score, d.lastScore + g, sizeof(float), cudaMemcpyDeviceToHost));
-  uint32_t fb[128];
-  SPCK(cudaMemcpy(fb, d.finalBoard + (size_t)g * 128, sizeof(fb), cudaMemcpyDeviceToHost));
-  for(int y = 0; y < d.Y; y++)
-    for(int x = 0; x < d.X; x++) {
-      finalColors[y * d.X + x] = (fb[y] >> x) & 1 ? 1 : (fb[32 + y] >> x) & 1 ? 2 : 0;
-      finalArea[y * d.X + x] = (fb[64 + y] >> x) & 1 ? 1 : (fb[96 + y] >> x) & 1 ? 2 : 0;
+KGB_API int kgb_selfplay_get_last_move(kgb_selfplay* sp, int game, int32_t* info, float* final_score, uint8_t* final_colors, uint8_t* final_area) {
+  return guarded([&] {
+    if(!sp || !info || !final_score || !final_colors || !final_area) throw std::invalid_argument("kgb_selfplay_get_last_move: NULL argument");
+    sp->enter();
+    const SPDev& d = sp->d;
+    sp->checkGame(game);
+    sp->download(info, d.lastMove + (size_t)game * 4, 4);
+    sp->download(final_score, d.lastScore + game, 1);
+    uint32_t fb[128];
+    sp->download(fb, d.finalBoard + (size_t)game * 128, 128);
+    for(int y = 0; y < d.Y; y++)
+      for(int x = 0; x < d.X; x++) {
+        final_colors[y * d.X + x] = (fb[y] >> x) & 1 ? 1 : (fb[32 + y] >> x) & 1 ? 2 : 0;
+        final_area[y * d.X + x] = (fb[64 + y] >> x) & 1 ? 1 : (fb[96 + y] >> x) & 1 ? 2 : 0;
+      }
+  });
+}
+
+KGB_API int kgb_selfplay_get_nn_row(kgb_selfplay* sp, int game, float* spatial, float* global) {
+  return guarded([&] {
+    if(!sp || !spatial || !global || game < 0 || game >= sp->d.numGames) throw std::invalid_argument("kgb_selfplay_get_nn_row: bad argument");
+    sp->enter();
+    const size_t XY = (size_t)sp->h->L.X * sp->h->L.Y;
+    sp->download(spatial, sp->h->dSpatial + (size_t)game * XY * 22, XY * 22);
+    sp->download(global, sp->h->dGlobal + (size_t)game * 19, 19);
+  });
+}
+
+KGB_API int kgb_selfplay_get_root_row(kgb_selfplay* sp, int game, float* spatial, float* global) {
+  return guarded([&] {
+    if(!sp || !spatial || !global || game < 0 || game >= sp->d.numGames) throw std::invalid_argument("kgb_selfplay_get_root_row: bad argument");
+    sp->enter();
+    const size_t n = (size_t)sp->d.XY * 22;
+    sp->download(spatial, sp->d.rootRow + (size_t)game * (n + 19), n);
+    sp->download(global, sp->d.rootRow + (size_t)game * (n + 19) + n, 19);
+  });
+}
+
+KGB_API int kgb_selfplay_get_leaf_path(kgb_selfplay* sp, int game, int32_t* moves_xy, int32_t max_len, int32_t* len_out, int32_t* valid_out) {
+  return guarded([&] {
+    if(!sp || !moves_xy || !len_out || !valid_out || max_len < 0) throw std::invalid_argument("kgb_selfplay_get_leaf_path: bad argument");
+    sp->enter();
+    const SPDev& d = sp->d;
+    sp->checkGame(game);
+    int len = 0;
+    sp->download(&len, d.pathLen + game, 1);
+    sp->download(valid_out, d.leafValid + game, 1);
+    std::vector<int> mv(len > 0 ? len : 1);
+    if(len > 0) sp->download(mv.data(), d.pathMove + (size_t)game * d.maxDepth, len);
+    for(int i = 0; i < len && i < max_len; i++) {
+      const bool pass = mv[i] == d.policySize - 1;
+      moves_xy[2 * i] = pass ? -1 : mv[i] % d.X; moves_xy[2 * i + 1] = pass ? -1 : mv[i] / d.X;
     }
+    *len_out = len;
+  });
 }
 
-int selfplayReadLeafPath(SelfplayImpl* sp, int g, int* movesXY, int maxLen, int* valid) {
-  const SPDev& d = sp->d;
-  if(g < 0 || g >= d.numGames) throw std::invalid_argument("selfplay: game index out of range");
-  int len = 0;
-  SPCK(cudaMemcpy(&len, d.pathLen + g, sizeof(int), cudaMemcpyDeviceToHost));
-  SPCK(cudaMemcpy(valid, d.leafValid + g, sizeof(int), cudaMemcpyDeviceToHost));
-  std::vector<int> mv(len > 0 ? len : 1);
-  if(len > 0) SPCK(cudaMemcpy(mv.data(), d.pathMove + (size_t)g * d.maxDepth, len * sizeof(int), cudaMemcpyDeviceToHost));
-  for(int i = 0; i < len && i < maxLen; i++) {
-    const bool pass = mv[i] == d.policySize - 1;
-    movesXY[2 * i] = pass ? -1 : mv[i] % d.X; movesXY[2 * i + 1] = pass ? -1 : mv[i] / d.X;
-  }
-  return len;
+KGB_API int kgb_selfplay_play_moves(kgb_selfplay* sp, const int8_t* moves_xy, int num_moves) {
+  return guarded([&] {
+    if(!sp || (!moves_xy && num_moves > 0) || num_moves < 0) throw std::invalid_argument("kgb_selfplay_play_moves: bad argument");
+    sp->enter(false);
+    sp->playMoves(moves_xy, num_moves, -1);
+  });
 }
 
-void selfplayReadGame(SelfplayImpl* sp, int g, uint8_t* colors, int* info) {
-  const SPDev& d = sp->d;
-  if(g < 0 || g >= d.numGames) throw std::invalid_argument("selfplay: game index out of range");
-  uint32_t b[32], w[32];
-  SPCK(cudaMemcpy(b, d.rootB + (size_t)g * 32, sizeof(b), cudaMemcpyDeviceToHost));
-  SPCK(cudaMemcpy(w, d.rootW + (size_t)g * 32, sizeof(w), cudaMemcpyDeviceToHost));
-  for(int y = 0; y < d.Y; y++)
-    for(int x = 0; x < d.X; x++) colors[y * d.X + x] = (b[y] >> x) & 1 ? 1 : (w[y] >> x) & 1 ? 2 : 0;
-  int h[6];
-  SPCK(cudaMemcpy(&h[0], d.moveNum + g, sizeof(int), cudaMemcpyDeviceToHost));
-  SPCK(cudaMemcpy(&h[1], d.rootBlackToMove + g, sizeof(int), cudaMemcpyDeviceToHost));
-  SPCK(cudaMemcpy(&h[2], d.rootKo + g, sizeof(int), cudaMemcpyDeviceToHost));
-  SPCK(cudaMemcpy(&h[3], d.rootCapB + g, sizeof(int), cudaMemcpyDeviceToHost));
-  SPCK(cudaMemcpy(&h[4], d.rootCapW + g, sizeof(int), cudaMemcpyDeviceToHost));
-  SPCK(cudaMemcpy(&h[5], d.nodeVisits + (size_t)g * d.maxNodes, sizeof(int), cudaMemcpyDeviceToHost));
-  for(int i = 0; i < 6; i++) info[i] = h[i];
+KGB_API int kgb_selfplay_play_moves_game(kgb_selfplay* sp, int game, const int8_t* moves_xy, int num_moves) {
+  return guarded([&] {
+    if(!sp || game < 0 || (!moves_xy && num_moves > 0) || num_moves < 0) throw std::invalid_argument("kgb_selfplay_play_moves_game: bad argument");
+    sp->enter();
+    sp->playMoves(moves_xy, num_moves, game);
+  });
 }
 
-void selfplayReadRootChildren(SelfplayImpl* sp, int g, int* visits, float* policy, double* utilSum) {
-  const SPDev& d = sp->d;
-  if(g < 0 || g >= d.numGames) throw std::invalid_argument("selfplay: game index out of range");
-  size_t nb = (size_t)g * d.maxNodes * d.policySize;
-  SPCK(cudaMemcpy(visits, d.childVisits + nb, d.policySize * sizeof(int), cudaMemcpyDeviceToHost));
-  SPCK(cudaMemcpy(policy, d.policy + nb, d.policySize * sizeof(float), cudaMemcpyDeviceToHost));
-  std::vector<int> child(d.policySize);
-  std::vector<double> avg(d.maxNodes);
-  SPCK(cudaMemcpy(child.data(), d.childNode + nb, d.policySize * sizeof(int), cudaMemcpyDeviceToHost));
-  SPCK(cudaMemcpy(avg.data(), d.nodeUtilAvg + (size_t)g * d.maxNodes, d.maxNodes * sizeof(double), cudaMemcpyDeviceToHost));
-  for(int i = 0; i < d.policySize; i++) utilSum[i] = child[i] >= 0 ? avg[child[i]] : 0.0;
+KGB_API int kgb_selfplay_get_play_selection_values(kgb_selfplay* sp, int game, double* values) {
+  return guarded([&] {
+    if(!sp || !values) throw std::invalid_argument("kgb_selfplay_get_play_selection_values: NULL argument");
+    sp->enter();
+    sp->checkGame(game);
+    Scratch<double> out(sp->d.policySize);
+    playSelectionKernel<<<1, 32, 0, sp->h->stream>>>(sp->d, game, out.p);
+    CK(cudaGetLastError());
+    sp->download(values, out.p, sp->d.policySize);
+  });
 }
 
-void selfplayReadPlaySelection(SelfplayImpl* sp, int g, double* out) {
-  const SPDev& d = sp->d;
-  if(g < 0 || g >= d.numGames) throw std::invalid_argument("selfplay: game index out of range");
-  double* dout;
-  SPCK(cudaMalloc(&dout, d.policySize * sizeof(double)));
-  playSelectionKernel<<<1, 32>>>(d, g, dout);
-  cudaError_t e = cudaDeviceSynchronize();
-  if(e == cudaSuccess) e = cudaMemcpy(out, dout, d.policySize * sizeof(double), cudaMemcpyDeviceToHost);
-  cudaFree(dout);
-  SPCK(e);
+KGB_API int kgb_selfplay_time_tree_kernels(kgb_selfplay* sp, int iters, float* ms_select, float* ms_backup) {
+  return guarded([&] {
+    if(!sp || iters < 1 || !ms_select || !ms_backup) throw std::invalid_argument("kgb_selfplay_time_tree_kernels: bad argument");
+    sp->enter();
+    cudaStream_t s = sp->h->stream;
+    cudaEvent_t e0, e1, e2;
+    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1)); CK(cudaEventCreate(&e2));
+    float accS = 0.f, accB = 0.f;
+    for(int i = 0; i < iters; i++) {   // the evaluator outputs of the last wave are reused: the trees keep growing normally
+      CK(cudaEventRecord(e0, s));
+      sp->launchSelect();
+      CK(cudaEventRecord(e1, s));
+      sp->launchBackup();
+      CK(cudaEventRecord(e2, s));
+      sp->sync();
+      float a = 0.f, b = 0.f;
+      CK(cudaEventElapsedTime(&a, e0, e1)); CK(cudaEventElapsedTime(&b, e1, e2));
+      accS += a; accB += b;
+    }
+    cudaEventDestroy(e0); cudaEventDestroy(e1); cudaEventDestroy(e2);
+    *ms_select = accS / iters; *ms_backup = accB / iters;
+  });
 }
 
-void chooseIndexTest(const char* seedString, const double* probs, int n, double temperature, double onlyBelowProb, int count, int* out) {
-  RefRand rr(seedString);
-  DevRandState st;
-  memset(&st, 0, sizeof(st));
-  uint64_t a[16], idx, pcg;
-  rr.exportState(a, idx, pcg);
-  for(int i = 0; i < 16; i++) st.a[i] = a[i];
-  st.aIdx = idx; st.pcg = pcg;
-  DevRandState* ds; double *dp, *dscr; int* dout;
-  SPCK(cudaMalloc(&ds, sizeof(st))); SPCK(cudaMalloc(&dp, n * sizeof(double))); SPCK(cudaMalloc(&dscr, n * sizeof(double))); SPCK(cudaMalloc(&dout, count * sizeof(int)));
-  SPCK(cudaMemcpy(ds, &st, sizeof(st), cudaMemcpyHostToDevice));
-  SPCK(cudaMemcpy(dp, probs, n * sizeof(double), cudaMemcpyHostToDevice));
-  chooseIndexTestKernel<<<1, 32>>>(ds, dp, n, temperature, onlyBelowProb, count, dout, dscr);
-  cudaError_t e = cudaDeviceSynchronize();
-  if(e == cudaSuccess) e = cudaMemcpy(out, dout, count * sizeof(int), cudaMemcpyDeviceToHost);
-  cudaFree(ds); cudaFree(dp); cudaFree(dscr); cudaFree(dout);
-  SPCK(e);
+KGB_API int kgb_selfplay_debug_cycles(kgb_selfplay* sp, int64_t* cycles /*[numGames][8]*/, int clear) {
+  return guarded([&] {
+    if(!sp || !cycles) throw std::invalid_argument("kgb_selfplay_debug_cycles: NULL argument");
+    sp->enter();
+    sp->download(cycles, sp->d.dbgCycles, (size_t)sp->d.numGames * 8);
+    if(clear) {
+      sp->fill(sp->d.dbgCycles, 0, (size_t)sp->d.numGames * 8);
+      sp->sync();
+    }
+  });
 }
 
-void historyReplay(int X, int Y, int koRule, int multiSuicide, int numGames, int maxMoves, const int8_t* moves, uint8_t* flags, uint8_t* legal,
-                   uint8_t* banned) {
-  if(X > 19 || Y > 19 || X < 2 || Y < 2) throw std::invalid_argument("history replay: board sizes 2..19 only");
-  const size_t nm = (size_t)numGames * maxMoves, cells = nm * X * Y;
-  int8_t* dMoves; uint8_t *dFlags, *dLegal, *dBanned; unsigned long long* dLists; ZobEntry* dZob;
-  const ZobristTables zt = makeZobristTables(X, Y);
-  SPCK(cudaMalloc(&dMoves, nm * 2)); SPCK(cudaMalloc(&dFlags, nm)); SPCK(cudaMalloc(&dLegal, cells)); SPCK(cudaMalloc(&dBanned, cells));
-  SPCK(cudaMalloc(&dLists, (size_t)numGames * 3 * (maxMoves + 2) * sizeof(unsigned long long))); SPCK(cudaMalloc(&dZob, zt.board.size() * sizeof(ZobEntry)));
-  SPCK(cudaMemcpy(dMoves, moves, nm * 2, cudaMemcpyHostToDevice));
-  SPCK(cudaMemcpy(dZob, zt.board.data(), zt.board.size() * sizeof(ZobEntry), cudaMemcpyHostToDevice));
-  SPCK(cudaMemset(dFlags, 0, nm)); SPCK(cudaMemset(dLegal, 0, cells)); SPCK(cudaMemset(dBanned, 0, cells));
-  historyReplayKernel<<<(numGames * 32 + 127) / 128, 128>>>(X, Y, koRule, multiSuicide, numGames, maxMoves, dMoves, dZob, dLists, dFlags, dLegal, dBanned);
-  cudaError_t e = cudaDeviceSynchronize();
-  if(e == cudaSuccess) { cudaMemcpy(flags, dFlags, nm, cudaMemcpyDeviceToHost); cudaMemcpy(legal, dLegal, cells, cudaMemcpyDeviceToHost); cudaMemcpy(banned, dBanned, cells, cudaMemcpyDeviceToHost); }
-  cudaFree(dMoves); cudaFree(dFlags); cudaFree(dLegal); cudaFree(dBanned); cudaFree(dLists); cudaFree(dZob);
-  SPCK(e);
+KGB_API int kgb_selfplay_launches_per_step(const kgb_selfplay* sp) { return sp ? sp->h->launchesPerForward + 2 : 0; }
+
+// ---- test hooks of the loop's device code: no handle, so on the default stream -------------------------------------------------
+KGB_API int kgb_test_choose_index_with_temperature(const char* seed_string, const double* relative_probs, int n, double temperature,
+                                                   double only_below_prob, int count, int32_t* chosen) {
+  return guarded([&] {
+    if(!seed_string || !relative_probs || !chosen || n < 1 || count < 1) throw std::invalid_argument("kgb_test_choose_index_with_temperature: bad argument");
+    const DevRandState st = devRandState(seed_string);
+    Scratch<DevRandState> ds(1);
+    Scratch<double> dp(n), dscr(n);
+    Scratch<int> dout(count);
+    CK(cudaMemcpy(ds.p, &st, sizeof(st), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(dp.p, relative_probs, n * sizeof(double), cudaMemcpyHostToDevice));
+    chooseIndexTestKernel<<<1, 32>>>(ds.p, dp.p, n, temperature, only_below_prob, count, dout.p, dscr.p);
+    CK(cudaGetLastError());
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpy(chosen, dout.p, count * sizeof(int), cudaMemcpyDeviceToHost));
+  });
 }
 
-void repBoundTest(int X, int Y, int numMoves, int bound, const int8_t* moves, uint8_t* out) {
-  int8_t* dm; uint8_t* dout;
-  SPCK(cudaMalloc(&dm, (size_t)numMoves * 3)); SPCK(cudaMalloc(&dout, numMoves));
-  SPCK(cudaMemcpy(dm, moves, (size_t)numMoves * 3, cudaMemcpyHostToDevice));
-  repBoundKernel<<<1, 32>>>(X, Y, numMoves, bound, dm, dout);
-  cudaError_t e = cudaDeviceSynchronize();
-  if(e == cudaSuccess) e = cudaMemcpy(out, dout, numMoves, cudaMemcpyDeviceToHost);
-  cudaFree(dm); cudaFree(dout);
-  SPCK(e);
+KGB_API int kgb_test_history_replay(int x_len, int y_len, int ko_rule, int multi_stone_suicide_legal, int num_games, int max_moves, const int8_t* moves_xy,
+                                    uint8_t* flags, uint8_t* legal_next, uint8_t* super_ko_banned) {
+  return guarded([&] {
+    if(!moves_xy || !flags || !legal_next || !super_ko_banned || num_games < 1 || max_moves < 1 || ko_rule < 0 || ko_rule > 3)
+      throw std::invalid_argument("kgb_test_history_replay: bad argument");
+    const int X = x_len, Y = y_len;
+    if(X > 19 || Y > 19 || X < 2 || Y < 2) throw std::invalid_argument("history replay: board sizes 2..19 only");
+    const size_t nm = (size_t)num_games * max_moves, cells = nm * X * Y;
+    const ZobristTables zt = makeZobristTables(X, Y);
+    Scratch<int8_t> dMoves(nm * 2);
+    Scratch<uint8_t> dFlags(nm), dLegal(cells), dBanned(cells);
+    Scratch<unsigned long long> dLists((size_t)num_games * 3 * (max_moves + 2));
+    Scratch<ZobEntry> dZob(zt.board.size());
+    CK(cudaMemcpy(dMoves.p, moves_xy, nm * 2, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(dZob.p, zt.board.data(), zt.board.size() * sizeof(ZobEntry), cudaMemcpyHostToDevice));
+    CK(cudaMemset(dFlags.p, 0, nm)); CK(cudaMemset(dLegal.p, 0, cells)); CK(cudaMemset(dBanned.p, 0, cells));
+    historyReplayKernel<<<(num_games * 32 + 127) / 128, 128>>>(X, Y, ko_rule, multi_stone_suicide_legal, num_games, max_moves, dMoves.p, dZob.p,
+                                                               dLists.p, dFlags.p, dLegal.p, dBanned.p);
+    CK(cudaGetLastError());
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpy(flags, dFlags.p, nm, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(legal_next, dLegal.p, cells, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(super_ko_banned, dBanned.p, cells, cudaMemcpyDeviceToHost));
+  });
 }
 
-void rootNoiseTest(const char* seedString, int X, int Y, int policySize, int turnNumber, int noise, double concentration, double weight,
-                   double temperature, double temperatureEarly, double halflife, const float* policyIn, float* policyOut) {
-  RefRand rr(seedString);
-  DevRandState st;
-  memset(&st, 0, sizeof(st));
-  uint64_t a[16], idx, pcg;
-  rr.exportState(a, idx, pcg);
-  for(int i = 0; i < 16; i++) st.a[i] = a[i];
-  st.aIdx = idx; st.pcg = pcg;
-  float* dp; DevRandState* ds; double* dr;
-  SPCK(cudaMalloc(&dp, policySize * sizeof(float))); SPCK(cudaMalloc(&ds, sizeof(st))); SPCK(cudaMalloc(&dr, 3 * policySize * sizeof(double)));
-  SPCK(cudaMemcpy(dp, policyIn, policySize * sizeof(float), cudaMemcpyHostToDevice));
-  SPCK(cudaMemcpy(ds, &st, sizeof(st), cudaMemcpyHostToDevice));
-  rootNoiseTestKernel<<<1, 32>>>(dp, policySize, X, Y, turnNumber, noise, concentration, weight, temperature, temperatureEarly, halflife, ds, dr);
-  cudaError_t e = cudaDeviceSynchronize();
-  if(e == cudaSuccess) e = cudaMemcpy(policyOut, dp, policySize * sizeof(float), cudaMemcpyDeviceToHost);
-  cudaFree(dp); cudaFree(ds); cudaFree(dr);
-  SPCK(e);
+KGB_API int kgb_test_repetition_bound(int x_len, int y_len, int num_moves, int bound, const int8_t* moves_xyp, uint8_t* out) {
+  return guarded([&] {
+    if(!moves_xyp || !out || num_moves < 1) throw std::invalid_argument("kgb_test_repetition_bound: bad argument");
+    Scratch<int8_t> dm((size_t)num_moves * 3);
+    Scratch<uint8_t> dout(num_moves);
+    CK(cudaMemcpy(dm.p, moves_xyp, (size_t)num_moves * 3, cudaMemcpyHostToDevice));
+    repBoundKernel<<<1, 32>>>(x_len, y_len, num_moves, bound, dm.p, dout.p);
+    CK(cudaGetLastError());
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpy(out, dout.p, num_moves, cudaMemcpyDeviceToHost));
+  });
 }
 
-void boardReplay(int X, int Y, int numBoards, int numMoves, int multiSuicide, const int8_t* moves, uint8_t* colors, int8_t* ko, int16_t* caps,
-                 uint8_t* libClass, uint8_t* legalNext, uint64_t* posHash, uint8_t* area) {
-  if(X > 19 || Y > 19 || X < 2 || Y < 2) throw std::invalid_argument("board replay: board sizes 2..19 only");
-  size_t nm = (size_t)numBoards * numMoves, cells = nm * X * Y;
-  int8_t *dMoves, *dKo; uint8_t *dColors, *dLib, *dLegal; int16_t* dCaps;
-  SPCK(cudaMalloc(&dMoves, nm * 3)); SPCK(cudaMalloc(&dKo, nm * 2)); SPCK(cudaMalloc(&dCaps, nm * 2 * sizeof(int16_t)));
-  SPCK(cudaMalloc(&dColors, cells)); SPCK(cudaMalloc(&dLib, cells)); SPCK(cudaMalloc(&dLegal, cells));
-  SPCK(cudaMemcpy(dMoves, moves, nm * 3, cudaMemcpyHostToDevice));
-  ZobristTables zt = makeZobristTables(X, Y);
-  ZobEntry* dZob; unsigned long long* dHash; uint8_t* dArea;
-  SPCK(cudaMalloc(&dZob, zt.board.size() * sizeof(ZobEntry))); SPCK(cudaMalloc(&dHash, nm * 2 * sizeof(unsigned long long)));
-  SPCK(cudaMalloc(&dArea, cells));
-  static_assert(sizeof(ZobEntry) == sizeof(Hash128), "layout");
-  SPCK(cudaMemcpy(dZob, zt.board.data(), zt.board.size() * sizeof(ZobEntry), cudaMemcpyHostToDevice));
-  int threads = 128;
-  boardReplayKernel<<<(numBoards * 32 + threads - 1) / threads, threads>>>(X, Y, numBoards, numMoves, multiSuicide, dMoves, dColors, dKo, dCaps, dLib, dLegal,
-                                                                           dZob, zt.sizeHash.h0, zt.sizeHash.h1, dHash, dArea);
-  cudaError_t e = cudaDeviceSynchronize();
-  if(e == cudaSuccess) { cudaMemcpy(posHash, dHash, nm * 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost); cudaMemcpy(area, dArea, cells, cudaMemcpyDeviceToHost); }
-  cudaFree(dZob); cudaFree(dHash); cudaFree(dArea);
-  if(e == cudaSuccess) {
-    cudaMemcpy(colors, dColors, cells, cudaMemcpyDeviceToHost); cudaMemcpy(libClass, dLib, cells, cudaMemcpyDeviceToHost);
-    cudaMemcpy(legalNext, dLegal, cells, cudaMemcpyDeviceToHost); cudaMemcpy(ko, dKo, nm * 2, cudaMemcpyDeviceToHost);
-    cudaMemcpy(caps, dCaps, nm * 2 * sizeof(int16_t), cudaMemcpyDeviceToHost);
-  }
-  cudaFree(dMoves); cudaFree(dKo); cudaFree(dCaps); cudaFree(dColors); cudaFree(dLib); cudaFree(dLegal);
-  SPCK(e);
+KGB_API int kgb_test_root_policy_noise(const char* seed_string, int x_len, int y_len, int policy_size, int turn_number, int noise_enabled,
+                                       double concentration, double weight, double temperature, double temperature_early, double halflife,
+                                       const float* policy_in, float* policy_out) {
+  return guarded([&] {
+    if(!seed_string || !policy_in || !policy_out || policy_size < 1 || policy_size > 362) throw std::invalid_argument("kgb_test_root_policy_noise: bad argument");
+    const DevRandState st = devRandState(seed_string);
+    Scratch<float> dp(policy_size);
+    Scratch<DevRandState> ds(1);
+    Scratch<double> dr(3 * (size_t)policy_size);
+    CK(cudaMemcpy(dp.p, policy_in, policy_size * sizeof(float), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(ds.p, &st, sizeof(st), cudaMemcpyHostToDevice));
+    rootNoiseTestKernel<<<1, 32>>>(dp.p, policy_size, x_len, y_len, turn_number, noise_enabled, concentration, weight, temperature, temperature_early,
+                                   halflife, ds.p, dr.p);
+    CK(cudaGetLastError());
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpy(policy_out, dp.p, policy_size * sizeof(float), cudaMemcpyDeviceToHost));
+  });
 }
 
-}  // namespace kgb
+KGB_API int kgb_test_board_replay(int x_size, int y_size, int num_boards, int num_moves, int multi_stone_suicide_legal, const int8_t* moves,
+                                  uint8_t* colors, int8_t* ko, int16_t* caps, uint8_t* lib_class, uint8_t* legal_next, uint64_t* pos_hash, uint8_t* area) {
+  return guarded([&] {
+    if(!moves || !colors || !ko || !caps || !lib_class || !legal_next || !pos_hash || !area || num_boards < 1 || num_moves < 1)
+      throw std::invalid_argument("kgb_test_board_replay: bad argument");
+    int count = 0;
+    if(cudaGetDeviceCount(&count) != cudaSuccess || count == 0) throw CudaFailure("libkgb200: no CUDA device is visible");
+    const int X = x_size, Y = y_size;
+    if(X > 19 || Y > 19 || X < 2 || Y < 2) throw std::invalid_argument("board replay: board sizes 2..19 only");
+    const size_t nm = (size_t)num_boards * num_moves, cells = nm * X * Y;
+    const ZobristTables zt = makeZobristTables(X, Y);
+    static_assert(sizeof(ZobEntry) == sizeof(Hash128), "layout");
+    Scratch<int8_t> dMoves(nm * 3), dKo(nm * 2);
+    Scratch<int16_t> dCaps(nm * 2);
+    Scratch<uint8_t> dColors(cells), dLib(cells), dLegal(cells), dArea(cells);
+    Scratch<ZobEntry> dZob(zt.board.size());
+    Scratch<unsigned long long> dHash(nm * 2);
+    CK(cudaMemcpy(dMoves.p, moves, nm * 3, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(dZob.p, zt.board.data(), zt.board.size() * sizeof(ZobEntry), cudaMemcpyHostToDevice));
+    int threads = 128;
+    boardReplayKernel<<<(num_boards * 32 + threads - 1) / threads, threads>>>(X, Y, num_boards, num_moves, multi_stone_suicide_legal, dMoves.p, dColors.p,
+                                                                               dKo.p, dCaps.p, dLib.p, dLegal.p, dZob.p, zt.sizeHash.h0, zt.sizeHash.h1,
+                                                                               dHash.p, dArea.p);
+    CK(cudaGetLastError());
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpy(pos_hash, dHash.p, nm * 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(area, dArea.p, cells, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(colors, dColors.p, cells, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(lib_class, dLib.p, cells, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(legal_next, dLegal.p, cells, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(ko, dKo.p, nm * 2, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(caps, dCaps.p, nm * 2 * sizeof(int16_t), cudaMemcpyDeviceToHost));
+  });
+}
+
+}  // extern "C"
