@@ -167,7 +167,8 @@ typedef struct kgb_selfplay_config {
   double win_loss_utility_factor;    /* winLossUtilityFactor   (1.0) */
   double no_result_utility_for_white;
   uint64_t seed;
-  int32_t debug_fake_nn;             /* TEST ONLY: replace the evaluator by the deterministic hash net of oracle/ref_driver.cpp */
+  int32_t debug_fake_nn;             /* TEST ONLY: replace the evaluator by the deterministic hash net of oracle/ref_driver.cpp; 1 = short-term
+                                        error channels 0 (its default), 2 = hash-derived raw values there (tests/cpp/uncertainty_search_driver.cpp) */
   int32_t disable_ladder_features;   /* 1 = leave NN input planes 14-17 zero (timing experiments only) */
   int32_t ladder_nodes_per_wave;     /* > 0: each of a game's 8 ladder-reader warps plays at most this many search moves per wave;
                                         a game whose searches are unfinished skips the wave (no visit) and resumes in the next.
@@ -234,6 +235,19 @@ typedef struct kgb_selfplay_config {
                                                      utility unless they capture / touch the opponent / connect groups that are not pass-alive
                                                      (Search::getEndingWhiteScoreBonus, searchhelpers.cpp:351-420; area scoring).  Needs the
                                                      root to be evaluated by the net (root_num_symmetries_to_sample >= 2 or the cache off). */
+  /* Uncertainty-weighted evaluations (Search::computeWeightFromNNOutput, searchupdatehelpers.cpp:114-136; on in the stock gatekeeper
+   * configs and under katago match, off in self-play).  With a net of model version >= 9 each evaluation enters the search with weight
+   * coeff / ((winLossUtilityFactor * shorttermWinlossError + dScoreUtility/dScore * shorttermScoreError)^exponent + coeff / max_weight)
+   * instead of 1, and terminal positions with max_weight.  Nets below version 9 report no short-term error: weight 1.  0 = off. */
+  int32_t use_uncertainty;                        /* useUncertainty */
+  double uncertainty_coeff;                       /* uncertaintyCoeff (0.25) */
+  double uncertainty_exponent;                    /* uncertaintyExponent (1.0; 1.0 and 0.5 are exact, other values use pow) */
+  double uncertainty_max_weight;                  /* uncertaintyMaxWeight (8.0) */
+  /* Noise pruning (Search::pruneNoiseWeight, searchupdatehelpers.cpp:495-539): in every backup, a child whose utility is below the
+   * average of the children before it (creation order) loses weight beyond twice its policy share of theirs.  0 = off. */
+  int32_t use_noise_pruning;                      /* useNoisePruning */
+  double noise_prune_utility_scale;               /* noisePruneUtilityScale (0.15) */
+  double noise_pruning_cap;                       /* noisePruningCap (1e50) */
 } kgb_selfplay_config;
 
 typedef struct kgb_selfplay_stats {
@@ -298,6 +312,16 @@ KGB_API int kgb_selfplay_get_root_children(kgb_selfplay* sp, int game, int32_t* 
 /* NodeStats moments (searchnode.h:17-41; white's perspective) of game g's root and of its children by move position:
  * winLossValueAvg, noResultValueAvg, scoreMeanAvg, scoreMeanSqAvg, leadAvg.  child_stats[(X*Y+1)*5] (0 where no child), root_stats[5]. */
 KGB_API int kgb_selfplay_get_root_value_stats(kgb_selfplay* sp, int game, double* child_stats, double* root_stats);
+/* NodeStats weightSum and weightSqSum of game g's root (root_weights[2]) and of its children by move position
+ * (child_weights[(X*Y+1)*2], 0 where there is no child): 1 per evaluation unless uncertainty weighting or noise pruning acts. */
+KGB_API int kgb_selfplay_get_root_weights(kgb_selfplay* sp, int game, double* child_weights, double* root_weights);
+/* TEST HOOK (row a20): the device loop's short-term error post-processing and evaluation weight on the host, n independent cases.
+ * raw[n][2] = score-value channels 4 and 5 as the net outputs them; params[n][12] = shortterm value / score error multipliers,
+ * uncertaintyCoeff, uncertaintyExponent, uncertaintyMaxWeight, winLossUtilityFactor, staticScoreUtilityFactor,
+ * dynamicScoreUtilityFactor, dynamicScoreCenterScale, recentScoreCenter, sqrtBoardArea, whiteScoreMean.  out[n][3] =
+ * shorttermWinlossError, shorttermScoreError (float as NNOutput keeps them; -1 below version 9) and the weight the search would use
+ * with useUncertainty on and a net that supports short-term errors. */
+KGB_API int kgb_test_uncertainty_weight(int n, const int32_t* model_version, const double* raw, const double* params, double* out);
 /* Game recording (SURVEY.md §8f row 2; replaces the bookkeeping around the search in Play::runGame, program/play.cpp:1757-1936).
  * With kgb_selfplay_config.debug_hold_at_max_visits = 1 a game whose search reached max_visits idles until it is released; the
  * host reads the finished search (getters above and below), releases, and the next wave lets the device choose and play the move

@@ -176,6 +176,13 @@ inline kgb_selfplay_config configFromCfg(const Cfg& c, int numGames) {
   k.use_non_buggy_lcb = c.flag("useNonBuggyLcb", false) ? 1 : 0;
   k.root_ending_bonus_points = c.num("rootEndingBonusPoints", 0.5);
   k.root_prune_useless_moves = c.flag("rootPruneUselessMoves", true) ? 1 : 0;
+  k.use_uncertainty = c.flag("useUncertainty", false) ? 1 : 0;
+  k.uncertainty_coeff = c.num("uncertaintyCoeff", 0.25);
+  k.uncertainty_exponent = c.num("uncertaintyExponent", 1.0);
+  k.uncertainty_max_weight = c.num("uncertaintyMaxWeight", 8.0);
+  k.use_noise_pruning = c.flag("useNoisePruning", false) ? 1 : 0;
+  k.noise_prune_utility_scale = c.num("noisePruneUtilityScale", 0.15);
+  k.noise_pruning_cap = c.num("noisePruningCap", 1e50);
   k.max_playouts_per_wave = (int32_t)c.num("b200MaxPlayoutsPerWave", 4);
   k.debug_hold_at_max_visits = 1;       // a slot whose search is finished waits for this host to read its move
   return k;
@@ -198,7 +205,8 @@ inline void printConfig(const kgb_selfplay_config& c) {
   FI(use_non_buggy_lcb); FD(lcb_stdevs); FD(min_visit_prop_for_lcb); FD(chosen_move_temperature); FD(chosen_move_temperature_early);
   FD(chosen_move_temperature_only_below_prob); FD(chosen_move_subtract); FD(chosen_move_prune); FI(nn_cache_size_power_of_two);
   FI(root_num_symmetries_to_sample); FI(ko_rule); FI(full_history_rules); FD(root_ending_bonus_points); FI(root_prune_useless_moves);
-  FI(max_playouts_per_wave);
+  FI(max_playouts_per_wave); FI(use_uncertainty); FD(uncertainty_coeff); FD(uncertainty_exponent); FD(uncertainty_max_weight);
+  FI(use_noise_pruning); FD(noise_prune_utility_scale); FD(noise_pruning_cap);
 #undef FI
 #undef FD
   std::printf("\"debug_hold_at_max_visits\":%d}\n", (int)c.debug_hold_at_max_visits);
@@ -272,7 +280,8 @@ inline const std::vector<std::string>& searchKeys() {
     "rootPolicyTemperatureEarly", "chosenMoveTemperature", "chosenMoveTemperatureEarly", "chosenMoveTemperatureHalflife", "chosenMoveTemperatureOnlyBelowProb",
     "chosenMoveSubtract", "chosenMovePrune", "useLcbForSelection", "lcbStdevs", "minVisitPropForLCB", "useNonBuggyLcb", "winLossUtilityFactor",
     "staticScoreUtilityFactor", "dynamicScoreUtilityFactor", "dynamicScoreCenterZeroWeight", "dynamicScoreCenterScale", "noResultUtilityForWhite",
-    "drawEquivalentWinsForWhite", "rootNumSymmetriesToSample", "nnCacheSizePowerOfTwo", "maxMovesPerGame", "rootEndingBonusPoints", "rootPruneUselessMoves"};
+    "drawEquivalentWinsForWhite", "rootNumSymmetriesToSample", "nnCacheSizePowerOfTwo", "maxMovesPerGame", "rootEndingBonusPoints", "rootPruneUselessMoves",
+    "useUncertainty", "uncertaintyCoeff", "uncertaintyExponent", "uncertaintyMaxWeight", "useNoisePruning", "noisePruneUtilityScale", "noisePruningCap"};
   return keys;
 }
 // The configuration bot `idx` of a match sees: a search key with the bot's index appended overrides the shared one; keys of other bots, bot

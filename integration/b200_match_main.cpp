@@ -51,6 +51,24 @@ int main(int argc, char** argv) {
   const int games = (int)std::max(2L, std::min(std::min((long)gamesPerGpu, (long)cfg.num("numGameThreads", gamesPerGpu)), total));
   check(kgb_global_init(), "kgb_global_init");
   log("Match Engine starting...");
+  {
+    // the reference's katago match loads its bots with SETUP_FOR_MATCH, where both default to true (program/setup.cpp:522-544); an unset
+    // key stays off here, so that existing match configurations keep playing the same games (katago_b200/match_cli.py match_default_note)
+    std::vector<std::string> absent;
+    for(const std::string k : {"useUncertainty", "useNoisePruning"}) {
+      bool set = cfg.has(k);
+      for(const auto& kv : cfg.kv)
+        set = set || (kv.first.size() > k.size() && kv.first.compare(0, k.size(), k) == 0 &&
+                      kv.first.find_first_not_of("0123456789", k.size()) == std::string::npos);
+      if(!set) absent.push_back(k);
+    }
+    if(!absent.empty()) {
+      std::string line = "[config] " + absent[0] + (absent.size() > 1 ? " and " + absent[1] : "") +
+                         " not set: off here, while the reference's katago match defaults " + (absent.size() > 1 ? "them" : "it") + " to true; set ";
+      for(size_t i = 0; i < absent.size(); i++) line += (i ? ", " : "") + absent[i] + " = true";
+      log(line + " to search like it");
+    }
+  }
 
   kgb_model* models[2]; kgb_context* ctxs[2]; kgb_handle* handles[2];
   std::unique_ptr<b200::GameSlots> loops[2];

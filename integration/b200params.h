@@ -66,6 +66,13 @@ inline kgb_selfplay_config configFromSearchParams(const SearchParams& p, const R
   c.value_weight_exponent = p.valueWeightExponent;
   c.subtree_value_bias_factor = p.subtreeValueBiasFactor;
   c.subtree_value_bias_weight_exponent = p.subtreeValueBiasWeightExponent;
+  c.use_uncertainty = p.useUncertainty ? 1 : 0;
+  c.uncertainty_coeff = p.uncertaintyCoeff;
+  c.uncertainty_exponent = p.uncertaintyExponent;
+  c.uncertainty_max_weight = p.uncertaintyMaxWeight;
+  c.use_noise_pruning = p.useNoisePruning ? 1 : 0;
+  c.noise_prune_utility_scale = p.noisePruneUtilityScale;
+  c.noise_pruning_cap = p.noisePruningCap;
   // graph search
   c.use_graph_search = p.useGraphSearch ? 1 : 0;
   c.graph_search_rep_bound = p.graphSearchRepBound;
@@ -94,8 +101,6 @@ inline kgb_selfplay_config configFromSearchParams(const SearchParams& p, const R
   // options of the reference's search that the device loop does not have: reported when they are switched on
   no(p.policyOptimism != 0.0, "policyOptimism = " + num(p.policyOptimism));
   no(p.rootPolicyOptimism != 0.0, "rootPolicyOptimism = " + num(p.rootPolicyOptimism));
-  no(p.useNoisePruning, "useNoisePruning = true");
-  no(p.useUncertainty, "useUncertainty = true");
   no(p.graphSearchCatchUpLeakProb != 0.0, "graphSearchCatchUpLeakProb = " + num(p.graphSearchCatchUpLeakProb));
   no(p.rootSymmetryPruning, "rootSymmetryPruning = true");
   no(p.conservativePass, "conservativePass = true");

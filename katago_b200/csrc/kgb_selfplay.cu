@@ -91,7 +91,8 @@ struct SPDev {
   int useGraphSearch, graphSearchRepBound, holdAtMaxVisits;
   // evaluation cache (NNCacheTable, nneval.cpp:1273-1353; key = NNInputs::getHash, nninputs.cpp:869-943): direct mapped, shared by
   // all games of the GPU.  An entry holds what NNOutput holds for the search: post-processed policy, white win/loss/noResult,
-  // white score mean / mean-square, plus the position's laddered stones (a function of the same position, needed by descendants).
+  // white score mean / mean-square / lead, the two short-term errors (not the weight: it depends on the search's score centre),
+  // plus the position's laddered stones (a function of the same position, needed by descendants).
   int cacheSize;                    // entries (power of two), 0 = off
   unsigned long long *cacheKey0, *cacheKey1;
   int* cacheLock;
@@ -104,10 +105,11 @@ struct SPDev {
   // root policy temperature and Dirichlet noise (searchhelpers.cpp:78-215)
   // rootNumSymmetriesToSample (searchnnhelpers.cpp:95-101, nneval.cpp:811-838, nninputs.cpp:324-430): the root is evaluated under
   // several distinct symmetries, one per wave, and the post-processed outputs are averaged
-  int rootNumSymmetries, fakeNN;
+  int rootNumSymmetries, fakeNN;    // fakeNN: 0 the evaluator, 1 the hash net, 2 the hash net with raw short-term error channels
   int* rootSymCount;                // [game] evaluations of the current root accumulated so far
   int* rootSymOrder;                // [game][8] the sampled symmetry order
-  float* rootSymAcc;                // [game][8] sums of whiteWin, whiteLoss, noResult, whiteScoreMean, whiteScoreMeanSq
+  float* rootSymAcc;                // [game][8] sums of whiteWin, whiteLoss, noResult, whiteScoreMean, whiteScoreMeanSq, whiteLead,
+                                    // shorttermWinlossError, shorttermScoreError (NNOutput(others), nninputs.cpp:327-363)
   int rootNoiseEnabled;
   double rootDirichletNoiseTotalConcentration, rootDirichletNoiseWeight, rootPolicyTemperature, rootPolicyTemperatureEarly, chosenMoveTemperatureHalflife;
   // root move choice (searchresults.cpp:24-330 play selection values, :573-598 getChosenMoveLoc, searchhelpers.cpp:12-76)
@@ -133,6 +135,15 @@ struct SPDev {
   double scoreMeanMultiplier, scoreStdevMultiplier;   // ModelPostProcessParams of the net
   const double* svTable;            // ScoreValue's expectedSVTable [842][421]
   double* recentScoreCenter;        // [game] Search::recentScoreCenter of the current root
+  // evaluation weights (Search::computeWeightFromNNOutput, searchupdatehelpers.cpp:114-136): useUncertainty = the switch and a net that
+  // reports short-term errors (model version >= 9, nneval.cpp:299); otherwise every evaluation has weight 1
+  int useUncertainty, modelVersion;
+  double uncertaintyCoeff, uncertaintyExponent, uncertaintyMaxWeight;
+  double shorttermValueErrorMultiplier, shorttermScoreErrorMultiplier;   // ModelPostProcessParams of the net
+  double* nodeNNWeight;             // [game][maxNodes] weight of the node's own evaluation (allocated when useUncertainty)
+  // Search::pruneNoiseWeight (searchupdatehelpers.cpp:495-539) in every recompute
+  int useNoisePruning;
+  double noisePruneUtilityScale, noisePruningCap;
   float* leafTerminalScore;         // [game] finalWhiteMinusBlackScore of a terminal leaf
   const float* nnScore;             // [game][6] raw score head (whiteScoreMean, stdev pre-softplus, lead, ...)
   uint64_t seed;
@@ -761,11 +772,12 @@ __device__ void rootAdvance(const SPDev& d, int g, int lane) {
 }
 
 __device__ void recomputeNodeStats(const SPDev& d, int g, int node, bool nodePlaWhite, double* sh, int lane);
-__device__ void finishPlayout(const SPDev& d, int g, int node, double u, bool terminal, bool leafBlack, int len, double* shSum, int lane);
+__device__ void finishPlayout(const SPDev& d, int g, int node, double u, double w, bool terminal, bool leafBlack, int len, double* shSum, int lane);
+__device__ __forceinline__ double evalWeight(const SPDev& d, int g, const float vals[8]);
 __device__ double utilityFromEval(const SPDev& d, int g, int node, float whiteWin, float whiteLoss, float noResult, float whiteScoreMeanF,
                                   float whiteScoreMeanSqF, float whiteLeadF, int lane);
 __device__ void maybeRootNoise(const SPDev& d, int g, int node, int lane);
-__device__ bool cacheLookup(const SPDev& d, int g, int node, unsigned long long k0, unsigned long long k1, float vals[6], int lane);
+__device__ bool cacheLookup(const SPDev& d, int g, int node, unsigned long long k0, unsigned long long k1, float vals[8], int lane);
 
 // Warp 0 of a game's block: PUCT descent, leaf board, legality and every feature except the leaf's own ladder searches.
 __device__ void spSelectWarp0(const SPDev& d, int g, int lane, uint32_t* shB, uint32_t* shW, uint32_t* shCand, int& shKo, int& shDoLadders,
@@ -1092,7 +1104,7 @@ __device__ void spSelectWarp0(const SPDev& d, int g, int lane, uint32_t* shB, ui
       k0 ^= kh; k1 ^= splitmix64(kh);
     }
     if(lane == 0) { d.leafKey[g * 2] = k0; d.leafKey[g * 2 + 1] = k1; }
-    float vals[6];
+    float vals[8];
     // a plain root (cheap search) is evaluated by the net even when the cache knows it: its input row is kept for the recorder; the key is
     // still set, so that the backup stores the fresh evaluation under it
     if(!(node == 0 && d.plainRoot[g]) && cacheLookup(d, g, node, k0, k1, vals, lane)) {
@@ -1100,7 +1112,7 @@ __device__ void spSelectWarp0(const SPDev& d, int g, int lane, uint32_t* shB, ui
         computeRootExtras(d, g, bd, black, false, 1, lane);     // a root served by the cache has no ownership map: allowed moves only
       maybeRootNoise(d, g, node, lane);
       const double u = utilityFromEval(d, g, node, vals[0], vals[1], vals[2], vals[3], vals[4], vals[5], lane);
-      finishPlayout(d, g, node, u, false, black, depth, shSum, lane);
+      finishPlayout(d, g, node, u, evalWeight(d, g, vals), false, black, depth, shSum, lane);
       if(lane == 0) atomicAdd(d.cacheHits, 1ULL);
       PF(pfBackup);
       continue;
@@ -1406,8 +1418,9 @@ __global__ void rootNoiseTestKernel(float* pol, int policySize, int X, int Y, in
                                       scratch + policySize, threadIdx.x);
 }
 
-// Search::recomputeNodeStats (searchupdatehelpers.cpp:167-360) for the parameter subset of the loop (no noise pruning, no root
-// noise subtraction, no subtree value bias, no uncertainty weights: the node's own evaluation has weight 1), one warp per node.
+// Search::recomputeNodeStats (searchupdatehelpers.cpp:167-360) for the parameter subset of the loop (no root noise subtraction:
+// chosenMoveSubtract / chosenMovePrune are not applied during the search), one warp per node.  Noise pruning and the node's own
+// evaluation weight (uncertainty) when switched on.
 // Children are visited in creation order and every sum is accumulated in that order (orderedAdd2), like the reference's loops.
 #ifdef KGB_PROFILE_DESCENT   // profiling build: cycles of the recompute's phases, accumulated per game (spBackupKernel zeroes the slots first)
 #define RPF(slot) do { const long long t_ = clock64(); if(lane == 0) d.dbgCycles[g * 8 + (slot)] += t_ - rpT; rpT = t_; } while(0)
@@ -1423,10 +1436,11 @@ __device__ void recomputeNodeStats(const SPDev& d, int g, int node, bool nodePla
   const int nc = d.nodeNumChildren[gn];
   double WA[12], CU[12], CUSQ[12], CWS[12], CWSQ[12];   // weightAdjusted, child utilityAvg / utilitySqAvg / weightSum / weightSqSum
   int CI[12];                                             // the child's node index
+  uint32_t GM[12];                                        // lanes holding a good child (noise pruning)
   double origTotal = 0.0, simpleValueSum = 0.0;
 #pragma unroll
   for(int ch = 0; ch < 12; ch++) {
-    WA[ch] = 0.0; CU[ch] = 0.0; CUSQ[ch] = 0.0; CWS[ch] = 1.0; CWSQ[ch] = 0.0; CI[ch] = 0;
+    WA[ch] = 0.0; CU[ch] = 0.0; CUSQ[ch] = 0.0; CWS[ch] = 1.0; CWSQ[ch] = 0.0; CI[ch] = 0; GM[ch] = 0;
     if(ch * 32 < nc) {
       const int k = ch * 32 + lane;
       const bool in = k < nc;
@@ -1437,6 +1451,7 @@ __device__ void recomputeNodeStats(const SPDev& d, int g, int node, bool nodePla
       const int cv = in ? d.nodeVisits[gb + c] : 0;
       const double cw = in ? d.nodeWeightSum[gb + c] : 0.0;
       const bool good = in && cv > 0 && cw > 0.0 && ev > 0;
+      if(d.useNoisePruning) GM[ch] = __ballot_sync(KGB_FULL, good);
       if(good) {
         WA[ch] = cw * ((double)ev / (double)(cv > 1 ? cv : 1));
         CU[ch] = d.nodeUtilAvg[gb + c]; CUSQ[ch] = d.nodeUtilSqAvg[gb + c]; CWS[ch] = cw; CWSQ[ch] = d.nodeWeightSqSum[gb + c];
@@ -1454,9 +1469,52 @@ __device__ void recomputeNodeStats(const SPDev& d, int g, int node, bool nodePla
       orderedAdd2(WA[ch], WA[ch] != 0.0 ? selfU * WA[ch] : 0.0, n, origTotal, simpleValueSum, sh, lane);
     }
   }
+  double curTotal = origTotal;   // currentTotalChildWeight
+  if(d.useNoisePruning && origTotal > 0.00001) {
+    // pruneNoiseWeight (:495-539): one pass over the good children in creation order, each step depending on the sums before it.
+    // Every lane runs the same pass on values broadcast from the lane that holds the child (warp-uniform), the owner keeps the result.
+    // Its running sums are the ones downweightBadChildrenAndNormalizeWeight then takes (same terms, same order).
+    int numGood = 0;
+#pragma unroll
+    for(int ch = 0; ch < 12; ch++) numGood += __popc(GM[ch]);
+    if(numGood > 1) {
+      const float* pol = d.policy + nb;   // the node's policy as the search sees it (noised at a noised root)
+      double utilitySoFar = 0.0, weightSoFar = 0.0, policySoFar = 0.0;
+#pragma unroll
+      for(int ch = 0; ch < 12; ch++) {
+        if(GM[ch] == 0) continue;
+        const int k = ch * 32 + lane;
+        const double rawPolicy = k < nc ? fmax(1e-30, (double)pol[d.childOrder[nb + k]]) : 0.0;
+        const double selfU = nodePlaWhite ? CU[ch] : -CU[ch];
+        for(uint32_t m = GM[ch]; m != 0; m &= m - 1) {
+          const int j = __ffs(m) - 1;
+          const double utility = __shfl_sync(KGB_FULL, selfU, j), oldWeight = __shfl_sync(KGB_FULL, WA[ch], j);
+          const double p = __shfl_sync(KGB_FULL, rawPolicy, j);
+          double newWeight = oldWeight;
+          if(weightSoFar > 0 && policySoFar > 0) {
+            const double utilityGap = utilitySoFar / weightSoFar - utility;
+            if(utilityGap > 0) {
+              const double lenientShare = 2.0 * (weightSoFar * p / policySoFar);
+              if(oldWeight > lenientShare) {
+                double weightToSubtract = (oldWeight - lenientShare) * (1.0 - exp(-utilityGap / d.noisePruneUtilityScale));
+                if(weightToSubtract > d.noisePruningCap) weightToSubtract = d.noisePruningCap;
+                newWeight = oldWeight - weightToSubtract;
+                if(lane == j) WA[ch] = newWeight;
+              }
+            }
+          }
+          utilitySoFar += utility * newWeight;
+          weightSoFar += newWeight;
+          policySoFar += p;
+        }
+      }
+      curTotal = weightSoFar;
+      simpleValueSum = utilitySoFar;
+    }
+  }
   // downweightBadChildrenAndNormalizeWeight (:402-491) with nothing to subtract or prune
-  if(d.valueWeightExponent != 0.0 && origTotal > 0.0) {
-    const double simpleValue = simpleValueSum / origTotal;
+  if(d.valueWeightExponent != 0.0 && curTotal > 0.0) {
+    const double simpleValue = simpleValueSum / curTotal;
     double totalNew = 0.0, unused = 0.0;
 #pragma unroll
     for(int ch = 0; ch < 12; ch++) {
@@ -1473,7 +1531,7 @@ __device__ void recomputeNodeStats(const SPDev& d, int g, int node, bool nodePla
         orderedAdd2(WA[ch], 0.0, n, totalNew, unused, sh, lane);
       }
     }
-    const double factor = origTotal / totalNew;
+    const double factor = curTotal / totalNew;
 #pragma unroll
     for(int ch = 0; ch < 12; ch++) WA[ch] *= factor;
   }
@@ -1512,17 +1570,18 @@ __device__ void recomputeNodeStats(const SPDev& d, int g, int node, bool nodePla
     }
   }
   RPF(6);
-  double weightSum = origTotal;
-  // the node's own evaluation, weight 1
+  double weightSum = curTotal;
+  // the node's own evaluation, with its weight (1 unless uncertainty weighting applies)
   double utility = d.nodeNNUtil[gn];
+  const double selfWeight = d.useUncertainty ? d.nodeNNWeight[gn] : 1.0;
   const int entry = d.subtreeValueBiasFactor != 0.0 ? d.nodeBiasEntry[gn] : -1;
   if(entry >= 0) {
     // searchupdatehelpers.cpp:273-310: the node reports how far its children's average is from its own evaluation to the entry
     // shared by all nodes reached by the same local move, and shifts its own evaluation by the entry's average observation
     const size_t te = (size_t)g * d.biasTableSize + entry;
     double newDelta, newWeight;
-    if(origTotal > 1e-10) {
-      const double utilityChildren = utilitySum / origTotal;
+    if(curTotal > 1e-10) {
+      const double utilityChildren = utilitySum / curTotal;
       const double biasWeight = pow(origTotal, d.subtreeValueBiasWeightExponent);
       const double biasDelta = (utilityChildren - utility) * biasWeight;
       newDelta = d.biasDeltaSum[te] + (biasDelta - d.nodeLastBiasDelta[gn]);
@@ -1533,13 +1592,13 @@ __device__ void recomputeNodeStats(const SPDev& d, int g, int node, bool nodePla
     else { newDelta = d.biasDeltaSum[te]; newWeight = d.biasWeightSum[te]; }
     if(newWeight > 0.001) utility += d.subtreeValueBiasFactor * newDelta / newWeight;
   }
-  utilitySum += utility * 1.0;
-  utilitySqSum += utility * utility * 1.0;
-  weightSqSum += 1.0 * 1.0;
-  weightSum += 1.0;
+  utilitySum += utility * selfWeight;
+  utilitySqSum += utility * utility * selfWeight;
+  weightSqSum += selfWeight * selfWeight;
+  weightSum += selfWeight;
   __syncwarp();
   if(lane == 0) {
-    for(int i = 0; i < 5; i++) d.nodeMoments[gn * 5 + i] = (mom[i] + d.nodeNNMoments[gn * 5 + i] * 1.0) / weightSum;
+    for(int i = 0; i < 5; i++) d.nodeMoments[gn * 5 + i] = (mom[i] + d.nodeNNMoments[gn * 5 + i] * selfWeight) / weightSum;
     d.nodeUtilAvg[gn] = utilitySum / weightSum;
     d.nodeUtilSqAvg[gn] = utilitySqSum / weightSum;
     d.nodeWeightSqSum[gn] = weightSqSum;
@@ -1548,6 +1607,52 @@ __device__ void recomputeNodeStats(const SPDev& d, int g, int node, bool nodePla
   }
   __syncwarp();
   RPF(7);
+}
+
+// Short-term errors of one evaluation from the raw score-value channels 4 and 5 (nneval.cpp:1161-1178, 1217-1226), by model version;
+// -1 for nets below version 9, which have no such outputs.  Host and device share it (kgb_test_uncertainty_weight).
+__host__ __device__ inline double spSoftPlus(double x) { return x > 40.0 ? x : log(1.0 + exp(x)); }
+__host__ __device__ inline void shorttermErrors(int version, double valueMult, double scoreMult, double rawWinloss, double rawScore, float& winlossError,
+                                                float& scoreError) {
+  double wl, se;
+  if(version >= 14) {
+    const double a = spSoftPlus(rawWinloss * 0.5), b = spSoftPlus(rawScore * 0.5);
+    wl = sqrt(a * a * valueMult);
+    se = sqrt(b * b * scoreMult);
+  }
+  else if(version >= 10) { wl = sqrt(spSoftPlus(rawWinloss) * valueMult); se = sqrt(spSoftPlus(rawScore) * scoreMult); }
+  else { wl = spSoftPlus(rawWinloss); se = spSoftPlus(rawScore) * 10.0; }
+  winlossError = version >= 9 ? (float)wl : -1.0f;
+  scoreError = version >= 9 ? (float)se : -1.0f;
+}
+// ScoreValue::whiteDScoreValueDScoreSmoothNoDrawAdjust (nninputs.cpp:64-69)
+__host__ __device__ inline double dScoreValueDScore(double score, double center, double scale, double sqrtBoardArea) {
+  const double adjustedScore = score - center;
+  const double scaleFactor = scale * sqrtBoardArea;
+  return scaleFactor / (scaleFactor * scaleFactor + adjustedScore * adjustedScore) * 0.63661977236758134308;
+}
+// Search::computeWeightFromNNOutput (searchupdatehelpers.cpp:114-136) with getApproxScoreUtilityDerivative (searchhelpers.cpp:296-301),
+// for a search whose switch applies (useUncertainty and a net of version >= 9)
+__host__ __device__ inline double uncertaintyWeight(double coeff, double exponent, double maxWeight, double winLossUtilityFactor, double staticFactor,
+                                                   double dynamicFactor, double dynamicScale, double center, double sqrtBoardArea, float whiteScoreMean,
+                                                   float winlossError, float scoreError) {
+  const double scoreMean = (double)whiteScoreMean;
+  const double derivative = dScoreValueDScore(scoreMean, 0.0, 2.0, sqrtBoardArea) * staticFactor +
+                            dScoreValueDScore(scoreMean, center, dynamicScale, sqrtBoardArea) * dynamicFactor;
+  const double uncertainty = winLossUtilityFactor * winlossError + derivative * scoreError;
+  const double powered = exponent == 1.0 ? uncertainty : exponent == 0.5 ? sqrt(uncertainty) : pow(uncertainty, exponent);
+  const double baseline = coeff / maxWeight;
+  return coeff / (powered + baseline);
+}
+// Board::sqrtBoardArea (board.cpp:234-239) of game g
+__device__ __forceinline__ double sqrtBoardAreaOf(const SPDev& d, int g) {
+  return d.gX[g] == d.gY[g] ? (double)d.gX[g] : sqrt((double)(d.gX[g] * d.gY[g]));
+}
+// The weight of an evaluation of game g's search (vals: whiteScoreMean at 3, the two short-term errors at 6 and 7)
+__device__ __forceinline__ double evalWeight(const SPDev& d, int g, const float vals[8]) {
+  if(!d.useUncertainty) return 1.0;
+  return uncertaintyWeight(d.uncertaintyCoeff, d.uncertaintyExponent, d.uncertaintyMaxWeight, d.winLossUtilityFactor, d.staticScoreUtilityFactor,
+                           d.dynamicScoreUtilityFactor, d.dynamicScoreCenterScale, d.recentScoreCenter[g], sqrtBoardAreaOf(d, g), vals[3], vals[6], vals[7]);
 }
 
 // Search::getScoreUtility (searchhelpers.cpp:272-279)
@@ -1683,18 +1788,18 @@ __device__ void maybeRootNoise(const SPDev& d, int g, int node, int lane) {
   }
 }
 // The end of a playout whose leaf value is known: the leaf's own statistics (Search::addLeafValue, searchupdatehelpers.cpp:11-81,
-// evaluation weight 1), then edge visit + recomputeNodeStats for every node on the path (updateStatsAfterPlayout).
-__device__ void finishPlayout(const SPDev& d, int g, int node, double u, bool terminal, bool leafBlack, int len, double* shSum, int lane) {
+// evaluation weight w), then edge visit + recomputeNodeStats for every node on the path (updateStatsAfterPlayout).
+__device__ void finishPlayout(const SPDev& d, int g, int node, double u, double w, bool terminal, bool leafBlack, int len, double* shSum, int lane) {
   const size_t gb = (size_t)g * d.maxNodes, gl = gb + node;
   const int leafVisits = d.nodeVisits[gl];
   __syncwarp();
   if(terminal) {
     if(lane == 0) {
-      const double oldW = d.nodeWeightSum[gl], newW = oldW + 1.0;
-      for(int i = 0; i < 5; i++) d.nodeMoments[gl * 5 + i] = (d.nodeMoments[gl * 5 + i] * oldW + d.leafMoments[g * 5 + i] * 1.0) / newW;
-      d.nodeUtilAvg[gl] = (d.nodeUtilAvg[gl] * oldW + u * 1.0) / newW;
-      d.nodeUtilSqAvg[gl] = (d.nodeUtilSqAvg[gl] * oldW + (u * u) * 1.0) / newW;
-      d.nodeWeightSqSum[gl] = d.nodeWeightSqSum[gl] + 1.0;
+      const double oldW = d.nodeWeightSum[gl], newW = oldW + w;
+      for(int i = 0; i < 5; i++) d.nodeMoments[gl * 5 + i] = (d.nodeMoments[gl * 5 + i] * oldW + d.leafMoments[g * 5 + i] * w) / newW;
+      d.nodeUtilAvg[gl] = (d.nodeUtilAvg[gl] * oldW + u * w) / newW;
+      d.nodeUtilSqAvg[gl] = (d.nodeUtilSqAvg[gl] * oldW + (u * u) * w) / newW;
+      d.nodeWeightSqSum[gl] = d.nodeWeightSqSum[gl] + w * w;
       d.nodeWeightSum[gl] = newW;
       d.nodeVisits[gl] = leafVisits + 1;
     }
@@ -1702,6 +1807,7 @@ __device__ void finishPlayout(const SPDev& d, int g, int node, double u, bool te
   else if(leafVisits == 0) {
     if(lane == 0) {
       d.nodeNNUtil[gl] = u;
+      if(d.useUncertainty) d.nodeNNWeight[gl] = w;
       for(int i = 0; i < 5; i++) { d.nodeNNMoments[gl * 5 + i] = d.leafMoments[g * 5 + i]; d.nodeMoments[gl * 5 + i] = d.leafMoments[g * 5 + i]; }
       const int entry = d.subtreeValueBiasFactor != 0.0 ? d.nodeBiasEntry[gl] : -1;
       if(entry >= 0) {   // searchupdatehelpers.cpp:26-36
@@ -1709,7 +1815,7 @@ __device__ void finishPlayout(const SPDev& d, int g, int node, double u, bool te
         const double ew = d.biasWeightSum[te];
         if(ew > 0.001) u += d.subtreeValueBiasFactor * d.biasDeltaSum[te] / ew;
       }
-      d.nodeUtilAvg[gl] = u; d.nodeUtilSqAvg[gl] = u * u; d.nodeWeightSqSum[gl] = 1.0; d.nodeWeightSum[gl] = 1.0;
+      d.nodeUtilAvg[gl] = u; d.nodeUtilSqAvg[gl] = u * u; d.nodeWeightSqSum[gl] = w * w; d.nodeWeightSum[gl] = w;
       d.nodeVisits[gl] = 1;
     }
   }
@@ -1732,7 +1838,7 @@ __device__ __forceinline__ size_t cacheSlotOf(const SPDev& d, unsigned long long
 }
 // Looks the leaf's key up; on a hit copies policy, values and laddered stones into the node (whole warp).  Writers hold the
 // entry's lock while they change it and readers check key and lock before and after copying, so a torn entry is never used.
-__device__ bool cacheLookup(const SPDev& d, int g, int node, unsigned long long k0, unsigned long long k1, float vals[6], int lane) {
+__device__ bool cacheLookup(const SPDev& d, int g, int node, unsigned long long k0, unsigned long long k1, float vals[8], int lane) {
   const size_t slot = cacheSlotOf(d, k0, k1);
   bool ok = false;
   if(lane == 0) ok = atomicAdd(&d.cacheLock[slot], 0) == 0 && __ldcg(d.cacheKey0 + slot) == k0 && __ldcg(d.cacheKey1 + slot) == k1;
@@ -1742,15 +1848,15 @@ __device__ bool cacheLookup(const SPDev& d, int g, int node, unsigned long long 
   const size_t gb = (size_t)g * d.maxNodes, nb = (gb + node) * d.policySize;
   for(int i = lane; i < d.policySize; i += 32) d.policy[nb + i] = __ldcg(d.cachePolicy + slot * d.policySize + i);
   d.nodeLad[(gb + node) * 32 + lane] = __ldcg(d.cacheLad + slot * 32 + lane);
-  float v = lane < 6 ? __ldcg(d.cacheVals + slot * 8 + lane) : 0.0f;
+  float v = lane < 8 ? __ldcg(d.cacheVals + slot * 8 + lane) : 0.0f;
   __threadfence();
   if(lane == 0) ok = atomicAdd(&d.cacheLock[slot], 0) == 0 && __ldcg(d.cacheKey0 + slot) == k0 && __ldcg(d.cacheKey1 + slot) == k1;
   ok = __shfl_sync(KGB_FULL, ok ? 1 : 0, 0) != 0;
 #pragma unroll
-  for(int i = 0; i < 6; i++) vals[i] = __shfl_sync(KGB_FULL, v, i);
+  for(int i = 0; i < 8; i++) vals[i] = __shfl_sync(KGB_FULL, v, i);
   return ok;
 }
-__device__ void cacheStore(const SPDev& d, int g, int node, unsigned long long k0, unsigned long long k1, const float vals[6], int lane) {
+__device__ void cacheStore(const SPDev& d, int g, int node, unsigned long long k0, unsigned long long k1, const float vals[8], int lane) {
   const size_t slot = cacheSlotOf(d, k0, k1);
   bool mine = false;
   if(lane == 0) mine = atomicCAS(&d.cacheLock[slot], 0, 1) == 0;
@@ -1761,7 +1867,7 @@ __device__ void cacheStore(const SPDev& d, int g, int node, unsigned long long k
   const size_t gb = (size_t)g * d.maxNodes, nb = (gb + node) * d.policySize;
   for(int i = lane; i < d.policySize; i += 32) d.cachePolicy[slot * d.policySize + i] = d.policy[nb + i];
   d.cacheLad[slot * 32 + lane] = d.nodeLad[(gb + node) * 32 + lane];
-  if(lane < 6) d.cacheVals[slot * 8 + lane] = vals[lane];
+  if(lane < 8) d.cacheVals[slot * 8 + lane] = vals[lane];
   __threadfence();
   __syncwarp();
   if(lane == 0) {
@@ -1798,7 +1904,8 @@ __global__ void spBackupKernel(const SPDev d) {
     for(int i = lane; i < n; i += 32) dst[i] = src[i];
     if(lane < 19) dst[n + lane] = d.nnGlobal[(size_t)g * 19 + lane];
   }
-  double u;
+  double u, weight = 1.0;
+  if(terminal) weight = d.useUncertainty ? d.uncertaintyMaxWeight : 1.0;   // search.cpp:1210, 1220
   if(d.leafTerminal[g] == 2) {
     // search.cpp:1204-1212: a game ended without result (long cycle under simple ko)
     u = 1.0 * d.noResultUtilityForWhite + scoreUtilityOf(d, g, 0.0, 0.0, d.recentScoreCenter[g]);
@@ -1883,9 +1990,12 @@ __global__ void spBackupKernel(const SPDev d) {
     scoreMean = scoreMean * (1.0 - n);
     scoreMeanSq = scoreMeanSq * (1.0 - n);
     const double lead = (double)sc[2] * d.leadMultiplier * (1.0 - n);
-    float vals[6];
+    float vals[8];
     vals[0] = leafBlack ? lf : wf; vals[1] = leafBlack ? wf : lf; vals[2] = nf;
     vals[3] = leafBlack ? -(float)scoreMean : (float)scoreMean; vals[4] = (float)scoreMeanSq; vals[5] = leafBlack ? -(float)lead : (float)lead;
+    vals[6] = 0.0f; vals[7] = 0.0f;
+    if(d.useUncertainty)   // channels 4 and 5: no colour flip
+      shorttermErrors(d.modelVersion, d.shorttermValueErrorMultiplier, d.shorttermScoreErrorMultiplier, (double)sc[4], (double)sc[5], vals[6], vals[7]);
     __syncwarp();
     const bool freshRoot = node == 0 && d.nodeVisits[gb] == 0;
     const bool wantRootExtras = freshRoot && (d.rootEndingBonusPoints != 0.0 || d.rootPruneUselessMoves);
@@ -1911,7 +2021,7 @@ __global__ void spBackupKernel(const SPDev d) {
         return;
       }
       float* acc = d.rootSymAcc + g * 8;
-      if(lane < 6) acc[lane] = symCount > 0 ? acc[lane] + vals[lane] : vals[lane];
+      if(lane < 8) acc[lane] = symCount > 0 ? acc[lane] + vals[lane] : vals[lane];
       __syncwarp();
       if(symCount + 1 < d.rootNumSymmetries) {
         if(lane == 0) { d.rootSymCount[g] = symCount + symLead + 1; atomicAdd(d.stalledWaves, 1ULL); }   // the root stays unvisited: next wave, next symmetry
@@ -1920,7 +2030,7 @@ __global__ void spBackupKernel(const SPDev d) {
       const float floatLen = (float)d.rootNumSymmetries;
       for(int i = lane; i < d.policySize; i += 32) d.policy[nb + i] = d.policy[nb + i] / floatLen;
 #pragma unroll
-      for(int i = 0; i < 6; i++) vals[i] = acc[i] / floatLen;
+      for(int i = 0; i < 8; i++) vals[i] = acc[i] / floatLen;
       if(lane == 0) d.rootSymCount[g] = 0;
       __syncwarp();
     }
@@ -1933,12 +2043,13 @@ __global__ void spBackupKernel(const SPDev d) {
     }
     maybeRootNoise(d, g, node, lane);
     u = utilityFromEval(d, g, node, vals[0], vals[1], vals[2], vals[3], vals[4], vals[5], lane);
+    weight = evalWeight(d, g, vals);   // after utilityFromEval: a fresh root's score centre is set there
   }
   __syncwarp();
 #ifdef KGB_PROFILE_DESCENT
   const long long tBk1 = clock64();
 #endif
-  finishPlayout(d, g, node, u, terminal, leafBlack, d.pathLen[g], shSum, lane);
+  finishPlayout(d, g, node, u, weight, terminal, leafBlack, d.pathLen[g], shSum, lane);
 #ifdef KGB_PROFILE_DESCENT
   if(lane == 0) { d.dbgCycles[g * 8 + 0] = clock64() - tBk0; d.dbgCycles[g * 8 + 2] = tBk1 - tBk0; d.dbgCycles[g * 8 + 3] = d.pathLen[g]; }   // whole warp, before the path update, path length
 #endif
@@ -1979,6 +2090,10 @@ __global__ void spFakeNNKernel(const SPDev d, float* policyOut, float* valueOut,
     scoreOut[g * 6 + 1] = (float)(uint32_t)(splitmix64(h ^ 0x4444ULL) >> 48) * (1.0f / 16384.0f) - 2.0f;
     scoreOut[g * 6 + 2] = (float)(uint32_t)(splitmix64(h ^ 0x5555ULL) >> 48) * (1.0f / 32768.0f) - 1.0f;
     scoreOut[g * 6 + 3] = 0.0f; scoreOut[g * 6 + 4] = 0.0f; scoreOut[g * 6 + 5] = 0.0f;
+    if(d.fakeNN == 2) {   // the variant with raw short-term error channels in [-2,2) (tests/cpp/uncertainty_search_driver.cpp gives the reference Search the same net)
+      scoreOut[g * 6 + 4] = (float)(uint32_t)(splitmix64(h ^ 0x6666ULL) >> 48) * (1.0f / 16384.0f) - 2.0f;
+      scoreOut[g * 6 + 5] = (float)(uint32_t)(splitmix64(h ^ 0x7777ULL) >> 48) * (1.0f / 16384.0f) - 2.0f;
+    }
   }
 }
 
@@ -2508,7 +2623,8 @@ static void initLoop(kgb_selfplay* sp, const kgb_selfplay_config& c) {
   d.gEverOcc = sp->alloc<uint32_t>(G * 32); d.rootBanned = sp->alloc<uint32_t>(G * 32);
   d.pKo = sp->alloc<unsigned long long>(G * d.pathCap); d.pPassB = sp->alloc<unsigned long long>(G * d.pathCap); d.pPassW = sp->alloc<unsigned long long>(G * d.pathCap);
   d.holdAtMaxVisits = c.debug_hold_at_max_visits ? 1 : 0;
-  d.fakeNN = c.debug_fake_nn ? 1 : 0;
+  if(c.debug_fake_nn < 0 || c.debug_fake_nn > 2) throw std::invalid_argument("selfplay: debug_fake_nn must be 0, 1 or 2");
+  d.fakeNN = c.debug_fake_nn;
   d.rootNumSymmetries = c.root_num_symmetries_to_sample > 1 ? (c.root_num_symmetries_to_sample > 8 ? 8 : c.root_num_symmetries_to_sample) : 1;
   d.rootSymCount = sp->alloc<int>(G); d.rootSymOrder = sp->alloc<int>(G * 8); d.rootSymAcc = sp->alloc<float>(G * 8);
   d.rootNoiseEnabled = c.root_noise_enabled ? 1 : 0;
@@ -2593,6 +2709,16 @@ static void initLoop(kgb_selfplay* sp, const kgb_selfplay_config& c) {
     d.vwCdfTable = dc;
   }
   d.recentScoreCenter = sp->alloc<double>(G); d.leafTerminalScore = sp->alloc<float>(G);
+  d.modelVersion = hd.model->version;
+  d.shorttermValueErrorMultiplier = hd.model->shorttermValueErrorMultiplier; d.shorttermScoreErrorMultiplier = hd.model->shorttermScoreErrorMultiplier;
+  d.useUncertainty = (c.use_uncertainty && d.modelVersion >= 9) ? 1 : 0;   // NNEvaluator::supportsShorttermError (nneval.cpp:299-301)
+  d.uncertaintyCoeff = c.uncertainty_coeff; d.uncertaintyExponent = c.uncertainty_exponent; d.uncertaintyMaxWeight = c.uncertainty_max_weight;
+  if(c.use_uncertainty && !(c.uncertainty_coeff > 0.0 && c.uncertainty_max_weight > 0.0))
+    throw std::invalid_argument("selfplay: use_uncertainty needs uncertainty_coeff > 0 and uncertainty_max_weight > 0");
+  d.nodeNNWeight = d.useUncertainty ? sp->alloc<double>(G * N) : nullptr;
+  d.useNoisePruning = c.use_noise_pruning ? 1 : 0;
+  d.noisePruneUtilityScale = c.noise_prune_utility_scale; d.noisePruningCap = c.noise_pruning_cap;
+  if(d.useNoisePruning && !(c.noise_prune_utility_scale > 0.0)) throw std::invalid_argument("selfplay: use_noise_pruning needs noise_prune_utility_scale > 0");
   sp->refused = sp->alloc<int>(1);
   // initial state: empty boards, black to move, history empty, one unevaluated root node per game
   std::vector<int> ones(G, 1), minus(G * 5, -1), kos(G, -1);
@@ -2704,6 +2830,39 @@ KGB_API int kgb_selfplay_get_root_children(kgb_selfplay* sp, int game, int32_t* 
     sp->download(child.data(), d.childNode + nb, d.policySize);
     sp->download(avg.data(), d.nodeUtilAvg + (size_t)game * d.maxNodes, d.maxNodes);
     for(int i = 0; i < d.policySize; i++) util_sum[i] = child[i] >= 0 ? avg[child[i]] : 0.0;
+  });
+}
+
+KGB_API int kgb_selfplay_get_root_weights(kgb_selfplay* sp, int game, double* child_weights, double* root_weights) {
+  return guarded([&] {
+    if(!sp || !child_weights || !root_weights) throw std::invalid_argument("kgb_selfplay_get_root_weights: NULL argument");
+    sp->enter();
+    const SPDev& d = sp->d;
+    sp->checkGame(game);
+    std::vector<int> child(d.policySize);
+    std::vector<double> ws(d.maxNodes), wsq(d.maxNodes);
+    sp->download(child.data(), d.childNode + (size_t)game * d.maxNodes * d.policySize, d.policySize);
+    sp->download(ws.data(), d.nodeWeightSum + (size_t)game * d.maxNodes, d.maxNodes);
+    sp->download(wsq.data(), d.nodeWeightSqSum + (size_t)game * d.maxNodes, d.maxNodes);
+    for(int i = 0; i < d.policySize; i++) {
+      child_weights[i * 2] = child[i] >= 0 ? ws[child[i]] : 0.0;
+      child_weights[i * 2 + 1] = child[i] >= 0 ? wsq[child[i]] : 0.0;
+    }
+    root_weights[0] = ws[0]; root_weights[1] = wsq[0];
+  });
+}
+
+KGB_API int kgb_test_uncertainty_weight(int n, const int32_t* model_version, const double* raw, const double* params, double* out) {
+  return guarded([&] {
+    if(n < 0 || !model_version || !raw || !params || !out) throw std::invalid_argument("kgb_test_uncertainty_weight: bad argument");
+    for(int i = 0; i < n; i++) {
+      const double* r = raw + (size_t)i * 2;
+      const double* p = params + (size_t)i * 12;
+      float wl, se;
+      shorttermErrors(model_version[i], p[0], p[1], r[0], r[1], wl, se);
+      out[i * 3] = wl; out[i * 3 + 1] = se;
+      out[i * 3 + 2] = uncertaintyWeight(p[2], p[3], p[4], p[5], p[6], p[7], p[8], p[9], p[10], (float)p[11], wl, se);
+    }
   });
 }
 

@@ -31,6 +31,18 @@ def bot_cfg(cfg, idx):
     return out
 
 
+def match_default_note(cfg):
+    """The log line for uncertainty weighting / noise pruning left unset: the reference's `katago match` loads its bots with
+    SETUP_FOR_MATCH, where both default to true (program/setup.cpp:522-544); here an unset key stays off, so that existing match
+    configurations keep playing the same games.  None when every bot sets both."""
+    import re
+    absent = [k for k in ("useUncertainty", "useNoisePruning") if not any(c == k or re.fullmatch(k + r"\d+", c) for c in cfg)]
+    if not absent:
+        return None
+    return (f"[config] {' and '.join(absent)} not set: off here, while the reference's katago match defaults "
+            f"{'them' if len(absent) > 1 else 'it'} to true; set {', '.join(k + ' = true' for k in absent)} to search like it")
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser(prog="katago_b200.match_cli", description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("-config", required=True)
@@ -72,6 +84,9 @@ def main(argv=None):
     games = max(2, min(a.games_per_gpu, int(cfg.get("numGameThreads", a.games_per_gpu)), total))
     gpu = int(os.environ.get("LOCAL_RANK", "0"))
     log("Match Engine starting...")
+    note = match_default_note(cfg)
+    if note:
+        log(note)
     loops, owned, data0 = [], [], None
     for i in range(2):
         kw, data, report = C.selfplay_kwargs_from_cfg({k: v for k, v in bot_cfg(cfg, i).items() if k not in ("numBots", "numGamesTotal")})

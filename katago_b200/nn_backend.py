@@ -63,6 +63,9 @@ class SelfplayConfig(C.Structure):
         ("chosen_move_subtract", C.c_double), ("chosen_move_prune", C.c_double),
         ("nn_cache_size_power_of_two", C.c_int32), ("root_num_symmetries_to_sample", C.c_int32),
         ("ko_rule", C.c_int32), ("full_history_rules", C.c_int32), ("root_ending_bonus_points", C.c_double),
+        ("use_uncertainty", C.c_int32), ("uncertainty_coeff", C.c_double), ("uncertainty_exponent", C.c_double),
+        ("uncertainty_max_weight", C.c_double), ("use_noise_pruning", C.c_int32), ("noise_prune_utility_scale", C.c_double),
+        ("noise_pruning_cap", C.c_double),
     ]
 
 
@@ -86,7 +89,7 @@ ABI_SYMBOLS = [
     "kgb_selfplay_debug_cycles", "kgb_selfplay_release", "kgb_selfplay_get_root_visits", "kgb_selfplay_get_root_extra", "kgb_selfplay_get_last_move",
     "kgb_selfplay_set_game_setup", "kgb_selfplay_get_game_setup", "kgb_selfplay_play_moves_game",
     "kgb_selfplay_set_next_search_limits", "kgb_selfplay_get_search_limits", "kgb_selfplay_set_policy_init", "kgb_selfplay_get_policy_init",
-    "kgb_selfplay_get_root_raw_policy_entropy", "kgb_selfplay_get_nn_symmetries",
+    "kgb_selfplay_get_root_raw_policy_entropy", "kgb_selfplay_get_nn_symmetries", "kgb_selfplay_get_root_weights", "kgb_test_uncertainty_weight",
 ]
 
 _lib = None
@@ -162,6 +165,8 @@ def load_library():
     lib.kgb_selfplay_play_moves.argtypes = [P, P, I]
     lib.kgb_selfplay_random_openings.argtypes = [P, I]
     lib.kgb_selfplay_get_root_value_stats.argtypes = [P, I, P, P]
+    lib.kgb_selfplay_get_root_weights.argtypes = [P, I, P, P]
+    lib.kgb_test_uncertainty_weight.argtypes = [I, P, P, P, P]
     lib.kgb_selfplay_release.argtypes = [P, P]
     lib.kgb_selfplay_get_root_visits.argtypes = [P, P]
     lib.kgb_selfplay_get_root_extra.argtypes = [P, I, P, P]
@@ -503,6 +508,24 @@ def expected_white_score_value(mean, stdev, center, scale, sqrt_board_area):
     return out
 
 
+def uncertainty_weight(model_version, raw_winloss, raw_score, value_error_multiplier=0.25, score_error_multiplier=30.0, coeff=0.25,
+                       exponent=1.0, max_weight=8.0, win_loss_utility_factor=1.0, static_score_utility_factor=0.0,
+                       dynamic_score_utility_factor=0.0, dynamic_score_center_scale=1.0, center=0.0, sqrt_board_area=19.0,
+                       white_score_mean=0.0):
+    """kgb_test_uncertainty_weight for arrays of arguments: (shorttermWinlossError, shorttermScoreError, weight), the short-term
+    error post-processing of the net's raw channels 4 and 5 and Search::computeWeightFromNNOutput as the device loop does them."""
+    ver = np.ascontiguousarray(np.asarray(model_version, np.int32).reshape(-1))
+    n = ver.size
+    col = lambda v: np.broadcast_to(np.asarray(v, np.float64).reshape(-1), (n,))
+    raw = np.ascontiguousarray(np.stack([col(raw_winloss), col(raw_score)], axis=1))
+    params = np.ascontiguousarray(np.stack([col(v) for v in (value_error_multiplier, score_error_multiplier, coeff, exponent, max_weight,
+                                                             win_loss_utility_factor, static_score_utility_factor, dynamic_score_utility_factor,
+                                                             dynamic_score_center_scale, center, sqrt_board_area, white_score_mean)], axis=1))
+    out = np.zeros((n, 3), np.float64)
+    _check(load_library().kgb_test_uncertainty_weight(n, ver.ctypes.data, raw.ctypes.data, params.ctypes.data, out.ctypes.data))
+    return out[:, 0], out[:, 1], out[:, 2]
+
+
 def board_replay(x_size: int, y_size: int, moves, multi_stone_suicide_legal: bool):
     """kgb_test_board_replay: moves int8 [boards, m, 3] = (x, y, pla) with (-1,-1) = pass, pla 1 black / 2 white.
     Returns dict(colors [b,m,Y,X], ko [b,m,2], caps [b,m,2], lib_class [b,m,Y,X], legal_next [b,m,Y,X])."""
@@ -527,7 +550,7 @@ class SelfPlay:
                  multi_stone_suicide_legal: bool = True, early_temperature_moves: int = 30, cpuct_exploration: float = 1.0,
                  cpuct_exploration_log: float = 0.45, cpuct_exploration_base: float = 500.0, fpu_reduction_max: float = 0.2,
                  root_fpu_reduction_max: float = 0.1, win_loss_utility_factor: float = 1.0, no_result_utility_for_white: float = 0.0,
-                 seed: int = 0, debug_fake_nn: bool = False, disable_ladder_features: bool = False, ladder_nodes_per_wave: int = 0, max_playouts_per_wave: int = 0,
+                 seed: int = 0, debug_fake_nn: int = 0, disable_ladder_features: bool = False, ladder_nodes_per_wave: int = 0, max_playouts_per_wave: int = 0,
                  static_score_utility_factor: float = 0.0, dynamic_score_utility_factor: float = 0.0,
                  dynamic_score_center_zero_weight: float = 0.0, dynamic_score_center_scale: float = 1.0,
                  draw_equivalent_wins_for_white: float = 0.5, value_weight_exponent: float = 0.0,
@@ -545,7 +568,10 @@ class SelfPlay:
                  chosen_move_temperature_early: float = 0.0, chosen_move_temperature_only_below_prob: float = 1.0,
                  chosen_move_subtract: float = 0.0, chosen_move_prune: float = 1.0, nn_cache_size_power_of_two: int = 0, root_num_symmetries_to_sample: int = 1,
                  ko_rule: int = 0, full_history_rules: bool = False, debug_fixed_symmetry: int = -1,
-                 root_ending_bonus_points: float = 0.0, root_prune_useless_moves: bool = False):
+                 root_ending_bonus_points: float = 0.0, root_prune_useless_moves: bool = False,
+                 use_uncertainty: bool = False, uncertainty_coeff: float = 0.25, uncertainty_exponent: float = 1.0,
+                 uncertainty_max_weight: float = 8.0, use_noise_pruning: bool = False, noise_prune_utility_scale: float = 0.15,
+                 noise_pruning_cap: float = 1e50):
         lib = load_library()
         self.handle = handle
         self.cfg = SelfplayConfig(num_games, max_visits, max_moves, int(multi_stone_suicide_legal), early_temperature_moves, komi,
@@ -563,7 +589,9 @@ class SelfPlay:
                                   int(use_play_selection), int(use_lcb_for_selection), int(use_non_buggy_lcb), int(root_prune_useless_moves), lcb_stdevs, min_visit_prop_for_lcb,
                                   chosen_move_temperature, chosen_move_temperature_early, chosen_move_temperature_only_below_prob,
                                   chosen_move_subtract, chosen_move_prune, int(nn_cache_size_power_of_two), int(root_num_symmetries_to_sample),
-                                  int(ko_rule), int(full_history_rules), float(root_ending_bonus_points))
+                                  int(ko_rule), int(full_history_rules), float(root_ending_bonus_points),
+                                  int(use_uncertainty), float(uncertainty_coeff), float(uncertainty_exponent), float(uncertainty_max_weight),
+                                  int(use_noise_pruning), float(noise_prune_utility_scale), float(noise_pruning_cap))
         self._p = C.c_void_p()
         _check(lib.kgb_selfplay_create(handle._p, C.byref(self.cfg), C.byref(self._p)))
         self.x, self.y = handle.context.nnXLen, handle.context.nnYLen
@@ -625,6 +653,12 @@ class SelfPlay:
         """(children [X*Y+1, 5], root [5]): winLossValueAvg, noResultValueAvg, scoreMeanAvg, scoreMeanSqAvg, leadAvg."""
         ch = np.zeros((self.x * self.y + 1, 5), np.float64); rt = np.zeros(5, np.float64)
         _check(load_library().kgb_selfplay_get_root_value_stats(self._p, g, ch.ctypes.data, rt.ctypes.data))
+        return ch, rt
+
+    def root_weights(self, g: int):
+        """(children [X*Y+1, 2], root [2]): NodeStats weightSum and weightSqSum of game g's root children and root."""
+        ch = np.zeros((self.x * self.y + 1, 2), np.float64); rt = np.zeros(2, np.float64)
+        _check(load_library().kgb_selfplay_get_root_weights(self._p, g, ch.ctypes.data, rt.ctypes.data))
         return ch, rt
 
     # ---- game recording (hold mode, kgb200.h) ----

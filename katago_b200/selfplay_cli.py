@@ -49,6 +49,10 @@ _SEARCH_KEYS = {
     "rootNumSymmetriesToSample": ("root_num_symmetries_to_sample", int), "nnCacheSizePowerOfTwo": ("nn_cache_size_power_of_two", int),
     "maxMovesPerGame": ("max_moves", int),
     "rootEndingBonusPoints": ("root_ending_bonus_points", float), "rootPruneUselessMoves": ("root_prune_useless_moves", _B),
+    "useUncertainty": ("use_uncertainty", _B), "uncertaintyCoeff": ("uncertainty_coeff", float),
+    "uncertaintyExponent": ("uncertainty_exponent", float), "uncertaintyMaxWeight": ("uncertainty_max_weight", float),
+    "useNoisePruning": ("use_noise_pruning", _B), "noisePruneUtilityScale": ("noise_prune_utility_scale", float),
+    "noisePruningCap": ("noise_pruning_cap", float),
 }
 # keys that only place or log the reference's own CPU threads / evaluator servers: nothing to do here
 _IRRELEVANT_PREFIXES = ("log", "cuda", "trt", "opencl", "eigen", "metal", "numNNServerThreads", "nnMaxBatchSize", "nnMutexPool", "numSearchThreads",
@@ -71,6 +75,8 @@ _REFERENCE_DEFAULTS = {
     "use_non_buggy_lcb": False, "lcb_stdevs": 5.0, "min_visit_prop_for_lcb": 0.15, "chosen_move_temperature": 0.10, "chosen_move_temperature_early": 0.50,
     "chosen_move_temperature_only_below_prob": 1.0, "chosen_move_subtract": 0.0, "chosen_move_prune": 1.0, "nn_cache_size_power_of_two": 0,
     "root_num_symmetries_to_sample": 1, "root_ending_bonus_points": 0.5, "root_prune_useless_moves": True,
+    "use_uncertainty": False, "uncertainty_coeff": 0.25, "uncertainty_exponent": 1.0, "uncertainty_max_weight": 8.0,
+    "use_noise_pruning": False, "noise_prune_utility_scale": 0.15, "noise_pruning_cap": 1e50,
 }
 # options the reference switches ON by default and the loop does not have: reported even when the key is absent (none at present)
 _DEFAULT_ON_NOT_BUILT = {}
