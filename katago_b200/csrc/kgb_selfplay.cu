@@ -417,6 +417,22 @@ __device__ __forceinline__ void rootHashesInit(const SPDev& d, int g, int lane) 
   }
   if(lane == 0) { d.nodePosH0[gb] = h0; d.nodePosH1[gb] = h1; d.nodeGH0[gb] = s0; d.nodeGH1[gb] = s1; }
 }
+// The transposition table emptied and the root node's hashes set from the stored root position.
+__device__ __forceinline__ void rootTableReset(const SPDev& d, int g, int lane) {
+  nodeTableClear(d, g, lane);
+  __syncwarp();
+  rootHashesInit(d, g, lane);
+  __syncwarp();
+}
+// After the root position changed: node 0 = the unevaluated root, every other node freed, every subtree value bias entry unused
+// and dropped (search.cpp:860-861).
+__device__ __forceinline__ void treeReset(const SPDev& d, int g, int lane) {
+  const size_t gb = (size_t)g * d.maxNodes;
+  if(lane == 0) { d.nodeCount[g] = 1; nodeStatsReset(d, gb, false); d.rootSymCount[g] = 0; }
+  nodeInit(d, gb * d.policySize, lane);
+  biasTableClear(d, g, lane);
+  rootTableReset(d, g, lane);
+}
 
 __device__ __forceinline__ double rootChildUtilityWithBonus(const SPDev& d, int g, size_t gb, int c, int mv, double utilityAvg);
 __device__ double scoreUtilityDiff(const SPDev& d, int g, double scoreMean, double scoreMeanSq, double delta, double center);
@@ -625,8 +641,83 @@ __device__ void gameOverStartNext(const SPDev& d, int g, WarpBoard& bd, bool noR
   __syncwarp();
   boardInit(bd, d.gX[g], d.gY[g]);
   gameHistReset(d, g, lane);
+  if(lane == 0) { d.passStreak[g * 2] = 0; d.passStreak[g * 2 + 1] = 0; }
+}
+
+// Game g's root board as stored; with withHash also its Zobrist hash (else 0, as boardInit leaves it).
+__device__ __forceinline__ void rootBoardLoad(const SPDev& d, int g, int lane, WarpBoard& bd, bool withHash) {
+  boardInit(bd, d.gX[g], d.gY[g]);
+  bd.b = d.rootB[g * 32 + lane]; bd.w = d.rootW[g * 32 + lane];
+  bd.ko = d.rootKo[g]; bd.capB = d.rootCapB[g]; bd.capW = d.rootCapW[g];
+  if(withHash) { bd.h0 = d.rootPosH[g * 2]; bd.h1 = d.rootPosH[g * 2 + 1]; }
+}
+// A game's root position while one warp plays moves there: the board and the per-game scalars in registers.  The last five moves
+// (hist) and the boards one and two moves ago (prevB/W/Ko, BoardHistory::getRecentBoard, for ladder planes 15/16) move along in
+// memory, so that rootAdvance holds no more registers across gameMakeMove than the board before the move.
+struct RootPos {
+  WarpBoard bd;
+  bool black;
+  int moveNum, passes;
+};
+__device__ __forceinline__ void rootLoad(const SPDev& d, int g, int lane, RootPos& rp) {
+  rootBoardLoad(d, g, lane, rp.bd, true);
+  rp.black = d.rootBlackToMove[g] != 0;
+  rp.moveNum = d.moveNum[g]; rp.passes = d.consecPasses[g];
+}
+__device__ __forceinline__ void rootStore(const SPDev& d, int g, int lane, const RootPos& rp) {
+  d.rootB[g * 32 + lane] = rp.bd.b; d.rootW[g * 32 + lane] = rp.bd.w;
+  if(lane == 0) {
+    d.rootKo[g] = rp.bd.ko; d.rootCapB[g] = rp.bd.capB; d.rootCapW[g] = rp.bd.capW;
+    d.rootPosH[g * 2] = rp.bd.h0; d.rootPosH[g * 2 + 1] = rp.bd.h1;
+    d.rootBlackToMove[g] = rp.black ? 1 : 0; d.moveNum[g] = rp.moveNum; d.consecPasses[g] = rp.passes;
+  }
+}
+// One move p (y*32+x, or -1 = pass) of the game at its root.
+__device__ __forceinline__ void rootPlay(const SPDev& d, int g, int lane, RootPos& rp, int p, bool& finished, bool& noResult) {
+  const uint32_t beforeB = rp.bd.b, beforeW = rp.bd.w; const int beforeKo = rp.bd.ko;
+  gameMakeMove(d, g, rp.bd, p, rp.black, lane, rp.passes, finished, noResult);
+  const int h = lane < 5 ? d.hist[g * 5 + lane] : -1;
+  const int older = __shfl_up_sync(KGB_FULL, h, 1);
+  if(lane < 5) d.hist[g * 5 + lane] = lane == 0 ? (p < 0 ? -2 : p) : older;
+  const size_t G32 = (size_t)d.numGames * 32;
+  d.prevB[G32 + g * 32 + lane] = d.prevB[g * 32 + lane]; d.prevW[G32 + g * 32 + lane] = d.prevW[g * 32 + lane];
+  d.prevB[g * 32 + lane] = beforeB; d.prevW[g * 32 + lane] = beforeW;
+  if(lane == 0) { d.prevKo[d.numGames + g] = d.prevKo[g]; d.prevKo[g] = beforeKo; }
+  rp.black = !rp.black;
+  rp.moveNum++;
+}
+// The root move record (lastMove): move position pos, end flags, the move's number, the game's index in its slot.
+__device__ __forceinline__ void recordRootMove(const SPDev& d, int g, int lane, int pos, bool over, bool finished, bool noResult, int moveNum) {
+  if(lane == 0) {
+    d.lastMove[g * 4 + 0] = pos;
+    d.lastMove[g * 4 + 1] = over ? (1 | (noResult ? 2 : 0) | (finished ? 0 : 4)) : 0;
+    d.lastMove[g * 4 + 2] = moveNum;
+    d.lastMove[g * 4 + 3] = (int)d.gameCounter[g];
+  }
+}
+// The root move just played ended the game: the slot's next game starts from an empty root without history.
+__device__ __forceinline__ void rootGameOver(const SPDev& d, int g, int lane, RootPos& rp, bool noResult) {
+  gameOverStartNext(d, g, rp.bd, noResult, lane);
+  rp.black = true; rp.moveNum = 0; rp.passes = 0;
+  const size_t G32 = (size_t)d.numGames * 32;
   if(lane < 5) d.hist[g * 5 + lane] = -1;
-  if(lane == 0) { d.rootBlackToMove[g] = 1; d.passStreak[g * 2] = 0; d.passStreak[g * 2 + 1] = 0; }
+  d.prevB[g * 32 + lane] = 0; d.prevW[g * 32 + lane] = 0; d.prevB[G32 + g * 32 + lane] = 0; d.prevW[G32 + g * 32 + lane] = 0;
+  if(lane == 0) { d.prevKo[g] = -1; d.prevKo[d.numGames + g] = -1; }
+}
+// Laddered stones of the two previous boards (planes 15/16 at the root), searched again after moves the search did not make.
+__device__ __forceinline__ void rootPrevLadders(const SPDev& d, int g, int lane) {
+  if(!d.enableLadders) return;
+  const size_t G32 = (size_t)d.numGames * 32;
+  const LadderScratch sc = ladderScratchAt(d.ladderScratch + (size_t)g * SP_LADDER_WARPS * ladderScratchWordsPerWarp());
+  __syncwarp();   // prevKo was written by lane 0
+  WarpBoard pb;
+  boardInit(pb, d.gX[g], d.gY[g]);
+  uint32_t l1, l2, wB, wW;
+  pb.b = d.prevB[g * 32 + lane]; pb.w = d.prevW[g * 32 + lane]; pb.ko = d.prevKo[g];
+  boardLadders(pb, sc, d.gX[g], d.gY[g], l1, wB, wW);
+  pb.b = d.prevB[G32 + g * 32 + lane]; pb.w = d.prevW[G32 + g * 32 + lane]; pb.ko = d.prevKo[d.numGames + g];
+  boardLadders(pb, sc, d.gX[g], d.gY[g], l2, wB, wW);
+  d.prevLad[g * 32 + lane] = l1; d.prevLad[G32 + g * 32 + lane] = l2;
 }
 
 // Choose and play the root move once the visit budget is spent; restart the game when it is over.
@@ -706,52 +797,21 @@ __device__ void rootAdvance(const SPDev& d, int g, int lane) {
   }
   if(bestV <= 0) best = d.policySize - 1;  // nothing searched (cannot happen with maxVisits >= 2): pass
   // play it on the root board
-  WarpBoard bd;
-  boardInit(bd, d.gX[g], d.gY[g]);
-  bd.b = d.rootB[g * 32 + lane]; bd.w = d.rootW[g * 32 + lane];
-  bd.ko = d.rootKo[g]; bd.capB = d.rootCapB[g]; bd.capW = d.rootCapW[g];
-  const bool black = d.rootBlackToMove[g] != 0;
-  const bool isPass = best == d.policySize - 1;
-  const int p = isPass ? -1 : pointOfPos(best, d.X);
-  const uint32_t beforeB = bd.b, beforeW = bd.w; const int beforeKo = bd.ko;
-  bd.h0 = d.rootPosH[g * 2]; bd.h1 = d.rootPosH[g * 2 + 1];
-  int passes = d.consecPasses[g];
+  RootPos rp;
+  rootLoad(d, g, lane, rp);
   bool finished = false, noResult = false;
-  gameMakeMove(d, g, bd, p, black, lane, passes, finished, noResult);
-  int mv = d.moveNum[g] + 1;
-  bool over = finished || mv >= d.maxMoves;
-  if(lane == 0) {
-    d.lastMove[g * 4 + 0] = best;
-    d.lastMove[g * 4 + 1] = over ? (1 | (noResult ? 2 : 0) | (finished ? 0 : 4)) : 0;
-    d.lastMove[g * 4 + 2] = mv - 1;
-    d.lastMove[g * 4 + 3] = (int)d.gameCounter[g];
-  }
-  if(over) {
-    gameOverStartNext(d, g, bd, noResult, lane);
-    passes = 0; mv = 0;
-  }
+  rootPlay(d, g, lane, rp, best == d.policySize - 1 ? -1 : pointOfPos(best, d.X), finished, noResult);
+  const bool over = finished || rp.moveNum >= d.maxMoves;
+  recordRootMove(d, g, lane, best, over, finished, noResult, rp.moveNum - 1);
+  if(over) rootGameOver(d, g, lane, rp, noResult);
   else {
-    int h = lane < 5 ? d.hist[g * 5 + lane] : -1;
-    int shifted = __shfl_up_sync(KGB_FULL, h, 1);
-    if(lane < 5) d.hist[g * 5 + lane] = lane == 0 ? (isPass ? -2 : p) : shifted;
-    if(lane == 0) d.rootBlackToMove[g] = black ? 0 : 1;
     const size_t G32 = (size_t)d.numGames * 32;
-    d.prevB[G32 + g * 32 + lane] = d.prevB[g * 32 + lane]; d.prevW[G32 + g * 32 + lane] = d.prevW[g * 32 + lane];
-    d.prevB[g * 32 + lane] = beforeB; d.prevW[g * 32 + lane] = beforeW;
-    if(lane == 0) { d.prevKo[d.numGames + g] = d.prevKo[g]; d.prevKo[g] = beforeKo; }
     d.prevLad[G32 + g * 32 + lane] = d.prevLad[g * 32 + lane];
     d.prevLad[g * 32 + lane] = d.nodeLad[gb * 32 + lane];   // the old root was evaluated, so its ladders are known
   }
-  d.rootB[g * 32 + lane] = bd.b; d.rootW[g * 32 + lane] = bd.w;
+  rootStore(d, g, lane, rp);
   if(lane == 0) {
-    d.rootKo[g] = bd.ko; d.rootCapB[g] = bd.capB; d.rootCapW[g] = bd.capW;
-    d.rootPosH[g * 2] = bd.h0; d.rootPosH[g * 2 + 1] = bd.h1;   // boardInit zeroes them for a new game
-    d.moveNum[g] = mv; d.consecPasses[g] = passes;
     atomicAdd(d.totalMoves, 1ULL);
-    // reset the tree: node 0 = unevaluated root
-    d.nodeCount[g] = 1;
-    nodeStatsReset(d, gb, false);
-    d.rootSymCount[g] = 0;
     // the new root's search limits (kgb_selfplay_set_next_search_limits)
     d.visitBudget[g] = d.nextBudget[g * 2 + (over ? 1 : 0)];
     d.plainRoot[g] = d.nextPlain[g * 2 + (over ? 1 : 0)];
@@ -763,12 +823,7 @@ __device__ void rootAdvance(const SPDev& d, int g, int lane) {
     }
     if(d.initMovesLeft[g] > 0) { d.visitBudget[g] = 1; d.plainRoot[g] = 1; }   // an opening root: one plain evaluation, then the policy draw
   }
-  nodeInit(d, rootBase, lane);
-  biasTableClear(d, g, lane);   // all nodes freed: every entry is unused and dropped (search.cpp:860-861)
-  nodeTableClear(d, g, lane);
-  __syncwarp();
-  rootHashesInit(d, g, lane);
-  __syncwarp();
+  treeReset(d, g, lane);
 }
 
 __device__ void recomputeNodeStats(const SPDev& d, int g, int node, bool nodePlaWhite, double* sh, int lane);
@@ -811,9 +866,7 @@ __device__ void spSelectWarp0(const SPDev& d, int g, int lane, uint32_t* shB, ui
     { const long long t_ = clock64(); pfAdvance += t_ - pfT; pfT = t_; }
 #endif
   }
-  boardInit(bd, d.gX[g], d.gY[g]);
-  bd.b = d.rootB[g * 32 + lane]; bd.w = d.rootW[g * 32 + lane];
-  bd.ko = d.rootKo[g]; bd.capB = d.rootCapB[g]; bd.capW = d.rootCapW[g];
+  rootBoardLoad(d, g, lane, bd, d.histRules != 0);   // under the full rules the hash follows the whole path: ko hashes are taken from it
   const bool rootBlack = d.rootBlackToMove[g] != 0;
   black = rootBlack;
   passes = d.consecPasses[g];
@@ -829,7 +882,6 @@ __device__ void spSelectWarp0(const SPDev& d, int g, int lane, uint32_t* shB, ui
     hst.passes = passes; hst.finished = false; hst.noResult = false;
     hst.everOcc = d.gEverOcc[g * 32 + lane]; hst.banned = d.rootBanned[g * 32 + lane];
     bannedValid = true;
-    bd.h0 = d.rootPosH[g * 2]; bd.h1 = d.rootPosH[g * 2 + 1];   // the hash follows the whole path: ko hashes are taken from it
   }
   bool instant = false;   // this playout ended on an existing edge: back it up here, no leaf
 #ifdef KGB_PROFILE_DESCENT   // build variant for tests/gpu_checks/descent_profile.py: where a descent step spends its cycles
@@ -1740,6 +1792,14 @@ __device__ void computeRootExtras(const SPDev& d, int g, const WarpBoard& bd, bo
   }
   __syncwarp();
 }
+// Search::recentScoreCenter of a fresh root from the expected score of its first evaluation (Search::beginSearch, search.cpp:1148-1153).
+__device__ __forceinline__ double rootScoreCenter(const SPDev& d, int g, double whiteScoreMean) {
+  double c = whiteScoreMean * (1.0 - d.dynamicScoreCenterZeroWeight);
+  const double cap = sqrt((double)(d.gX[g] * d.gY[g])) * d.dynamicScoreCenterScale;
+  if(c > whiteScoreMean + cap) c = whiteScoreMean + cap;
+  if(c < whiteScoreMean - cap) c = whiteScoreMean - cap;
+  return c;
+}
 // Search::getUtilityFromNN (searchhelpers.cpp:304-307) from the NNOutput fields (floats, white's perspective); a fresh root
 // first centres the dynamic score utility on its expected score (Search::beginSearch, search.cpp:1125-1154).
 __device__ double utilityFromEval(const SPDev& d, int g, int node, float whiteWin, float whiteLoss, float noResult, float whiteScoreMeanF,
@@ -1754,10 +1814,7 @@ __device__ double utilityFromEval(const SPDev& d, int g, int node, float whiteWi
   if(d.staticScoreUtilityFactor != 0.0 || d.dynamicScoreUtilityFactor != 0.0) {
     const double whiteScoreMean = (double)whiteScoreMeanF, whiteScoreMeanSq = (double)whiteScoreMeanSqF;
     if(node == 0 && d.nodeVisits[gb] == 0 && rootSyms(d, g) <= 1) {
-      double c = whiteScoreMean * (1.0 - d.dynamicScoreCenterZeroWeight);
-      const double cap = sqrt((double)(d.gX[g] * d.gY[g])) * d.dynamicScoreCenterScale;
-      if(c > whiteScoreMean + cap) c = whiteScoreMean + cap;
-      if(c < whiteScoreMean - cap) c = whiteScoreMean - cap;
+      const double c = rootScoreCenter(d, g, whiteScoreMean);
       __syncwarp();
       if(lane == 0) d.recentScoreCenter[g] = c;
       __syncwarp();
@@ -2012,11 +2069,7 @@ __global__ void spBackupKernel(const SPDev d) {
     if(multiSymRoot) {
       if(symCount < 0) {
         // the centring evaluation: recentScoreCenter from its expected score (search.cpp:1148-1153), nothing else is kept
-        const double whiteScoreMean = (double)vals[3];
-        double c = whiteScoreMean * (1.0 - d.dynamicScoreCenterZeroWeight);
-        const double cap = sqrt((double)(d.gX[g] * d.gY[g])) * d.dynamicScoreCenterScale;
-        if(c > whiteScoreMean + cap) c = whiteScoreMean + cap;
-        if(c < whiteScoreMean - cap) c = whiteScoreMean - cap;
+        const double c = rootScoreCenter(d, g, (double)vals[3]);
         if(lane == 0) { d.recentScoreCenter[g] = c; d.rootSymCount[g] = 1; atomicAdd(d.stalledWaves, 1ULL); }   // a wave without a playout
         return;
       }
@@ -2037,8 +2090,7 @@ __global__ void spBackupKernel(const SPDev d) {
     else if(d.cacheSize > 0) cacheStore(d, g, node, d.leafKey[g * 2], d.leafKey[g * 2 + 1], vals, lane);   // before any root noise: the raw evaluation
     if(wantRootExtras) {
       WarpBoard rb;
-      boardInit(rb, d.gX[g], d.gY[g]);
-      rb.b = d.rootB[g * 32 + lane]; rb.w = d.rootW[g * 32 + lane]; rb.ko = d.rootKo[g];
+      rootBoardLoad(d, g, lane, rb, false);
       computeRootExtras(d, g, rb, leafBlack, true, multiSymRoot ? d.rootNumSymmetries : 1, lane);
     }
     maybeRootNoise(d, g, node, lane);
@@ -2102,71 +2154,24 @@ __global__ void spPlayMovesKernel(const SPDev d, const int8_t* moves, int numMov
   const int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if(g >= d.numGames || (onlyGame >= 0 && g != onlyGame)) return;
-  WarpBoard bd;
-  boardInit(bd, d.gX[g], d.gY[g]);
-  bd.b = d.rootB[g * 32 + lane]; bd.w = d.rootW[g * 32 + lane];
-  bd.ko = d.rootKo[g]; bd.capB = d.rootCapB[g]; bd.capW = d.rootCapW[g];
-  bool black = d.rootBlackToMove[g] != 0;
-  int passes = d.consecPasses[g], mv = d.moveNum[g];
-  int h[5];
-  for(int k = 0; k < 5; k++) h[k] = d.hist[g * 5 + k];
-  const size_t G32 = (size_t)d.numGames * 32;
-  uint32_t p1B = d.prevB[g * 32 + lane], p1W = d.prevW[g * 32 + lane], p2B = d.prevB[G32 + g * 32 + lane], p2W = d.prevW[G32 + g * 32 + lane];
-  int p1Ko = d.prevKo[g], p2Ko = d.prevKo[d.numGames + g];
-  bd.h0 = d.rootPosH[g * 2]; bd.h1 = d.rootPosH[g * 2 + 1];
+  RootPos rp;
+  rootLoad(d, g, lane, rp);
   for(int m = 0; m < numMoves; m++) {
-    const bool isPass = moves[m * 2] < 0;
-    const int p = isPass ? -1 : (moves[m * 2 + 1] * 32 + moves[m * 2]);
-    p2B = p1B; p2W = p1W; p2Ko = p1Ko; p1B = bd.b; p1W = bd.w; p1Ko = bd.ko;
+    const int p = moves[m * 2] < 0 ? -1 : (moves[m * 2 + 1] * 32 + moves[m * 2]);
     bool fin, nores;
-    gameMakeMove(d, g, bd, p, black, lane, passes, fin, nores);
-    for(int k = 4; k > 0; k--) h[k] = h[k - 1];
-    h[0] = isPass ? -2 : p;
-    black = !black;
-    mv++;
-    if(endGames && (fin || mv >= d.maxMoves)) {
+    rootPlay(d, g, lane, rp, p, fin, nores);
+    if(endGames && (fin || rp.moveNum >= d.maxMoves)) {
       // a move of the list ended the game (match play mirrors the opponent's moves into this loop, kgb_selfplay_play_moves_game): the same
       // game-over handling as when the loop's own move ends it - result kept readable, next game started; further moves go to that game
-      if(lane == 0) {
-        d.lastMove[g * 4 + 0] = isPass ? d.policySize - 1 : posOf(p, d.X);
-        d.lastMove[g * 4 + 1] = 1 | (nores ? 2 : 0) | (fin ? 0 : 4);
-        d.lastMove[g * 4 + 2] = mv - 1;
-        d.lastMove[g * 4 + 3] = (int)d.gameCounter[g];
-      }
+      recordRootMove(d, g, lane, p < 0 ? d.policySize - 1 : posOf(p, d.X), true, fin, nores, rp.moveNum - 1);
       __syncwarp();
-      gameOverStartNext(d, g, bd, nores, lane);
-      passes = 0; mv = 0; black = true;
-      for(int k = 0; k < 5; k++) h[k] = -1;
-      p1B = 0; p1W = 0; p2B = 0; p2W = 0; p1Ko = -1; p2Ko = -1;
+      rootGameOver(d, g, lane, rp, nores);
     }
   }
-  d.rootB[g * 32 + lane] = bd.b; d.rootW[g * 32 + lane] = bd.w;
-  d.prevB[g * 32 + lane] = p1B; d.prevW[g * 32 + lane] = p1W; d.prevB[G32 + g * 32 + lane] = p2B; d.prevW[G32 + g * 32 + lane] = p2W;
-  if(d.enableLadders) {
-    const LadderScratch sc = ladderScratchAt(d.ladderScratch + (size_t)g * SP_LADDER_WARPS * ladderScratchWordsPerWarp());
-    WarpBoard pb = bd;
-    uint32_t l1, l2, wB, wW;
-    pb.b = p1B; pb.w = p1W; pb.ko = p1Ko;
-    boardLadders(pb, sc, d.gX[g], d.gY[g], l1, wB, wW);
-    pb.b = p2B; pb.w = p2W; pb.ko = p2Ko;
-    boardLadders(pb, sc, d.gX[g], d.gY[g], l2, wB, wW);
-    d.prevLad[g * 32 + lane] = l1; d.prevLad[G32 + g * 32 + lane] = l2;
-  }
-  const size_t gb = (size_t)g * d.maxNodes;
-  if(lane == 0) {
-    d.prevKo[g] = p1Ko; d.prevKo[d.numGames + g] = p2Ko;
-    d.rootKo[g] = bd.ko; d.rootCapB[g] = bd.capB; d.rootCapW[g] = bd.capW;
-    d.rootBlackToMove[g] = black ? 1 : 0; d.consecPasses[g] = passes; d.moveNum[g] = mv;
-    for(int k = 0; k < 5; k++) d.hist[g * 5 + k] = h[k];
-    d.nodeCount[g] = 1; nodeStatsReset(d, gb, false);
-    d.ladPending[g] = 0; d.leafValid[g] = 0; d.rootSymCount[g] = 0;
-    d.rootPosH[g * 2] = bd.h0; d.rootPosH[g * 2 + 1] = bd.h1;
-  }
-  nodeInit(d, gb * d.policySize, lane);
-  biasTableClear(d, g, lane);
-  nodeTableClear(d, g, lane);
-  __syncwarp();
-  rootHashesInit(d, g, lane);
+  rootStore(d, g, lane, rp);
+  rootPrevLadders(d, g, lane);
+  if(lane == 0) { d.ladPending[g] = 0; d.leafValid[g] = 0; }
+  treeReset(d, g, lane);
 }
 
 // Desynchronise the games: every game's root is advanced by its own random number (0..maxLen) of uniformly random legal
@@ -2176,18 +2181,9 @@ __global__ void spRandomOpeningsKernel(const SPDev d, int maxLen) {
   const int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if(g >= d.numGames) return;
-  WarpBoard bd;
-  boardInit(bd, d.gX[g], d.gY[g]);
-  bd.b = d.rootB[g * 32 + lane]; bd.w = d.rootW[g * 32 + lane];
-  bd.ko = d.rootKo[g]; bd.capB = d.rootCapB[g]; bd.capW = d.rootCapW[g];
-  bd.h0 = d.rootPosH[g * 2]; bd.h1 = d.rootPosH[g * 2 + 1];
-  bool black = d.rootBlackToMove[g] != 0;
-  int mv = d.moveNum[g];
-  int h[5];
-  for(int k = 0; k < 5; k++) h[k] = d.hist[g * 5 + k];
-  const size_t G32 = (size_t)d.numGames * 32;
-  uint32_t p1B = d.prevB[g * 32 + lane], p1W = d.prevW[g * 32 + lane], p2B = d.prevB[G32 + g * 32 + lane], p2W = d.prevW[G32 + g * 32 + lane];
-  int p1Ko = d.prevKo[g], p2Ko = d.prevKo[d.numGames + g];
+  RootPos rp;
+  rootLoad(d, g, lane, rp);
+  rp.passes = 0;   // every move counts passes from 0 and the game's end is ignored; no move is a pass, so the count stays 0
   DevRand rand;
   if(lane == 0) rand.s = d.nonSearchRand[g];
   unsigned len = 0;
@@ -2195,8 +2191,8 @@ __global__ void spRandomOpeningsKernel(const SPDev d, int maxLen) {
   len = __shfl_sync(KGB_FULL, len, 0);
   for(unsigned m = 0; m < len; m++) {
     uint32_t l1, l2, l3;
-    boardLibertyClasses(bd, l1, l2, l3);
-    const uint32_t legal = boardLegalMask(bd, black, d.gMultiSuicide[g] != 0, l1) & ~(d.histRules ? d.rootBanned[g * 32 + lane] : 0u);
+    boardLibertyClasses(rp.bd, l1, l2, l3);
+    const uint32_t legal = boardLegalMask(rp.bd, rp.black, d.gMultiSuicide[g] != 0, l1) & ~(d.histRules ? d.rootBanned[g * 32 + lane] : 0u);
     const int n = warpCount(legal);
     if(n == 0) break;
     unsigned r = 0;
@@ -2214,52 +2210,21 @@ __global__ void spRandomOpeningsKernel(const SPDev d, int maxLen) {
     }
     const unsigned who = __ballot_sync(KGB_FULL, p >= 0);
     p = __shfl_sync(KGB_FULL, p, __ffs(who) - 1);
-    p2B = p1B; p2W = p1W; p2Ko = p1Ko; p1B = bd.b; p1W = bd.w; p1Ko = bd.ko;
-    int passesTmp = 0; bool fin, nores;
-    gameMakeMove(d, g, bd, p, black, lane, passesTmp, fin, nores);
-    for(int k = 4; k > 0; k--) h[k] = h[k - 1];
-    h[0] = p;
-    black = !black;
-    mv++;
+    bool fin, nores;
+    rootPlay(d, g, lane, rp, p, fin, nores);
   }
-  d.rootB[g * 32 + lane] = bd.b; d.rootW[g * 32 + lane] = bd.w;
-  d.prevB[g * 32 + lane] = p1B; d.prevW[g * 32 + lane] = p1W; d.prevB[G32 + g * 32 + lane] = p2B; d.prevW[G32 + g * 32 + lane] = p2W;
-  if(d.enableLadders) {
-    const LadderScratch sc = ladderScratchAt(d.ladderScratch + (size_t)g * SP_LADDER_WARPS * ladderScratchWordsPerWarp());
-    WarpBoard pb = bd;
-    uint32_t la, lb, wB, wW;
-    pb.b = p1B; pb.w = p1W; pb.ko = p1Ko;
-    boardLadders(pb, sc, d.gX[g], d.gY[g], la, wB, wW);
-    pb.b = p2B; pb.w = p2W; pb.ko = p2Ko;
-    boardLadders(pb, sc, d.gX[g], d.gY[g], lb, wB, wW);
-    d.prevLad[g * 32 + lane] = la; d.prevLad[G32 + g * 32 + lane] = lb;
-  }
-  const size_t gb = (size_t)g * d.maxNodes;
-  if(lane == 0) {
-    d.nonSearchRand[g] = rand.s;
-    d.prevKo[g] = p1Ko; d.prevKo[d.numGames + g] = p2Ko;
-    d.rootKo[g] = bd.ko; d.rootCapB[g] = bd.capB; d.rootCapW[g] = bd.capW;
-    d.rootBlackToMove[g] = black ? 1 : 0; d.consecPasses[g] = 0; d.moveNum[g] = mv;
-    for(int k = 0; k < 5; k++) d.hist[g * 5 + k] = h[k];
-    d.nodeCount[g] = 1; nodeStatsReset(d, gb, false);
-    d.ladPending[g] = 0; d.leafValid[g] = 0; d.rootSymCount[g] = 0;
-    d.rootPosH[g * 2] = bd.h0; d.rootPosH[g * 2 + 1] = bd.h1;
-  }
-  nodeInit(d, gb * d.policySize, lane);
-  biasTableClear(d, g, lane);
-  nodeTableClear(d, g, lane);
-  __syncwarp();
-  rootHashesInit(d, g, lane);
+  rootStore(d, g, lane, rp);
+  rootPrevLadders(d, g, lane);
+  if(lane == 0) { d.nonSearchRand[g] = rand.s; d.ladPending[g] = 0; d.leafValid[g] = 0; }
+  treeReset(d, g, lane);
 }
 
 __global__ void spInitRootsKernel(const SPDev d) {
   const int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if(g >= d.numGames) return;
-  nodeTableClear(d, g, lane);
   gameHistReset(d, g, lane);
-  __syncwarp();
-  rootHashesInit(d, g, lane);
+  rootTableReset(d, g, lane);
 }
 
 // ------------------------------------------------------------------------------------------------------------
