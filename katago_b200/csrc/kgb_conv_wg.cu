@@ -144,25 +144,55 @@ __device__ __forceinline__ int slice_offset(int r, int c, bool fp32) {
   return r * 64 + ((((c >> 3) ^ ((r >> 1) & 3)) << 4) | ((c & 7) << 1));
 }
 
-// Epilogue of two adjacent columns (col, col+1) of one accumulator row: r = the residual (used when p.residual is set), sc / bi =
+// What an epilogue does, as bits.  The kernel has one straight-line copy of the slice epilogue for every combination the nets
+// launch (epiDispatch below), with these choices made at compile time: a thread's 8 column pairs of a slice then form one run of
+// instructions whose shared-memory loads, ex2 and rcp overlap each other.  With the choices read from ConvParams per pair, each
+// pair is a chain of branches that waits out its own latencies, with two warps per scheduler to hide them.  Everything else (an
+// activation other than mish, in practice test launches) takes the EPI_RUNTIME copy.  Same arithmetic in every copy.
+enum EpiFlags {
+  EPI_RES = 1,       // + residual, read from the stream slice
+  EPI_RAW = 2,       // raw output written to the stream slice
+  EPI_FP32 = 4,      // the stream is fp32 (else fp16)
+  EPI_MISH = 8,      // BN + mish + mask -> fp16 operand
+  EPI_SPLIT = 16,    // the operand also gets its lo half
+  EPI_NCBIAS = 32,   // + per-image bias
+  EPI_RUNTIME = -1   // every choice read from ConvParams
+};
+__host__ __device__ inline int epiFlags(const ConvParams& p) {
+  if(p.act_out != nullptr && p.act != 2) return EPI_RUNTIME;
+  const bool stream = p.residual != nullptr || p.raw_out != nullptr;
+  return (p.residual != nullptr ? EPI_RES : 0) | (p.raw_out != nullptr ? EPI_RAW : 0) | (stream && streamFp32(p) ? EPI_FP32 : 0) |
+         (p.act_out != nullptr ? EPI_MISH | (p.split ? EPI_SPLIT : 0) : 0) | (p.ncbias != nullptr ? EPI_NCBIAS : 0);
+}
+
+// Epilogue of two adjacent columns (col, col+1) of one accumulator row: r = the residual (used when there is one), sc / bi =
 // the BN constants of col in shared memory.  raw goes to `raw_dst` in the stream slice, the activated operand to `act_dst` (and
 // its lo half to `act_lo_dst` in split mode).
+template <int F>
 __device__ __forceinline__ void epilogue_store(const ConvParams& p, int row, int col, float v0, float v1, float maskv, float2 r,
                                                const float* sc, const float* bi, uint8_t* raw_dst, uint8_t* act_dst,
                                                uint8_t* act_lo_dst) {
-  if(p.ncbias != nullptr) {
+  constexpr bool rt = F == EPI_RUNTIME;
+  const bool has_ncbias = rt ? p.ncbias != nullptr : (F & EPI_NCBIAS) != 0;
+  const bool has_res = rt ? p.residual != nullptr : (F & EPI_RES) != 0;
+  const bool has_raw = rt ? p.raw_out != nullptr : (F & EPI_RAW) != 0;
+  const bool raw_fp32 = rt ? p.raw_fp32 != 0 : (F & EPI_FP32) != 0;
+  const bool has_act = rt ? p.act_out != nullptr : (F & EPI_MISH) != 0;
+  const bool mish = rt ? p.act == 2 : true;
+  const bool split = rt ? p.split != 0 : (F & EPI_SPLIT) != 0;
+  if(has_ncbias) {
     const float2 b = __ldg(reinterpret_cast<const float2*>(p.ncbias + (size_t)(row / p.P) * p.cout_p + col));
     v0 += b.x; v1 += b.y;
   }
-  if(p.residual != nullptr) { v0 += r.x; v1 += r.y; }
-  if(p.raw_out != nullptr) {
-    if(p.raw_fp32) *reinterpret_cast<float2*>(raw_dst) = make_float2(v0 * maskv, v1 * maskv);
+  if(has_res) { v0 += r.x; v1 += r.y; }
+  if(has_raw) {
+    if(raw_fp32) *reinterpret_cast<float2*>(raw_dst) = make_float2(v0 * maskv, v1 * maskv);
     else *reinterpret_cast<__half2*>(raw_dst) = __floats2half2_rn(v0 * maskv, v1 * maskv);
   }
-  if(p.act_out != nullptr) {
+  if(has_act) {
     float a0 = fmaf(v0, sc[0], bi[0]);
     float a1 = fmaf(v1, sc[1], bi[1]);
-    if(p.act == 2) {   // mish(x) = x - 2x / (e^x (e^x + 2) + 2): overflow of e gives x, underflow gives 0, no clamps needed
+    if(mish) {   // mish(x) = x - 2x / (e^x (e^x + 2) + 2): overflow of e gives x, underflow gives 0, no clamps needed
       const float e0 = kgb_ex2(a0 * 1.4426950408889634f), e1 = kgb_ex2(a1 * 1.4426950408889634f);
       a0 = fmaf(-2.0f, a0 * kgb_rcp(fmaf(e0, e0 + 2.0f, 2.0f)), a0);
       a1 = fmaf(-2.0f, a1 * kgb_rcp(fmaf(e1, e1 + 2.0f, 2.0f)), a1);
@@ -174,11 +204,66 @@ __device__ __forceinline__ void epilogue_store(const ConvParams& p, int row, int
     if(maskv == 0.0f) { a0 = 0.0f; a1 = 0.0f; }   // pad and off-board rows (also guards NaN/inf garbage there)
     const __half2 h = __floats2half2_rn(a0, a1);
     *reinterpret_cast<__half2*>(act_dst) = h;
-    if(p.split) {
+    if(split) {
       const float2 hf = __half22float2(h);
       *reinterpret_cast<__half2*>(act_lo_dst) = __floats2half2_rn(a0 - hf.x, a1 - hf.y);
     }
   }
+}
+
+// One thread's part of slice s of a tile: 2 rows (rloc, rloc + 8) x 4 column pairs out of the accumulators into the slice's
+// stream and act slots.
+template <int F, int N>
+__device__ __forceinline__ void epilogue_slice(const ConvParams& p, const float (&acc)[N / 2], int s, int m0, int n0, int rloc, int lane,
+                                               float mask0, float mask1, const float* s_scale, const float* s_bias, uint8_t* slot,
+                                               uint8_t* aslot) {
+  constexpr bool rt = F == EPI_RUNTIME;
+  const bool has_res = rt ? p.residual != nullptr : (F & EPI_RES) != 0;
+  const bool s_fp32 = rt ? streamFp32(p) : (F & EPI_FP32) != 0;
+#pragma unroll
+  for(int h = 0; h < 2; h++) {
+    const int rl = rloc + 8 * h, row = m0 + rl;
+    if(row >= p.M) continue;   // no ncbias entry for rows past the batch; the TMA stores clip them
+    const float maskv = h ? mask1 : mask0;
+#pragma unroll
+    for(int jj = 0; jj < RES_COLS / 8; jj++) {
+      const int j = s * (RES_COLS / 8) + jj, lc = 8 * j + 2 * (lane & 3), c = lc - s * RES_COLS;
+      uint8_t* const rp = slot + slice_offset(rl, c, s_fp32);
+      uint8_t* const ap = aslot + slice_offset(rl, c, false);
+      const float2 r = has_res ? (s_fp32 ? *reinterpret_cast<const float2*>(rp) : __half22float2(*reinterpret_cast<const __half2*>(rp)))
+                               : make_float2(0.0f, 0.0f);
+      epilogue_store<F>(p, row, n0 + lc, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], maskv, r, s_scale + lc, s_bias + lc, rp, ap,
+                        ap + ACT_SLICE_BYTES);
+    }
+  }
+}
+
+// The compile-time copies: what the evaluator launches in fp16 mode (fp16 or fp32 streams) and in fp32-equivalent mode (split
+// operands, fp32 streams).  `flags` is the same for every thread of the launch.
+template <int N>
+__device__ __forceinline__ void epiDispatch(int flags, const ConvParams& p, const float (&acc)[N / 2], int s, int m0, int n0, int rloc,
+                                            int lane, float mask0, float mask1, const float* s_scale, const float* s_bias, uint8_t* slot,
+                                            uint8_t* aslot) {
+#define KGB_EPI(F) case (F): epilogue_slice<(F), N>(p, acc, s, m0, n0, rloc, lane, mask0, mask1, s_scale, s_bias, slot, aslot); break;
+  switch(flags) {
+    KGB_EPI(EPI_RAW | EPI_FP32)                                     // raw fp32 only: the gpool unit's first conv, the heads' 1x1
+    KGB_EPI(EPI_MISH)                                               // the first conv of a residual unit
+    KGB_EPI(EPI_RES | EPI_RAW | EPI_MISH)                           // the second conv of a unit, a nested block's post conv
+    KGB_EPI(EPI_RES | EPI_RAW | EPI_FP32 | EPI_MISH)
+    KGB_EPI(EPI_RES | EPI_MISH)                                     // the trunk's last block: the stream is not kept
+    KGB_EPI(EPI_RES | EPI_FP32 | EPI_MISH)
+    KGB_EPI(EPI_RAW | EPI_MISH)                                     // a nested block's pre conv
+    KGB_EPI(EPI_RAW | EPI_FP32 | EPI_MISH)
+    KGB_EPI(EPI_RAW | EPI_MISH | EPI_NCBIAS)                        // the initial conv
+    KGB_EPI(EPI_RAW | EPI_FP32 | EPI_MISH | EPI_NCBIAS)
+    KGB_EPI(EPI_MISH | EPI_SPLIT)                                   // fp32-equivalent mode
+    KGB_EPI(EPI_RES | EPI_RAW | EPI_FP32 | EPI_MISH | EPI_SPLIT)
+    KGB_EPI(EPI_RES | EPI_FP32 | EPI_MISH | EPI_SPLIT)
+    KGB_EPI(EPI_RAW | EPI_FP32 | EPI_MISH | EPI_SPLIT)
+    KGB_EPI(EPI_RAW | EPI_FP32 | EPI_MISH | EPI_SPLIT | EPI_NCBIAS)
+    default: epilogue_slice<EPI_RUNTIME, N>(p, acc, s, m0, n0, rloc, lane, mask0, mask1, s_scale, s_bias, slot, aslot);
+  }
+#undef KGB_EPI
 }
 
 template <int N>
@@ -195,6 +280,7 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
   constexpr int slices = N / RES_COLS;
   const int r_slots = streamSlots(p), r_slot_bytes = streamSlotBytes(p), act_slot_bytes = actSlotBytes(p);
   const bool s_fp32 = streamFp32(p);
+  const int flags = epiFlags(p);
   const uint32_t smem_r = smem_base + 2 * a_buf_bytes;
   const uint32_t smem_act = smem_r + r_slots * r_slot_bytes;
   const uint32_t smem_b = smem_act + ACT_SLOTS * act_slot_bytes;
@@ -362,23 +448,7 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
       uint8_t* const slot = ring + rs * r_slot_bytes;
       uint8_t* const aslot = act_ring + as * act_slot_bytes;
       if(p.residual != nullptr) mbar_wait(smem_u32(&bars->r_full[rs]), rphase);
-#pragma unroll
-      for(int h = 0; h < 2; h++) {
-        const int rl = rloc + 8 * h, row = m0 + rl;
-        if(row >= p.M) continue;   // no ncbias entry for rows past the batch; the TMA stores clip them
-        const float maskv = h ? mask1 : mask0;
-#pragma unroll
-        for(int jj = 0; jj < RES_COLS / 8; jj++) {
-          const int j = s * (RES_COLS / 8) + jj, lc = 8 * j + 2 * (lane & 3), c = lc - s * RES_COLS;
-          uint8_t* const rp = slot + slice_offset(rl, c, s_fp32);
-          uint8_t* const ap = aslot + slice_offset(rl, c, false);
-          const float2 r = p.residual != nullptr ? (s_fp32 ? *reinterpret_cast<const float2*>(rp)
-                                                           : __half22float2(*reinterpret_cast<const __half2*>(rp)))
-                                                 : make_float2(0.0f, 0.0f);
-          epilogue_store(p, row, n0 + lc, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], maskv, r, s_scale + lc, s_bias + lc, rp, ap,
-                         ap + ACT_SLICE_BYTES);
-        }
-      }
+      epiDispatch<N>(flags, p, acc, s, m0, n0, rloc, lane, mask0, mask1, s_scale, s_bias, slot, aslot);
       fence_proxy_async();
       if(leader) {
         // the previous slice's stores have read their slots: its act slot (the next slice's) and its stream slot are free again
