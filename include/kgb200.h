@@ -470,6 +470,18 @@ KGB_API int kgb_test_conv_ex(int ky, int kx, int in_c, int out_c, const float* w
                              int epilogue_kind, const float* input, const int32_t* board_xy, const float* ncbias, const float* residual_in,
                              const float* bn_scale, const float* bn_bias, int activation, float* raw_out, float* act_hi_out,
                              float* act_lo_out);
+/* Test hook for the fused nested-block boundary (DESIGN.md §4): a block's exit 1x1 (inner_c -> trunk_c, + the trunk stream) and
+ * the next block's entry 1x1 (trunk_c -> inner_c, mish at both ends) on inputs and weights drawn from `seed`, run once as one fused
+ * launch and once as two launches.  board_xy [n][2] or NULL as in kgb_test_conv_ex; the trunk stream is fp32 when trunk_fp32, the
+ * inner one when inner_fp32 (which needs trunk_fp32, as KGB_STREAM_FP32=all).  out[0..2]: elements of the trunk stream, the inner
+ * stream and the inner operand whose bits differ between the two; out[3..5]: nonzero elements of the fused outputs in masked rows
+ * or padded channels.  Fails when the fused kernel does not take the shape. */
+KGB_API int kgb_test_conv_boundary(int inner_c, int trunk_c, int n, int nn_x_len, int nn_y_len, const int32_t* board_xy, int trunk_fp32,
+                                   int inner_fp32, uint32_t seed, int64_t* out);
+/* Timing hook of the same boundary (whole boards): ms per boundary, fused (one launch) or not (two launches), cycling through
+ * `rotate` buffer sets. */
+KGB_API int kgb_bench_conv_boundary(int inner_c, int trunk_c, int n, int nn_x_len, int nn_y_len, int trunk_fp32, int inner_fp32, int fused,
+                                    int rotate, int warmup, int iters, float* ms_per_boundary);
 
 #ifdef __cplusplus
 }

@@ -13,6 +13,8 @@
 #include <dlfcn.h>
 #include <nccl.h>      // types only: the library is looked up at run time (ncclApi below), libkgb200.so does not link against it
 
+#include <cmath>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -209,6 +211,57 @@ struct Builder {
     return d;
   }
 
+  // The launch parameters of one convolution at batch n
+  static ConvParams convParams(const kgb_handle& hh, int n, const ConvWeights& cw, const void* residual, bool residualFp32, const float* ncbias,
+                               void* rawOut, bool rawFp32, __half* actOut, BNDev bn) {
+    ConvParams p;
+    memset(&p, 0, sizeof(p));
+    p.M = n * hh.L.P;
+    p.P = hh.L.P;
+    p.Wp = hh.L.Wp;
+    p.ky = cw.ky; p.kx = cw.kx;
+    p.cin_p = cw.cin_p; p.cout_p = cw.cout_p;
+    p.n_tile = cw.n_tile;
+    p.num_m_tiles = (p.M + 127) / 128;
+    p.num_n_tiles = cw.num_n_tiles;
+    p.split = hh.split;
+    p.residual = residual; p.residual_fp32 = residualFp32 ? 1 : 0;
+    p.ncbias = ncbias;
+    p.raw_out = rawOut; p.raw_fp32 = rawFp32 ? 1 : 0;
+    p.act_out = actOut;
+    p.bn_scale = bn.scale; p.bn_bias = bn.bias; p.act = bn.act;
+    p.mask = hh.dMask;
+    return p;
+  }
+
+  // Emit a block boundary as one op (launchConvPair): the exit conv `wpost` of a nested block (operand innerA, residual stream S
+  // updated in place, the next block's preBN `bn1`) and the entry conv `wpre` of the next nested block (raw stream innerS, activated
+  // operand innerAOut, its first inner block's preBN `bn2`).  The trunk operand between them never leaves the kernel.  innerAOut may
+  // be innerA: levels of one width share their buffers, and the kernel reads each tile's operand rows before it writes them.
+  // Returns false, emitting nothing, when the kernel does not take these shapes or epilogues.
+  bool emitConvPair(const ConvWeights& wpost, const __half* innerA, void* S, bool sFp32, BNDev bn1, const ConvWeights& wpre, void* innerS,
+                    bool innerFp32, __half* innerAOut, BNDev bn2) {
+    if(!convPairSupported(convParams(h, h.maxBatch, wpost, S, sFp32, nullptr, S, sFp32, nullptr, bn1),
+                          convParams(h, h.maxBatch, wpre, nullptr, false, nullptr, innerS, innerFp32, innerAOut, bn2)))
+      return false;
+    kgb_handle* hp = &h;
+    h.ops.push_back([=](int n, cudaStream_t s) {
+      const ConvParams p1 = convParams(*hp, n, wpost, S, sFp32, nullptr, S, sFp32, nullptr, bn1);
+      const ConvParams p2 = convParams(*hp, n, wpre, nullptr, false, nullptr, innerS, innerFp32, innerAOut, bn2);
+      ConvPairTmaps tm;
+      memset(&tm, 0, sizeof(tm));
+      tm.A = makeTmap2D(innerA, (uint64_t)p1.M, (uint64_t)wpost.cin_p, (uint32_t)convABoxRows(1, 1, p1.Wp));
+      tm.W1 = makeTmap2D(wpost.w, (uint64_t)wpost.cout_p, (uint64_t)wpost.cin_p, (uint32_t)kConvPairChunk);
+      tm.W2 = wpre.tmapB;
+      tm.stream1 = makeTmapSlices(S, (uint64_t)p1.M, (uint64_t)wpost.cout_p, sFp32);
+      tm.stream2 = makeTmapSlices(innerS, (uint64_t)p1.M, (uint64_t)wpre.cout_p, innerFp32);
+      tm.act2 = makeTmapSlices(innerAOut, (uint64_t)p1.M, (uint64_t)wpre.cout_p, false);
+      CK(launchConvPair(tm, p1, p2, s));
+    });
+    h.launchesPerForward++;
+    return true;
+  }
+
   // Emit one convolution op.  residual/rawOut may alias (in-place residual update).
   void emitConv(const ConvWeights& cw, const __half* A, const void* residual, bool residualFp32, const float* ncbias, void* rawOut,
                 bool rawFp32, __half* actOut, BNDev bn) {
@@ -221,23 +274,7 @@ struct Builder {
     kgb_handle* hp = &h;
     const int actMulL = actMul;
     h.ops.push_back([=](int n, cudaStream_t s) {
-      ConvParams p;
-      memset(&p, 0, sizeof(p));
-      p.M = n * hp->L.P;
-      p.P = hp->L.P;
-      p.Wp = hp->L.Wp;
-      p.ky = cw.ky; p.kx = cw.kx;
-      p.cin_p = cw.cin_p; p.cout_p = cw.cout_p;
-      p.n_tile = cw.n_tile;
-      p.num_m_tiles = (p.M + 127) / 128;
-      p.num_n_tiles = cw.num_n_tiles;
-      p.split = hp->split;
-      p.residual = residual; p.residual_fp32 = residualFp32 ? 1 : 0;
-      p.ncbias = ncbias;
-      p.raw_out = rawOut; p.raw_fp32 = rawFp32 ? 1 : 0;
-      p.act_out = actOut;
-      p.bn_scale = bn.scale; p.bn_bias = bn.bias; p.act = bn.act;
-      p.mask = hp->dMask;
+      const ConvParams p = convParams(*hp, n, cw, residual, residualFp32, ncbias, rawOut, rawFp32, actOut, bn);
       ConvTmaps tm;
       memset(&tm, 0, sizeof(tm));
       tm.A = makeTmap2D(A, (uint64_t)p.M, (uint64_t)cw.cin_p * actMulL, (uint32_t)convABoxRows(cw.ky, cw.kx, p.Wp));
@@ -252,6 +289,13 @@ struct Builder {
 
   // blocks operate on stream lv.S, with lv.A = act(preBN_0(S)) on entry and = act(finalBN(S_out)) on exit.
   void emitBlocks(const std::vector<BlockDesc>& blocks, Level& lv, const BNDesc& finalBN, int finalAct, bool keepFinalRaw) {
+    // A nested block followed by another nested block holds its exit conv back: the next block's entry conv goes out with it as
+    // one launch when emitConvPair takes the pair, else the two go out as before.  Either way the weights are packed in the same
+    // order, so the arena layout does not depend on the choice.
+    bool exitPending = false;
+    ConvWeights pendingW;
+    __half* pendingA = nullptr;
+    BNDev pendingBN;
     for(size_t i = 0; i < blocks.size(); i++) {
       const BlockDesc& b = blocks[i];
       bool last = i + 1 == blocks.size();
@@ -293,9 +337,17 @@ struct Builder {
         ConvWeights wpost = packConv({&b.conv2});
         Level inner = makeLevel(b.conv1.cout, h.streamInnerFp32, b.blocks);
         BNDev innerPre = uploadBN(b.blocks[0].preBN, b.blocks[0].preAct, inner.cp);
-        emitConv(wpre, lv.A, nullptr, false, nullptr, inner.S, inner.fp32, inner.A, innerPre);
+        if(!exitPending || !emitConvPair(pendingW, pendingA, lv.S, lv.fp32, pendingBN, wpre, inner.S, inner.fp32, inner.A, innerPre)) {
+          if(exitPending) emitConv(pendingW, pendingA, lv.S, lv.fp32, nullptr, lv.S, lv.fp32, lv.A, pendingBN);
+          emitConv(wpre, lv.A, nullptr, false, nullptr, inner.S, inner.fp32, inner.A, innerPre);
+        }
+        exitPending = false;
         emitBlocks(b.blocks, inner, b.midBN, b.midAct, false);
-        emitConv(wpost, inner.A, lv.S, lv.fp32, nullptr, rawOut, lv.fp32, lv.A, nextBN);
+        if(h.fuseBoundaries && !last && blocks[i + 1].kind == BLOCK_NESTED) {
+          exitPending = true;
+          pendingW = wpost; pendingA = inner.A; pendingBN = nextBN;
+        }
+        else emitConv(wpost, inner.A, lv.S, lv.fp32, nullptr, rawOut, lv.fp32, lv.A, nextBN);
       }
     }
   }
@@ -552,6 +604,7 @@ static void ncclCheck(ncclResult_t r, const char* what) {
 static void copyBuildSettings(kgb_handle& dst, const kgb_handle& src) {
   dst.device = src.device; dst.model = src.model; dst.L = src.L; dst.maxBatch = src.maxBatch; dst.split = src.split;
   dst.nhwc = src.nhwc; dst.streamTrunkFp32 = src.streamTrunkFp32; dst.streamInnerFp32 = src.streamInnerFp32;
+  dst.fuseBoundaries = src.fuseBoundaries;
 }
 
 // Makes device `dev` (-1: the current device) current, after checking that it exists and is the sm_90a device the kernels are
@@ -630,6 +683,9 @@ KGB_API int kgb_handle_create(kgb_context* ctx, const kgb_model* model, int max_
     std::string streams = h.split ? "all" : (env ? env : "none");
     h.streamTrunkFp32 = streams != "none";
     h.streamInnerFp32 = streams == "all";
+    // KGB_FUSE_BOUNDARY=0 keeps every nested block boundary as two launches (same-build A/B runs and tests; the results are the same)
+    const char* fuse = getenv("KGB_FUSE_BOUNDARY");
+    h.fuseBoundaries = !h.split && !(fuse && std::string(fuse) == "0");
     CK(cudaStreamCreateWithFlags(&h.stream, cudaStreamNonBlocking));
     CK(convWGInit());
     CK(cudaStreamCreateWithFlags(&h.copyStream, cudaStreamNonBlocking));
@@ -927,6 +983,112 @@ struct SingleConv {
   void run() { h.ops[next](n, h.stream); next = (next + 1) % rotate; }
 };
 
+// A nested-block boundary on its own: the exit 1x1 (inner_c -> trunk_c, + the trunk stream) of one block and the entry 1x1
+// (trunk_c -> inner_c) of the next, with seeded random weights, BN constants and inputs.  Buffer set 2r runs it as one fused launch
+// (launchConvPair), set 2r + 1 as the two launches of the unfused path, on the same inputs; `rotate` pairs of sets are cycled
+// through by run() so that a timing loop does not live in L2.
+struct BoundaryConv {
+  kgb_handle h;
+  ModelDesc dummy;
+  ConvWeights wpost, wpre;
+  int n, innerCp = 0, trunkCp = 0, rotate, next = 0;
+  bool trunkF32, innerF32;
+  size_t M;
+  struct Set {
+    __half *innerA = nullptr, *trunkA = nullptr;
+    void *trunkS = nullptr, *innerS = nullptr;
+  };
+  std::vector<Set> sets;
+  std::vector<float> mask;
+  BoundaryConv(int inner_c, int trunk_c, int n_, int X, int Y, const int32_t* boardXY, bool trunkFp32, bool innerFp32, uint32_t seed, int rotate_)
+      : n(n_), rotate(rotate_ < 1 ? 1 : rotate_), trunkF32(trunkFp32), innerF32(innerFp32) {
+    h.device = selectDevice(-1);
+    h.model = &dummy;
+    h.maxBatch = n;
+    h.L = boardLayout(X, Y, 1);
+    CK(cudaStreamCreateWithFlags(&h.stream, cudaStreamNonBlocking));
+    CK(convWGInit());
+    uint32_t st = seed * 2654435761u + 12345u;
+    auto uni = [&]() { st = st * 1664525u + 1013904223u; return (st >> 8) * (1.0f / 16777216.0f); };
+    ConvDesc post, pre;
+    post.ky = post.kx = pre.ky = pre.kx = 1;
+    post.cin = pre.cout = inner_c; post.cout = pre.cin = trunk_c;
+    for(ConvDesc* c : {&post, &pre}) {
+      c->w.resize((size_t)c->cin * c->cout);
+      for(auto& v : c->w) v = (uni() - 0.5f) * 4.0f / std::sqrt((float)c->cin);
+    }
+    auto randBN = [&](int c) {
+      BNDesc bn;
+      bn.c = c;
+      for(int i = 0; i < c; i++) { bn.scale.push_back(0.5f + uni()); bn.bias.push_back(uni() - 0.5f); }
+      return bn;
+    };
+    const BNDesc bnTrunk = randBN(trunk_c), bnInner = randBN(inner_c);
+    Builder::BNDev bn1, bn2;
+    buildWeights(h, [&](kgb_handle& hh) {
+      Builder b(hh);
+      wpost = b.packConv({&post});
+      wpre = b.packConv({&pre});
+      bn1 = b.uploadBN(bnTrunk, ACT_MISH, wpost.cout_p);
+      bn2 = b.uploadBN(bnInner, ACT_MISH, wpre.cout_p);
+    });
+    innerCp = wpost.cin_p; trunkCp = wpost.cout_p;
+    M = (size_t)n * h.L.P;
+    h.dMask = h.dalloc<float>(M + 128);
+    mask.assign(M, 0.0f);
+    for(int i = 0; i < n; i++) {
+      const int bx = boardXY ? boardXY[2 * i] : X, by = boardXY ? boardXY[2 * i + 1] : Y;
+      for(int y = 0; y < by; y++)
+        for(int x = 0; x < bx; x++) mask[(size_t)i * h.L.P + (size_t)(y + h.L.pad) * h.L.Wp + x] = 1.0f;
+    }
+    CK(cudaMemcpyAsync(h.dMask, mask.data(), M * sizeof(float), cudaMemcpyHostToDevice, h.stream));
+    // inputs as the previous layers leave them: zero in masked rows and padded channels
+    std::vector<__half> hA(M * innerCp, __float2half(0.0f));
+    std::vector<float> hS(M * trunkCp, 0.0f);
+    for(size_t r = 0; r < M; r++) {
+      if(mask[r] == 0.0f) continue;
+      for(int c = 0; c < inner_c; c++) hA[r * innerCp + c] = __float2half_rn(uni() * 2.0f);
+      for(int c = 0; c < trunk_c; c++) hS[r * trunkCp + c] = (uni() - 0.5f) * 8.0f;
+    }
+    std::vector<__half> hS16(hS.size());
+    for(size_t k = 0; k < hS.size(); k++) hS16[k] = __float2half_rn(hS[k]);
+    Builder b(h);
+    for(int k = 0; k < 2 * rotate; k++) {
+      Set s;
+      s.innerA = h.dalloc<__half>(M * innerCp);
+      s.trunkA = h.dalloc<__half>(M * trunkCp);
+      s.trunkS = trunkF32 ? (void*)h.dalloc<float>(M * trunkCp) : (void*)h.dalloc<__half>(M * trunkCp);
+      s.innerS = innerF32 ? (void*)h.dalloc<float>(M * innerCp) : (void*)h.dalloc<__half>(M * innerCp);
+      CK(cudaMemcpyAsync(s.innerA, hA.data(), hA.size() * sizeof(__half), cudaMemcpyHostToDevice, h.stream));
+      if(trunkF32) CK(cudaMemcpyAsync(s.trunkS, hS.data(), hS.size() * sizeof(float), cudaMemcpyHostToDevice, h.stream));
+      else CK(cudaMemcpyAsync(s.trunkS, hS16.data(), hS16.size() * sizeof(__half), cudaMemcpyHostToDevice, h.stream));
+      sets.push_back(s);
+      if(k % 2 == 0) {
+        if(!b.emitConvPair(wpost, s.innerA, s.trunkS, trunkF32, bn1, wpre, s.innerS, innerF32, s.innerA, bn2))
+          throw std::invalid_argument("the fused boundary kernel does not take " + std::to_string(inner_c) + " / " + std::to_string(trunk_c) +
+                                      " channels with these streams");
+      }
+      else {
+        // one op per launch, as emitBlocks emits an unfused boundary
+        b.emitConv(wpost, s.innerA, s.trunkS, trunkF32, nullptr, s.trunkS, trunkF32, s.trunkA, bn1);
+        b.emitConv(wpre, s.trunkA, nullptr, false, nullptr, s.innerS, innerF32, s.innerA, bn2);
+      }
+    }
+    CK(cudaStreamSynchronize(h.stream));
+  }
+  ~BoundaryConv() {
+    for(void* p : h.allocs) cudaFree(p);
+    if(h.wHost) cudaFreeHost(h.wHost);
+    if(h.stream) cudaStreamDestroy(h.stream);
+  }
+  // ops: set 2r's fused op is op 3r, set 2r + 1's two launches ops 3r + 1 and 3r + 2
+  void run(bool fused) {
+    if(fused) h.ops[3 * next](n, h.stream);
+    else { h.ops[3 * next + 1](n, h.stream); h.ops[3 * next + 2](n, h.stream); }
+    next = (next + 1) % rotate;
+  }
+};
+
 // kgb_test_conv_ex and its two narrower forms kgb_test_conv (kind 0) and kgb_test_conv_epilogue (kinds 1-4): one launch, NHWC in
 // and out.  act_lo_out is written in split mode only.
 void testConv(const char* fn, int ky, int kx, int in_c, int out_c, const float* weights, int n, int nn_x_len, int nn_y_len, int use_fp16, int kind,
@@ -1072,6 +1234,74 @@ KGB_API int kgb_bench_conv_ex(int ky, int kx, int in_c, int out_c, int n, int nn
     CK(cudaEventElapsedTime(&ms, e0, e1));
     cudaEventDestroy(e0); cudaEventDestroy(e1);
     *ms_per_launch = ms / iters;
+  });
+}
+
+KGB_API int kgb_test_conv_boundary(int inner_c, int trunk_c, int n, int nn_x_len, int nn_y_len, const int32_t* board_xy, int trunk_fp32,
+                                   int inner_fp32, uint32_t seed, int64_t* out) {
+  return guarded([&] {
+    if(!out || n < 1 || inner_c < 1 || trunk_c < 1 || nn_x_len < 2 || nn_y_len < 2 || (inner_fp32 && !trunk_fp32))
+      throw std::invalid_argument("kgb_test_conv_boundary: bad argument");
+    if(board_xy)
+      for(int i = 0; i < n; i++)
+        if(board_xy[2 * i] < 1 || board_xy[2 * i] > nn_x_len || board_xy[2 * i + 1] < 1 || board_xy[2 * i + 1] > nn_y_len)
+          throw std::invalid_argument("kgb_test_conv_boundary: board size of image " + std::to_string(i) + " not in the frame");
+    BoundaryConv bc(inner_c, trunk_c, n, nn_x_len, nn_y_len, board_xy, trunk_fp32 != 0, inner_fp32 != 0, seed, 1);
+    bc.run(true);
+    bc.run(false);
+    const cudaStream_t s = bc.h.stream;
+    auto download = [&](const void* src, size_t bytes) {
+      std::vector<uint8_t> v(bytes);
+      CK(cudaMemcpyAsync(v.data(), src, bytes, cudaMemcpyDeviceToHost, s));
+      CK(cudaStreamSynchronize(s));
+      return v;
+    };
+    // out[0..2]: elements of trunk.S, inner.S, inner.A whose bits differ between the fused launch and the two launches;
+    // out[3..5]: nonzero elements of the fused outputs in masked rows or padded channels
+    struct Out { size_t off; int cp, c, esize; };
+    const Out outs[3] = {{offsetof(BoundaryConv::Set, trunkS), bc.trunkCp, trunk_c, trunk_fp32 ? 4 : 2},
+                         {offsetof(BoundaryConv::Set, innerS), bc.innerCp, inner_c, inner_fp32 ? 4 : 2},
+                         {offsetof(BoundaryConv::Set, innerA), bc.innerCp, inner_c, 2}};
+    for(int k = 0; k < 3; k++) {
+      const Out& o = outs[k];
+      auto ptr = [&](const BoundaryConv::Set& st) { return *reinterpret_cast<void* const*>(reinterpret_cast<const uint8_t*>(&st) + o.off); };
+      const size_t bytes = bc.M * o.cp * o.esize;
+      const std::vector<uint8_t> f = download(ptr(bc.sets[0]), bytes), u = download(ptr(bc.sets[1]), bytes);
+      int64_t diff = 0, nonzero = 0;
+      for(size_t r = 0; r < bc.M; r++)
+        for(int c = 0; c < o.cp; c++) {
+          const size_t e = (r * o.cp + c) * o.esize;
+          if(memcmp(&f[e], &u[e], o.esize) != 0) diff++;
+          if(bc.mask[r] == 0.0f || c >= o.c) {
+            float v;
+            if(o.esize == 4) memcpy(&v, &f[e], 4);
+            else { __half hv; memcpy(&hv, &f[e], 2); v = __half2float(hv); }
+            if(v != 0.0f) nonzero++;
+          }
+        }
+      out[k] = diff;
+      out[3 + k] = nonzero;
+    }
+  });
+}
+
+KGB_API int kgb_bench_conv_boundary(int inner_c, int trunk_c, int n, int nn_x_len, int nn_y_len, int trunk_fp32, int inner_fp32, int fused,
+                                    int rotate, int warmup, int iters, float* ms_per_boundary) {
+  return guarded([&] {
+    if(!ms_per_boundary || n < 1 || iters < 1 || (inner_fp32 && !trunk_fp32)) throw std::invalid_argument("kgb_bench_conv_boundary: bad argument");
+    BoundaryConv bc(inner_c, trunk_c, n, nn_x_len, nn_y_len, nullptr, trunk_fp32 != 0, inner_fp32 != 0, 1, rotate);
+    for(int i = 0; i < warmup; i++) bc.run(fused != 0);
+    cudaEvent_t e0, e1;
+    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
+    CK(cudaStreamSynchronize(bc.h.stream));
+    CK(cudaEventRecord(e0, bc.h.stream));
+    for(int i = 0; i < iters; i++) bc.run(fused != 0);
+    CK(cudaEventRecord(e1, bc.h.stream));
+    CK(cudaStreamSynchronize(bc.h.stream));
+    float ms = 0.0f;
+    CK(cudaEventElapsedTime(&ms, e0, e1));
+    cudaEventDestroy(e0); cudaEventDestroy(e1);
+    *ms_per_boundary = ms / iters;
   });
 }
 

@@ -79,4 +79,21 @@ inline int convABoxRows(int ky, int kx, int Wp) { return 128 + 2 * ((ky / 2) * W
 inline int convSliceBoxRows() { return 64; }  // TMA box rows of the epilogue's slices: one consumer warpgroup's half of a tile
 cudaError_t convWGInit();  // per device, before the first launch (sets the kernels' shared-memory limit, reads the SM count)
 
+// A block boundary in one launch: p1 = a nested block's exit 1x1 (inner -> trunk channels, + residual, raw stream written in
+// place, p1.act_out unused), p2 = the next nested block's entry 1x1 (trunk -> inner channels, raw stream + activated operand).  The
+// activated trunk operand that p1 would write and p2 would read stays in shared memory, 64 columns at a time, each chunk an entry
+// k-block.  Every output element is summed in the same order and goes through the same epilogue as with two launchConvWG calls,
+// so the results are bit-identical.  p2.act_out may be the same buffer as p1's A (a tile reads all of its rows of A before its
+// epilogue writes them, and there is no halo).  Tensor maps: A = p1's operand, box {64, 128}; W1 = the exit's packed weights, box
+// {64, 64}; W2 = the entry's, box {64, p2.n_tile}; stream1 = p1's residual and raw stream, stream2 = p2.raw_out, act2 = p2.act_out
+// (slice boxes as in ConvTmaps).
+struct ConvPairTmaps {
+  CUtensorMap A, W1, W2, stream1, stream2, act2;
+};
+static constexpr int kConvPairChunk = 64;   // box rows of W1
+// Whether launchConvPair takes these launches: fp16 operands, mish at both ends, 1x1 filters, (inner, trunk) widths the kernel is
+// compiled for, and rings that fit in shared memory.
+bool convPairSupported(const ConvParams& p1, const ConvParams& p2);
+cudaError_t launchConvPair(const ConvPairTmaps& tm, const ConvParams& p1, const ConvParams& p2, cudaStream_t stream);
+
 }  // namespace kgb

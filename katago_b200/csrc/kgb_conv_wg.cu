@@ -474,6 +474,7 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
 }
 
 static int g_smCount[64];   // per device ordinal, read by convWGInit
+static cudaError_t convPairInit();
 
 cudaError_t convWGInit() {
   int dev = 0;
@@ -489,7 +490,8 @@ cudaError_t convWGInit() {
                        cudaFuncSetAttribute(kgb_conv_wg_kernel<160>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
                        cudaFuncSetAttribute(kgb_conv_wg_kernel<192>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
                        cudaFuncSetAttribute(kgb_conv_wg_kernel<224>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
-                       cudaFuncSetAttribute(kgb_conv_wg_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT)})
+                       cudaFuncSetAttribute(kgb_conv_wg_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
+                       convPairInit()})
     if(e != cudaSuccess) return e;
   return cudaSuccess;
 }
@@ -533,6 +535,365 @@ cudaError_t launchConvWG(const ConvTmaps& tm, const ConvParams& p, cudaStream_t 
     case 256: return launchN<256>(tm, p, grid, stages, smem, stream);
     default: return cudaErrorInvalidValue;
   }
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// Fused block boundary (launchConvPair): exit 1x1 of nested block i + entry 1x1 of nested block i+1
+// ------------------------------------------------------------------------------------------------------------
+// Both layers are bound by HBM bytes; in two launches the activated trunk operand (fp16, trunk channels) is written by the exit
+// and read straight back by the entry.  Here one persistent CTA per SM walks 128-row tiles; for one tile:
+//   phase 1  the exit's output in chunks of PAIR_NC columns: acc1[128 x 64] = A[128 x K1] * W1[chunk], the inner operand A resident
+//            in shared memory for the whole tile (1x1: no halo).  Its epilogue is the exit's (residual slice in, raw stream out by
+//            TMA store), except that the activated operand goes into a shared-memory chunk slot T, 64B-swizzled 32-column slices.
+//   phase 2  each finished chunk is one k-block of the entry: acc2[128 x N2] += T * W2[chunk], both operands by shared-memory
+//            descriptor.  After the last chunk, the entry's epilogue writes the inner raw stream and activated operand.
+// The loop per chunk c issues P1(c+1) and P2(c) together and waits for P1(c+1) only, so P2(c) runs under chunk c+1's epilogue;
+// T has two slots for that.  Weight stages hold one chunk of W1 (K1/64 boxes {64, 64}) or of W2 (one box {64, N2}), both
+// N2 * 128 bytes, in the order the consumers take them: W1(0), then W1(c+1), W2(c) for each c.  acc2 sums over K in the order of
+// the entry's own launch (chunk = k-block, then k16), acc1 in that of the exit's, and the epilogues are the same code.
+static constexpr int PAIR_NC = kConvPairChunk;
+static constexpr int PAIR_T_BYTES = BLOCK_M * PAIR_NC * 2;   // one chunk slot: PAIR_NC / 32 act slices
+
+struct __align__(8) PairBars {
+  uint64_t full[MAX_STAGES];
+  uint64_t empty[MAX_STAGES];
+  uint64_t a_full, a_empty;     // the inner operand tile of the current tile
+  uint64_t r_full[RES_SLOTS];
+  uint64_t r_empty[RES_SLOTS];
+};
+
+// 64B-swizzled K-major operand (the act slices, slice_offset's fp16 layout): 64 B rows, 8-row groups 512 B apart
+__device__ __forceinline__ uint64_t make_smem_desc_sw64(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(512 >> 4) << 32;
+  d |= (uint64_t)2 << 62;
+  return d;
+}
+
+// dynamic smem: [<=1023 B slack][A tile: K1/64 x 16 KB][2 x T slot][residual ring][2 x raw staging][2 x act slice][stages x weights]
+//               [PairBars][BN scale / bias: exit N1, entry N2]
+struct PairLayout {
+  int r_slots = 0, stages = 0, smem = 0;
+};
+static PairLayout pairLayout(const ConvParams& p1, const ConvParams& p2) {
+  PairLayout l;
+  const int n2 = p2.cout_p, n1 = p1.cout_p;
+  const int r1 = BLOCK_M * RES_COLS * (p1.residual_fp32 ? 4 : 2), r2 = BLOCK_M * RES_COLS * (p2.raw_fp32 ? 4 : 2);
+  const int wBytes = n2 * PAIR_NC * 2;
+  // a full residual ring when it leaves room for three weight stages, else half of one
+  for(int rs : {RES_SLOTS, 2}) {
+    const int fixed = 1024 + BLOCK_M * n2 * 2 + 2 * PAIR_T_BYTES + rs * r1 + STAGE_SLOTS * r2 + ACT_SLOTS * ACT_SLICE_BYTES +
+                      (int)sizeof(PairBars) + 2 * (n1 + n2) * (int)sizeof(float);
+    const int stages = std::min(MAX_STAGES, (SMEM_LIMIT - fixed) / wBytes);
+    if(stages >= 3 || (rs == 2 && stages >= 2)) {
+      l.r_slots = rs; l.stages = stages; l.smem = fixed + stages * wBytes;
+      return l;
+    }
+  }
+  return l;
+}
+
+template <int N2, int N1, bool S1_FP32, bool S2_FP32>
+__global__ void __launch_bounds__(THREADS, 1)
+kgb_conv_pair_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapW1,
+                     const __grid_constant__ CUtensorMap tmapW2, const __grid_constant__ CUtensorMap tmapS1,
+                     const __grid_constant__ CUtensorMap tmapS2, const __grid_constant__ CUtensorMap tmapA2,
+                     const __grid_constant__ ConvParams p1, const __grid_constant__ ConvParams p2, int stages, int r_slots) {
+  constexpr int F1 = EPI_RES | EPI_RAW | EPI_MISH | (S1_FP32 ? EPI_FP32 : 0);
+  constexpr int F2 = EPI_RAW | EPI_MISH | (S2_FP32 ? EPI_FP32 : 0);
+  constexpr int K1 = N2;                             // the exit's K = the entry's N = the inner channels
+  constexpr int A_BYTES = BLOCK_M * K1 * 2;          // K1 / 64 boxes {64, 128}
+  constexpr int W_BYTES = N2 * PAIR_NC * 2;
+  constexpr int R1_BYTES = BLOCK_M * RES_COLS * (S1_FP32 ? 4 : 2), R2_BYTES = BLOCK_M * RES_COLS * (S2_FP32 ? 4 : 2);
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t smem_t = smem_base + A_BYTES;
+  const uint32_t smem_r = smem_t + 2 * PAIR_T_BYTES;
+  const uint32_t smem_stg = smem_r + r_slots * R1_BYTES;
+  const uint32_t smem_act = smem_stg + STAGE_SLOTS * R2_BYTES;
+  const uint32_t smem_w = smem_act + ACT_SLOTS * ACT_SLICE_BYTES;
+  uint8_t* const smem = smem_raw + (smem_base - smem_u32(smem_raw));
+  PairBars* bars = reinterpret_cast<PairBars*>(smem + (smem_w - smem_base) + (size_t)stages * W_BYTES);
+  constexpr int chunks = N1 / PAIR_NC;
+  float* const s_scale1 = reinterpret_cast<float*>(bars + 1);
+  float* const s_bias1 = s_scale1 + N1;
+  float* const s_scale2 = s_bias1 + N1;
+  float* const s_bias2 = s_scale2 + N2;
+
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  const int tiles = p1.num_m_tiles;
+
+  if(threadIdx.x == 0) {
+    for(const CUtensorMap* m : {&tmapA, &tmapW1, &tmapW2, &tmapS1, &tmapS2, &tmapA2})
+      asm volatile("prefetch.tensormap [%0];" ::"l"(m) : "memory");
+    for(int s = 0; s < stages; s++) {
+      mbar_init(smem_u32(&bars->full[s]), 1);
+      mbar_init(smem_u32(&bars->empty[s]), CONSUMER_WARPS);
+    }
+    mbar_init(smem_u32(&bars->a_full), 1);
+    mbar_init(smem_u32(&bars->a_empty), CONSUMER_WARPS);
+    for(int s = 0; s < RES_SLOTS; s++) {
+      mbar_init(smem_u32(&bars->r_full[s]), 1);
+      mbar_init(smem_u32(&bars->r_empty[s]), 2);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if(warp < 4) {
+    // ===================== TMA producers =====================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if(warp == 0 && lane == 0) {
+      // the inner operand tile, then the weight chunks in consumption order
+      int stage = 0;
+      uint32_t phase = 0, aphase = 0;
+      auto loadW = [&](bool entry, int c) {
+        mbar_wait(smem_u32(&bars->empty[stage]), phase ^ 1);
+        const uint32_t full = smem_u32(&bars->full[stage]), dst = smem_w + stage * W_BYTES;
+        mbar_arrive_expect_tx(full, (uint32_t)W_BYTES);
+        if(entry) {
+          for(int j = 0; j < PAIR_NC / BLOCK_K; j++) tma_load_2d(dst + j * N2 * 128, &tmapW2, full, c * PAIR_NC + j * BLOCK_K, 0);
+        }
+        else {
+          for(int kb = 0; kb < K1 / BLOCK_K; kb++) tma_load_2d(dst + kb * PAIR_NC * 128, &tmapW1, full, kb * BLOCK_K, c * PAIR_NC);
+        }
+        if(++stage == stages) { stage = 0; phase ^= 1; }
+      };
+      for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        const int m0 = tile * BLOCK_M;
+        mbar_wait(smem_u32(&bars->a_empty), aphase ^ 1);
+        const uint32_t afull = smem_u32(&bars->a_full);
+        mbar_arrive_expect_tx(afull, (uint32_t)A_BYTES);
+        for(int kb = 0; kb < K1 / BLOCK_K; kb++) tma_load_2d(smem_base + kb * BLOCK_M * 128, &tmapA, afull, kb * BLOCK_K, m0);
+        aphase ^= 1;
+        loadW(false, 0);
+        for(int c = 0; c < chunks; c++) {
+          if(c + 1 < chunks) loadW(false, c + 1);
+          loadW(true, c);
+        }
+      }
+    }
+    else if(warp == 1 && lane == 0) {
+      // the exit's residual slices
+      int rs = 0;
+      uint32_t rphase = 0;
+      for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        const int m0 = tile * BLOCK_M;
+        for(int s = 0; s < N1 / RES_COLS; s++) {
+          mbar_wait(smem_u32(&bars->r_empty[rs]), rphase ^ 1);
+          const uint32_t rfull = smem_u32(&bars->r_full[rs]), dst = smem_r + rs * R1_BYTES;
+          mbar_arrive_expect_tx(rfull, (uint32_t)R1_BYTES);
+          tma_load_2d(dst, &tmapS1, rfull, s * RES_COLS, m0);
+          tma_load_2d(dst + R1_BYTES / 2, &tmapS1, rfull, s * RES_COLS, m0 + BLOCK_M / 2);
+          if(++rs == r_slots) { rs = 0; rphase ^= 1; }
+        }
+      }
+    }
+    return;
+  }
+
+  // ===================== consumers: warpgroup g owns tile rows 64g..64g+63 =====================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int g = (warp - 4) >> 2, q = warp & 3;
+  const bool leader = q == 0 && lane == 0;
+  const int rloc = g * 64 + q * 16 + (lane >> 2);
+  for(int i = threadIdx.x - 128; i < N1; i += 32 * CONSUMER_WARPS) { s_scale1[i] = __ldg(p1.bn_scale + i); s_bias1[i] = __ldg(p1.bn_bias + i); }
+  for(int i = threadIdx.x - 128; i < N2; i += 32 * CONSUMER_WARPS) { s_scale2[i] = __ldg(p2.bn_scale + i); s_bias2[i] = __ldg(p2.bn_bias + i); }
+  consumer_sync();
+
+  int stage = 0, rs = 0, prev_rs = -1, ps = 0, as = 0;
+  uint32_t phase = 0, rphase = 0, aphase = 0;
+  uint8_t* const ring = smem + (smem_r - smem_base);
+  uint8_t* const t_ring = smem + (smem_t - smem_base);
+  uint8_t* const stg_ring = smem + (smem_stg - smem_base);
+  uint8_t* const act_ring = smem + (smem_act - smem_base);
+  auto take = [&]() {
+    const int st = stage;
+    mbar_wait(smem_u32(&bars->full[st]), phase);
+    if(++stage == stages) { stage = 0; phase ^= 1; }
+    return st;
+  };
+  auto release = [&](uint32_t bar) {
+    __syncwarp();
+    if(lane == 0) mbar_arrive(bar);
+  };
+  for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int m0 = tile * BLOCK_M;
+    const float mask0 = m0 + rloc < p1.M ? __ldg(p1.mask + m0 + rloc) : 0.0f;
+    const float mask1 = m0 + rloc + 8 < p1.M ? __ldg(p1.mask + m0 + rloc + 8) : 0.0f;
+    float acc1[PAIR_NC / 2], acc2[N2 / 2];
+#pragma unroll
+    for(int i = 0; i < N2 / 2; i++) acc2[i] = 0.0f;
+    // P1: acc1 = A rows 64g.. x W1 chunk in stage st (K1 / 64 k-blocks of 4 k16 steps, as the exit's launch sums them)
+    auto issueP1 = [&](int st) {
+      const uint32_t w = smem_w + st * W_BYTES, a = smem_base + g * 64 * 128;
+#pragma unroll
+      for(int kb = 0; kb < K1 / BLOCK_K; kb++)
+#pragma unroll
+        for(int k = 0; k < 4; k++)
+          WgmmaSS<PAIR_NC>::mma(acc1, make_smem_desc(a + kb * BLOCK_M * 128) + 2 * k, make_smem_desc(w + kb * PAIR_NC * 128) + 2 * k);
+      wgmma_commit();
+    };
+    // P2: acc2 += T slot rows 64g.. x W2 chunk in stage st (the chunk's k16 steps in order)
+    auto issueP2 = [&](int st, int slot) {
+      const uint32_t w = smem_w + st * W_BYTES, t = smem_t + slot * PAIR_T_BYTES + g * 64 * 64;
+#pragma unroll
+      for(int k = 0; k < PAIR_NC / 16; k++)
+        WgmmaSS<N2>::mma(acc2, make_smem_desc_sw64(t + (k / 2) * ACT_SLICE_BYTES) + 2 * (k & 1),
+                         make_smem_desc(w + (k / 4) * N2 * 128) + 2 * (k & 3));
+      wgmma_commit();
+    };
+    auto zeroAcc1 = [&]() {
+#pragma unroll
+      for(int i = 0; i < PAIR_NC / 2; i++) acc1[i] = 0.0f;
+    };
+
+    mbar_wait(smem_u32(&bars->a_full), aphase);
+    aphase ^= 1;
+    zeroAcc1();
+    fence_acc(acc1);
+    fence_acc(acc2);
+    int st1 = take(), st2 = -1;
+    wgmma_fence();
+    issueP1(st1);
+    wgmma_wait0();
+    fence_acc(acc1);
+    release(smem_u32(&bars->empty[st1]));
+    if(chunks == 1) release(smem_u32(&bars->a_empty));
+#pragma unroll
+    for(int c = 0; c < chunks; c++) {
+      // ---- the exit's epilogue of chunk c: residual in, raw stream out, activated operand into T slot c & 1 ----
+#pragma unroll
+      for(int s = 0; s < PAIR_NC / RES_COLS; s++) {
+        uint8_t* const slot = ring + rs * R1_BYTES;
+        mbar_wait(smem_u32(&bars->r_full[rs]), rphase);
+        epilogue_slice<F1, PAIR_NC>(p1, acc1, s, m0, c * PAIR_NC, rloc, lane, mask0, mask1, s_scale1 + c * PAIR_NC, s_bias1 + c * PAIR_NC,
+                                    slot, t_ring + (c & 1) * PAIR_T_BYTES + s * ACT_SLICE_BYTES);
+        fence_proxy_async();   // the raw slice for its TMA store, the T slice for the wgmma that reads it
+        if(leader) {
+          bulk_wait_read0();
+          if(prev_rs >= 0) mbar_arrive(smem_u32(&bars->r_empty[prev_rs]));
+        }
+        warpgroup_sync(g);
+        if(leader) {
+          tma_store_2d(&tmapS1, smem_u32(slot + g * (R1_BYTES / 2)), c * PAIR_NC + s * RES_COLS, m0 + g * (BLOCK_M / 2));
+          bulk_commit();
+        }
+        prev_rs = rs;
+        if(++rs == r_slots) { rs = 0; rphase ^= 1; }
+      }
+      // P2(c - 1) has read T slot (c - 1) & 1 and its weight stage
+      if(c > 0) {
+        wgmma_wait0();
+        release(smem_u32(&bars->empty[st2]));
+      }
+      zeroAcc1();
+      fence_acc(acc1);
+      fence_acc(acc2);
+      wgmma_fence();
+      if(c + 1 < chunks) {
+        st1 = take();
+        issueP1(st1);
+      }
+      st2 = take();
+      issueP2(st2, c & 1);
+      if(c + 1 < chunks) {
+        wgmma_wait1();   // P1(c + 1) done, P2(c) may still run under the next chunk's epilogue
+        fence_acc(acc1);
+        release(smem_u32(&bars->empty[st1]));
+        if(c + 2 == chunks) release(smem_u32(&bars->a_empty));   // the tile's last P1: the next tile's A may land
+      }
+    }
+    wgmma_wait0();
+    fence_acc(acc2);
+    release(smem_u32(&bars->empty[st2]));
+
+    // ---- the entry's epilogue: raw inner stream and activated inner operand, one 32-column slice at a time ----
+#pragma unroll
+    for(int s = 0; s < N2 / RES_COLS; s++) {
+      uint8_t* const slot = stg_ring + ps * R2_BYTES;
+      uint8_t* const aslot = act_ring + as * ACT_SLICE_BYTES;
+      epilogue_slice<F2, N2>(p2, acc2, s, m0, 0, rloc, lane, mask0, mask1, s_scale2, s_bias2, slot, aslot);
+      fence_proxy_async();
+      if(leader) {
+        bulk_wait_read0();
+        if(prev_rs >= 0) mbar_arrive(smem_u32(&bars->r_empty[prev_rs]));
+      }
+      prev_rs = -1;
+      warpgroup_sync(g);
+      if(leader) {
+        const int c0 = s * RES_COLS, r0 = m0 + g * (BLOCK_M / 2);
+        tma_store_2d(&tmapS2, smem_u32(slot + g * (R2_BYTES / 2)), c0, r0);
+        tma_store_2d(&tmapA2, smem_u32(aslot + g * (ACT_SLICE_BYTES / 2)), c0, r0);
+        bulk_commit();
+      }
+      ps ^= 1;
+      as ^= 1;
+    }
+  }
+  if(leader) bulk_wait0();
+}
+
+template <int N2, int N1>
+static cudaError_t pairFuncAttrs() {
+  for(cudaError_t e : {cudaFuncSetAttribute(kgb_conv_pair_kernel<N2, N1, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
+                       cudaFuncSetAttribute(kgb_conv_pair_kernel<N2, N1, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
+                       cudaFuncSetAttribute(kgb_conv_pair_kernel<N2, N1, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT)})
+    if(e != cudaSuccess) return e;
+  return cudaSuccess;
+}
+
+// The (inner, trunk) widths of the nested-bottleneck nets: tiny_nbt, mid_nbt, b18c384nbt.  b28c512nbt's (256, 512) spills with fp32
+// streams (256-column acc2 next to acc1), so its boundaries keep two launches.
+#define KGB_PAIR_SHAPES(X) X(64, 64) X(64, 128) X(192, 384)
+
+static cudaError_t convPairInit() {
+#define KGB_PAIR_ATTR(N2, N1) pairFuncAttrs<N2, N1>(),
+  for(cudaError_t e : {KGB_PAIR_SHAPES(KGB_PAIR_ATTR)})
+    if(e != cudaSuccess) return e;
+#undef KGB_PAIR_ATTR
+  return cudaSuccess;
+}
+
+static bool pairShapeCompiled(int n2, int n1) {
+#define KGB_PAIR_IS(N2, N1) (n2 == N2 && n1 == N1) ||
+  return KGB_PAIR_SHAPES(KGB_PAIR_IS) false;
+#undef KGB_PAIR_IS
+}
+
+bool convPairSupported(const ConvParams& p1, const ConvParams& p2) {
+  const int n2 = p2.cout_p;
+  return p1.ky == 1 && p1.kx == 1 && p2.ky == 1 && p2.kx == 1 && !p1.split && !p2.split && p1.cin_p == n2 && p2.cin_p == p1.cout_p &&
+         pairShapeCompiled(n2, p1.cout_p) && p2.n_tile == n2 && p1.M == p2.M &&
+         p1.residual != nullptr && p1.raw_out != nullptr && p1.ncbias == nullptr && p1.act == 2 && p2.residual == nullptr &&
+         p2.raw_out != nullptr && p2.act_out != nullptr && p2.ncbias == nullptr && p2.act == 2 &&
+         (p1.residual_fp32 != 0) == (p1.raw_fp32 != 0) && !(p2.raw_fp32 && !p1.raw_fp32) && pairLayout(p1, p2).stages >= 2;
+}
+
+template <int N2, int N1>
+static cudaError_t launchPairN(const ConvPairTmaps& tm, const ConvParams& p1, const ConvParams& p2, int grid, const PairLayout& l,
+                               cudaStream_t stream) {
+  auto k = p1.raw_fp32 ? (p2.raw_fp32 ? kgb_conv_pair_kernel<N2, N1, true, true> : kgb_conv_pair_kernel<N2, N1, true, false>)
+                       : kgb_conv_pair_kernel<N2, N1, false, false>;
+  k<<<grid, THREADS, l.smem, stream>>>(tm.A, tm.W1, tm.W2, tm.stream1, tm.stream2, tm.act2, p1, p2, l.stages, l.r_slots);
+  return cudaGetLastError();
+}
+
+cudaError_t launchConvPair(const ConvPairTmaps& tm, const ConvParams& p1, const ConvParams& p2, cudaStream_t stream) {
+  if(!convPairSupported(p1, p2)) return cudaErrorInvalidValue;
+  int dev = 0;
+  const cudaError_t e = cudaGetDevice(&dev);
+  if(e != cudaSuccess) return e;
+  if(dev < 0 || dev >= 64 || g_smCount[dev] < 1) return cudaErrorInitializationError;
+  const PairLayout l = pairLayout(p1, p2);
+  const int grid = std::min(p1.num_m_tiles, g_smCount[dev]);
+#define KGB_PAIR_LAUNCH(N2, N1) if(p2.cout_p == N2 && p1.cout_p == N1) return launchPairN<N2, N1>(tm, p1, p2, grid, l, stream);
+  KGB_PAIR_SHAPES(KGB_PAIR_LAUNCH)
+#undef KGB_PAIR_LAUNCH
+  return cudaErrorInvalidValue;
 }
 
 }  // namespace kgb

@@ -58,6 +58,7 @@ struct kgb_handle {
   int split = 0;          // fp32-equivalent mode
   bool nhwc = true;
   bool streamTrunkFp32 = true, streamInnerFp32 = false;
+  bool fuseBoundaries = false;   // consecutive nested blocks' exit + entry 1x1 as one launch (launchConvPair)
   std::vector<void*> allocs;
   // inputs / outputs (device, fixed addresses so graphs can be replayed)
   float *dSpatial = nullptr, *dGlobal = nullptr, *dOptimism = nullptr;
