@@ -112,6 +112,11 @@ KGB_API int kgb_handle_sync(kgb_handle* handle);
 KGB_API uint64_t kgb_handle_stream(kgb_handle* handle);
 /* Number of kernel launches one kgb_forward of batch n issues (for bench.py's gpu_launches accounting). */
 KGB_API int kgb_handle_launches_per_forward(const kgb_handle* handle);
+/* The row layout the last forward or self-play wave on the handle used (waits for the handle's stream): the rows and 128-row
+ * tiles every convolution ran over, and the number of segments (board widths).  Each image takes (h+pad)*(w+pad) rows for the
+ * bounding box w x h of its mask, so a batch of small boards takes fewer rows than n*(nnYLen+pad)*(nnXLen+pad).  All zero
+ * before the first forward. */
+KGB_API int kgb_handle_get_layout_stats(kgb_handle* handle, int64_t* rows, int64_t* m_tiles, int64_t* segments);
 
 /* New weights into a live handle.  The reference polls its models directory and builds a fresh NNEvaluator for every new net
  * (command/selfplay.cpp:142-231 loadLatestNeuralNetIntoManager, :336-352 the polling thread; dataio/loadmodel.cpp:58

@@ -121,7 +121,7 @@ struct Builder {
   const ModelDesc& m;
   size_t Mmax;
   int actMul;  // 2 in split mode ([hi | lo])
-  Builder(kgb_handle& hh) : h(hh), m(*hh.model), Mmax((size_t)hh.maxBatch * hh.L.P), actMul(hh.split ? 2 : 1) {}
+  Builder(kgb_handle& hh) : h(hh), m(*hh.model), Mmax(hh.planRows(hh.maxBatch)), actMul(hh.split ? 2 : 1) {}
 
   struct Level {
     int C = 0, cp = 0;
@@ -216,9 +216,11 @@ struct Builder {
                                void* rawOut, bool rawFp32, __half* actOut, BNDev bn) {
     ConvParams p;
     memset(&p, 0, sizeof(p));
-    p.M = n * hh.L.P;
-    p.P = hh.L.P;
+    p.M = (int)hh.planRows(n);
     p.Wp = hh.L.Wp;
+    p.tile_wp = hh.plan.tileWp;
+    p.row_img = hh.plan.rowImg;
+    p.m_tiles = hh.plan.stats + 1;
     p.ky = cw.ky; p.kx = cw.kx;
     p.cin_p = cw.cin_p; p.cout_p = cw.cout_p;
     p.n_tile = cw.n_tile;
@@ -325,9 +327,9 @@ struct Builder {
         float* G = lv.G; __half* T = lv.T;
         const int gld = w1.cout_p, tcp = w2.cin_p, split = h.split;
         h.ops.push_back([=](int n, cudaStream_t s) {
-          CK(launchGPool(G, 1, gld, regC, gC, gbn.scale, gbn.bias, gbn.act, hp->dMask, hp->dMaskSum, n, hp->L, 0, pooled, s));
+          CK(launchGPool(G, 1, gld, regC, gC, gbn.scale, gbn.bias, gbn.act, hp->dMask, hp->dMaskSum, n, hp->L, hp->plan, 0, pooled, s));
           CK(launchMatMulNC(pooled, 3 * gC, Wg, nullptr, n, 3 * gC, regC, ACT_IDENTITY, bias, regC, s));
-          CK(launchBiasAct(G, 1, gld, regC, bias, regC, mid.scale, mid.bias, mid.act, hp->dMask, n * hp->L.P, hp->L.P, T, tcp, split, s));
+          CK(launchBiasAct(G, 1, gld, regC, bias, regC, mid.scale, mid.bias, mid.act, hp->dMask, (int)hp->planRows(n), hp->plan, T, tcp, split, s));
         });
         h.launchesPerForward += 3;
         emitConv(w2, lv.T, lv.S, lv.fp32, nullptr, rawOut, lv.fp32, lv.A, nextBN);
@@ -367,13 +369,20 @@ struct Builder {
     h.dOwnership = h.dalloc<float>((size_t)h.maxBatch * XY);
     h.dMask = h.dalloc<float>(Mmax + 128);
     h.dMaskSum = h.dalloc<float>(h.maxBatch);
+    h.plan.box = h.dalloc<int4>(h.maxBatch);
+    h.plan.base = h.dalloc<int>(h.maxBatch);
+    h.plan.tileWp = h.dalloc<int>(Mmax / 128);
+    h.plan.rowImg = h.dalloc<int>(Mmax);
+    h.plan.stats = h.dalloc<int>(3);
     __half* inAct = h.dalloc<__half>(Mmax * cinP * actMul);
     kgb_handle* hp = &h;
     const int C = m.numInputChannels, split = h.split;
     h.ops.push_back([=](int n, cudaStream_t s) {
-      CK(launchPackInput(hp->dSpatial, n, C, hp->nhwc, hp->dSymmetry, hp->L, inAct, cinP, split, hp->dMask, hp->dMaskSum, s));
+      CK(launchPlanRows(hp->dSpatial, n, C, hp->nhwc, hp->dSymmetry, hp->L, hp->plan, s));
+      CK(launchPackInput(hp->dSpatial, n, C, hp->nhwc, hp->dSymmetry, hp->L, hp->plan, hp->planRows(n), inAct, cinP, split, hp->dMask,
+                         hp->dMaskSum, s));
     });
-    h.launchesPerForward += 4;
+    h.launchesPerForward += 6;
     // trunk
     Level trunk = makeLevel(m.trunkC, h.streamTrunkFp32, m.blocks);
     float* initBias = h.dalloc<float>((size_t)h.maxBatch * trunk.cp);
@@ -420,10 +429,10 @@ struct Builder {
     const float* Wown = h.upload(m.ownershipConv.w);
     h.ops.push_back([=](int n, cudaStream_t s) {
       // policy head
-      CK(launchGPool(H, 1, hld, p1C, g1C, g1bn.scale, g1bn.bias, g1bn.act, hp->dMask, hp->dMaskSum, n, hp->L, 0, g1pool, s));
+      CK(launchGPool(H, 1, hld, p1C, g1C, g1bn.scale, g1bn.bias, g1bn.act, hp->dMask, hp->dMaskSum, n, hp->L, hp->plan, 0, g1pool, s));
       CK(launchMatMulNC(g1pool, 3 * g1C, Wg2b, nullptr, n, 3 * g1C, p1C, ACT_IDENTITY, g1bias, p1C, s));
       CK(launchPolicyOut(H, hld, 0, p1C, g1bias, p1C, p1bn.scale, p1bn.bias, p1bn.act, Wp2, cp2, hp->dMask, hp->dSymmetry,
-                         hp->dOptimism, n, hp->L, hp->dPolicy, s));
+                         hp->dOptimism, n, hp->L, hp->plan, hp->dPolicy, s));
       if(version >= 15) {
         CK(launchMatMulNC(g1pool, 3 * g1C, Wpass, passBias, n, 3 * g1C, passMid, passAct, passH, passMid, s));
         CK(launchMatMulNC(passH, passMid, Wpass2, nullptr, n, passMid, cp2, ACT_IDENTITY, passLogits, 4, s));
@@ -432,11 +441,11 @@ struct Builder {
         CK(launchMatMulNC(g1pool, 3 * g1C, Wpass, nullptr, n, 3 * g1C, cp2, ACT_IDENTITY, passLogits, 4, s));
       }
       // value head
-      CK(launchGPool(H, 1, hld, p1C + g1C, v1C, v1bn.scale, v1bn.bias, v1bn.act, hp->dMask, hp->dMaskSum, n, hp->L, 1, v1pool, s));
+      CK(launchGPool(H, 1, hld, p1C + g1C, v1C, v1bn.scale, v1bn.bias, v1bn.act, hp->dMask, hp->dMaskSum, n, hp->L, hp->plan, 1, v1pool, s));
       CK(launchMatMulNC(v1pool, 3 * v1C, Wv2, bv2, n, 3 * v1C, v2C, v2Act, v2, v2C, s));
       CK(launchMatMulNC(v2, v2C, Wv3, bv3, n, v2C, 3, ACT_IDENTITY, value, 3, s));
       CK(launchMatMulNC(v2, v2C, Wsv3, bsv3, n, v2C, numSV, ACT_IDENTITY, sv, numSV, s));
-      CK(launchOwnershipOut(H, hld, p1C + g1C, v1C, v1bn.scale, v1bn.bias, v1bn.act, Wown, hp->dMask, hp->dSymmetry, n, hp->L,
+      CK(launchOwnershipOut(H, hld, p1C + g1C, v1C, v1bn.scale, v1bn.bias, v1bn.act, Wown, hp->dMask, hp->dSymmetry, n, hp->L, hp->plan,
                             hp->dOwnership, s));
       CK(launchFinalize(passLogits, 4, cp2, hp->dOptimism, value, sv, numSV, version, n, hp->L.X * hp->L.Y + 1, hp->dPolicy,
                         hp->dValue, hp->dScore, s));
@@ -686,6 +695,10 @@ KGB_API int kgb_handle_create(kgb_context* ctx, const kgb_model* model, int max_
     // KGB_FUSE_BOUNDARY=0 keeps every nested block boundary as two launches (same-build A/B runs and tests; the results are the same)
     const char* fuse = getenv("KGB_FUSE_BOUNDARY");
     h.fuseBoundaries = !h.split && !(fuse && std::string(fuse) == "0");
+    // KGB_RAGGED_ROWS=0 lays every image out at the full frame (the reference plan of the tests and same-build A/B runs; the
+    // results are the same)
+    const char* ragged = getenv("KGB_RAGGED_ROWS");
+    h.plan.ragged = !(ragged && std::string(ragged) == "0");
     CK(cudaStreamCreateWithFlags(&h.stream, cudaStreamNonBlocking));
     CK(convWGInit());
     CK(cudaStreamCreateWithFlags(&h.copyStream, cudaStreamNonBlocking));
@@ -824,6 +837,17 @@ KGB_API int kgb_handle_is_fp16(const kgb_handle* handle) { return handle && !han
 KGB_API uint64_t kgb_handle_stream(kgb_handle* handle) { return handle ? (uint64_t)(uintptr_t)handle->stream : 0; }
 KGB_API int kgb_handle_launches_per_forward(const kgb_handle* handle) { return handle ? handle->launchesPerForward : 0; }
 
+KGB_API int kgb_handle_get_layout_stats(kgb_handle* handle, int64_t* rows, int64_t* m_tiles, int64_t* segments) {
+  return guarded([&] {
+    if(!handle || !rows || !m_tiles || !segments) throw std::invalid_argument("kgb_handle_get_layout_stats: NULL argument");
+    CK(cudaSetDevice(handle->device));
+    int st[3] = {0, 0, 0};
+    CK(cudaMemcpyAsync(st, handle->plan.stats, sizeof(st), cudaMemcpyDeviceToHost, handle->stream));
+    CK(cudaStreamSynchronize(handle->stream));
+    *rows = st[0]; *m_tiles = st[1]; *segments = st[2];
+  });
+}
+
 KGB_API int kgb_handle_sync(kgb_handle* handle) {
   return guarded([&] {
     if(!handle) throw std::invalid_argument("kgb_handle_sync: NULL handle");
@@ -900,6 +924,29 @@ KGB_API int kgb_forward_device(kgb_handle* h, int n, const float* d_spatial, con
 
 // Stand-alone single convolution (testEvaluateConv / kernel-level roofline timing).
 namespace {
+// The frame layout as a fixed plan for h.maxBatch images: image i at row i*P, no gap rows (the single-layer hooks lay out and
+// mask their rows on the host).
+void uploadFramePlan(kgb_handle& h) {
+  const int n = h.maxBatch, P = h.L.P;
+  h.fixedPlan = true;
+  const size_t M = h.planRows(n), tiles = (M + 127) / 128;
+  std::vector<int4> box(n, make_int4(0, 0, h.L.X, h.L.Y));
+  std::vector<int> base(n), tileWp(tiles, h.L.Wp), rowImg(M), stats = {(int)M, (int)tiles, 1};
+  for(int i = 0; i < n; i++) base[i] = i * P;
+  for(size_t r = 0; r < M; r++) rowImg[r] = (int)(r / P);
+  h.plan.box = h.dalloc<int4>(n);
+  h.plan.base = h.dalloc<int>(n);
+  h.plan.tileWp = h.dalloc<int>(tiles);
+  h.plan.rowImg = h.dalloc<int>(M);
+  h.plan.stats = h.dalloc<int>(3);
+  CK(cudaMemcpyAsync(h.plan.box, box.data(), n * sizeof(int4), cudaMemcpyHostToDevice, h.stream));
+  CK(cudaMemcpyAsync(h.plan.base, base.data(), n * sizeof(int), cudaMemcpyHostToDevice, h.stream));
+  CK(cudaMemcpyAsync(h.plan.tileWp, tileWp.data(), tiles * sizeof(int), cudaMemcpyHostToDevice, h.stream));
+  CK(cudaMemcpyAsync(h.plan.rowImg, rowImg.data(), M * sizeof(int), cudaMemcpyHostToDevice, h.stream));
+  CK(cudaMemcpyAsync(h.plan.stats, stats.data(), 3 * sizeof(int), cudaMemcpyHostToDevice, h.stream));
+  CK(cudaStreamSynchronize(h.stream));
+}
+
 struct SingleConv {
   kgb_handle h;
   ModelDesc dummy;
@@ -929,6 +976,7 @@ struct SingleConv {
     h.streamTrunkFp32 = h.streamInnerFp32 = h.split != 0;
     CK(cudaStreamCreateWithFlags(&h.stream, cudaStreamNonBlocking));
     CK(convWGInit());
+    uploadFramePlan(h);
     ConvDesc cd;
     cd.ky = ky; cd.kx = kx; cd.cin = in_c; cd.cout = out_c;
     cd.w.assign(weights, weights + (size_t)ky * kx * in_c * out_c);
@@ -967,7 +1015,7 @@ struct SingleConv {
   void setInput(const float* input /* NHWC */, const int32_t* boardXY = nullptr) {
     float* dIn = h.dalloc<float>((size_t)n * X * Y * cin);
     CK(cudaMemcpyAsync(dIn, input, (size_t)n * X * Y * cin * sizeof(float), cudaMemcpyHostToDevice, h.stream));
-    CK(launchPackInput(dIn, n, cin, true, nullptr, h.L, As[0], cw.cin_p, h.split, h.dMask, h.dMaskSum, h.stream));
+    CK(launchPackInput(dIn, n, cin, true, nullptr, h.L, h.plan, M, As[0], cw.cin_p, h.split, h.dMask, h.dMaskSum, h.stream));
     for(size_t r = 1; r < As.size(); r++)
       CK(cudaMemcpyAsync(As[r], As[0], M * cw.cin_p * (h.split ? 2 : 1) * sizeof(__half), cudaMemcpyDeviceToDevice, h.stream));
     // the mask of a bare convolution is "every point of the image's board", not input channel 0
@@ -1008,6 +1056,7 @@ struct BoundaryConv {
     h.L = boardLayout(X, Y, 1);
     CK(cudaStreamCreateWithFlags(&h.stream, cudaStreamNonBlocking));
     CK(convWGInit());
+    uploadFramePlan(h);
     uint32_t st = seed * 2654435761u + 12345u;
     auto uni = [&]() { st = st * 1664525u + 1013904223u; return (st >> 8) * (1.0f / 16777216.0f); };
     ConvDesc post, pre;

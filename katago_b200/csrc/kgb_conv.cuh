@@ -16,25 +16,29 @@ namespace kgb {
 //   (cudabackend.cpp:788-841) [beta=1 residual accumulate]  [-> addNCBiasInplace* (cudahelpers.cu:1250-1364)]
 // i.e. NormActConv::apply / ConvLayer::apply of the Eigen path (eigenbackend.cpp:448-701, 1065-1077).
 //
-// Data layout ("padded rows"): activations are 2-D row-major [M = n*P rows][C_p channels], C_p a multiple of 64,
-// where every image owns P = (Y+pad)*(X+pad) rows: `pad` zero rows on top and `pad` zero columns at the right of each
-// board row (pad = largest conv radius of the net).  A (dy,dx) filter tap is then the same matrix shifted by
-// dy*(X+pad)+dx rows, the zero padding of the convolution is physically present (or supplied by TMA out-of-bounds
-// fill at the two ends), and boards smaller than (X,Y) are handled by the same mask that zeroes the pad rows.
+// Data layout ("padded rows"): activations are 2-D row-major [M rows][C_p channels], C_p a multiple of 64, where every image
+// owns (h+pad)*(w+pad) rows for its board box w x h: `pad` zero rows on top and `pad` zero columns at the right of each board
+// row (pad = largest conv radius of the net), pitch w+pad.  A (dy,dx) filter tap is then the same matrix shifted by
+// dy*(w+pad)+dx rows, and the zero padding of the convolution is physically present (or supplied by TMA out-of-bounds fill at
+// the two ends).  Images of one width are laid out back to back in segments of whole 128-row tiles (RowPlan, kgb_kernels.cuh),
+// so each tile has one pitch; points of the box that are off the board are handled by the same mask that zeroes the pad rows.
+// The frame layout is the case where every box is the full X x Y frame: image i at row i*(Y+pad)*(X+pad).
 struct ConvParams {
-  int M;            // valid rows (= batch * P)
-  int P;            // rows per image
-  int Wp;           // X + pad (row pitch of the board inside an image)
+  int M;            // rows the buffers hold (at least the plan's rows)
+  int Wp;           // X + pad, the frame's pitch: the A halo box is sized for it, the widest pitch a tile can have
+  const int* tile_wp;     // [num_m_tiles] row pitch of each 128-row tile
+  const int* row_img;     // [M] image of each board row, read for ncbias (other rows are masked: -1 or any image)
+  const int* m_tiles;     // the number of 128-row tiles the plan uses (device), at most num_m_tiles
   int ky, kx;       // filter size
   int cin_p;        // padded input channels (multiple of 64)
   int cout_p;       // padded output channels (multiple of 64)
   int n_tile;       // wgmma N (cout_p / num_n_tiles), multiple of 32, <= 256
-  int num_m_tiles, num_n_tiles;
+  int num_m_tiles, num_n_tiles;   // num_m_tiles: the most tiles a plan can use (sizes the persistent grid)
   int split;        // 0: fp16 operands; 1: 3-term split-fp16 ("fp32-equivalent") - A and W carry [hi | lo] halves
   // epilogue
   const void* residual;   // [M][cout_p] or null
   int residual_fp32;
-  const float* ncbias;    // [batch][cout_p] or null
+  const float* ncbias;    // [batch][cout_p] or null, by row_img
   void* raw_out;          // [M][cout_p] or null
   int raw_fp32;
   __half* act_out;        // [M][cout_p * (split ? 2 : 1)] or null

@@ -121,6 +121,7 @@ struct __align__(8) Bars {
   uint64_t a_empty[2];          // A halo tile consumed by all of its taps
   uint64_t r_full[RES_SLOTS];   // residual slice landed
   uint64_t r_empty[RES_SLOTS];  // residual slice read, and the raw stream written over it stored, by both consumer warpgroups
+  int a_wp[2];                  // row pitch of the tile whose A halo tile is in the slot (written before the slot's a_full arrive)
 };
 
 // dynamic smem: [<=1023 B slack][2 x A halo tile][stream ring][ACT_SLOTS x act slice (x 2 split)][stages x weight tile][Bars]
@@ -181,7 +182,7 @@ __device__ __forceinline__ void epilogue_store(const ConvParams& p, int row, int
   const bool mish = rt ? p.act == 2 : true;
   const bool split = rt ? p.split != 0 : (F & EPI_SPLIT) != 0;
   if(has_ncbias) {
-    const float2 b = __ldg(reinterpret_cast<const float2*>(p.ncbias + (size_t)(row / p.P) * p.cout_p + col));
+    const float2 b = __ldg(reinterpret_cast<const float2*>(p.ncbias + (size_t)max(__ldg(p.row_img + row), 0) * p.cout_p + col));   // off-board rows are masked
     v0 += b.x; v1 += b.y;
   }
   if(has_res) { v0 += r.x; v1 += r.y; }
@@ -274,7 +275,7 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr int b_tile_bytes = N * BLOCK_K * 2;               // one tap's weight tile
-  const int halo = (p.ky / 2) * p.Wp + (p.kx / 2);            // rows of A above / below the tile that the taps reach
+  const int halo = (p.ky / 2) * p.Wp + (p.kx / 2);            // rows of A above / below the tile that the widest pitch's taps reach
   const int a_tx_bytes = (BLOCK_M + 2 * halo) * BLOCK_K * 2;
   const int a_buf_bytes = (a_tx_bytes + 1023) / 1024 * 1024;
   constexpr int slices = N / RES_COLS;
@@ -291,7 +292,7 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
-  const int tiles = p.num_m_tiles * p.num_n_tiles;
+  const int tiles = __ldg(p.m_tiles) * p.num_n_tiles;        // the plan's tiles; a CTA past them has nothing to do
   const int n0 = (blockIdx.x % p.num_n_tiles) * N;            // gridDim.x is a multiple of num_n_tiles: one n0 per CTA
   const int taps = p.ky * p.kx;
   const int parts = p.split ? 3 : 1;
@@ -328,6 +329,7 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
       uint32_t phase = 0;
       for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
         const int m0 = (tile / p.num_n_tiles) * BLOCK_M;
+        const int wp = __ldg(p.tile_wp + m0 / BLOCK_M);       // loaded here, ahead of the consumers, who read it from the A slot
         for(int ph = 0; ph < phases; ph++, ac++) {
           const int kb = ph / parts, part = ph - kb * parts;
           const int colA = kb * BLOCK_K + (part == 1 ? p.cin_p : 0);
@@ -335,6 +337,7 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
           const int abuf = ac & 1;
           mbar_wait(smem_u32(&bars->a_empty[abuf]), ((ac >> 1) & 1) ^ 1);
           const uint32_t afull = smem_u32(&bars->a_full[abuf]);
+          bars->a_wp[abuf] = wp;
           mbar_arrive_expect_tx(afull, (uint32_t)a_tx_bytes);
           tma_load_2d(smem_base + abuf * a_buf_bytes, &tmapA, afull, colA, m0 - halo);
           for(int t = 0; t < taps; t++) {
@@ -390,6 +393,7 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
   uint8_t* const act_ring = smem + (smem_act - smem_base);
   for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
     const int m0 = (tile / p.num_n_tiles) * BLOCK_M;
+    int wp = 0;                                               // the tile's row pitch, from the A slot
     // this thread's two epilogue rows' mask values; the loads complete during the main loop
     const float mask0 = m0 + rloc < p.M ? __ldg(p.mask + m0 + rloc) : 0.0f;
     const float mask1 = m0 + rloc + 8 < p.M ? __ldg(p.mask + m0 + rloc + 8) : 0.0f;
@@ -400,13 +404,17 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
     // One step = one (k-block, tap): ldmatrix the tap's A fragments into `af` and issue its 4 wgmma as one group.  Steps alternate
     // between two fragment buffers; wait_group 1 after issuing step i means step i-1's group has finished, so its weight stage can
     // be released and its fragment buffer is free for step i+1.  The MMAs reach the accumulators in k-block, tap, k16 order.
-    int prev_stage = -1, t = 0, dy = -ry, dx = -rx;
+    // the tap is (dy, dx); the k-block's first tap is (-ry, -rx), its last (ry, rx)
+    int prev_stage = -1, dy = -ry, dx = -rx;
     auto step = [&](uint32_t (&af)[4][4]) {
       const int abuf = ph & 1;
-      if(t == 0) mbar_wait(smem_u32(&bars->a_full[abuf]), (ph >> 1) & 1);
+      if(dy == -ry && dx == -rx) {
+        mbar_wait(smem_u32(&bars->a_full[abuf]), (ph >> 1) & 1);
+        wp = bars->a_wp[abuf];
+      }
       const uint32_t a_base = smem_base + abuf * a_buf_bytes;
-      // tap (dy,dx) = the tile's rows shifted by `halo + dy*Wp + dx`; the 128B swizzle puts 16-byte chunk c of row r at c ^ (r & 7)
-      const uint32_t r = (uint32_t)(lrow + halo + dy * p.Wp + dx);
+      // tap (dy,dx) = the tile's rows shifted by `halo + dy*wp + dx`; the 128B swizzle puts 16-byte chunk c of row r at c ^ (r & 7)
+      const uint32_t r = (uint32_t)(lrow + halo + dy * wp + dx);
 #pragma unroll
       for(int k = 0; k < 4; k++) ldmatrix_x4(a_base + r * 128u + (((2u * k + lchunk) ^ (r & 7u)) << 4), af[k]);
       mbar_wait(smem_u32(&bars->full[stage]), phase);
@@ -416,7 +424,7 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
       for(int k = 0; k < 4; k++) Wgmma<N>::mma(acc, af[k], db + 2 * k);
       wgmma_commit();
       // the wgmma issue above consumed the fragments of the k-block's last tap, so its A halo tile may be refilled
-      if(t == taps - 1) {
+      if(dy == ry && dx == rx) {
         __syncwarp();
         if(lane == 0) mbar_arrive(smem_u32(&bars->a_empty[abuf]));
       }
@@ -427,8 +435,10 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
       }
       prev_stage = stage;
       if(++stage == stages) { stage = 0; phase ^= 1; }
-      if(++dx > rx) { dx = -rx; dy++; }
-      if(++t == taps) { t = 0; dy = -ry; ph++; }
+      if(++dx > rx) {
+        dx = -rx;
+        if(++dy > ry) { dy = -ry; ph++; }
+      }
     };
     const int steps = phases * taps;
     uint32_t af0[4][4], af1[4][4];
@@ -624,7 +634,7 @@ kgb_conv_pair_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_con
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
-  const int tiles = p1.num_m_tiles;
+  const int tiles = __ldg(p1.m_tiles);
 
   if(threadIdx.x == 0) {
     for(const CUtensorMap* m : {&tmapA, &tmapW1, &tmapW2, &tmapS1, &tmapS2, &tmapA2})

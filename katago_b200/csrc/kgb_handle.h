@@ -69,6 +69,12 @@ struct kgb_handle {
         *hOwnership = nullptr;
   int* hSymmetry = nullptr;
   float *dMask = nullptr, *dMaskSum = nullptr;
+  // The rows of the current forward (kgb_kernels.cuh RowPlan), planned on the device at the start of every forward; plan.ragged
+  // is off with KGB_RAGGED_ROWS=0 (every image at the full frame).  The single-layer test hooks upload the frame layout once
+  // instead (fixedPlan): n*P rows, no gap.
+  kgb::RowPlan plan{};
+  bool fixedPlan = false;
+  size_t planRows(int n) const { return fixedPlan ? (size_t)n * L.P : kgb::planRowCapacity(L, n); }   // rows the row buffers hold
   std::vector<std::function<void(int, cudaStream_t)>> ops;
   int launchesPerForward = 0;
   std::map<int, cudaGraphExec_t> graphs;

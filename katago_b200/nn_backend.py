@@ -80,7 +80,7 @@ ABI_SYMBOLS = [
     "kgb_global_init", "kgb_global_cleanup", "kgb_last_error", "kgb_device_count", "kgb_device_name",
     "kgb_model_load_file", "kgb_model_free", "kgb_model_get_info", "kgb_context_create", "kgb_context_free",
     "kgb_handle_create", "kgb_handle_free", "kgb_handle_is_fp16", "kgb_forward", "kgb_forward_device", "kgb_handle_sync",
-    "kgb_handle_stream", "kgb_handle_launches_per_forward", "kgb_test_conv", "kgb_bench_conv_ex", "kgb_test_conv_epilogue",
+    "kgb_handle_stream", "kgb_handle_launches_per_forward", "kgb_handle_get_layout_stats", "kgb_test_conv", "kgb_bench_conv_ex", "kgb_test_conv_epilogue",
     "kgb_test_conv_ex", "kgb_test_conv_boundary", "kgb_bench_conv_boundary",
     "kgb_selfplay_create", "kgb_selfplay_free", "kgb_selfplay_run", "kgb_selfplay_get_stats", "kgb_selfplay_get_game",
     "kgb_selfplay_get_root_children", "kgb_selfplay_launches_per_step", "kgb_selfplay_play_moves", "kgb_selfplay_time_tree_kernels", "kgb_zobrist_tables", "kgb_selfplay_get_nn_row", "kgb_selfplay_get_root_row", "kgb_test_board_replay", "kgb_selfplay_get_leaf_path", "kgb_expected_white_score_value", "kgb_value_weight_cdf_table", "kgb_rand_uint32_stream", "kgb_test_root_policy_noise", "kgb_test_history_replay", "kgb_test_repetition_bound", "kgb_selfplay_get_play_selection_values", "kgb_selfplay_random_openings", "kgb_selfplay_set_search_rand", "kgb_selfplay_get_root_value_stats", "kgb_test_choose_index_with_temperature",
@@ -150,6 +150,7 @@ def load_library():
     lib.kgb_handle_stream.argtypes = [P]
     lib.kgb_handle_stream.restype = C.c_uint64
     lib.kgb_handle_launches_per_forward.argtypes = [P]
+    lib.kgb_handle_get_layout_stats.argtypes = [P, P, P, P]
     lib.kgb_test_conv.argtypes = [I, I, I, I, P, I, I, I, I, P, P]
     lib.kgb_bench_conv_ex.argtypes = [I, I, I, I, I, I, I, I, I, I, I, I, F]
     lib.kgb_test_conv_epilogue.argtypes = [I, I, I, I, P, I, I, I, I, I, P, P, P, P, I, P, P]
@@ -254,6 +255,13 @@ class ComputeHandle:
     @property
     def launches_per_forward(self) -> int:
         return load_library().kgb_handle_launches_per_forward(self._p)
+
+    def layout_stats(self) -> dict:
+        """The row layout of the last forward or self-play wave on this handle (waits for its stream): rows and 128-row tiles
+        the convolutions ran over, and segments (board widths)."""
+        v = [C.c_int64() for _ in range(3)]
+        _check(load_library().kgb_handle_get_layout_stats(self._p, *(C.byref(x) for x in v)))
+        return dict(zip(("rows", "m_tiles", "segments"), (int(x.value) for x in v)))
 
     @property
     def stream(self) -> int:
