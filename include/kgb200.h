@@ -483,6 +483,45 @@ KGB_API int kgb_test_conv_ex(int ky, int kx, int in_c, int out_c, const float* w
  * or padded channels.  Fails when the fused kernel does not take the shape. */
 KGB_API int kgb_test_conv_boundary(int inner_c, int trunk_c, int n, int nn_x_len, int nn_y_len, const int32_t* board_xy, int trunk_fp32,
                                    int inner_fp32, uint32_t seed, int64_t* out);
+/* Plan mode of the layer hooks.  The rows are planned on the device as a forward plans them (launchPlanRows, then launchPackInput):
+ * image i's mask is 1 on the top-left board_xy[i] of the frame ({0, 0}: an empty mask) and 0 elsewhere, moved by symmetry[i] (NULL:
+ * all 0); ragged 1 lays each board out at its own box, ragged 0 every image at the full frame.  Row buffers are sized for the largest
+ * plan of n images.  Every input but `input` (given before the symmetry, zero off the board, as fillRowV7 writes it) and every
+ * output is NHWC in the coordinates after the symmetry.  Rows of the operand at or past the plan's end hold a finite sentinel (fp16
+ * 1024), as a larger earlier forward can leave them; rows of the outputs there are filled with all-ones bytes (NaN) before the launch.
+ * The hook fails if an output row past the plan's end was written, or if any channel of a row below it that is not a board position
+ * (pad rows and columns, gap rows, the tail up to 128 rows), or a padded channel of any row, is not exactly zero.  layout_stats [3]
+ * (rows, 128-row tiles, segments) and plan_out [n][5] (box x0, y0, w, h and first row; -1 for an empty mask), either may be NULL. */
+KGB_API int kgb_test_conv_plan(int ky, int kx, int in_c, int out_c, const float* weights, int n, int nn_x_len, int nn_y_len, int use_fp16,
+                               int epilogue_kind, const float* input, const int32_t* board_xy, const int32_t* symmetry, int ragged,
+                               const float* ncbias, const float* residual_in, const float* bn_scale, const float* bn_bias, int activation,
+                               float* raw_out, float* act_hi_out, float* act_lo_out, int64_t* layout_stats, int32_t* plan_out);
+/* kgb_test_conv_boundary under a plan made as for kgb_test_conv_plan, every buffer's rows past the plan's end NaN.  out [12]:
+ * out[0..5] as kgb_test_conv_boundary over the rows below the plan's end; out[6..8] NaN elements of the fused outputs there;
+ * out[9..11] bytes past the plan's end that either path changed.  layout_stats [3] or NULL. */
+KGB_API int kgb_test_conv_boundary_plan(int inner_c, int trunk_c, int n, int nn_x_len, int nn_y_len, const int32_t* board_xy,
+                                        const int32_t* symmetry, int ragged, int trunk_fp32, int inner_fp32, uint32_t seed, int64_t* out,
+                                        int64_t* layout_stats);
+/* Test hook of the evaluator's fp32 kernels: one launch of kernel `which` on caller-given fp32 tensors, in a frame of
+ * nn_x_len x nn_y_len with `pad` (1 or 2).  Kernels that read rows run under a plan made as for kgb_test_conv_plan (board_xy,
+ * symmetry, ragged; layout_stats and plan_out as there); their row inputs are NHWC [n][y][x][C] after the symmetry and are placed
+ * in the rows of the board positions, every other element of the row buffer NaN.  Outputs the kernel does not write hold NaN.
+ *   0 pack     iparams {C, split, nhwc}; inputs {spatial [n][C][y][x] or [n][y][x][C], channel 0 the mask}, planned from the
+ *              spatial itself (board_xy unused); outputs {hi [n][y][x][C], lo (split) or NULL, mask sums [n], mask [n][y][x]}, after
+ *              the symmetry.  Fails if a row that is not a board position, or a padded channel, is not zero.
+ *   1 gpool    iparams {C, act, valueHead, rawFp32, c0, ldr}; inputs {raw (stored as fp16 when !rawFp32), bn scale [C], bias [C]};
+ *              outputs {pooled [n][3C]}.
+ *   2 biasAct  iparams {C, act, split, rawFp32}; inputs {raw, ncbias [n][C] or NULL, scale, bias}; outputs {hi, lo (split) or NULL}
+ *              NHWC after the symmetry.  Fails as pack does, or if a row past the plan's end was written.
+ *   3 matMulNC iparams {cin, cout, act, ldi, ldo}; inputs {in [n][ldi], W [cin][cout], bias [cout] or NULL}; outputs {[n][ldo]}.
+ *   4 policy   iparams {C, act, cp2, c0, ldr}; inputs {raw, g1bias [n][C], scale, bias, Wp2 [C][cp2], optimism [n] or NULL};
+ *              outputs {policy [n][x*y+1]}.
+ *   5 ownership iparams {C, act, c0, ldr}; inputs {raw, scale, bias, Wown [C]}; outputs {ownership [n][x*y]}.
+ *   6 finalize iparams {cp2, numSV, version, ldp}; inputs {pass logits [n][ldp], optimism [n] or NULL, value [n][3], score values
+ *              [n][numSV]}; outputs {policy [n][x*y+1], value [n][3], score [n][6]}. */
+KGB_API int kgb_test_head_kernel(int which, int n, int nn_x_len, int nn_y_len, int pad, const int32_t* board_xy, const int32_t* symmetry,
+                                 int ragged, const int32_t* iparams, int num_iparams, const float* const* inputs, int num_inputs,
+                                 float* const* outputs, int num_outputs, int64_t* layout_stats, int32_t* plan_out);
 /* Timing hook of the same boundary (whole boards): ms per boundary, fused (one launch) or not (two launches), cycling through
  * `rotate` buffer sets. */
 KGB_API int kgb_bench_conv_boundary(int inner_c, int trunk_c, int n, int nn_x_len, int nn_y_len, int trunk_fp32, int inner_fp32, int fused,

@@ -947,6 +947,106 @@ void uploadFramePlan(kgb_handle& h) {
   CK(cudaStreamSynchronize(h.stream));
 }
 
+// Plan mode of the test hooks: the row plan the evaluator makes at the start of a forward, for boards given by size.
+// The plan's buffers for h.maxBatch images, sized as Builder::build sizes them.
+void allocPlan(kgb_handle& h) {
+  const size_t Mmax = h.planRows(h.maxBatch);
+  h.dMask = h.dalloc<float>(Mmax + 128);
+  h.dMaskSum = h.dalloc<float>(h.maxBatch);
+  h.plan.box = h.dalloc<int4>(h.maxBatch);
+  h.plan.base = h.dalloc<int>(h.maxBatch);
+  h.plan.tileWp = h.dalloc<int>(Mmax / 128);
+  h.plan.rowImg = h.dalloc<int>(Mmax);
+  h.plan.stats = h.dalloc<int>(3);
+  h.dSymmetry = h.dalloc<int>(h.maxBatch);
+}
+
+// A plan as the device holds it after launchPlanRows + launchPackInput.
+struct HostPlan {
+  std::vector<int4> box;
+  std::vector<int> base;
+  std::vector<float> mask;   // [M]
+  int stats[3] = {0, 0, 0};
+  // row of frame position (y, x) of image i, or -1 outside its box (planRow)
+  long row(const Layout& L, int i, int y, int x) const {
+    const int4 b = box[i];
+    const int yy = y - b.y, xx = x - b.x;
+    if(yy < 0 || xx < 0 || yy >= b.w || xx >= b.z) return -1;
+    return (long)base[i] + (long)(yy + L.pad) * (b.z + L.pad) + xx;
+  }
+  void copyOut(int n, int64_t* statsOut, int32_t* planOut) const {
+    if(statsOut) for(int k = 0; k < 3; k++) statsOut[k] = stats[k];
+    if(planOut)
+      for(int i = 0; i < n; i++) {
+        const int4 b = box[i];
+        const int32_t v[5] = {b.x, b.y, b.z, b.w, base[i]};
+        memcpy(planOut + 5 * i, v, sizeof(v));
+      }
+  }
+};
+
+void checkBoards(const char* fn, int n, int X, int Y, const int32_t* board_xy, const int32_t* symmetry, bool allowEmpty) {
+  for(int i = 0; board_xy && i < n; i++) {
+    const int bx = board_xy[2 * i], by = board_xy[2 * i + 1];
+    if(!(allowEmpty && bx == 0 && by == 0) && (bx < 1 || bx > X || by < 1 || by > Y))
+      throw std::invalid_argument(std::string(fn) + ": board size of image " + std::to_string(i) + " not in the frame");
+  }
+  for(int i = 0; symmetry && i < n; i++)
+    if(symmetry[i] < 0 || symmetry[i] > 7) throw std::invalid_argument(std::string(fn) + ": symmetry must be in 0..7");
+}
+
+// Step 1: the mask of image i is 1 on the top-left board_xy[i] of the frame (0 x 0: an empty mask), as fillRowV7 places boards,
+// before symmetry[i]; launchPlanRows plans the rows from it (h.plan.ragged chooses the plan).  Returns the mask input (NHWC, 1 channel).
+float* planBoards(kgb_handle& h, int n, const int32_t* board_xy, const int32_t* symmetry) {
+  const Layout& L = h.L;
+  std::vector<float> m((size_t)n * L.X * L.Y, 0.0f);
+  std::vector<int> sym(n, 0);
+  for(int i = 0; i < n; i++) {
+    const int bx = board_xy ? board_xy[2 * i] : L.X, by = board_xy ? board_xy[2 * i + 1] : L.Y;
+    for(int y = 0; y < by; y++)
+      for(int x = 0; x < bx; x++) m[((size_t)i * L.Y + y) * L.X + x] = 1.0f;
+    if(symmetry) sym[i] = symmetry[i];
+  }
+  float* dm = h.dalloc<float>(m.size());
+  CK(cudaMemcpyAsync(dm, m.data(), m.size() * sizeof(float), cudaMemcpyHostToDevice, h.stream));
+  CK(cudaMemcpyAsync(h.dSymmetry, sym.data(), n * sizeof(int), cudaMemcpyHostToDevice, h.stream));
+  CK(launchPlanRows(dm, n, 1, true, h.dSymmetry, L, h.plan, h.stream));
+  return dm;
+}
+
+// Step 2 (after the caller packed its own features, which sets the mask from their channel 0): the mask packed as the mask,
+// with its sums and the row -> image table, and the plan read back.
+HostPlan readPlan(kgb_handle& h, int n);
+HostPlan finishPlan(kgb_handle& h, int n, const float* dMaskIn) {
+  const size_t M = h.planRows(n);
+  __half* scratch = h.dalloc<__half>(M * 64);
+  CK(launchPackInput(dMaskIn, n, 1, true, h.dSymmetry, h.L, h.plan, M, scratch, 64, 0, h.dMask, h.dMaskSum, h.stream));
+  return readPlan(h, n);
+}
+HostPlan readPlan(kgb_handle& h, int n) {
+  const size_t M = h.planRows(n);
+  HostPlan hp;
+  hp.box.resize(n); hp.base.resize(n); hp.mask.resize(M);
+  CK(cudaMemcpyAsync(hp.box.data(), h.plan.box, n * sizeof(int4), cudaMemcpyDeviceToHost, h.stream));
+  CK(cudaMemcpyAsync(hp.base.data(), h.plan.base, n * sizeof(int), cudaMemcpyDeviceToHost, h.stream));
+  CK(cudaMemcpyAsync(hp.mask.data(), h.dMask, M * sizeof(float), cudaMemcpyDeviceToHost, h.stream));
+  CK(cudaMemcpyAsync(hp.stats, h.plan.stats, sizeof(hp.stats), cudaMemcpyDeviceToHost, h.stream));
+  CK(cudaStreamSynchronize(h.stream));
+  if(hp.stats[0] < 0 || (size_t)hp.stats[0] > M || hp.stats[0] % 128 != 0 || hp.stats[1] * 128 != hp.stats[0])
+    throw std::runtime_error("the plan's rows " + std::to_string(hp.stats[0]) + " do not fit its buffers of " + std::to_string(M) + " rows");
+  return hp;
+}
+
+// Rows at or past the plan's end are filled with all-ones bytes (a NaN in fp16 and fp32) before a launch; no launch may write them.
+void poisonTail(kgb_handle& h, void* buf, size_t rowBytes, size_t fromRow, size_t M) {
+  if(buf && fromRow < M) CK(cudaMemsetAsync((uint8_t*)buf + fromRow * rowBytes, 0xFF, (M - fromRow) * rowBytes, h.stream));
+}
+size_t countTouchedTail(const std::vector<uint8_t>& v, size_t rowBytes, size_t fromRow) {
+  size_t k = 0;
+  for(size_t b = fromRow * rowBytes; b < v.size(); b++) k += v[b] != 0xFF;
+  return k;
+}
+
 struct SingleConv {
   kgb_handle h;
   ModelDesc dummy;
@@ -966,7 +1066,8 @@ struct SingleConv {
   // with KGB_STREAM_FP32=trunk.  In fp32-equivalent mode every stream is fp32.  `rotate` independent buffer sets are cycled through
   // by run() so that a timing loop does not live in L2.
   SingleConv(int ky, int kx, int in_c, int out_c, const float* weights, int n_, int X_, int Y_, int use_fp16, int kind, int rotate_ = 1,
-             const float* bnScale = nullptr, const float* bnBias = nullptr, int actKind = ACT_MISH, bool withNcbias = false)
+             const float* bnScale = nullptr, const float* bnBias = nullptr, int actKind = ACT_MISH, bool withNcbias = false,
+             int ragged = -1)
       : n(n_), X(X_), Y(Y_), cin(in_c), cout(out_c), rotate(rotate_ < 1 ? 1 : rotate_) {
     h.device = selectDevice(-1);
     h.model = &dummy;
@@ -976,7 +1077,12 @@ struct SingleConv {
     h.streamTrunkFp32 = h.streamInnerFp32 = h.split != 0;
     CK(cudaStreamCreateWithFlags(&h.stream, cudaStreamNonBlocking));
     CK(convWGInit());
-    uploadFramePlan(h);
+    // ragged < 0: the fixed frame layout, masked on the host (setInput); else plan mode (setInputPlanned)
+    if(ragged < 0) uploadFramePlan(h);
+    else {
+      h.plan.ragged = ragged;
+      allocPlan(h);
+    }
     ConvDesc cd;
     cd.ky = ky; cd.kx = kx; cd.cin = in_c; cd.cout = out_c;
     cd.w.assign(weights, weights + (size_t)ky * kx * in_c * out_c);
@@ -991,9 +1097,11 @@ struct SingleConv {
       dev = b.uploadBN(bn, actKind, cw.cout_p);
     });
     Builder b(h);
-    M = (size_t)n * h.L.P;
-    h.dMask = h.dalloc<float>(M + 128);
-    h.dMaskSum = h.dalloc<float>(n);
+    M = h.planRows(n);
+    if(ragged < 0) {
+      h.dMask = h.dalloc<float>(M + 128);
+      h.dMaskSum = h.dalloc<float>(n);
+    }
     rawF32 = kind == 0 || kind == 4 || h.split != 0;
     if(withNcbias) ncbias = h.dalloc<float>((size_t)n * cw.cout_p);
     for(int r = 0; r < rotate; r++) {
@@ -1028,6 +1136,21 @@ struct SingleConv {
     mask = hm;
     CK(cudaMemcpyAsync(h.dMask, hm.data(), M * sizeof(float), cudaMemcpyHostToDevice, h.stream));
   }
+  // Plan mode: the real launchPlanRows and launchPackInput for boards board_xy moved by `symmetry`.  The input is given before
+  // the symmetry and must be zero off the board, as fillRowV7 leaves it.  Rows of the operand at or past the plan's end hold
+  // finite garbage (fp16 1024), as an earlier, larger forward can leave them: a board row whose tap reached them would be wrong.
+  HostPlan setInputPlanned(const float* input /* NHWC */, const int32_t* boardXY, const int32_t* symmetry) {
+    float* dIn = h.dalloc<float>((size_t)n * X * Y * cin);
+    CK(cudaMemcpyAsync(dIn, input, (size_t)n * X * Y * cin * sizeof(float), cudaMemcpyHostToDevice, h.stream));
+    const float* dMaskIn = planBoards(h, n, boardXY, symmetry);
+    CK(launchPackInput(dIn, n, cin, true, h.dSymmetry, h.L, h.plan, M, As[0], cw.cin_p, h.split, h.dMask, h.dMaskSum, h.stream));
+    HostPlan hp = finishPlan(h, n, dMaskIn);
+    const size_t ld = (size_t)cw.cin_p * (h.split ? 2 : 1);
+    const std::vector<__half> tail((M - hp.stats[0]) * ld, __float2half(1024.0f));
+    if(!tail.empty()) CK(cudaMemcpyAsync(As[0] + hp.stats[0] * ld, tail.data(), tail.size() * sizeof(__half), cudaMemcpyHostToDevice, h.stream));
+    mask = hp.mask;
+    return hp;
+  }
   void run() { h.ops[next](n, h.stream); next = (next + 1) % rotate; }
 };
 
@@ -1048,7 +1171,10 @@ struct BoundaryConv {
   };
   std::vector<Set> sets;
   std::vector<float> mask;
-  BoundaryConv(int inner_c, int trunk_c, int n_, int X, int Y, const int32_t* boardXY, bool trunkFp32, bool innerFp32, uint32_t seed, int rotate_)
+  HostPlan hp;   // plan mode: the plan; every buffer's rows from hp.stats[0] on hold all-ones bytes before the launches
+  // ragged < 0: the fixed frame layout; else plan mode, boards moved by `symmetry` (planBoards)
+  BoundaryConv(int inner_c, int trunk_c, int n_, int X, int Y, const int32_t* boardXY, bool trunkFp32, bool innerFp32, uint32_t seed, int rotate_,
+               const int32_t* symmetry = nullptr, int ragged = -1)
       : n(n_), rotate(rotate_ < 1 ? 1 : rotate_), trunkF32(trunkFp32), innerF32(innerFp32) {
     h.device = selectDevice(-1);
     h.model = &dummy;
@@ -1056,7 +1182,12 @@ struct BoundaryConv {
     h.L = boardLayout(X, Y, 1);
     CK(cudaStreamCreateWithFlags(&h.stream, cudaStreamNonBlocking));
     CK(convWGInit());
-    uploadFramePlan(h);
+    if(ragged < 0) uploadFramePlan(h);
+    else {
+      h.plan.ragged = ragged;
+      allocPlan(h);
+      hp = finishPlan(h, n, planBoards(h, n, boardXY, symmetry));
+    }
     uint32_t st = seed * 2654435761u + 12345u;
     auto uni = [&]() { st = st * 1664525u + 1013904223u; return (st >> 8) * (1.0f / 16777216.0f); };
     ConvDesc post, pre;
@@ -1082,15 +1213,18 @@ struct BoundaryConv {
       bn2 = b.uploadBN(bnInner, ACT_MISH, wpre.cout_p);
     });
     innerCp = wpost.cin_p; trunkCp = wpost.cout_p;
-    M = (size_t)n * h.L.P;
-    h.dMask = h.dalloc<float>(M + 128);
-    mask.assign(M, 0.0f);
-    for(int i = 0; i < n; i++) {
-      const int bx = boardXY ? boardXY[2 * i] : X, by = boardXY ? boardXY[2 * i + 1] : Y;
-      for(int y = 0; y < by; y++)
-        for(int x = 0; x < bx; x++) mask[(size_t)i * h.L.P + (size_t)(y + h.L.pad) * h.L.Wp + x] = 1.0f;
+    M = h.planRows(n);
+    if(ragged < 0) {
+      h.dMask = h.dalloc<float>(M + 128);
+      mask.assign(M, 0.0f);
+      for(int i = 0; i < n; i++) {
+        const int bx = boardXY ? boardXY[2 * i] : X, by = boardXY ? boardXY[2 * i + 1] : Y;
+        for(int y = 0; y < by; y++)
+          for(int x = 0; x < bx; x++) mask[(size_t)i * h.L.P + (size_t)(y + h.L.pad) * h.L.Wp + x] = 1.0f;
+      }
+      CK(cudaMemcpyAsync(h.dMask, mask.data(), M * sizeof(float), cudaMemcpyHostToDevice, h.stream));
     }
-    CK(cudaMemcpyAsync(h.dMask, mask.data(), M * sizeof(float), cudaMemcpyHostToDevice, h.stream));
+    else mask = hp.mask;
     // inputs as the previous layers leave them: zero in masked rows and padded channels
     std::vector<__half> hA(M * innerCp, __float2half(0.0f));
     std::vector<float> hS(M * trunkCp, 0.0f);
@@ -1111,6 +1245,12 @@ struct BoundaryConv {
       CK(cudaMemcpyAsync(s.innerA, hA.data(), hA.size() * sizeof(__half), cudaMemcpyHostToDevice, h.stream));
       if(trunkF32) CK(cudaMemcpyAsync(s.trunkS, hS.data(), hS.size() * sizeof(float), cudaMemcpyHostToDevice, h.stream));
       else CK(cudaMemcpyAsync(s.trunkS, hS16.data(), hS16.size() * sizeof(__half), cudaMemcpyHostToDevice, h.stream));
+      if(ragged >= 0) {   // 1x1 convolutions: no tap reaches past a tile's own rows, so every buffer can hold NaN there
+        poisonTail(h, s.innerA, (size_t)innerCp * 2, hp.stats[0], M);
+        poisonTail(h, s.trunkA, (size_t)trunkCp * 2, hp.stats[0], M);
+        poisonTail(h, s.trunkS, (size_t)trunkCp * (trunkF32 ? 4 : 2), hp.stats[0], M);
+        poisonTail(h, s.innerS, (size_t)innerCp * (innerF32 ? 4 : 2), hp.stats[0], M);
+      }
       sets.push_back(s);
       if(k % 2 == 0) {
         if(!b.emitConvPair(wpost, s.innerA, s.trunkS, trunkF32, bn1, wpre, s.innerS, innerF32, s.innerA, bn2))
@@ -1140,27 +1280,39 @@ struct BoundaryConv {
 
 // kgb_test_conv_ex and its two narrower forms kgb_test_conv (kind 0) and kgb_test_conv_epilogue (kinds 1-4): one launch, NHWC in
 // and out.  act_lo_out is written in split mode only.
+//
+// ragged >= 0 is plan mode (kgb_test_conv_plan): the plan is made on the device for boards board_xy moved by `symmetry`, every input
+// but `input` and every output is in the coordinates after the symmetry, and rows at or past the plan's end must come back as the
+// all-ones bytes they were filled with.  stats_out [3] and plan_out [n][5] (x0, y0, w, h, first row) report the plan.
 void testConv(const char* fn, int ky, int kx, int in_c, int out_c, const float* weights, int n, int nn_x_len, int nn_y_len, int use_fp16, int kind,
               const float* input, const int32_t* board_xy, const float* ncbias, const float* residual_in, const float* bn_scale,
-              const float* bn_bias, int activation, float* raw_out, float* act_hi_out, float* act_lo_out) {
+              const float* bn_bias, int activation, float* raw_out, float* act_hi_out, float* act_lo_out, const int32_t* symmetry = nullptr,
+              int ragged = -1, int64_t* stats_out = nullptr, int32_t* plan_out = nullptr) {
   const bool hasResidual = kind == 2 || kind == 4;
+  const bool planned = ragged >= 0;
   if(!weights || !input || n < 1 || kind < 0 || kind > 4 || activation < ACT_IDENTITY || activation > ACT_SILU ||
      (kind == 0 ? !raw_out : !act_hi_out))
     throw std::invalid_argument(std::string(fn) + ": bad argument");
   if(hasResidual && !residual_in) throw std::invalid_argument(std::string(fn) + ": kinds 2 and 4 need residual_in");
   if(kind >= 2 && !raw_out) throw std::invalid_argument(std::string(fn) + ": kinds 2 to 4 need raw_out");
-  if(board_xy)
-    for(int i = 0; i < n; i++)
-      if(board_xy[2 * i] < 1 || board_xy[2 * i] > nn_x_len || board_xy[2 * i + 1] < 1 || board_xy[2 * i + 1] > nn_y_len)
-        throw std::invalid_argument(std::string(fn) + ": board size of image " + std::to_string(i) + " not in the frame");
-  SingleConv sc(ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16, kind, 1, bn_scale, bn_bias, activation, ncbias != nullptr);
-  sc.setInput(input, board_xy);
+  checkBoards(fn, n, nn_x_len, nn_y_len, board_xy, symmetry, planned);
+  SingleConv sc(ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16, kind, 1, bn_scale, bn_bias, activation, ncbias != nullptr,
+                planned ? (ragged != 0) : -1);
+  HostPlan hp;
+  if(planned) {
+    hp = sc.setInputPlanned(input, board_xy, symmetry);
+    hp.copyOut(n, stats_out, plan_out);
+  }
+  else sc.setInput(input, board_xy);
+  const size_t used = planned ? (size_t)hp.stats[0] : sc.M;   // rows the launch may write
   const int cp = sc.cw.cout_p;
   const bool f32 = sc.rawF32;
   const bool split = sc.h.split != 0;
   const cudaStream_t s = sc.h.stream;
   if(split && kind != 0 && !act_lo_out) throw std::invalid_argument(std::string(fn) + ": split mode needs act_lo_out");
-  auto rowOf = [&](int i, int y, int x) { return (size_t)i * sc.h.L.P + (size_t)(y + sc.h.L.pad) * sc.h.L.Wp + x; };
+  auto rowOf = [&](int i, int y, int x) -> long {
+    return planned ? hp.row(sc.h.L, i, y, x) : (long)((size_t)i * sc.h.L.P + (size_t)(y + sc.h.L.pad) * sc.h.L.Wp + x);
+  };
   if(ncbias) {
     std::vector<float> hb((size_t)n * cp, 0.0f);
     for(int i = 0; i < n; i++) for(int c = 0; c < out_c; c++) hb[(size_t)i * cp + c] = ncbias[(size_t)i * out_c + c];
@@ -1169,8 +1321,11 @@ void testConv(const char* fn, int ky, int kx, int in_c, int out_c, const float* 
   if(hasResidual) {
     // given as fp32; an fp16 stream holds it rounded to nearest
     std::vector<float> hf(sc.M * cp, 0.0f);
-    for(int i = 0; i < n; i++) for(int y = 0; y < nn_y_len; y++) for(int x = 0; x < nn_x_len; x++) for(int c = 0; c < out_c; c++)
-      hf[rowOf(i, y, x) * cp + c] = residual_in[(((size_t)i * nn_y_len + y) * nn_x_len + x) * out_c + c];
+    for(int i = 0; i < n; i++) for(int y = 0; y < nn_y_len; y++) for(int x = 0; x < nn_x_len; x++) {
+      const long row = rowOf(i, y, x);
+      if(row < 0) continue;
+      for(int c = 0; c < out_c; c++) hf[row * cp + c] = residual_in[(((size_t)i * nn_y_len + y) * nn_x_len + x) * out_c + c];
+    }
     if(f32) CK(cudaMemcpyAsync(sc.raws[0], hf.data(), hf.size() * sizeof(float), cudaMemcpyHostToDevice, s));
     else {
       std::vector<__half> hh(hf.size());
@@ -1178,12 +1333,17 @@ void testConv(const char* fn, int ky, int kx, int in_c, int out_c, const float* 
       CK(cudaMemcpyAsync(sc.raws[0], hh.data(), hh.size() * sizeof(__half), cudaMemcpyHostToDevice, s));
     }
   }
+  const int am = split ? 2 : 1;
+  const size_t rawRowBytes = (size_t)cp * (f32 ? 4 : 2), actRowBytes = (size_t)cp * am * 2;
+  if(planned) {
+    if(!sc.raws.empty()) poisonTail(sc.h, sc.raws[0], rawRowBytes, used, sc.M);
+    if(!sc.acts.empty()) poisonTail(sc.h, sc.acts[0], actRowBytes, used, sc.M);
+  }
   sc.run();
   auto download = [&](void* dst, const void* src, size_t bytes) {
     CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
   };
-  const int am = split ? 2 : 1;
   std::vector<__half> ha;
   if(!sc.acts.empty()) {
     ha.resize(sc.M * cp * am);
@@ -1199,11 +1359,29 @@ void testConv(const char* fn, int ky, int kx, int in_c, int out_c, const float* 
       for(size_t k = 0; k < hr.size(); k++) hr[k] = __half2float(hh[k]);
     }
   }
+  if(planned) {
+    // the rows past the plan: the bytes they were filled with (no tile writes there)
+    auto tail = [&](const char* what, const void* p, size_t rowBytes) {
+      std::vector<uint8_t> v(sc.M * rowBytes);
+      memcpy(v.data(), p, v.size());
+      if(const size_t k = countTouchedTail(v, rowBytes, used))
+        throw std::runtime_error(std::string(fn) + ": " + what + " was written past the plan's " + std::to_string(used) + " rows (" +
+                                 std::to_string(k) + " bytes)");
+    };
+    if(!sc.raws.empty() && f32) tail("the raw output", hr.data(), rawRowBytes);
+    if(!sc.raws.empty() && !f32) {
+      std::vector<__half> hh(sc.M * cp);
+      download(hh.data(), sc.raws[0], hh.size() * sizeof(__half));
+      tail("the raw output", hh.data(), rawRowBytes);
+    }
+    if(!ha.empty()) tail("the activated operand", ha.data(), actRowBytes);
+  }
   // Exact zeros where the next layer relies on them: every column of a row the mask zeroes (pad rows and columns, and points off
-  // a smaller board), which the next conv's halo reads as its zero padding; and the padded channels cout..cout_p of every row, which
-  // the next conv reads as part of K (0 x NaN is not 0).  The raw output is checked too, and in split mode the lo half.
+  // a smaller board; in plan mode also the gap rows that end a segment and the rows up to the next 128), which the next conv's halo
+  // reads as its zero padding; and the padded channels cout..cout_p of every row, which the next conv reads as part of K (0 x NaN is
+  // not 0).  The raw output is checked too, and in split mode the lo half.
   auto check = [&](const char* what, int ld, int col0, auto value) {
-    for(size_t r = 0; r < sc.M; r++) {
+    for(size_t r = 0; r < used; r++) {
       const bool off = sc.mask[r] == 0.0f;
       for(int c = off ? 0 : out_c; c < cp; c++)
         if(value(r * ld + col0 + c) != 0.0f)
@@ -1217,12 +1395,249 @@ void testConv(const char* fn, int ky, int kx, int in_c, int out_c, const float* 
     if(split) check("the activated operand's lo half", cp * am, cp, [&](size_t k) { return __half2float(ha[k]); });
   }
   for(int i = 0; i < n; i++) for(int y = 0; y < nn_y_len; y++) for(int x = 0; x < nn_x_len; x++) for(int c = 0; c < out_c; c++) {
-    const size_t row = rowOf(i, y, x), o = (((size_t)i * nn_y_len + y) * nn_x_len + x) * out_c + c;
+    const long prow = rowOf(i, y, x);
+    const size_t row = (size_t)prow, o = (((size_t)i * nn_y_len + y) * nn_x_len + x) * out_c + c;
+    if(prow < 0) {   // outside the image's box: a mask-0 position, whose outputs are zero
+      if(!ha.empty()) { act_hi_out[o] = 0.0f; if(split) act_lo_out[o] = 0.0f; }
+      if(!hr.empty()) raw_out[o] = 0.0f;
+      continue;
+    }
     if(!ha.empty()) {
       act_hi_out[o] = __half2float(ha[row * cp * am + c]);
       if(split) act_lo_out[o] = __half2float(ha[row * cp * am + cp + c]);
     }
     if(!hr.empty()) raw_out[o] = hr[row * cp + c];
+  }
+}
+
+// kgb_test_conv_boundary (ragged < 0, the frame layout) and kgb_test_conv_boundary_plan.  out[0..2]: elements of trunk.S, inner.S,
+// inner.A whose bits differ between the fused launch and the two launches; out[3..5]: nonzero elements of the fused outputs in masked
+// rows or padded channels.  Plan mode, over the rows below the plan's end, and out[6..8]: NaN elements of the fused outputs there;
+// out[9..11]: bytes at or past the plan's end that either path changed.
+void testBoundary(const char* fn, int inner_c, int trunk_c, int n, int nn_x_len, int nn_y_len, const int32_t* board_xy, const int32_t* symmetry,
+                  int ragged, int trunk_fp32, int inner_fp32, uint32_t seed, int64_t* out, int64_t* stats_out) {
+  const bool planned = ragged >= 0;
+  if(!out || n < 1 || inner_c < 1 || trunk_c < 1 || nn_x_len < 2 || nn_y_len < 2 || (inner_fp32 && !trunk_fp32))
+    throw std::invalid_argument(std::string(fn) + ": bad argument");
+  checkBoards(fn, n, nn_x_len, nn_y_len, board_xy, symmetry, planned);
+  BoundaryConv bc(inner_c, trunk_c, n, nn_x_len, nn_y_len, board_xy, trunk_fp32 != 0, inner_fp32 != 0, seed, 1, symmetry, planned ? (ragged != 0) : -1);
+  if(planned) bc.hp.copyOut(n, stats_out, nullptr);
+  const size_t used = planned ? (size_t)bc.hp.stats[0] : bc.M;
+  bc.run(true);
+  bc.run(false);
+  const cudaStream_t s = bc.h.stream;
+  auto download = [&](const void* src, size_t bytes) {
+    std::vector<uint8_t> v(bytes);
+    CK(cudaMemcpyAsync(v.data(), src, bytes, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    return v;
+  };
+  struct Out { size_t off; int cp, c, esize; };
+  const Out outs[3] = {{offsetof(BoundaryConv::Set, trunkS), bc.trunkCp, trunk_c, trunk_fp32 ? 4 : 2},
+                       {offsetof(BoundaryConv::Set, innerS), bc.innerCp, inner_c, inner_fp32 ? 4 : 2},
+                       {offsetof(BoundaryConv::Set, innerA), bc.innerCp, inner_c, 2}};
+  for(int k = 0; k < 3; k++) {
+    const Out& o = outs[k];
+    auto ptr = [&](const BoundaryConv::Set& st) { return *reinterpret_cast<void* const*>(reinterpret_cast<const uint8_t*>(&st) + o.off); };
+    const size_t bytes = bc.M * o.cp * o.esize;
+    const std::vector<uint8_t> f = download(ptr(bc.sets[0]), bytes), u = download(ptr(bc.sets[1]), bytes);
+    int64_t diff = 0, nonzero = 0, nan = 0;
+    for(size_t r = 0; r < used; r++)
+      for(int c = 0; c < o.cp; c++) {
+        const size_t e = (r * o.cp + c) * o.esize;
+        if(memcmp(&f[e], &u[e], o.esize) != 0) diff++;
+        float v;
+        if(o.esize == 4) memcpy(&v, &f[e], 4);
+        else { __half hv; memcpy(&hv, &f[e], 2); v = __half2float(hv); }
+        if(std::isnan(v)) nan++;
+        if((bc.mask[r] == 0.0f || c >= o.c) && v != 0.0f) nonzero++;
+      }
+    out[k] = diff;
+    out[3 + k] = nonzero;
+    if(planned) {
+      out[6 + k] = nan;
+      out[9 + k] = (int64_t)(countTouchedTail(f, (size_t)o.cp * o.esize, used) + countTouchedTail(u, (size_t)o.cp * o.esize, used));
+    }
+  }
+}
+
+// kgb_test_head_kernel (include/kgb200.h): one launch of one of the evaluator's fp32 kernels on the caller's tensors.
+enum { HK_PACK = 0, HK_GPOOL = 1, HK_BIASACT = 2, HK_MATMUL = 3, HK_POLICY = 4, HK_OWNERSHIP = 5, HK_FINALIZE = 6 };
+
+void testHead(int which, int n, int X, int Y, int pad, const int32_t* board_xy, const int32_t* symmetry, int ragged, const int32_t* ip, int nip,
+              const float* const* in, int nin, float* const* out, int nout, int64_t* stats_out, int32_t* plan_out) {
+  static const int needIp[7] = {3, 6, 4, 5, 5, 4, 4}, needIn[7] = {1, 3, 4, 3, 6, 4, 4}, needOut[7] = {4, 1, 2, 1, 1, 1, 3};
+  const char* fn = "kgb_test_head_kernel";
+  if(which < 0 || which > 6 || n < 1 || X < 2 || Y < 2 || X > 37 || Y > 37 || pad < 1 || pad > 2 || (ragged != 0 && ragged != 1) || !ip ||
+     nip != needIp[which] || !in || nin != needIn[which] || !out || nout != needOut[which])
+    throw std::invalid_argument(std::string(fn) + ": bad argument");
+  checkBoards(fn, n, X, Y, board_xy, symmetry, true);
+  kgb_handle h;
+  struct Release {
+    kgb_handle& h;
+    ~Release() { for(void* p : h.allocs) cudaFree(p); if(h.stream) cudaStreamDestroy(h.stream); }
+  } release{h};
+  ModelDesc dummy;
+  h.device = selectDevice(-1);
+  h.model = &dummy;
+  h.maxBatch = n;
+  h.L = boardLayout(X, Y, pad);
+  h.plan.ragged = ragged;
+  CK(cudaStreamCreateWithFlags(&h.stream, cudaStreamNonBlocking));
+  const cudaStream_t s = h.stream;
+  const Layout L = h.L;
+  const int XY = X * Y;
+  auto up = [&](const float* p, size_t count) -> float* {
+    if(!p) return nullptr;
+    float* d = h.dalloc<float>(count);
+    CK(cudaMemcpyAsync(d, p, count * sizeof(float), cudaMemcpyHostToDevice, s));
+    return d;
+  };
+  auto down = [&](void* dst, const void* src, size_t bytes) {
+    CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+  };
+  auto poisoned = [&](size_t count) {   // an fp32 output, all-ones bytes (NaN) where the kernel does not write
+    float* d = h.dalloc<float>(count);
+    CK(cudaMemsetAsync(d, 0xFF, count * sizeof(float), s));
+    return d;
+  };
+  auto need = [&](bool ok) { if(!ok) throw std::invalid_argument(std::string(fn) + ": bad argument for kernel " + std::to_string(which)); };
+  auto isOnes = [](const void* p, size_t bytes) {
+    for(size_t b = 0; b < bytes; b++) if(((const uint8_t*)p)[b] != 0xFF) return false;
+    return true;
+  };
+
+  if(which == HK_MATMUL) {
+    const int cin = ip[0], cout = ip[1], act = ip[2], ldi = ip[3], ldo = ip[4];
+    need(cin >= 1 && cin <= ldi && cin <= 8192 && cout >= 1 && cout <= ldo && act >= ACT_IDENTITY && act <= ACT_SILU && in[0] && in[1]);
+    float* o = poisoned((size_t)n * ldo);
+    CK(launchMatMulNC(up(in[0], (size_t)n * ldi), ldi, up(in[1], (size_t)cin * cout), up(in[2], cout), n, cin, cout, act, o, ldo, s));
+    down(out[0], o, (size_t)n * ldo * sizeof(float));
+    return;
+  }
+  if(which == HK_FINALIZE) {
+    const int cp2 = ip[0], numSV = ip[1], version = ip[2], ldp = ip[3];
+    need(cp2 >= 1 && cp2 <= ldp && numSV >= (version >= 9 ? 6 : version >= 8 ? 4 : version >= 4 ? 2 : 1) && in[0] && in[2] && in[3] &&
+         out[0] && out[1] && out[2]);
+    float *pol = poisoned((size_t)n * (XY + 1)), *val = poisoned((size_t)n * 3), *score = poisoned((size_t)n * 6);
+    CK(launchFinalize(up(in[0], (size_t)n * ldp), ldp, cp2, up(in[1], n), up(in[2], (size_t)n * 3), up(in[3], (size_t)n * numSV), numSV, version,
+                      n, XY + 1, pol, val, score, s));
+    down(out[0], pol, (size_t)n * (XY + 1) * sizeof(float));
+    down(out[1], val, (size_t)n * 3 * sizeof(float));
+    down(out[2], score, (size_t)n * 6 * sizeof(float));
+    return;
+  }
+
+  allocPlan(h);
+  const size_t M = h.planRows(n);
+  HostPlan hp;
+  if(which == HK_PACK) {
+    // the plan from the input itself (its channel 0 is the mask), as a forward plans it
+    const int C = ip[0], split = ip[1], nhwc = ip[2];
+    need(C >= 1 && C <= 64 && (split == 0 || split == 1) && in[0] && out[0] && out[2] && out[3] && (!split || out[1]));
+    const float* sp = up(in[0], (size_t)n * C * XY);
+    std::vector<int> sym(n, 0);
+    for(int i = 0; symmetry && i < n; i++) sym[i] = symmetry[i];
+    CK(cudaMemcpyAsync(h.dSymmetry, sym.data(), n * sizeof(int), cudaMemcpyHostToDevice, s));
+    const int cinP = cpad(C), ld = cinP * (split ? 2 : 1);
+    __half* act = h.dalloc<__half>(M * ld);
+    CK(launchPlanRows(sp, n, C, nhwc != 0, h.dSymmetry, L, h.plan, s));
+    CK(launchPackInput(sp, n, C, nhwc != 0, h.dSymmetry, L, h.plan, M, act, cinP, split, h.dMask, h.dMaskSum, s));
+    hp = readPlan(h, n);
+    std::vector<__half> ha(M * ld);
+    down(ha.data(), act, ha.size() * sizeof(__half));
+    down(out[2], h.dMaskSum, n * sizeof(float));
+    // a row that is not a board position is zero in every channel, and so is every padded channel
+    for(size_t r = 0; r < (size_t)hp.stats[0]; r++)
+      for(int c = 0; c < ld; c++)
+        if((hp.mask[r] == 0.0f || c % cinP >= C) && __half2float(ha[r * ld + c]) != 0.0f)
+          throw std::runtime_error(std::string(fn) + ": the packed input is not zero at row " + std::to_string(r) + ", column " + std::to_string(c));
+    for(int i = 0; i < n; i++)
+      for(int y = 0; y < Y; y++)
+        for(int x = 0; x < X; x++) {
+          const long row = hp.row(L, i, y, x);
+          const size_t o = ((size_t)i * Y + y) * X + x;
+          out[3][o] = row < 0 ? 0.0f : hp.mask[row];
+          for(int c = 0; c < C; c++) {
+            out[0][o * C + c] = row < 0 ? 0.0f : __half2float(ha[row * ld + c]);
+            if(split) out[1][o * C + c] = row < 0 ? 0.0f : __half2float(ha[row * ld + cinP + c]);
+          }
+        }
+    hp.copyOut(n, stats_out, plan_out);
+    return;
+  }
+  hp = finishPlan(h, n, planBoards(h, n, board_xy, symmetry));
+  hp.copyOut(n, stats_out, plan_out);
+  // t [n][Y][X][C] (the coordinates after the symmetry) into rows of ld columns from column c0: every other element, and every row
+  // that is not a board position, NaN; the kernels must read neither
+  auto placeRows = [&](const float* t, int C, int ld, int c0, bool fp16) -> void* {
+    std::vector<float> v(M * ld, NAN);
+    for(int i = 0; i < n; i++)
+      for(int y = 0; y < Y; y++)
+        for(int x = 0; x < X; x++) {
+          const long row = hp.row(L, i, y, x);
+          if(row < 0 || hp.mask[row] != 1.0f) continue;
+          for(int c = 0; c < C; c++) v[row * ld + c0 + c] = t[(((size_t)i * Y + y) * X + x) * C + c];
+        }
+    if(!fp16) return up(v.data(), v.size());
+    std::vector<__half> hv(v.size());
+    for(size_t k = 0; k < v.size(); k++) hv[k] = __float2half_rn(v[k]);
+    __half* d = h.dalloc<__half>(hv.size());
+    CK(cudaMemcpyAsync(d, hv.data(), hv.size() * sizeof(__half), cudaMemcpyHostToDevice, s));
+    return d;
+  };
+  if(which == HK_GPOOL) {
+    const int C = ip[0], act = ip[1], valueHead = ip[2], rawFp32 = ip[3], c0 = ip[4], ldr = ip[5];
+    need(C >= 1 && c0 >= 0 && c0 + C <= ldr && act >= ACT_IDENTITY && act <= ACT_SILU && in[0] && in[1] && in[2]);
+    float* pooled = poisoned((size_t)n * 3 * C);
+    CK(launchGPool(placeRows(in[0], C, ldr, c0, !rawFp32), rawFp32 ? 1 : 0, ldr, c0, C, up(in[1], C), up(in[2], C), act, h.dMask, h.dMaskSum, n, L,
+                   h.plan, valueHead ? 1 : 0, pooled, s));
+    down(out[0], pooled, (size_t)n * 3 * C * sizeof(float));
+  }
+  else if(which == HK_BIASACT) {
+    const int C = ip[0], act = ip[1], split = ip[2], rawFp32 = ip[3];
+    need(C >= 1 && (split == 0 || split == 1) && act >= ACT_IDENTITY && act <= ACT_SILU && in[0] && in[2] && in[3] && out[0] && (!split || out[1]));
+    const int cp = cpad(C), ld = cp * (split ? 2 : 1);
+    __half* actOut = h.dalloc<__half>(M * ld);
+    CK(cudaMemsetAsync(actOut, 0xFF, M * ld * sizeof(__half), s));
+    CK(launchBiasAct(placeRows(in[0], C, cp, 0, !rawFp32), rawFp32 ? 1 : 0, cp, C, up(in[1], (size_t)n * C), C, up(in[2], C), up(in[3], C), act,
+                     h.dMask, (int)M, h.plan, actOut, cp, split, s));
+    std::vector<__half> ha(M * ld);
+    down(ha.data(), actOut, ha.size() * sizeof(__half));
+    const size_t used = hp.stats[0];
+    if(!isOnes(ha.data() + used * ld, (M - used) * ld * sizeof(__half)))
+      throw std::runtime_error(std::string(fn) + ": biasAct wrote past the plan's " + std::to_string(used) + " rows");
+    for(size_t r = 0; r < used; r++)
+      for(int c = 0; c < ld; c++)
+        if((hp.mask[r] == 0.0f || c % cp >= C) && __half2float(ha[r * ld + c]) != 0.0f)
+          throw std::runtime_error(std::string(fn) + ": biasAct's output is not zero at row " + std::to_string(r) + ", column " + std::to_string(c));
+    for(int i = 0; i < n; i++)
+      for(int y = 0; y < Y; y++)
+        for(int x = 0; x < X; x++) {
+          const long row = hp.row(L, i, y, x);
+          const size_t o = (((size_t)i * Y + y) * X + x) * C;
+          for(int c = 0; c < C; c++) {
+            out[0][o + c] = row < 0 ? 0.0f : __half2float(ha[row * ld + c]);
+            if(split) out[1][o + c] = row < 0 ? 0.0f : __half2float(ha[row * ld + cp + c]);
+          }
+        }
+  }
+  else if(which == HK_POLICY) {
+    const int C = ip[0], act = ip[1], cp2 = ip[2], c0 = ip[3], ldr = ip[4];
+    need(C >= 1 && cp2 >= 1 && cp2 <= 4 && c0 >= 0 && c0 + C <= ldr && act >= ACT_IDENTITY && act <= ACT_SILU && in[0] && in[1] && in[2] && in[3] && in[4]);
+    float* pol = poisoned((size_t)n * (XY + 1));
+    CK(launchPolicyOut((const float*)placeRows(in[0], C, ldr, c0, false), ldr, c0, C, up(in[1], (size_t)n * C), C, up(in[2], C), up(in[3], C), act,
+                       up(in[4], (size_t)C * cp2), cp2, h.dMask, h.dSymmetry, up(in[5], n), n, L, h.plan, pol, s));
+    down(out[0], pol, (size_t)n * (XY + 1) * sizeof(float));
+  }
+  else {   // HK_OWNERSHIP
+    const int C = ip[0], act = ip[1], c0 = ip[2], ldr = ip[3];
+    need(C >= 1 && c0 >= 0 && c0 + C <= ldr && act >= ACT_IDENTITY && act <= ACT_SILU && in[0] && in[1] && in[2] && in[3]);
+    float* own = poisoned((size_t)n * XY);
+    CK(launchOwnershipOut((const float*)placeRows(in[0], C, ldr, c0, false), ldr, c0, C, up(in[1], C), up(in[2], C), act, up(in[3], C), h.dMask,
+                          h.dSymmetry, n, L, h.plan, own, s));
+    down(out[0], own, (size_t)n * XY * sizeof(float));
   }
 }
 }  // namespace
@@ -1260,6 +1675,17 @@ KGB_API int kgb_test_conv_ex(int ky, int kx, int in_c, int out_c, const float* w
   });
 }
 
+KGB_API int kgb_test_conv_plan(int ky, int kx, int in_c, int out_c, const float* weights, int n, int nn_x_len, int nn_y_len, int use_fp16,
+                               int epilogue_kind, const float* input, const int32_t* board_xy, const int32_t* symmetry, int ragged,
+                               const float* ncbias, const float* residual_in, const float* bn_scale, const float* bn_bias, int activation,
+                               float* raw_out, float* act_hi_out, float* act_lo_out, int64_t* layout_stats, int32_t* plan_out) {
+  return guarded([&] {
+    if(ragged < 0) throw std::invalid_argument("kgb_test_conv_plan: ragged must be 0 or 1");
+    testConv("kgb_test_conv_plan", ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16, epilogue_kind, input, board_xy, ncbias,
+             residual_in, bn_scale, bn_bias, activation, raw_out, act_hi_out, act_lo_out, symmetry, ragged, layout_stats, plan_out);
+  });
+}
+
 KGB_API int kgb_bench_conv_ex(int ky, int kx, int in_c, int out_c, int n, int nn_x_len, int nn_y_len, int use_fp16, int epilogue_kind, int rotate,
                       int warmup, int iters, float* ms_per_launch) {
   return guarded([&] {
@@ -1288,49 +1714,26 @@ KGB_API int kgb_bench_conv_ex(int ky, int kx, int in_c, int out_c, int n, int nn
 
 KGB_API int kgb_test_conv_boundary(int inner_c, int trunk_c, int n, int nn_x_len, int nn_y_len, const int32_t* board_xy, int trunk_fp32,
                                    int inner_fp32, uint32_t seed, int64_t* out) {
+  return guarded([&] { testBoundary("kgb_test_conv_boundary", inner_c, trunk_c, n, nn_x_len, nn_y_len, board_xy, nullptr, -1, trunk_fp32,
+                                    inner_fp32, seed, out, nullptr); });
+}
+
+KGB_API int kgb_test_conv_boundary_plan(int inner_c, int trunk_c, int n, int nn_x_len, int nn_y_len, const int32_t* board_xy,
+                                        const int32_t* symmetry, int ragged, int trunk_fp32, int inner_fp32, uint32_t seed, int64_t* out,
+                                        int64_t* layout_stats) {
   return guarded([&] {
-    if(!out || n < 1 || inner_c < 1 || trunk_c < 1 || nn_x_len < 2 || nn_y_len < 2 || (inner_fp32 && !trunk_fp32))
-      throw std::invalid_argument("kgb_test_conv_boundary: bad argument");
-    if(board_xy)
-      for(int i = 0; i < n; i++)
-        if(board_xy[2 * i] < 1 || board_xy[2 * i] > nn_x_len || board_xy[2 * i + 1] < 1 || board_xy[2 * i + 1] > nn_y_len)
-          throw std::invalid_argument("kgb_test_conv_boundary: board size of image " + std::to_string(i) + " not in the frame");
-    BoundaryConv bc(inner_c, trunk_c, n, nn_x_len, nn_y_len, board_xy, trunk_fp32 != 0, inner_fp32 != 0, seed, 1);
-    bc.run(true);
-    bc.run(false);
-    const cudaStream_t s = bc.h.stream;
-    auto download = [&](const void* src, size_t bytes) {
-      std::vector<uint8_t> v(bytes);
-      CK(cudaMemcpyAsync(v.data(), src, bytes, cudaMemcpyDeviceToHost, s));
-      CK(cudaStreamSynchronize(s));
-      return v;
-    };
-    // out[0..2]: elements of trunk.S, inner.S, inner.A whose bits differ between the fused launch and the two launches;
-    // out[3..5]: nonzero elements of the fused outputs in masked rows or padded channels
-    struct Out { size_t off; int cp, c, esize; };
-    const Out outs[3] = {{offsetof(BoundaryConv::Set, trunkS), bc.trunkCp, trunk_c, trunk_fp32 ? 4 : 2},
-                         {offsetof(BoundaryConv::Set, innerS), bc.innerCp, inner_c, inner_fp32 ? 4 : 2},
-                         {offsetof(BoundaryConv::Set, innerA), bc.innerCp, inner_c, 2}};
-    for(int k = 0; k < 3; k++) {
-      const Out& o = outs[k];
-      auto ptr = [&](const BoundaryConv::Set& st) { return *reinterpret_cast<void* const*>(reinterpret_cast<const uint8_t*>(&st) + o.off); };
-      const size_t bytes = bc.M * o.cp * o.esize;
-      const std::vector<uint8_t> f = download(ptr(bc.sets[0]), bytes), u = download(ptr(bc.sets[1]), bytes);
-      int64_t diff = 0, nonzero = 0;
-      for(size_t r = 0; r < bc.M; r++)
-        for(int c = 0; c < o.cp; c++) {
-          const size_t e = (r * o.cp + c) * o.esize;
-          if(memcmp(&f[e], &u[e], o.esize) != 0) diff++;
-          if(bc.mask[r] == 0.0f || c >= o.c) {
-            float v;
-            if(o.esize == 4) memcpy(&v, &f[e], 4);
-            else { __half hv; memcpy(&hv, &f[e], 2); v = __half2float(hv); }
-            if(v != 0.0f) nonzero++;
-          }
-        }
-      out[k] = diff;
-      out[3 + k] = nonzero;
-    }
+    if(ragged < 0) throw std::invalid_argument("kgb_test_conv_boundary_plan: ragged must be 0 or 1");
+    testBoundary("kgb_test_conv_boundary_plan", inner_c, trunk_c, n, nn_x_len, nn_y_len, board_xy, symmetry, ragged, trunk_fp32, inner_fp32,
+                 seed, out, layout_stats);
+  });
+}
+
+KGB_API int kgb_test_head_kernel(int which, int n, int nn_x_len, int nn_y_len, int pad, const int32_t* board_xy, const int32_t* symmetry,
+                                 int ragged, const int32_t* iparams, int num_iparams, const float* const* inputs, int num_inputs,
+                                 float* const* outputs, int num_outputs, int64_t* layout_stats, int32_t* plan_out) {
+  return guarded([&] {
+    testHead(which, n, nn_x_len, nn_y_len, pad, board_xy, symmetry, ragged, iparams, num_iparams, inputs, num_inputs, outputs, num_outputs,
+             layout_stats, plan_out);
   });
 }
 

@@ -81,7 +81,8 @@ ABI_SYMBOLS = [
     "kgb_model_load_file", "kgb_model_free", "kgb_model_get_info", "kgb_context_create", "kgb_context_free",
     "kgb_handle_create", "kgb_handle_free", "kgb_handle_is_fp16", "kgb_forward", "kgb_forward_device", "kgb_handle_sync",
     "kgb_handle_stream", "kgb_handle_launches_per_forward", "kgb_handle_get_layout_stats", "kgb_test_conv", "kgb_bench_conv_ex", "kgb_test_conv_epilogue",
-    "kgb_test_conv_ex", "kgb_test_conv_boundary", "kgb_bench_conv_boundary",
+    "kgb_test_conv_ex", "kgb_test_conv_boundary", "kgb_bench_conv_boundary", "kgb_test_conv_plan", "kgb_test_conv_boundary_plan",
+    "kgb_test_head_kernel",
     "kgb_selfplay_create", "kgb_selfplay_free", "kgb_selfplay_run", "kgb_selfplay_get_stats", "kgb_selfplay_get_game",
     "kgb_selfplay_get_root_children", "kgb_selfplay_launches_per_step", "kgb_selfplay_play_moves", "kgb_selfplay_time_tree_kernels", "kgb_zobrist_tables", "kgb_selfplay_get_nn_row", "kgb_selfplay_get_root_row", "kgb_test_board_replay", "kgb_selfplay_get_leaf_path", "kgb_expected_white_score_value", "kgb_value_weight_cdf_table", "kgb_rand_uint32_stream", "kgb_test_root_policy_noise", "kgb_test_history_replay", "kgb_test_repetition_bound", "kgb_selfplay_get_play_selection_values", "kgb_selfplay_random_openings", "kgb_selfplay_set_search_rand", "kgb_selfplay_get_root_value_stats", "kgb_test_choose_index_with_temperature",
     "kgb_handle_weights_bytes", "kgb_handle_stage_weights", "kgb_handle_commit_weights", "kgb_handle_wait_staged", "kgb_nccl_unique_id", "kgb_handle_comm_init",
@@ -155,6 +156,9 @@ def load_library():
     lib.kgb_bench_conv_ex.argtypes = [I, I, I, I, I, I, I, I, I, I, I, I, F]
     lib.kgb_test_conv_epilogue.argtypes = [I, I, I, I, P, I, I, I, I, I, P, P, P, P, I, P, P]
     lib.kgb_test_conv_ex.argtypes = [I, I, I, I, P, I, I, I, I, I, P, P, P, P, P, P, I, P, P, P]
+    lib.kgb_test_conv_plan.argtypes = [I, I, I, I, P, I, I, I, I, I, P, P, P, I, P, P, P, P, I, P, P, P, P, P]
+    lib.kgb_test_conv_boundary_plan.argtypes = [I, I, I, I, I, P, P, I, I, I, C.c_uint32, P, P]
+    lib.kgb_test_head_kernel.argtypes = [I, I, I, I, I, P, P, I, P, I, P, I, P, I, P, P]
     lib.kgb_selfplay_create.argtypes = [P, C.POINTER(SelfplayConfig), C.POINTER(P)]
     lib.kgb_selfplay_free.argtypes = [P]
     lib.kgb_selfplay_free.restype = None
@@ -453,6 +457,53 @@ def test_conv_ex(ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16, 
     _check(lib.kgb_test_conv_ex(ky, kx, in_c, out_c, w.ctypes.data, n, nn_x_len, nn_y_len, int(bool(use_fp16)), kind, xx.ctypes.data,
                                 ptr(bxy), *[ptr(a) for a in opt], activation, ptr(raw), ptr(hi), ptr(lo)))
     return raw, hi, lo
+
+
+def test_conv_plan(ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16, kind, x, board_xy, symmetry, ragged, ncbias=None,
+                   residual=None, bn_scale=None, bn_bias=None, activation=2):
+    """test_conv_ex under a row plan made on the device (include/kgb200.h kgb_test_conv_plan): boards board_xy [n][2] ((0, 0): an empty
+    mask) moved by symmetry [n], ragged or at the full frame.  x is given before the symmetry and must be zero off the board; residual,
+    ncbias and the outputs are after it.  Returns (raw, hi, lo, layout stats dict, plan int32 [n][5] = box x0, y0, w, h, first row)."""
+    lib = load_library()
+    shape = (n, nn_y_len, nn_x_len, out_c)
+    w, xx = _f32(weights), _f32(x)
+    raw = np.zeros(shape, np.float32) if kind != 1 else None
+    hi = np.zeros(shape, np.float32) if kind != 0 else None
+    lo = np.zeros(shape, np.float32) if kind != 0 and not use_fp16 else None
+    bxy = np.ascontiguousarray(board_xy, dtype=np.int32)
+    sym = np.ascontiguousarray(symmetry, dtype=np.int32)
+    opt = [_f32(a) if a is not None else None for a in (ncbias, residual, bn_scale, bn_bias)]
+    stats = np.zeros(3, np.int64)
+    plan = np.zeros((n, 5), np.int32)
+    ptr = lambda a: a.ctypes.data if a is not None else None
+    _check(lib.kgb_test_conv_plan(ky, kx, in_c, out_c, w.ctypes.data, n, nn_x_len, nn_y_len, int(bool(use_fp16)), kind, xx.ctypes.data,
+                                  bxy.ctypes.data, sym.ctypes.data, int(bool(ragged)), *[ptr(a) for a in opt], activation, ptr(raw), ptr(hi),
+                                  ptr(lo), stats.ctypes.data, plan.ctypes.data))
+    return raw, hi, lo, dict(rows=int(stats[0]), m_tiles=int(stats[1]), segments=int(stats[2])), plan
+
+
+HEAD_KERNELS = {"pack": 0, "gpool": 1, "bias_act": 2, "matmul": 3, "policy": 4, "ownership": 5, "finalize": 6}
+
+
+def test_head_kernel(which, n, nn_x_len, nn_y_len, iparams, inputs, output_shapes, board_xy=None, symmetry=None, ragged=True, pad=1):
+    """One launch of an fp32 evaluator kernel (include/kgb200.h kgb_test_head_kernel).  inputs: arrays or None, in the hook's order;
+    output_shapes: a shape per output, or None for an output not asked for.  Returns (outputs, layout stats dict or None, plan)."""
+    lib = load_library()
+    ins = [None if a is None else _f32(a) for a in inputs]
+    outs = [None if s is None else np.zeros(s, np.float32) for s in output_shapes]
+    in_ptrs = (C.c_void_p * len(ins))(*[None if a is None else a.ctypes.data for a in ins])
+    out_ptrs = (C.c_void_p * len(outs))(*[None if a is None else a.ctypes.data for a in outs])
+    ip = np.ascontiguousarray(iparams, dtype=np.int32)
+    bxy = None if board_xy is None else np.ascontiguousarray(board_xy, dtype=np.int32)
+    sym = None if symmetry is None else np.ascontiguousarray(symmetry, dtype=np.int32)
+    stats = np.zeros(3, np.int64)
+    plan = np.zeros((n, 5), np.int32)
+    ptr = lambda a: a.ctypes.data if a is not None else None
+    _check(lib.kgb_test_head_kernel(HEAD_KERNELS[which], n, nn_x_len, nn_y_len, pad, ptr(bxy), ptr(sym), int(bool(ragged)), ip.ctypes.data, len(ip),
+                                    C.cast(in_ptrs, C.c_void_p), len(ins), C.cast(out_ptrs, C.c_void_p), len(outs), stats.ctypes.data,
+                                    plan.ctypes.data))
+    planned = which not in ("matmul", "finalize")
+    return outs, (dict(rows=int(stats[0]), m_tiles=int(stats[1]), segments=int(stats[2])) if planned else None), plan
 
 
 def zobrist_tables(x_size: int, y_size: int):
