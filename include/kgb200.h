@@ -54,6 +54,7 @@ typedef struct kgb_model_info {
   float shortterm_value_error_multiplier;
   float shortterm_score_error_multiplier;
   int64_t conv_macs_per_position; /* direct-convolution MACs per board point (ModelDesc::iterConvLayers, desc.cpp:2643) */
+  int32_t num_input_meta_channels; /* 192 for an SGF-metadata (human SL) net, which needs kgb_forward_meta; 0 otherwise */
 } kgb_model_info;
 
 /* NeuralNet::globalInitialize / globalCleanup (nninterface.h:34-36). */
@@ -107,10 +108,20 @@ KGB_API int kgb_forward(kgb_handle* handle, int n, const float* spatial, const f
 KGB_API int kgb_forward_device(kgb_handle* handle, int n, const float* d_spatial, const float* d_global, const int32_t* d_symmetry,
                        const float* d_policy_optimism, float* d_policy, float* d_value, float* d_score_value,
                        float* d_ownership);
+/* The same two entry points for an SGF-metadata (human SL) net (kgb_model_info.num_input_meta_channels = 192), with one more input:
+ *   meta           [n][192]   NNResultBuf::rowMetaBuf (SGFMetadata::fillMetadataRow output)
+ * The net's metadata encoder (three fully connected layers) turns each row into a per-image bias of the initial convolution, added
+ * to the global inputs' one (eigenbackend.cpp:1927-1932).  kgb_forward / kgb_forward_device on such a net, and these two on a net
+ * without an encoder, are KGB_ERR_INVALID. */
+KGB_API int kgb_forward_meta(kgb_handle* handle, int n, const float* spatial, const float* global, const float* meta, const int32_t* symmetry,
+                             const float* policy_optimism, float* policy, float* value, float* score_value, float* ownership);
+KGB_API int kgb_forward_device_meta(kgb_handle* handle, int n, const float* d_spatial, const float* d_global, const float* d_meta,
+                                    const int32_t* d_symmetry, const float* d_policy_optimism, float* d_policy, float* d_value,
+                                    float* d_score_value, float* d_ownership);
 KGB_API int kgb_handle_sync(kgb_handle* handle);
 /* cudaStream_t of the handle (as an integer) so a torch/CUDA caller can order its own work against it. */
 KGB_API uint64_t kgb_handle_stream(kgb_handle* handle);
-/* Number of kernel launches one kgb_forward of batch n issues (for bench.py's gpu_launches accounting). */
+/* Number of kernel launches one kgb_forward of batch n issues (for bench.py's gpu_launches accounting); a metadata net's encoder adds 3. */
 KGB_API int kgb_handle_launches_per_forward(const kgb_handle* handle);
 /* The row layout the last forward or self-play wave on the handle used (waits for the handle's stream): the rows and 128-row
  * tiles every convolution ran over, and the number of segments (board widths).  Each image takes (h+pad)*(w+pad) rows for the

@@ -40,10 +40,10 @@ struct ComputeContext {
 struct ComputeHandle {
   kgb_handle* kh;
   int nnXLen, nnYLen, maxBatchSize, modelVersion;
-  int numSpatial, numGlobal;
+  int numSpatial, numGlobal, numMeta;   // numMeta: 192 for an SGF-metadata (human SL) net, else 0
   bool inputsUseNHWC;
   // contiguous host staging (the C ABI takes plain row-major arrays)
-  vector<float> spatial, global, optimism, policy, value, score, ownership;
+  vector<float> spatial, global, meta, optimism, policy, value, score, ownership;
   vector<int32_t> symmetry;
 };
 
@@ -97,10 +97,12 @@ ComputeHandle* NeuralNet::createComputeHandle(
   h->modelVersion = loadedModel->modelDesc.modelVersion;
   h->numSpatial = NNModelVersion::getNumSpatialFeatures(h->modelVersion);
   h->numGlobal = NNModelVersion::getNumGlobalFeatures(h->modelVersion);
+  h->numMeta = loadedModel->modelDesc.numInputMetaChannels;
   h->inputsUseNHWC = inputsUseNHWC;
   const size_t xy = (size_t)h->nnXLen * h->nnYLen;
   h->spatial.resize((size_t)maxBatchSize * h->numSpatial * xy);
   h->global.resize((size_t)maxBatchSize * h->numGlobal);
+  h->meta.resize((size_t)maxBatchSize * h->numMeta);
   h->optimism.resize(maxBatchSize);
   h->symmetry.resize(maxBatchSize);
   h->policy.resize((size_t)maxBatchSize * (xy + 1));
@@ -137,15 +139,21 @@ void NeuralNet::getOutput(
   for(int i = 0; i < n; i++) {
     const NNResultBuf* rb = inputBufs[i];
     if(rb->rowSpatialBuf.size() < spElts || rb->rowGlobalBuf.size() < (size_t)h->numGlobal) throw StringError("H100 backend: row buffers too small");
-    if(rb->hasRowMeta) throw StringError("H100 backend: SGF metadata inputs are not supported");
+    // NNEvaluator fills rowMetaBuf (SGFMetadata::fillMetadataRow) exactly when the net has an encoder (nneval.cpp:466-484)
+    if(rb->hasRowMeta != (h->numMeta > 0) || rb->rowMetaBuf.size() < (size_t)h->numMeta) throw StringError("H100 backend: metadata row does not match the net");
     std::copy(rb->rowSpatialBuf.begin(), rb->rowSpatialBuf.begin() + spElts, h->spatial.begin() + i * spElts);
     std::copy(rb->rowGlobalBuf.begin(), rb->rowGlobalBuf.begin() + h->numGlobal, h->global.begin() + (size_t)i * h->numGlobal);
+    std::copy(rb->rowMetaBuf.begin(), rb->rowMetaBuf.begin() + h->numMeta, h->meta.begin() + (size_t)i * h->numMeta);
     h->symmetry[i] = rb->symmetry;
     h->optimism[i] = (float)rb->policyOptimism;
     anyOwner = anyOwner || outputs[i]->whiteOwnerMap != NULL;
   }
-  kgbCheck(kgb_forward(h->kh, n, h->spatial.data(), h->global.data(), h->symmetry.data(), h->optimism.data(), h->policy.data(),
-                       h->value.data(), h->score.data(), anyOwner ? h->ownership.data() : NULL), "getOutput");
+  if(h->numMeta > 0)
+    kgbCheck(kgb_forward_meta(h->kh, n, h->spatial.data(), h->global.data(), h->meta.data(), h->symmetry.data(), h->optimism.data(),
+                              h->policy.data(), h->value.data(), h->score.data(), anyOwner ? h->ownership.data() : NULL), "getOutput");
+  else
+    kgbCheck(kgb_forward(h->kh, n, h->spatial.data(), h->global.data(), h->symmetry.data(), h->optimism.data(), h->policy.data(),
+                         h->value.data(), h->score.data(), anyOwner ? h->ownership.data() : NULL), "getOutput");
   for(int i = 0; i < n; i++) {
     NNOutput* o = outputs[i];
     std::copy(h->policy.begin() + i * (xy + 1), h->policy.begin() + (i + 1) * (xy + 1), o->policyProbs);

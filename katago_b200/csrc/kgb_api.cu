@@ -392,6 +392,23 @@ struct Builder {
       CK(launchMatMulNC(hp->dGlobal, G, Wglob, nullptr, n, G, trunkC, ACT_IDENTITY, initBias, trunkCp, s));
     });
     h.launchesPerForward++;
+    if(m.numInputMetaChannels > 0) {
+      // the SGF-metadata encoder in fp32 in both modes; its output joins the global inputs' bias (eigenbackend.cpp:1839-1857, 1927-1932)
+      const MetaEncoderDesc& e = m.metaEncoder;
+      h.dMeta = h.dalloc<float>((size_t)h.maxBatch * m.numInputMetaChannels);
+      const float *W1 = h.upload(e.mul1.w), *b1 = h.upload(e.bias1.w), *W2 = h.upload(e.mul2.w), *b2 = h.upload(e.bias2.w), *W3 = h.upload(e.mul3.w);
+      const int cm = m.numInputMetaChannels, c1 = e.mul1.cout, c2 = e.mul2.cout, act1 = e.act1, act2 = e.act2;
+      float* mid1 = h.dalloc<float>((size_t)h.maxBatch * c1);
+      float* mid2 = h.dalloc<float>((size_t)h.maxBatch * c2);
+      h.ops.push_back([=](int n, cudaStream_t s) {
+        CK(launchMatMulNC(hp->dMeta, cm, W1, b1, n, cm, c1, act1, mid1, c1, s));
+        CK(launchMatMulNC(mid1, c1, W2, b2, n, c1, c2, act2, mid2, c2, s));
+        CK(launchMatMulNC(mid2, c2, W3, nullptr, n, c2, trunkC, ACT_IDENTITY, initBias, trunkCp, s, true));
+      });
+      h.launchesPerForward += 3;
+      h.wSignature += "meta" + std::to_string(cm) + ":" + std::to_string(c1) + "," + std::to_string(c2) + "," + std::to_string(act1) + "," +
+                      std::to_string(act2) + ";";
+    }
     ConvWeights winit = packConv({&m.initialConv});
     BNDev firstPre = uploadBN(m.blocks[0].preBN, m.blocks[0].preAct, trunk.cp);
     emitConv(winit, inAct, nullptr, false, initBias, trunk.S, trunk.fp32, trunk.A, firstPre);
@@ -555,6 +572,7 @@ KGB_API int kgb_model_get_info(const kgb_model* model, kgb_model_info* out) {
     out->shortterm_value_error_multiplier = d.shorttermValueErrorMultiplier;
     out->shortterm_score_error_multiplier = d.shorttermScoreErrorMultiplier;
     out->conv_macs_per_position = d.convMacsPerPosition();
+    out->num_input_meta_channels = d.numInputMetaChannels;
   });
 }
 
@@ -660,7 +678,7 @@ static void destroyHandle(kgb_handle* h) {
   if(h->ncclComm && ncclApi().ok) ncclApi().commDestroy((ncclComm_t)h->ncclComm);
   for(cudaEvent_t e : {h->stagedEvent, h->bcastStart, h->bcastStop}) if(e) cudaEventDestroy(e);
   if(h->copyStream) cudaStreamDestroy(h->copyStream);
-  for(void* p : {(void*)h->hSpatial, (void*)h->hGlobal, (void*)h->hOptimism, (void*)h->hPolicy, (void*)h->hValue, (void*)h->hScore,
+  for(void* p : {(void*)h->hSpatial, (void*)h->hGlobal, (void*)h->hMeta, (void*)h->hOptimism, (void*)h->hPolicy, (void*)h->hValue, (void*)h->hScore,
                  (void*)h->hOwnership, (void*)h->hSymmetry})
     if(p) cudaFreeHost(p);
   if(h->stream) cudaStreamDestroy(h->stream);
@@ -710,6 +728,7 @@ KGB_API int kgb_handle_create(kgb_context* ctx, const kgb_model* model, int max_
     const ModelDesc& m = *h.model;
     CK(cudaMallocHost((void**)&h.hSpatial, (size_t)h.maxBatch * m.numInputChannels * XY * sizeof(float)));
     CK(cudaMallocHost((void**)&h.hGlobal, (size_t)h.maxBatch * m.numInputGlobalChannels * sizeof(float)));
+    if(m.numInputMetaChannels > 0) CK(cudaMallocHost((void**)&h.hMeta, (size_t)h.maxBatch * m.numInputMetaChannels * sizeof(float)));
     CK(cudaMallocHost((void**)&h.hOptimism, (size_t)h.maxBatch * sizeof(float)));
     CK(cudaMallocHost((void**)&h.hSymmetry, (size_t)h.maxBatch * sizeof(int)));
     CK(cudaMallocHost((void**)&h.hPolicy, (size_t)h.maxBatch * (XY + 1) * sizeof(float)));
@@ -862,37 +881,86 @@ static void checkForwardArgs(kgb_handle* h, int n, const void* a, const void* b,
   if(!a || !b || !c || !d || !e) throw std::invalid_argument("kgb_forward: NULL buffer");
 }
 
+// A metadata net needs its rows (the reference's fatalError when they are missing, nneval.cpp:471-474), and rows need a metadata net
+static void checkMetaArgs(const kgb_handle* h, const void* meta, const char* fn) {
+  const bool hasEncoder = h->model->numInputMetaChannels > 0;
+  if(hasEncoder && !meta)
+    throw std::invalid_argument(std::string(fn) + ": the net has an SGF-metadata encoder and needs a metadata row per image (kgb_forward_meta / kgb_forward_device_meta)");
+  if(!hasEncoder && meta) throw std::invalid_argument(std::string(fn) + ": metadata rows given for a net without an SGF-metadata encoder");
+}
+
+static void forwardHost(kgb_handle* h, int n, const float* spatial, const float* global, const float* meta, const int32_t* symmetry,
+                        const float* policy_optimism, float* policy, float* value, float* score_value, float* ownership) {
+  CK(cudaSetDevice(h->device));
+  const ModelDesc& m = *h->model;
+  const int XY = h->L.X * h->L.Y;
+  const size_t spB = (size_t)n * m.numInputChannels * XY * sizeof(float);
+  const size_t glB = (size_t)n * m.numInputGlobalChannels * sizeof(float);
+  const size_t metaB = (size_t)n * m.numInputMetaChannels * sizeof(float);
+  memcpy(h->hSpatial, spatial, spB);
+  memcpy(h->hGlobal, global, glB);
+  if(meta) memcpy(h->hMeta, meta, metaB);
+  for(int i = 0; i < n; i++) {
+    h->hSymmetry[i] = symmetry ? symmetry[i] : 0;
+    h->hOptimism[i] = policy_optimism ? policy_optimism[i] : 0.0f;
+    if(h->hSymmetry[i] < 0 || h->hSymmetry[i] > 7) throw std::invalid_argument("kgb_forward: symmetry must be in 0..7");
+  }
+  cudaStream_t s = h->stream;
+  CK(cudaMemcpyAsync(h->dSpatial, h->hSpatial, spB, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(h->dGlobal, h->hGlobal, glB, cudaMemcpyHostToDevice, s));
+  if(meta) CK(cudaMemcpyAsync(h->dMeta, h->hMeta, metaB, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(h->dSymmetry, h->hSymmetry, n * sizeof(int), cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(h->dOptimism, h->hOptimism, n * sizeof(float), cudaMemcpyHostToDevice, s));
+  runOps(h, n);
+  CK(cudaMemcpyAsync(h->hPolicy, h->dPolicy, (size_t)n * (XY + 1) * sizeof(float), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(h->hValue, h->dValue, (size_t)n * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(h->hScore, h->dScore, (size_t)n * 6 * sizeof(float), cudaMemcpyDeviceToHost, s));
+  if(ownership) CK(cudaMemcpyAsync(h->hOwnership, h->dOwnership, (size_t)n * XY * sizeof(float), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  memcpy(policy, h->hPolicy, (size_t)n * (XY + 1) * sizeof(float));
+  memcpy(value, h->hValue, (size_t)n * 3 * sizeof(float));
+  memcpy(score_value, h->hScore, (size_t)n * 6 * sizeof(float));
+  if(ownership) memcpy(ownership, h->hOwnership, (size_t)n * XY * sizeof(float));
+}
+
+static void forwardDevice(kgb_handle* h, int n, const float* d_spatial, const float* d_global, const float* d_meta, const int32_t* d_symmetry,
+                          const float* d_policy_optimism, float* d_policy, float* d_value, float* d_score_value, float* d_ownership) {
+  CK(cudaSetDevice(h->device));
+  const ModelDesc& m = *h->model;
+  const int XY = h->L.X * h->L.Y;
+  cudaStream_t s = h->stream;
+  if(d_spatial != h->dSpatial)
+    CK(cudaMemcpyAsync(h->dSpatial, d_spatial, (size_t)n * m.numInputChannels * XY * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  if(d_global != h->dGlobal)
+    CK(cudaMemcpyAsync(h->dGlobal, d_global, (size_t)n * m.numInputGlobalChannels * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  if(d_meta && d_meta != h->dMeta)
+    CK(cudaMemcpyAsync(h->dMeta, d_meta, (size_t)n * m.numInputMetaChannels * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  if(d_symmetry) CK(cudaMemcpyAsync(h->dSymmetry, d_symmetry, n * sizeof(int), cudaMemcpyDeviceToDevice, s));
+  else CK(cudaMemsetAsync(h->dSymmetry, 0, n * sizeof(int), s));
+  if(d_policy_optimism) CK(cudaMemcpyAsync(h->dOptimism, d_policy_optimism, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  else CK(cudaMemsetAsync(h->dOptimism, 0, n * sizeof(float), s));
+  runOps(h, n);
+  CK(cudaMemcpyAsync(d_policy, h->dPolicy, (size_t)n * (XY + 1) * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  CK(cudaMemcpyAsync(d_value, h->dValue, (size_t)n * 3 * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  CK(cudaMemcpyAsync(d_score_value, h->dScore, (size_t)n * 6 * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  if(d_ownership) CK(cudaMemcpyAsync(d_ownership, h->dOwnership, (size_t)n * XY * sizeof(float), cudaMemcpyDeviceToDevice, s));
+}
+
 KGB_API int kgb_forward(kgb_handle* h, int n, const float* spatial, const float* global, const int32_t* symmetry, const float* policy_optimism,
                 float* policy, float* value, float* score_value, float* ownership) {
   return guarded([&] {
     checkForwardArgs(h, n, spatial, global, policy, value, score_value);
-    CK(cudaSetDevice(h->device));
-    const ModelDesc& m = *h->model;
-    const int XY = h->L.X * h->L.Y;
-    const size_t spB = (size_t)n * m.numInputChannels * XY * sizeof(float);
-    const size_t glB = (size_t)n * m.numInputGlobalChannels * sizeof(float);
-    memcpy(h->hSpatial, spatial, spB);
-    memcpy(h->hGlobal, global, glB);
-    for(int i = 0; i < n; i++) {
-      h->hSymmetry[i] = symmetry ? symmetry[i] : 0;
-      h->hOptimism[i] = policy_optimism ? policy_optimism[i] : 0.0f;
-      if(h->hSymmetry[i] < 0 || h->hSymmetry[i] > 7) throw std::invalid_argument("kgb_forward: symmetry must be in 0..7");
-    }
-    cudaStream_t s = h->stream;
-    CK(cudaMemcpyAsync(h->dSpatial, h->hSpatial, spB, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(h->dGlobal, h->hGlobal, glB, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(h->dSymmetry, h->hSymmetry, n * sizeof(int), cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(h->dOptimism, h->hOptimism, n * sizeof(float), cudaMemcpyHostToDevice, s));
-    runOps(h, n);
-    CK(cudaMemcpyAsync(h->hPolicy, h->dPolicy, (size_t)n * (XY + 1) * sizeof(float), cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(h->hValue, h->dValue, (size_t)n * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(h->hScore, h->dScore, (size_t)n * 6 * sizeof(float), cudaMemcpyDeviceToHost, s));
-    if(ownership) CK(cudaMemcpyAsync(h->hOwnership, h->dOwnership, (size_t)n * XY * sizeof(float), cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    memcpy(policy, h->hPolicy, (size_t)n * (XY + 1) * sizeof(float));
-    memcpy(value, h->hValue, (size_t)n * 3 * sizeof(float));
-    memcpy(score_value, h->hScore, (size_t)n * 6 * sizeof(float));
-    if(ownership) memcpy(ownership, h->hOwnership, (size_t)n * XY * sizeof(float));
+    checkMetaArgs(h, nullptr, "kgb_forward");
+    forwardHost(h, n, spatial, global, nullptr, symmetry, policy_optimism, policy, value, score_value, ownership);
+  });
+}
+
+KGB_API int kgb_forward_meta(kgb_handle* h, int n, const float* spatial, const float* global, const float* meta, const int32_t* symmetry,
+                             const float* policy_optimism, float* policy, float* value, float* score_value, float* ownership) {
+  return guarded([&] {
+    checkForwardArgs(h, n, spatial, global, policy, value, score_value);
+    checkMetaArgs(h, meta, "kgb_forward_meta");
+    forwardHost(h, n, spatial, global, meta, symmetry, policy_optimism, policy, value, score_value, ownership);
   });
 }
 
@@ -900,23 +968,18 @@ KGB_API int kgb_forward_device(kgb_handle* h, int n, const float* d_spatial, con
                        const float* d_policy_optimism, float* d_policy, float* d_value, float* d_score_value, float* d_ownership) {
   return guarded([&] {
     checkForwardArgs(h, n, d_spatial, d_global, d_policy, d_value, d_score_value);
-    CK(cudaSetDevice(h->device));
-    const ModelDesc& m = *h->model;
-    const int XY = h->L.X * h->L.Y;
-    cudaStream_t s = h->stream;
-    if(d_spatial != h->dSpatial)
-      CK(cudaMemcpyAsync(h->dSpatial, d_spatial, (size_t)n * m.numInputChannels * XY * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    if(d_global != h->dGlobal)
-      CK(cudaMemcpyAsync(h->dGlobal, d_global, (size_t)n * m.numInputGlobalChannels * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    if(d_symmetry) CK(cudaMemcpyAsync(h->dSymmetry, d_symmetry, n * sizeof(int), cudaMemcpyDeviceToDevice, s));
-    else CK(cudaMemsetAsync(h->dSymmetry, 0, n * sizeof(int), s));
-    if(d_policy_optimism) CK(cudaMemcpyAsync(h->dOptimism, d_policy_optimism, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    else CK(cudaMemsetAsync(h->dOptimism, 0, n * sizeof(float), s));
-    runOps(h, n);
-    CK(cudaMemcpyAsync(d_policy, h->dPolicy, (size_t)n * (XY + 1) * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    CK(cudaMemcpyAsync(d_value, h->dValue, (size_t)n * 3 * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    CK(cudaMemcpyAsync(d_score_value, h->dScore, (size_t)n * 6 * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    if(d_ownership) CK(cudaMemcpyAsync(d_ownership, h->dOwnership, (size_t)n * XY * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    checkMetaArgs(h, nullptr, "kgb_forward_device");
+    forwardDevice(h, n, d_spatial, d_global, nullptr, d_symmetry, d_policy_optimism, d_policy, d_value, d_score_value, d_ownership);
+  });
+}
+
+KGB_API int kgb_forward_device_meta(kgb_handle* h, int n, const float* d_spatial, const float* d_global, const float* d_meta,
+                                    const int32_t* d_symmetry, const float* d_policy_optimism, float* d_policy, float* d_value,
+                                    float* d_score_value, float* d_ownership) {
+  return guarded([&] {
+    checkForwardArgs(h, n, d_spatial, d_global, d_policy, d_value, d_score_value);
+    checkMetaArgs(h, d_meta, "kgb_forward_device_meta");
+    forwardDevice(h, n, d_spatial, d_global, d_meta, d_symmetry, d_policy_optimism, d_policy, d_value, d_score_value, d_ownership);
   });
 }
 

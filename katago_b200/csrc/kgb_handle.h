@@ -61,11 +61,11 @@ struct kgb_handle {
   bool fuseBoundaries = false;   // consecutive nested blocks' exit + entry 1x1 as one launch (launchConvPair)
   std::vector<void*> allocs;
   // inputs / outputs (device, fixed addresses so graphs can be replayed)
-  float *dSpatial = nullptr, *dGlobal = nullptr, *dOptimism = nullptr;
+  float *dSpatial = nullptr, *dGlobal = nullptr, *dMeta = nullptr, *dOptimism = nullptr;   // dMeta: SGF-metadata nets only
   int* dSymmetry = nullptr;
   float *dPolicy = nullptr, *dValue = nullptr, *dScore = nullptr, *dOwnership = nullptr;
   // pinned staging
-  float *hSpatial = nullptr, *hGlobal = nullptr, *hOptimism = nullptr, *hPolicy = nullptr, *hValue = nullptr, *hScore = nullptr,
+  float *hSpatial = nullptr, *hGlobal = nullptr, *hMeta = nullptr, *hOptimism = nullptr, *hPolicy = nullptr, *hValue = nullptr, *hScore = nullptr,
         *hOwnership = nullptr;
   int* hSymmetry = nullptr;
   float *dMask = nullptr, *dMaskSum = nullptr;

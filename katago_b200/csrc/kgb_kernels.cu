@@ -164,7 +164,7 @@ cudaError_t launchPackInput(const float* spatial, int n, int C, bool nhwc, const
 
 // ------------------------------------------------------------------------------------------------------------
 __global__ void matMulNCKernel(const float* __restrict__ in, int ldi, const float* __restrict__ W, const float* __restrict__ bias,
-                               int cin, int cout, int act, float* __restrict__ out, int ldo) {
+                               int cin, int cout, int act, float* __restrict__ out, int ldo, bool accumulate) {
   extern __shared__ float sIn[];
   int img = blockIdx.x;
   for(int k = threadIdx.x; k < cin; k += blockDim.x) sIn[k] = in[(size_t)img * ldi + k];
@@ -175,14 +175,15 @@ __global__ void matMulNCKernel(const float* __restrict__ in, int ldi, const floa
       for(int k = 0; k < cin; k++) v = fmaf(sIn[k], W[(size_t)k * cout + co], v);
       if(bias) v += bias[co];
       v = kgb_activate(v, act);
+      if(accumulate) v = out[(size_t)img * ldo + co] + v;
     }
     out[(size_t)img * ldo + co] = v;
   }
 }
 
 cudaError_t launchMatMulNC(const float* in, int ldi, const float* W, const float* bias, int n, int cin, int cout, int act, float* out,
-                           int ldo, cudaStream_t s) {
-  matMulNCKernel<<<n, 128, cin * sizeof(float), s>>>(in, ldi, W, bias, cin, cout, act, out, ldo);
+                           int ldo, cudaStream_t s, bool accumulate) {
+  matMulNCKernel<<<n, 128, cin * sizeof(float), s>>>(in, ldi, W, bias, cin, cout, act, out, ldo, accumulate);
   return cudaGetLastError();
 }
 

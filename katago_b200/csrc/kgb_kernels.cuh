@@ -55,9 +55,10 @@ cudaError_t launchPackInput(const float* spatial, int n, int C, bool nhwc, const
                             __half* act, int cin_p, int split, float* mask, float* maskSum, cudaStream_t s);
 
 // out[n][co] = act( sum_k in[n][k] * W[k][co] + bias[co] )   (MatMulLayer / MatBiasLayer / ActivationLayer,
-// eigenbackend.cpp:811-862); out has leading dimension ldo and is zero-filled in [cout, ldo).
+// eigenbackend.cpp:811-862); out has leading dimension ldo and is zero-filled in [cout, ldo).  accumulate: out = out + that instead
+// (the metadata encoder's output added to the global inputs' bias, eigenbackend.cpp:1927-1932).
 cudaError_t launchMatMulNC(const float* in, int ldi, const float* W, const float* bias, int n, int cin, int cout, int act,
-                           float* out, int ldo, cudaStream_t s);
+                           float* out, int ldo, cudaStream_t s, bool accumulate = false);
 
 // Global pooling of act(BN(raw[:, c0:c0+C])) * mask  ->  pooled [n][3C]
 //   valueHead == 0: mean, mean*(sqrt(area)-14)/10, max       (poolRowsGPool, eigenbackend.cpp:152-177)

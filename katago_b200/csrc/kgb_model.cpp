@@ -201,6 +201,27 @@ MatBiasDesc parseMatBias(Reader& r) {
 
 void parseBlockStack(Reader& r, int version, int n, int expectC, std::vector<BlockDesc>& out);
 
+MetaEncoderDesc parseMetaEncoder(Reader& r, int version, int expectInputs) {  // desc.cpp:1571-1617
+  MetaEncoderDesc e;
+  e.name = r.tok("sgf metadata encoder name");
+  const int numInputs = r.readInt("sgf metadata encoder num input channels");
+  if(numInputs != expectInputs)
+    throw std::runtime_error(e.name + ": number of in channels (" + std::to_string(numInputs) + ") did not match expected (" +
+                             std::to_string(expectInputs) + ")");
+  e.mul1 = parseMatMul(r); e.bias1 = parseMatBias(r); e.act1 = parseAct(r, version);
+  e.mul2 = parseMatMul(r); e.bias2 = parseMatBias(r); e.act2 = parseAct(r, version);
+  e.mul3 = parseMatMul(r);
+  if(e.mul1.cout != e.bias1.c)
+    throw std::runtime_error(e.name + ": mul1.outChannels (" + std::to_string(e.mul1.cout) + ") != bias1.numChannels (" + std::to_string(e.bias1.c) + ")");
+  if(e.mul2.cin != e.mul1.cout)
+    throw std::runtime_error(e.name + ": mul2.inChannels (" + std::to_string(e.mul2.cin) + ") != mul1.outChannels (" + std::to_string(e.mul1.cout) + ")");
+  if(e.mul2.cout != e.bias2.c)
+    throw std::runtime_error(e.name + ": mul2.outChannels (" + std::to_string(e.mul2.cout) + ") != bias2.numChannels (" + std::to_string(e.bias2.c) + ")");
+  if(e.mul2.cout != e.mul3.cin)
+    throw std::runtime_error(e.name + ": mul2.outChannels (" + std::to_string(e.mul2.cout) + ") != mul3.inChannels (" + std::to_string(e.mul3.cin) + ")");
+  return e;
+}
+
 BlockDesc parseBlock(Reader& r, int version, const std::string& kind) {
   BlockDesc b;
   b.name = r.tok("block name");
@@ -316,6 +337,7 @@ void ModelDesc::transformToReduceActivations() {  // desc.cpp:1911-1972
   tipBN.extractFactorsAbsLtOneWithInverses(f, inv);
   initialConv.scaleOutputChannels(f);
   initialMatMul.scaleOutputChannels(f);
+  if(numInputMetaChannels > 0) metaEncoder.mul3.scaleOutputChannels(f);
   for(auto& b : blocks) { b.preBN.scaleInputChannels(inv); b.conv2.scaleOutputChannels(f); }
   for(auto& b : blocks) b.transformToReduceActivations();
 }
@@ -373,15 +395,19 @@ std::unique_ptr<ModelDesc> parseModel(const std::string& data, bool binaryFloats
     }
   }
   if(v >= 15) {
-    int metaEncoderVersion = r.readInt("metaEncoderVersion");
-    if(metaEncoderVersion != 0) throw std::runtime_error(m.name + ": SGF-metadata (humanSL) nets are not supported by the H100 backend");
+    int metaEncoderVersion = r.readInt("metaEncoderVersion");   // desc.cpp:2519-2533, modelversion.cpp:83-89
+    if(metaEncoderVersion < 0) throw std::runtime_error(m.name + ": model metaEncoderVersion unexpected value: " + std::to_string(metaEncoderVersion));
+    if(metaEncoderVersion > 1)
+      throw std::runtime_error(m.name + ": model metaEncoderVersion not implemented, you may need a newer KataGo version, value was: " +
+                               std::to_string(metaEncoderVersion));
+    m.numInputMetaChannels = metaEncoderVersion == 1 ? 192 : 0;
     m.preferPassAliveUnderSuicideRules = r.readInt("preferPassAliveUnderSuicideRules");
     if(m.preferPassAliveUnderSuicideRules != 0 && m.preferPassAliveUnderSuicideRules != 1)
       throw std::runtime_error(m.name + ": model preferPassAliveUnderSuicideRules unexpected value");
     expectZeros(r, 6, "model option");
   }
   // Trunk
-  r.tok("trunk name");
+  const std::string trunkName = r.tok("trunk name");
   int numBlocks = r.readInt("trunk numBlocks");
   m.trunkC = r.readInt("trunkNumChannels"); m.midC = r.readInt("midNumChannels"); m.regularC = r.readInt("regularNumChannels");
   r.readInt("dilatedNumChannels");
@@ -397,6 +423,16 @@ std::unique_ptr<ModelDesc> parseModel(const std::string& data, bool binaryFloats
   m.initialMatMul = parseMatMul(r);
   if(m.initialConv.cout != m.trunkC || m.initialMatMul.cout != m.trunkC) throw std::runtime_error(m.name + ": initial conv/matmul outChannels != trunkNumChannels");
   if(m.initialConv.cin != m.numInputChannels || m.initialMatMul.cin != m.numInputGlobalChannels) throw std::runtime_error(m.name + ": initial conv/matmul inChannels mismatch");
+  if(m.numInputMetaChannels > 0) {
+    m.metaEncoder = parseMetaEncoder(r, v, m.numInputMetaChannels);
+    const MetaEncoderDesc& e = m.metaEncoder;
+    if(e.mul1.cin != m.numInputMetaChannels)  // desc.cpp:1729-1746
+      throw std::runtime_error(trunkName + ": " + e.name + " sgfMetadataEncoder.mul1.inChannels (" + std::to_string(e.mul1.cin) +
+                               ") != numInputMetaChannels (" + std::to_string(m.numInputMetaChannels) + ")");
+    if(e.mul3.cout != m.trunkC)
+      throw std::runtime_error(trunkName + ": " + e.name + " sgfMetadataEncoder.mul3.outChannels (" + std::to_string(e.mul3.cout) +
+                               ") != trunkNumChannels (" + std::to_string(m.trunkC) + ")");
+  }
   parseBlockStack(r, v, numBlocks, m.trunkC, m.blocks);
   m.tipBN = parseBN(r);
   m.tipAct = parseAct(r, v);

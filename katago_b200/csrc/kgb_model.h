@@ -4,7 +4,8 @@
 // folding as the reference: BN merge (cpp/neuralnet/desc.cpp:282-289) and transformToReduceActivations
 // (desc.cpp:627-632, 745-758, 944-1001, 1911-1972, applied at :2810).  The grammar is SURVEY.md Appendix A
 // (desc.cpp:110-155, 208-289, 382-403, 451-535, 566-576, 652-666, 783-801, 1444-1562, 1669-1764, 2051-2103,
-// 2242-2272, 2441-2574).  Transformer / SGF-metadata nets are rejected (out of scope, SURVEY.md §2).
+// 2242-2272, 2441-2574, and the SGF-metadata encoder 1571-1617, 1729-1746).  Transformer nets and RMSNorm trunk tips are rejected
+// (out of scope, SURVEY.md §2).
 #pragma once
 #include <cstdint>
 #include <memory>
@@ -44,6 +45,15 @@ struct MatBiasDesc {
   std::vector<float> w;
 };
 
+// SGF-metadata encoder of human-SL nets (desc.cpp:1571-1617): 192 metadata inputs -> mul1 + bias1, act1 -> mul2 + bias2, act2 -> mul3
+// (trunk channels), added to the initial convolution's per-image bias (eigenbackend.cpp:1839-1857, 1927-1932)
+struct MetaEncoderDesc {
+  std::string name;
+  MatMulDesc mul1; MatBiasDesc bias1; int act1 = ACT_RELU;
+  MatMulDesc mul2; MatBiasDesc bias2; int act2 = ACT_RELU;
+  MatMulDesc mul3;
+};
+
 enum BlockKind : int { BLOCK_ORDINARY = 0, BLOCK_GPOOL = 1, BLOCK_NESTED = 2 };
 
 struct BlockDesc {
@@ -70,9 +80,11 @@ struct ModelDesc {
   float tdScoreMultiplier = 20.f, scoreMeanMultiplier = 20.f, scoreStdevMultiplier = 20.f, leadMultiplier = 20.f,
         varianceTimeMultiplier = 40.f, shorttermValueErrorMultiplier = 0.25f, shorttermScoreErrorMultiplier = 30.f;
   int preferPassAliveUnderSuicideRules = 0;
+  int numInputMetaChannels = 0;   // 192 when the net has an SGF-metadata encoder (metaEncoderVersion 1), else 0
   // trunk
   int trunkC = 0, midC = 0, regularC = 0, gpoolC = 0;
   ConvDesc initialConv; MatMulDesc initialMatMul;
+  MetaEncoderDesc metaEncoder;    // only when numInputMetaChannels > 0
   std::vector<BlockDesc> blocks;
   BNDesc tipBN; int tipAct = ACT_RELU;
   // policy head

@@ -2709,6 +2709,8 @@ KGB_API int kgb_selfplay_create(kgb_handle* handle, const kgb_selfplay_config* c
     if(!handle->nhwc) throw std::invalid_argument("kgb_selfplay_create: the handle must be created with inputs_nhwc = 1");
     if(handle->model->numInputChannels != 22 || handle->model->numInputGlobalChannels != 19)
       throw std::invalid_argument("kgb_selfplay_create: the device loop writes V7 features (22 spatial, 19 global)");
+    if(handle->model->numInputMetaChannels > 0)
+      throw std::invalid_argument("kgb_selfplay_create: SGF-metadata nets need a metadata row per evaluation; the self-play loop has none");
     CK(cudaSetDevice(handle->device));
     std::unique_ptr<kgb_selfplay> sp(new kgb_selfplay());
     sp->h = handle;

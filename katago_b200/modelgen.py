@@ -117,8 +117,14 @@ def _nested(w, rng, name, c, cmid, cg: Optional[int], act, ninner=2):
 
 
 def model_bytes(config: str, seed: int = 0, name: Optional[str] = None, activation: str = "ACTIVATION_MISH",
-                version: int = 15, num_input_channels: int = 22, num_global: int = 19) -> bytes:
+                version: int = 15, num_input_channels: int = 22, num_global: int = 19, meta_channels: int = 0,
+                meta_out_gain: float = 1.0) -> bytes:
+    """meta_channels > 0 adds an SGF-metadata encoder of that internal width (metaEncoderVersion 1, as the reference's
+    `-meta` configs export it: desc.cpp:1571-1617, export_model_pytorch.py write_metadata_encoder), drawn from its own generator so
+    that the trunk and heads equal those of the net without it; meta_out_gain scales its last layer (0: an encoder that adds nothing)."""
     cfg = CONFIGS[config]
+    if meta_channels and version < 15:
+        raise ValueError("SGF-metadata encoders need model version >= 15")
     rng = np.random.default_rng(seed)
     w = _Writer(version)
     act = activation
@@ -130,13 +136,20 @@ def model_bytes(config: str, seed: int = 0, name: Optional[str] = None, activati
     if version >= 13:
         w.line(20.0, 20.0, 20.0, 20.0, 40.0, 0.25, 30.0)
     if version >= 15:
-        w.line(0, 0, 0, 0, 0, 0, 0, 0)
+        w.line(1 if meta_channels else 0, 0, 0, 0, 0, 0, 0, 0)
     w.line("trunk")
     w.line(len(cfg["blocks"]), c, cmid, cmid - cg, cmid - cg, cg)
     if version >= 15:
         w.line(0, 0, 0, 0, 0, 0)
     _conv(w, rng, "conv1", 3, num_input_channels, c)
     _matmul(w, rng, "ginputw", num_global, c)
+    if meta_channels:
+        mrng = np.random.default_rng([seed, 192])
+        w.line("sgf_metadata_encoder")
+        w.line(192)
+        _matmul(w, mrng, "meta.mul1", 192, meta_channels); _matbias(w, mrng, "meta.bias1", meta_channels); _act(w, "meta.act1", act)
+        _matmul(w, mrng, "meta.mul2", meta_channels, meta_channels); _matbias(w, mrng, "meta.bias2", meta_channels); _act(w, "meta.act2", act)
+        _matmul(w, mrng, "meta.mul3", meta_channels, c, gain=meta_out_gain)
     for i, kind in enumerate(cfg["blocks"]):
         nm = f"block{i}"
         if kind == "r":

@@ -31,7 +31,7 @@ class _ModelInfo(C.Structure):
         ("td_score_multiplier", C.c_float), ("score_mean_multiplier", C.c_float), ("score_stdev_multiplier", C.c_float),
         ("lead_multiplier", C.c_float), ("variance_time_multiplier", C.c_float),
         ("shortterm_value_error_multiplier", C.c_float), ("shortterm_score_error_multiplier", C.c_float),
-        ("conv_macs_per_position", C.c_int64),
+        ("conv_macs_per_position", C.c_int64), ("num_input_meta_channels", C.c_int32),
     ]
 
 
@@ -79,7 +79,7 @@ class SelfplayStats(C.Structure):
 ABI_SYMBOLS = [
     "kgb_global_init", "kgb_global_cleanup", "kgb_last_error", "kgb_device_count", "kgb_device_name",
     "kgb_model_load_file", "kgb_model_free", "kgb_model_get_info", "kgb_context_create", "kgb_context_free",
-    "kgb_handle_create", "kgb_handle_free", "kgb_handle_is_fp16", "kgb_forward", "kgb_forward_device", "kgb_handle_sync",
+    "kgb_handle_create", "kgb_handle_free", "kgb_handle_is_fp16", "kgb_forward", "kgb_forward_device", "kgb_forward_meta", "kgb_forward_device_meta", "kgb_handle_sync",
     "kgb_handle_stream", "kgb_handle_launches_per_forward", "kgb_handle_get_layout_stats", "kgb_test_conv", "kgb_bench_conv_ex", "kgb_test_conv_epilogue",
     "kgb_test_conv_ex", "kgb_test_conv_boundary", "kgb_bench_conv_boundary", "kgb_test_conv_plan", "kgb_test_conv_boundary_plan",
     "kgb_test_head_kernel",
@@ -147,6 +147,8 @@ def load_library():
     lib.kgb_selfplay_get_leaf_cache_key.argtypes = [P, I, P]
     lib.kgb_forward.argtypes = [P, I, P, P, P, P, P, P, P, P]
     lib.kgb_forward_device.argtypes = [P, I, P, P, P, P, P, P, P, P]
+    lib.kgb_forward_meta.argtypes = [P, I, P, P, P, P, P, P, P, P, P]
+    lib.kgb_forward_device_meta.argtypes = [P, I, P, P, P, P, P, P, P, P, P]
     lib.kgb_handle_sync.argtypes = [P]
     lib.kgb_handle_stream.argtypes = [P]
     lib.kgb_handle_stream.restype = C.c_uint64
@@ -386,9 +388,10 @@ class NeuralNet:
         return bool(load_library().kgb_handle_is_fp16(h._p))
 
     @staticmethod
-    def getOutput(handle: ComputeHandle, spatial, global_, symmetry=None, policyOptimism=None, includeOwnerMap=True) -> dict:
+    def getOutput(handle: ComputeHandle, spatial, global_, symmetry=None, policyOptimism=None, includeOwnerMap=True, meta=None) -> dict:
         """spatial [n, C*X*Y] (layout per inputsUseNHWC), global_ [n, G] -> dict(policy [n,X*Y+1], value [n,3],
-        score_value [n,6], ownership [n,X*Y] or None); raw logits as NeuralNet::getOutput writes into NNOutput."""
+        score_value [n,6], ownership [n,X*Y] or None); raw logits as NeuralNet::getOutput writes into NNOutput.  meta [n, 192]:
+        the SGF-metadata rows (SGFMetadata::fillMetadataRow) an SGF-metadata net needs, and only such a net takes."""
         lib = load_library()
         sp, gl = _f32(spatial), _f32(global_)
         n = sp.shape[0]
@@ -402,9 +405,14 @@ class NeuralNet:
         value = np.empty((n, 3), np.float32)
         score = np.empty((n, 6), np.float32)
         own = np.empty((n, xy), np.float32) if includeOwnerMap else None
-        _check(lib.kgb_forward(handle._p, n, sp.ctypes.data, gl.ctypes.data, sym.ctypes.data, opt.ctypes.data,
-                               policy.ctypes.data, value.ctypes.data, score.ctypes.data,
-                               own.ctypes.data if own is not None else None))
+        outs = (policy.ctypes.data, value.ctypes.data, score.ctypes.data, own.ctypes.data if own is not None else None)
+        if meta is None:
+            _check(lib.kgb_forward(handle._p, n, sp.ctypes.data, gl.ctypes.data, sym.ctypes.data, opt.ctypes.data, *outs))
+        else:
+            mt = _f32(meta)
+            if mt.size != n * 192:
+                raise KGBError("getOutput: meta must hold 192 floats per row")
+            _check(lib.kgb_forward_meta(handle._p, n, sp.ctypes.data, gl.ctypes.data, mt.ctypes.data, sym.ctypes.data, opt.ctypes.data, *outs))
         return dict(policy=policy, value=value, score_value=score, ownership=own)
 
     @staticmethod
