@@ -184,7 +184,9 @@ typedef struct kgb_selfplay_config {
   double no_result_utility_for_white;
   uint64_t seed;
   int32_t debug_fake_nn;             /* TEST ONLY: replace the evaluator by the deterministic hash net of oracle/ref_driver.cpp; 1 = short-term
-                                        error channels 0 (its default), 2 = hash-derived raw values there (tests/cpp/uncertainty_search_driver.cpp) */
+                                        error channels 0 (its default), 2 = hash-derived raw values there (tests/cpp/uncertainty_search_driver.cpp),
+                                        3 = the table net: each game's evaluations return the raw outputs set by kgb_selfplay_debug_set_raw_outputs,
+                                        4 = the wide hash net of oracle/ref_driver.cpp (KGREF_FAKE_WIDE=1): the same hash, wider output ranges */
   int32_t disable_ladder_features;   /* 1 = leave NN input planes 14-17 zero (timing experiments only) */
   int32_t ladder_nodes_per_wave;     /* > 0: each of a game's 8 ladder-reader warps plays at most this many search moves per wave;
                                         a game whose searches are unfinished skips the wave (no visit) and resumes in the next.
@@ -331,6 +333,15 @@ KGB_API int kgb_selfplay_get_root_value_stats(kgb_selfplay* sp, int game, double
 /* NodeStats weightSum and weightSqSum of game g's root (root_weights[2]) and of its children by move position
  * (child_weights[(X*Y+1)*2], 0 where there is no child): 1 per evaluation unless uncertainty weighting or noise pruning acts. */
 KGB_API int kgb_selfplay_get_root_weights(kgb_selfplay* sp, int game, double* child_weights, double* root_weights);
+/* Game g's root utility (white's perspective): utility[0] = the utility of its own evaluation (Search::getUtilityFromNN),
+ * utility[1] = NodeStats utilityAvg. */
+KGB_API int kgb_selfplay_get_root_utility(kgb_selfplay* sp, int game, double* utility);
+/* TEST ONLY (debug_fake_nn = 3): the raw net outputs every later evaluation of game g returns, in the evaluator's frame and from the
+ * mover's perspective as the net gives them: policy logits [X*Y+1] (pass last), value logits [3] (win, loss, no result),
+ * score-value channels [6] (mean, stdev before softplus, lead, variance of time left, short-term value and score errors before
+ * softplus), ownership logits [X*Y]. */
+KGB_API int kgb_selfplay_debug_set_raw_outputs(kgb_selfplay* sp, int game, const float* policy, const float* value, const float* score,
+                                               const float* ownership);
 /* TEST HOOK (row a20): the device loop's short-term error post-processing and evaluation weight on the host, n independent cases.
  * raw[n][2] = score-value channels 4 and 5 as the net outputs them; params[n][12] = shortterm value / score error multipliers,
  * uncertaintyCoeff, uncertaintyExponent, uncertaintyMaxWeight, winLossUtilityFactor, staticScoreUtilityFactor,

@@ -105,7 +105,10 @@ struct SPDev {
   // root policy temperature and Dirichlet noise (searchhelpers.cpp:78-215)
   // rootNumSymmetriesToSample (searchnnhelpers.cpp:95-101, nneval.cpp:811-838, nninputs.cpp:324-430): the root is evaluated under
   // several distinct symmetries, one per wave, and the post-processed outputs are averaged
-  int rootNumSymmetries, fakeNN;    // fakeNN: 0 the evaluator, 1 the hash net, 2 the hash net with raw short-term error channels
+  int rootNumSymmetries, fakeNN;    // fakeNN: 0 the evaluator, 1 the hash net, 2 the hash net with raw short-term error channels,
+                                    // 3 the table net: every evaluation of game g returns the raw outputs in fakeTable,
+                                    // 4 the wide hash net (same hash, wider output ranges)
+  float* fakeTable;                 // [game][policySize + 3 + 6 + XY] raw policy logits, value, score-value and ownership (fakeNN 3 only)
   int* rootSymCount;                // [game] evaluations of the current root accumulated so far
   int* rootSymOrder;                // [game][8] the sampled symmetry order
   float* rootSymAcc;                // [game][8] sums of whiteWin, whiteLoss, noResult, whiteScoreMean, whiteScoreMeanSq, whiteLead,
@@ -2115,6 +2118,15 @@ __global__ void spFakeNNKernel(const SPDev d, float* policyOut, float* valueOut,
   const int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if(g >= d.numGames) return;
+  if(d.fakeNN == 3) {   // the table net: the outputs the host chose for this game (kgb_selfplay_debug_set_raw_outputs), whatever the position
+    const float* t = d.fakeTable + (size_t)g * (d.policySize + 9 + d.XY);
+    for(int i = lane; i < d.policySize; i += 32) policyOut[(size_t)g * d.policySize + i] = t[i];
+    if(lane < 3) valueOut[g * 3 + lane] = t[d.policySize + lane];
+    if(lane < 6) scoreOut[g * 6 + lane] = t[d.policySize + 3 + lane];
+    if(ownershipOut != nullptr)
+      for(int i = lane; i < d.XY; i += 32) ownershipOut[(size_t)g * d.XY + i] = t[d.policySize + 9 + i];
+    return;
+  }
   const float* row = d.nnSpatial + (size_t)g * d.XY * 22;
   uint64_t h = 0;
   for(int pos = lane; pos < d.XY; pos += 32) {
@@ -2125,16 +2137,27 @@ __global__ void spFakeNNKernel(const SPDev d, float* policyOut, float* valueOut,
   for(int o = 16; o > 0; o >>= 1) h += __shfl_xor_sync(KGB_FULL, h, o);
   if(d.nnGlobal[(size_t)g * 19 + 5] < 0.0f) h ^= 0xABCDEFULL;
   if(d.nnSymmetry[g] != 0) h ^= splitmix64(0x5151ULL + (uint64_t)d.nnSymmetry[g]);   // outputs differ per symmetry, in the original orientation
+  const bool wide = d.fakeNN == 4;   // oracle/ref_driver.cpp with KGREF_FAKE_WIDE=1: the same hash, outputs over wider ranges
   for(int i = lane; i < d.policySize; i += 32) {
     uint32_t u = (uint32_t)(splitmix64(h + (uint64_t)(i + 1) * 0x9E3779B97F4A7C15ULL) >> 48);
-    float logit = (float)u * (1.0f / 8192.0f) - 4.0f;
+    float logit = wide ? (float)u * (3.0f / 4096.0f) - 24.0f : (float)u * (1.0f / 8192.0f) - 4.0f;
+    if(wide && (u & 15u) == 0u) logit -= 96.0f;   // one point in 16 far below the rest: its exp underflows to 0 in float
     if(i == d.policySize - 1) logit -= 3.0f;
     policyOut[(size_t)g * d.policySize + i] = logit;
   }
   if(ownershipOut != nullptr)   // raw ownership logits in [-4,4) per point, mover's perspective (oracle/ref_driver.cpp's fake net)
     for(int i = lane; i < d.XY; i += 32)
       ownershipOut[(size_t)g * d.XY + i] = (float)(uint32_t)(splitmix64(h + (uint64_t)(i + 1) * 0xD1B54A32D192ED03ULL) >> 48) * (1.0f / 8192.0f) - 4.0f;
-  if(lane == 0) {
+  if(lane == 0 && wide) {   // win, loss and no result from [-6,6), stdev pre-softplus from [-8,56), mean and lead from [-3,3)
+    valueOut[g * 3 + 0] = (float)(uint32_t)(splitmix64(h ^ 0x1111ULL) >> 48) * (3.0f / 16384.0f) - 6.0f;
+    valueOut[g * 3 + 1] = (float)(uint32_t)(splitmix64(h ^ 0x2222ULL) >> 48) * (3.0f / 16384.0f) - 6.0f;
+    valueOut[g * 3 + 2] = (float)(uint32_t)(splitmix64(h ^ 0x8888ULL) >> 48) * (3.0f / 16384.0f) - 6.0f;
+    scoreOut[g * 6 + 0] = (float)(uint32_t)(splitmix64(h ^ 0x3333ULL) >> 48) * (3.0f / 32768.0f) - 3.0f;
+    scoreOut[g * 6 + 1] = (float)(uint32_t)(splitmix64(h ^ 0x4444ULL) >> 48) * (1.0f / 1024.0f) - 8.0f;
+    scoreOut[g * 6 + 2] = (float)(uint32_t)(splitmix64(h ^ 0x5555ULL) >> 48) * (3.0f / 32768.0f) - 3.0f;
+    scoreOut[g * 6 + 3] = 0.0f; scoreOut[g * 6 + 4] = 0.0f; scoreOut[g * 6 + 5] = 0.0f;
+  }
+  else if(lane == 0) {
     valueOut[g * 3 + 0] = (float)(uint32_t)(splitmix64(h ^ 0x1111ULL) >> 48) * (1.0f / 8192.0f) - 4.0f;
     valueOut[g * 3 + 1] = (float)(uint32_t)(splitmix64(h ^ 0x2222ULL) >> 48) * (1.0f / 8192.0f) - 4.0f;
     valueOut[g * 3 + 2] = -30.0f;
@@ -2588,8 +2611,9 @@ static void initLoop(kgb_selfplay* sp, const kgb_selfplay_config& c) {
   d.gEverOcc = sp->alloc<uint32_t>(G * 32); d.rootBanned = sp->alloc<uint32_t>(G * 32);
   d.pKo = sp->alloc<unsigned long long>(G * d.pathCap); d.pPassB = sp->alloc<unsigned long long>(G * d.pathCap); d.pPassW = sp->alloc<unsigned long long>(G * d.pathCap);
   d.holdAtMaxVisits = c.debug_hold_at_max_visits ? 1 : 0;
-  if(c.debug_fake_nn < 0 || c.debug_fake_nn > 2) throw std::invalid_argument("selfplay: debug_fake_nn must be 0, 1 or 2");
+  if(c.debug_fake_nn < 0 || c.debug_fake_nn > 4) throw std::invalid_argument("selfplay: debug_fake_nn must be 0 to 4");
   d.fakeNN = c.debug_fake_nn;
+  d.fakeTable = d.fakeNN == 3 ? sp->alloc<float>(G * (PS + 9 + (size_t)X * Y)) : nullptr;
   d.rootNumSymmetries = c.root_num_symmetries_to_sample > 1 ? (c.root_num_symmetries_to_sample > 8 ? 8 : c.root_num_symmetries_to_sample) : 1;
   d.rootSymCount = sp->alloc<int>(G); d.rootSymOrder = sp->alloc<int>(G * 8); d.rootSymAcc = sp->alloc<float>(G * 8);
   d.rootNoiseEnabled = c.root_noise_enabled ? 1 : 0;
@@ -2816,6 +2840,35 @@ KGB_API int kgb_selfplay_get_root_weights(kgb_selfplay* sp, int game, double* ch
       child_weights[i * 2 + 1] = child[i] >= 0 ? wsq[child[i]] : 0.0;
     }
     root_weights[0] = ws[0]; root_weights[1] = wsq[0];
+  });
+}
+
+KGB_API int kgb_selfplay_get_root_utility(kgb_selfplay* sp, int game, double* utility) {
+  return guarded([&] {
+    if(!sp || !utility) throw std::invalid_argument("kgb_selfplay_get_root_utility: NULL argument");
+    sp->enter();
+    const SPDev& d = sp->d;
+    sp->checkGame(game);
+    sp->download(utility, d.nodeNNUtil + (size_t)game * d.maxNodes, 1);
+    sp->download(utility + 1, d.nodeUtilAvg + (size_t)game * d.maxNodes, 1);
+  });
+}
+
+KGB_API int kgb_selfplay_debug_set_raw_outputs(kgb_selfplay* sp, int game, const float* policy, const float* value, const float* score,
+                                               const float* ownership) {
+  return guarded([&] {
+    if(!sp || !policy || !value || !score || !ownership) throw std::invalid_argument("kgb_selfplay_debug_set_raw_outputs: NULL argument");
+    sp->enter();
+    const SPDev& d = sp->d;
+    sp->checkGame(game);
+    if(d.fakeNN != 3) throw std::invalid_argument("kgb_selfplay_debug_set_raw_outputs: the loop was not created with debug_fake_nn = 3");
+    const size_t stride = (size_t)d.policySize + 9 + d.XY;
+    float* t = d.fakeTable + (size_t)game * stride;
+    sp->upload(t, policy, d.policySize);
+    sp->upload(t + d.policySize, value, 3);
+    sp->upload(t + d.policySize + 3, score, 6);
+    sp->upload(t + d.policySize + 9, ownership, d.XY);
+    sp->sync();
   });
 }
 

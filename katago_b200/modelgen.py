@@ -118,10 +118,12 @@ def _nested(w, rng, name, c, cmid, cg: Optional[int], act, ninner=2):
 
 def model_bytes(config: str, seed: int = 0, name: Optional[str] = None, activation: str = "ACTIVATION_MISH",
                 version: int = 15, num_input_channels: int = 22, num_global: int = 19, meta_channels: int = 0,
-                meta_out_gain: float = 1.0) -> bytes:
+                meta_out_gain: float = 1.0, postprocess: Optional[tuple] = None) -> bytes:
     """meta_channels > 0 adds an SGF-metadata encoder of that internal width (metaEncoderVersion 1, as the reference's
     `-meta` configs export it: desc.cpp:1571-1617, export_model_pytorch.py write_metadata_encoder), drawn from its own generator so
-    that the trunk and heads equal those of the net without it; meta_out_gain scales its last layer (0: an encoder that adds nothing)."""
+    that the trunk and heads equal those of the net without it; meta_out_gain scales its last layer (0: an encoder that adds nothing).
+    postprocess: the 7 ModelPostProcessParams multipliers of a version >= 13 net (td score, score mean, score stdev, lead, variance of
+    time, short-term value error, short-term score error; desc.cpp:2476-2512), instead of the exporter's defaults."""
     cfg = CONFIGS[config]
     if meta_channels and version < 15:
         raise ValueError("SGF-metadata encoders need model version >= 15")
@@ -134,7 +136,7 @@ def model_bytes(config: str, seed: int = 0, name: Optional[str] = None, activati
     w.line(num_input_channels)
     w.line(num_global)
     if version >= 13:
-        w.line(20.0, 20.0, 20.0, 20.0, 40.0, 0.25, 30.0)
+        w.line(*(postprocess or (20.0, 20.0, 20.0, 20.0, 40.0, 0.25, 30.0)))
     if version >= 15:
         w.line(1 if meta_channels else 0, 0, 0, 0, 0, 0, 0, 0)
     w.line("trunk")

@@ -91,6 +91,7 @@ ABI_SYMBOLS = [
     "kgb_selfplay_set_game_setup", "kgb_selfplay_get_game_setup", "kgb_selfplay_play_moves_game",
     "kgb_selfplay_set_next_search_limits", "kgb_selfplay_get_search_limits", "kgb_selfplay_set_policy_init", "kgb_selfplay_get_policy_init",
     "kgb_selfplay_get_root_raw_policy_entropy", "kgb_selfplay_get_nn_symmetries", "kgb_selfplay_get_root_weights", "kgb_test_uncertainty_weight",
+    "kgb_selfplay_get_root_utility", "kgb_selfplay_debug_set_raw_outputs",
 ]
 
 _lib = None
@@ -173,6 +174,8 @@ def load_library():
     lib.kgb_selfplay_random_openings.argtypes = [P, I]
     lib.kgb_selfplay_get_root_value_stats.argtypes = [P, I, P, P]
     lib.kgb_selfplay_get_root_weights.argtypes = [P, I, P, P]
+    lib.kgb_selfplay_get_root_utility.argtypes = [P, I, P]
+    lib.kgb_selfplay_debug_set_raw_outputs.argtypes = [P, I, P, P, P, P]
     lib.kgb_test_uncertainty_weight.argtypes = [I, P, P, P, P]
     lib.kgb_selfplay_release.argtypes = [P, P]
     lib.kgb_selfplay_get_root_visits.argtypes = [P, P]
@@ -721,6 +724,21 @@ class SelfPlay:
         ch = np.zeros((self.x * self.y + 1, 5), np.float64); rt = np.zeros(5, np.float64)
         _check(load_library().kgb_selfplay_get_root_value_stats(self._p, g, ch.ctypes.data, rt.ctypes.data))
         return ch, rt
+
+    def root_utility(self, g: int):
+        """(utility of the root's own evaluation, NodeStats utilityAvg) of game g, white's perspective."""
+        out = np.zeros(2, np.float64)
+        _check(load_library().kgb_selfplay_get_root_utility(self._p, g, out.ctypes.data))
+        return float(out[0]), float(out[1])
+
+    def debug_set_raw_outputs(self, g: int, policy, value, score, ownership=None):
+        """debug_fake_nn = 3: every later evaluation of game g returns these raw net outputs (frame-indexed policy logits [X*Y+1],
+        value logits [3], score-value channels [6], ownership logits [X*Y]; mover's perspective)."""
+        n = self.x * self.y
+        arrs = [np.ascontiguousarray(a, np.float32).reshape(-1) for a in (policy, value, score, np.zeros(n) if ownership is None else ownership)]
+        if [a.size for a in arrs] != [n + 1, 3, 6, n]:
+            raise ValueError(f"raw outputs of sizes {[a.size for a in arrs]}, want {[n + 1, 3, 6, n]}")
+        _check(load_library().kgb_selfplay_debug_set_raw_outputs(self._p, g, *(a.ctypes.data for a in arrs)))
 
     def root_weights(self, g: int):
         """(children [X*Y+1, 2], root [2]): NodeStats weightSum and weightSqSum of game g's root children and root."""

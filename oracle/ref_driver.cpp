@@ -5,7 +5,9 @@
 //   kgref_driver searchfake MODELFILE X Y MAXVISITS "x,y x,y pass ..." [STATIC DYNAMIC ZEROWEIGHT SCALE]
 //       reference Search (search/search.cpp) with the deterministic hash-based fake net defined below as its NeuralNet
 //       backend (this file IS the backend TU of the driver); prints the root children's visit counts.  The device loop
-//       has the same fake net (kgb_selfplay_config.debug_fake_nn) so tree parity is tested without any real net.
+//       has the same fake net (kgb_selfplay_config.debug_fake_nn) so tree parity is tested without any real net.  With env
+//       KGREF_FAKE_TABLE=<file> the net is the table net instead: fixed raw outputs read from the file (debug_fake_nn = 3); with
+//       KGREF_FAKE_WIDE=1 the wide hash net (debug_fake_nn = 4), and the counts of the branches its evaluations took.
 //   kgref_driver featstream X Y MULTISUICIDE KOMI "x,y x,y pass ..." EVERY OUT.bin
 //       NNInputs::fillRowV7 (neuralnet/nninputs.cpp:2288-2731) rows along a game played through BoardHistory with the rule
 //       subset of the device loop (area scoring, simple ko, no tax): after every EVERY-th move writes the NHWC row + globals.
@@ -13,6 +15,8 @@
 //       random legal move stream on a reference Board (game/board.h): after every move records the board, ko, capture
 //       counters, pos_hash, per-stone liberty counts, the legality mask of the player to move next and the Benson pass-alive /
 //       territory area (Board::calculateArea, all flags on).
+#include <fstream>
+
 #include "game/board.h"
 #include "game/boardhistory.h"
 #include "game/rules.h"
@@ -127,6 +131,17 @@ static inline uint64_t splitmix64(uint64_t x) {
   x = (x ^ (x >> 27)) * 0x94D049BB133111EBULL;
   return x ^ (x >> 31);
 }
+// The table net (env KGREF_FAKE_TABLE=<file> of searchfake): every evaluation returns the raw outputs listed in the file, whatever the
+// position - policy logits [nnXLen*nnYLen+1], value logits [3], score-value channels [6], ownership logits [nnXLen*nnYLen], as text floats
+// (the device loop's debug_fake_nn = 3 is given the same numbers)
+static std::vector<float> fakeTable;
+// The wide hash net (env KGREF_FAKE_WIDE=1 of searchfake; the device loop's debug_fake_nn = 4): the same hash with wider output
+// ranges, and how many of its evaluations took each branch of the post-processing that the narrow net never reaches: P(no result)
+// > 0.05; superko removing a no-result probability > 0.05; stdev logit > 40 (linear softplus branch); a policy term whose exp
+// underflows to 0 in float
+static bool fakeWide = false;
+static bool fakeSuperko = false;
+static long long wideBranches[4] = {0, 0, 0, 0};
 #ifndef KGREF_EXTERNAL_BACKEND   // kgref_driver_b200 (oracle/Makefile.drivers) links integration/b200backend.cpp instead: the same commands on a real net
 struct LoadedModel { ModelDesc modelDesc; };
 struct ComputeContext { int nnXLen, nnYLen; };
@@ -157,6 +172,20 @@ InputBuffers* NeuralNet::createInputBuffers(const LoadedModel*, int, int, int) {
 void NeuralNet::freeInputBuffers(InputBuffers* b) { delete b; }
 void NeuralNet::getOutput(ComputeHandle* h, InputBuffers*, int n, NNResultBuf** inputBufs, vector<NNOutput*>& outputs) {
   const int xy = h->nnXLen * h->nnYLen;
+  if(!fakeTable.empty()) {
+    if(fakeTable.size() != (size_t)(2 * xy + 10)) throw StringError("KGREF_FAKE_TABLE: wrong number of values for the frame");
+    for(int r = 0; r < n; r++) {
+      NNOutput* o = outputs[r];
+      const float* t = fakeTable.data();
+      std::copy(t, t + xy + 1, o->policyProbs);
+      t += xy + 1;
+      o->whiteWinProb = t[0]; o->whiteLossProb = t[1]; o->whiteNoResultProb = t[2];
+      o->whiteScoreMean = t[3]; o->whiteScoreMeanSq = t[4]; o->whiteLead = t[5];
+      o->varTimeLeft = t[6]; o->shorttermWinlossError = t[7]; o->shorttermScoreError = t[8];
+      if(o->whiteOwnerMap != NULL) std::copy(t + 9, t + 9 + xy, o->whiteOwnerMap);
+    }
+    return;
+  }
   for(int r = 0; r < n; r++) {
     const float* sp = inputBufs[r]->rowSpatialBuf.data();
     const float* gl = inputBufs[r]->rowGlobalBuf.data();
@@ -169,12 +198,32 @@ void NeuralNet::getOutput(ComputeHandle* h, InputBuffers*, int n, NNResultBuf** 
     // a net that answers differently per requested symmetry (always in the original orientation), for rootNumSymmetriesToSample
     if(inputBufs[r]->symmetry != 0) hsh ^= splitmix64(0x5151ULL + (uint64_t)inputBufs[r]->symmetry);
     NNOutput* o = outputs[r];
+    float maxLogit = -1e30f;
     for(int i = 0; i <= xy; i++) {
       uint32_t u = (uint32_t)(splitmix64(hsh + (uint64_t)(i + 1) * 0x9E3779B97F4A7C15ULL) >> 48);
-      float logit = (float)u * (1.0f / 8192.0f) - 4.0f;
+      float logit = fakeWide ? (float)u * (3.0f / 4096.0f) - 24.0f : (float)u * (1.0f / 8192.0f) - 4.0f;
+      if(fakeWide && (u & 15u) == 0u) logit -= 96.0f;
       if(i == xy) logit -= 3.0f;
       o->policyProbs[i] = logit;
+      maxLogit = std::max(maxLogit, logit);
     }
+    if(fakeWide) {
+      o->whiteWinProb = (float)(uint32_t)(splitmix64(hsh ^ 0x1111ULL) >> 48) * (3.0f / 16384.0f) - 6.0f;
+      o->whiteLossProb = (float)(uint32_t)(splitmix64(hsh ^ 0x2222ULL) >> 48) * (3.0f / 16384.0f) - 6.0f;
+      o->whiteNoResultProb = (float)(uint32_t)(splitmix64(hsh ^ 0x8888ULL) >> 48) * (3.0f / 16384.0f) - 6.0f;
+      o->whiteScoreMean = (float)(uint32_t)(splitmix64(hsh ^ 0x3333ULL) >> 48) * (3.0f / 32768.0f) - 3.0f;
+      o->whiteScoreMeanSq = (float)(uint32_t)(splitmix64(hsh ^ 0x4444ULL) >> 48) * (1.0f / 1024.0f) - 8.0f;
+      o->whiteLead = (float)(uint32_t)(splitmix64(hsh ^ 0x5555ULL) >> 48) * (3.0f / 32768.0f) - 3.0f;
+      o->varTimeLeft = 0; o->shorttermWinlossError = 0; o->shorttermScoreError = 0;
+      const double w = o->whiteWinProb, l = o->whiteLossProb, nr = o->whiteNoResultProb, m = std::max(std::max(w, l), nr);
+      const double pNoResult = exp(nr - m) / (exp(w - m) + exp(l - m) + exp(nr - m));
+      if(pNoResult > 0.05) { wideBranches[0]++; if(fakeSuperko) wideBranches[1]++; }
+      if(o->whiteScoreMeanSq > 40.0f) wideBranches[2]++;
+      bool underflow = false;
+      for(int i = 0; i <= xy; i++) underflow = underflow || expf(o->policyProbs[i] - maxLogit) == 0.0f;
+      if(underflow) wideBranches[3]++;
+    }
+    else {
     o->whiteWinProb = (float)(uint32_t)(splitmix64(hsh ^ 0x1111ULL) >> 48) * (1.0f / 8192.0f) - 4.0f;
     o->whiteLossProb = (float)(uint32_t)(splitmix64(hsh ^ 0x2222ULL) >> 48) * (1.0f / 8192.0f) - 4.0f;
     o->whiteNoResultProb = -30.0f;
@@ -183,6 +232,7 @@ void NeuralNet::getOutput(ComputeHandle* h, InputBuffers*, int n, NNResultBuf** 
     o->whiteScoreMeanSq = (float)(uint32_t)(splitmix64(hsh ^ 0x4444ULL) >> 48) * (1.0f / 16384.0f) - 2.0f;
     o->whiteLead = (float)(uint32_t)(splitmix64(hsh ^ 0x5555ULL) >> 48) * (1.0f / 32768.0f) - 1.0f;
     o->varTimeLeft = 0; o->shorttermWinlossError = 0; o->shorttermScoreError = 0;
+    }
     // raw ownership logits in [-4,4) per point (mover's perspective; NNEvaluator applies tanh and the colour flip, nneval.cpp:1233-1250):
     // about half of the points end beyond |tanh| = 0.95, where Search::getEndingWhiteScoreBonus acts
     if(o->whiteOwnerMap != NULL)
@@ -207,6 +257,16 @@ static int cmdSearchFake(int argc, char** argv) {
   ConfigParser cfg;
   // KGREF_NN_CACHE_POW2 = -1 switches NNEvaluator's evaluation cache off (it is keyed by the situation, not the history: with a real net a
   // transposition then returns the output computed for another move order - fine for play, but not what a cache-less search sees)
+  if(getenv("KGREF_FAKE_TABLE")) {
+#ifdef KGREF_EXTERNAL_BACKEND
+    cerr << "KGREF_FAKE_TABLE needs the driver's own fake backend" << endl; return 1;
+#endif
+    std::ifstream in(getenv("KGREF_FAKE_TABLE"));
+    float v;
+    while(in >> v) fakeTable.push_back(v);
+    if(fakeTable.empty()) { cerr << "KGREF_FAKE_TABLE: no values read" << endl; return 1; }
+  }
+  fakeWide = getenv("KGREF_FAKE_WIDE") && atoi(getenv("KGREF_FAKE_WIDE")) != 0;
   const int cachePow2 = getenv("KGREF_NN_CACHE_POW2") ? atoi(getenv("KGREF_NN_CACHE_POW2")) : 10;
   // KGREF_NN_LEN = L: the evaluator's frame is L x L while the board is X x Y (nnXLen > board size: padded rows + mask, nneval.cpp:874-883;
   // BASELINE config 4 "mixed board sizes"); move positions and the policy are then indexed in the frame (NNPos::locToPos)
@@ -266,10 +326,18 @@ static int cmdSearchFake(int argc, char** argv) {
     else if(k == "subtreeValueBiasWeightExponent") params.subtreeValueBiasWeightExponent = v;
     else if(k == "rootEndingBonusPoints") params.rootEndingBonusPoints = v;
     else if(k == "rootPruneUselessMoves") params.rootPruneUselessMoves = v != 0;
+    else if(k == "noResultUtilityForWhite") params.noResultUtilityForWhite = v;
+    else if(k == "winLossUtilityFactor") params.winLossUtilityFactor = v;
+    else if(k == "drawEquivalentWinsForWhite") params.drawEquivalentWinsForWhite = v;
+    else if(k == "useUncertainty") params.useUncertainty = v != 0;
+    else if(k == "uncertaintyCoeff") params.uncertaintyCoeff = v;
+    else if(k == "uncertaintyExponent") params.uncertaintyExponent = v;
+    else if(k == "uncertaintyMaxWeight") params.uncertaintyMaxWeight = v;
     else { cerr << "unknown override " << k << endl; return 1; }
   }
   Rules rules;  // defaults, then the rule subset of the loop
   rules.koRule = koRuleOverride == 1 ? Rules::KO_POSITIONAL : koRuleOverride == 2 ? Rules::KO_SITUATIONAL : Rules::KO_SIMPLE;
+  fakeSuperko = rules.koRule != Rules::KO_SIMPLE;
   rules.scoringRule = Rules::SCORING_AREA; rules.taxRule = Rules::TAX_NONE;
   rules.multiStoneSuicideLegal = true; rules.hasButton = false; rules.whiteHandicapBonusRule = Rules::WHB_ZERO;
   rules.friendlyPassOk = false; rules.komi = 7.5f;
@@ -323,7 +391,11 @@ static int cmdSearchFake(int argc, char** argv) {
     }
     cout << endl;
   }
+  cout << "rootweight " << Global::strprintf("%.17g %.17g", root->stats.weightSum.load(), root->stats.weightSqSum.load()) << endl;
   const NNOutput* nn = root->getNNOutput();
+  // the root's own evaluation as NNEvaluator post-processed it (nneval.cpp:1112-1215; white's perspective, floats)
+  cout << "nnoutput " << Global::strprintf("%.9g %.9g %.9g %.9g %.9g %.9g %.9g %.9g", nn->whiteWinProb, nn->whiteLossProb, nn->whiteNoResultProb,
+                                           nn->whiteScoreMean, nn->whiteScoreMeanSq, nn->whiteLead, nn->shorttermWinlossError, nn->shorttermScoreError) << endl;
   cout << "policy";
   for(int i = 0; i <= NX * NY; i++) cout << " " << Global::strprintf("%.9g", nn->getPolicyProbsMaybeNoised()[i]);
   cout << endl;
@@ -344,15 +416,19 @@ static int cmdSearchFake(int argc, char** argv) {
       int x = loc == Board::PASS_LOC ? -1 : Location::getX(loc, X), y = loc == Board::PASS_LOC ? -1 : Location::getY(loc, X);
       cout << "qtarget " << x << " " << y << " " << Global::strprintf("%.9g %.9g", (float)cv.winLossValue, (float)cv.expectedScore) << " " << cv.visits << endl;
     }
-    vector<PolicyTargetMove> pt; vector<Loc> locsBuf; vector<double> psvBuf;
-    Play::extractPolicyTarget(pt, search, root, locsBuf, psvBuf);
-    cout << "policytarget";
-    for(const PolicyTargetMove& m : pt) {
-      int x = m.loc == Board::PASS_LOC ? -1 : Location::getX(m.loc, X), y = m.loc == Board::PASS_LOC ? -1 : Location::getY(m.loc, X);
-      cout << " " << x << " " << y << " " << m.policyTarget;
+    if(children.getCapacity() > 0 && children[0].getIfAllocated() != NULL) {   // a 1-visit search has no child to take targets from
+      vector<PolicyTargetMove> pt; vector<Loc> locsBuf; vector<double> psvBuf;
+      Play::extractPolicyTarget(pt, search, root, locsBuf, psvBuf);
+      cout << "policytarget";
+      for(const PolicyTargetMove& m : pt) {
+        int x = m.loc == Board::PASS_LOC ? -1 : Location::getX(m.loc, X), y = m.loc == Board::PASS_LOC ? -1 : Location::getY(m.loc, X);
+        cout << " " << x << " " << y << " " << m.policyTarget;
+      }
+      cout << endl;
     }
-    cout << endl;
   }
+  if(fakeWide)
+    cout << "widebranches " << wideBranches[0] << " " << wideBranches[1] << " " << wideBranches[2] << " " << wideBranches[3] << endl;
   delete search;
   delete nnEval;
   return 0;
