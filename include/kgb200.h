@@ -245,9 +245,6 @@ typedef struct kgb_selfplay_config {
   int32_t nn_cache_size_power_of_two;             /* nnCacheSizePowerOfTwo: evaluation cache shared by the games of this GPU (0 = off) */
   int32_t root_num_symmetries_to_sample;          /* rootNumSymmetriesToSample (4): the root is evaluated under that many symmetries, one per wave */
   int32_t ko_rule;                                /* Rules::koRule: 0 simple, 1 positional superko, 2 situational superko, 3 spight (area scoring) */
-  int32_t full_history_rules;                     /* 1 = BoardHistory's game-end rules also under simple ko: a pass in a situation the same
-                                                     player already passed in ends the game, a third repetition since the last pass is "no
-                                                     result".  Implied by ko_rule != 0.  0 = two consecutive passes only. */
   double root_ending_bonus_points;                /* rootEndingBonusPoints (0.5 in the stock configs): at the root, moves into territory the net's
                                                      ownership head is sure about (|ownership| >= 0.95) lose up to this many points of score
                                                      utility unless they capture / touch the opponent / connect groups that are not pass-alive
@@ -369,7 +366,7 @@ KGB_API int kgb_selfplay_get_komi(kgb_selfplay* sp, float* current, float* last_
  * move positions stay y * nn_x_len + x (NNPos::locToPos, neuralnet/nninputs.cpp:27-33), input plane 0 marks the board and the conv
  * trunk masks everything outside it (nneval.cpp:874-883 does the same with nnXLen > board size).  The values become each slot's NEXT
  * game's; also_current_games != 0 applies them to the games in progress too, which must not have started (no move, no visit) -
- * KGB_ERR_INVALID otherwise, nothing changed for those.  A ko rule different from the configuration's needs full_history_rules = 1.
+ * KGB_ERR_INVALID otherwise, nothing changed for those.
  * kgb_selfplay_get_game_setup: setup of the game in progress and of the slot's last finished game (either pointer may be NULL).
  * The evaluation cache keys on board size and rules as NNInputs::getHash does, so such games never share an entry. */
 KGB_API int kgb_selfplay_set_game_setup(kgb_selfplay* sp, const int32_t* setup, int also_current_games);

@@ -123,7 +123,6 @@ inline kgb_selfplay_config configFromCfg(const Cfg& c, int numGames) {
   // rules, board size and komi are drawn per game (b200_gameinit.h); the loop's own configuration carries the first listed values
   k.ko_rule = koRuleOf(c.list("koRules", "SIMPLE")[0]);
   k.multi_stone_suicide_legal = boolOf("multiStoneSuicideLegals", c.list("multiStoneSuicideLegals", "true")[0]) ? 1 : 0;
-  k.full_history_rules = 1;
   c.supportedOf("scoringRules", "AREA", {"AREA"}); c.supportedOf("taxRules", "NONE", {"NONE"}); c.supportedOf("hasButtons", "false", {"false"});
   c.neutral("handicapProb", "0.0"); c.neutral("compensateAfterPolicyInitProb", "0.0"); c.neutral("sekiForkHackProb", "0.0");
   c.neutral("handicapAsymmetricPlayoutProb", "0.0"); c.neutral("normalAsymmetricPlayoutProb", "0.0"); c.neutral("switchNetsMidGame", "true");
@@ -204,7 +203,7 @@ inline void printConfig(const kgb_selfplay_config& c) {
   FD(root_policy_temperature); FD(root_policy_temperature_early); FD(chosen_move_temperature_halflife); FI(use_play_selection); FI(use_lcb_for_selection);
   FI(use_non_buggy_lcb); FD(lcb_stdevs); FD(min_visit_prop_for_lcb); FD(chosen_move_temperature); FD(chosen_move_temperature_early);
   FD(chosen_move_temperature_only_below_prob); FD(chosen_move_subtract); FD(chosen_move_prune); FI(nn_cache_size_power_of_two);
-  FI(root_num_symmetries_to_sample); FI(ko_rule); FI(full_history_rules); FD(root_ending_bonus_points); FI(root_prune_useless_moves);
+  FI(root_num_symmetries_to_sample); FI(ko_rule); FD(root_ending_bonus_points); FI(root_prune_useless_moves);
   FI(max_playouts_per_wave); FI(use_uncertainty); FD(uncertainty_coeff); FD(uncertainty_exponent); FD(uncertainty_max_weight);
   FI(use_noise_pruning); FD(noise_prune_utility_scale); FD(noise_pruning_cap);
 #undef FI

@@ -32,7 +32,6 @@ inline kgb_selfplay_config configFromSearchParams(const SearchParams& p, const R
   c.komi = rules.komi;
   c.multi_stone_suicide_legal = rules.multiStoneSuicideLegal ? 1 : 0;
   c.ko_rule = rules.koRule == Rules::KO_POSITIONAL ? 1 : rules.koRule == Rules::KO_SITUATIONAL ? 2 : rules.koRule == Rules::KO_SPIGHT ? 3 : 0;
-  c.full_history_rules = 1;
   no(rules.scoringRule != Rules::SCORING_AREA, "scoringRule = " + Rules::writeScoringRule(rules.scoringRule));
   no(rules.taxRule != Rules::TAX_NONE, "taxRule = " + Rules::writeTaxRule(rules.taxRule));
   no(rules.hasButton, "hasButton = true");

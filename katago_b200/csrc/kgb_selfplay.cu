@@ -19,10 +19,10 @@
 // Backup = the reference's recompute (searchupdatehelpers.cpp:139-360): every node on the path re-derives its statistics from
 // its children (value weighting by the t-CDF of each child's z-score, :402-491) and its own evaluation.
 //
-// NN input planes written this round: 0 on-board, 1/2 own/opp stones, 3/4/5 liberties 1/2/3, 6 simple-ko ban,
+// NN input planes written this round: 0 on-board, 1/2 own/opp stones, 3/4/5 liberties 1/2/3, 6 simple-ko ban and superko bans,
 // 9-13 previous five move locations, 18/19 pass-alive + territory area (Benson, kgb_board.cuh); globals 0-4 pass history,
 // 5 selfKomi/20, 8 multi-stone suicide, 14 pass would end the phase, 18 komi parity wave; ladder planes 14-17 (kgb_ladder.cuh).
-// NOT written (stay 0, not reachable under the supported rule subset): superko bans in plane 6, encore planes 7/8/20/21.
+// NOT written (stay 0, not reachable under the supported rule subset): encore planes 7/8/20/21.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -51,8 +51,7 @@ static constexpr int SP_LADDER_WARPS = 8;   // warps per game in the select kern
 
 struct SPDev {
   // configuration
-  int X, Y, XY, policySize, numGames, maxVisits, maxNodes, maxDepth, maxMoves, multiSuicide, earlyMoves;
-  float komi;
+  int X, Y, XY, policySize, numGames, maxVisits, maxNodes, maxDepth, maxMoves, earlyMoves;
   // per-game board size and rules (GameInitializer::createGameSharedUnsynchronized, program/play.cpp:330-650 draws them per game): the
   // evaluator's frame is X x Y (nnXLen x nnYLen), a game's board gX x gY <= the frame sits in its top-left corner, move positions are
   // y * X + x in the frame (NNPos::locToPos, nninputs.cpp:27-33) and plane 0 marks the board.  setup arrays are [game][4] = X, Y, koRule, multiSuicide.
@@ -82,7 +81,7 @@ struct SPDev {
   double *biasDeltaSum, *biasWeightSum;   // [game][biasTableSize] SubtreeValueBiasEntry
   int* nodeBiasEntry;               // [game][maxNodes] slot or -1
   // full ko rules / game end (kgb_history.cuh): ko-hash history, pass situations, ever-occupied points, superko bans
-  int histRules, koRule, histCap, pathCap;
+  int histCap, pathCap;
   unsigned long long *gKo, *gPassB, *gPassW;   // [game][histCap]
   int *gKoLen, *gPassBLen, *gPassWLen;         // [game]
   uint32_t *gEverOcc, *rootBanned;             // [game][32]
@@ -101,7 +100,6 @@ struct SPDev {
   uint32_t* cacheLad;               // [cacheSize][32]
   unsigned long long *leafKey;      // [game][2] cache key of the current leaf
   unsigned long long *cacheHits, *cacheStores;
-  int trackPosHash;                 // graph search or cache: nodes carry their Zobrist position hash
   // root policy temperature and Dirichlet noise (searchhelpers.cpp:78-215)
   // rootNumSymmetriesToSample (searchnnhelpers.cpp:95-101, nneval.cpp:811-838, nninputs.cpp:324-430): the root is evaluated under
   // several distinct symmetries, one per wave, and the post-processed outputs are averaged
@@ -304,22 +302,19 @@ __device__ __forceinline__ void orderedAdd2(double a, double b, int n, double& a
 }
 
 // GraphHash::getStateHash (game/graphhash.cpp:4-24) for the rule subset: position, player to move, ko point, whether a pass
-// ends the phase, game over, consecutive passes.  (Own mixing constants: only equality of hashes matters to the search.)
-__device__ __forceinline__ void stateHash(unsigned long long posH0, unsigned long long posH1, bool nextBlack, int ko, int passes, bool gameOver,
-                                          unsigned long long& s0, unsigned long long& s1) {
+// ends the phase (passEnds: BoardHistory::passWouldEndPhase), game over, consecutive passes and the superko bans, which are part
+// of the situation (boardhistory.cpp:1238-1244).  (Own mixing constants: only equality of hashes matters to the search.)
+__device__ __forceinline__ void stateHashX(unsigned long long posH0, unsigned long long posH1, bool nextBlack, int ko, int passes, bool gameOver,
+                                           bool passEnds, unsigned long long bannedHash, unsigned long long& s0, unsigned long long& s1) {
   s0 = posH0 ^ (nextBlack ? 0x8F1BBCDCA62C1D6BULL : 0x5A827999ED9EBA1FULL);
   s1 = posH1 ^ (nextBlack ? 0xC3A5C85C97CB3127ULL : 0xB492B66FBE98F273ULL);
   if(ko >= 0) { const unsigned long long k = splitmix64((unsigned long long)ko + 0x51ED27ULL); s0 ^= k; s1 ^= splitmix64(k); }
-  if(passes >= 1) { s0 ^= 0x9AE16A3B2F90404FULL; s1 ^= 0xCBF29CE484222325ULL; }     // passWouldEndPhase
+  // passEnds enters as two XORs, one on each side of the pass count: reordering them would change every key, and with the
+  // keys which positions share an evaluation cache slot
+  if(passes >= 1) { s0 ^= 0x9AE16A3B2F90404FULL; s1 ^= 0xCBF29CE484222325ULL; }
   if(gameOver) { s0 ^= 0x2545F4914F6CDD1DULL; s1 ^= 0x106689D45497FDB5ULL; }
   s0 += 2862933555777941757ULL * (unsigned long long)passes;
   s1 += 3202034522624059733ULL * (unsigned long long)passes;
-}
-// The same with the full rules: a pass can also end the phase because the situation was passed in before, and the superko bans
-// are part of the situation (boardhistory.cpp:1238-1244).
-__device__ __forceinline__ void stateHashX(unsigned long long posH0, unsigned long long posH1, bool nextBlack, int ko, int passes, bool gameOver,
-                                           bool passEnds, unsigned long long bannedHash, unsigned long long& s0, unsigned long long& s1) {
-  stateHash(posH0, posH1, nextBlack, ko, passes, gameOver, s0, s1);
   if(passEnds != (passes >= 1)) { s0 ^= 0x9AE16A3B2F90404FULL; s1 ^= 0xCBF29CE484222325ULL; }
   s0 ^= bannedHash; s1 ^= splitmix64(bannedHash + 0x1234567ULL) * (bannedHash != 0 ? 1ULL : 0ULL);
 }
@@ -344,19 +339,12 @@ __device__ __forceinline__ HistLists playoutLists(const SPDev& d, int g) {
 }
 // A fresh game: the history starts with the initial situation (BoardHistory::clear).
 __device__ __forceinline__ void gameHistReset(const SPDev& d, int g, int lane) {
-  if(!d.histRules) return;
   d.gEverOcc[g * 32 + lane] = 0; d.rootBanned[g * 32 + lane] = 0;
   if(lane == 0) { d.gKo[(size_t)g * d.histCap] = koHashOf(d.gKoRule[g], 0ULL, true); d.gKoLen[g] = 1; d.gPassBLen[g] = 0; d.gPassWLen[g] = 0; }
 }
-// One move of the GAME (root): board, Zobrist hash, pass count and - with the full rules - the game's lists, bans and end flags.
+// One move of the GAME (root): board, Zobrist hash, pass count, the game's lists, bans and end flags.
 __device__ void gameMakeMove(const SPDev& d, int g, WarpBoard& bd, int p, bool black, int lane, int& passes, bool& finished, bool& noResult) {
   if(lane == 0) d.passStreak[g * 2 + (black ? 0 : 1)] = p < 0 ? d.passStreak[g * 2 + (black ? 0 : 1)] + 1 : 0;
-  if(!d.histRules) {
-    boardPlay(bd, p, black, d.zob);
-    passes = p < 0 ? passes + 1 : 0;
-    finished = passes >= 2; noResult = false;
-    return;
-  }
   HistLists L = gameLists(d, g);
   HistState st;
   st.passes = passes; st.finished = false; st.noResult = false; st.everOcc = d.gEverOcc[g * 32 + lane]; st.banned = 0;
@@ -406,18 +394,15 @@ __device__ __forceinline__ void nodeTableClear(const SPDev& d, int g, int lane) 
 __device__ __forceinline__ void rootHashesInit(const SPDev& d, int g, int lane) {
   const size_t gb = (size_t)g * d.maxNodes;
   const unsigned long long h0 = d.rootPosH[g * 2], h1 = d.rootPosH[g * 2 + 1];
+  WarpBoard bd;
+  boardInit(bd, d.gX[g], d.gY[g]);
+  bd.h0 = h0;
+  HistLists L = playoutLists(d, g);
+  HistState st;
+  st.passes = d.consecPasses[g]; st.finished = false; st.noResult = false; st.everOcc = 0; st.banned = d.rootBanned[g * 32 + lane];
+  const bool black = d.rootBlackToMove[g] != 0;
   unsigned long long s0, s1;
-  if(!d.histRules) stateHash(h0, h1, d.rootBlackToMove[g] != 0, d.rootKo[g], d.consecPasses[g], false, s0, s1);
-  else {
-    WarpBoard bd;
-    boardInit(bd, d.gX[g], d.gY[g]);
-    bd.h0 = h0;
-    HistLists L = playoutLists(d, g);
-    HistState st;
-    st.passes = d.consecPasses[g]; st.finished = false; st.noResult = false; st.everOcc = 0; st.banned = d.rootBanned[g * 32 + lane];
-    const bool black = d.rootBlackToMove[g] != 0;
-    stateHashX(h0, h1, black, d.rootKo[g], st.passes, false, histPassWouldEndPhase(bd, st, L, black, d.gKoRule[g]), pointSetHash(st.banned), s0, s1);
-  }
+  stateHashX(h0, h1, black, d.rootKo[g], st.passes, false, histPassWouldEndPhase(bd, st, L, black, d.gKoRule[g]), pointSetHash(st.banned), s0, s1);
   if(lane == 0) { d.nodePosH0[gb] = h0; d.nodePosH1[gb] = h1; d.nodeGH0[gb] = s0; d.nodeGH1[gb] = s1; }
 }
 // The transposition table emptied and the root node's hashes set from the stored root position.
@@ -844,12 +829,11 @@ __device__ void spSelectWarp0(const SPDev& d, int g, int lane, uint32_t* shB, ui
   const size_t G32 = (size_t)d.numGames * 32;
   WarpBoard bd;
   bool black = true, terminal = false, gotLeaf = false;
-  int passes = 0, h0 = -1, h1 = -1, h2 = -1, h3 = -1, h4 = -1, node = 0, depth = 0;
+  int h0 = -1, h1 = -1, h2 = -1, h3 = -1, h4 = -1, node = 0, depth = 0;
   uint32_t lad1 = 0, lad2 = 0;
-  HistLists HL = playoutLists(d, g);
-  HistState hst;
-  hst.passes = 0; hst.finished = false; hst.noResult = false; hst.everOcc = 0; hst.banned = 0;
-  bool bannedValid = false;     // hst.banned belongs to the current position
+  HistLists HL;                 // BoardHistory along the playout (kgb_history.cuh): the game's lists + the path part, and the
+  HistState hst;                // pass count, end flags and bans of the current position
+  bool bannedValid;             // hst.banned belongs to the current position
   const long long tW0 = clock64();
 #ifdef KGB_PROFILE_DESCENT
   long long pfGather = 0, pfSelect = 0, pfMove = 0, pfEdge = 0, pfSteps = 0, pfT = clock64(), pfBackup = 0, pfAttempts = 0, pfAdvance = 0;
@@ -869,10 +853,9 @@ __device__ void spSelectWarp0(const SPDev& d, int g, int lane, uint32_t* shB, ui
     { const long long t_ = clock64(); pfAdvance += t_ - pfT; pfT = t_; }
 #endif
   }
-  rootBoardLoad(d, g, lane, bd, d.histRules != 0);   // under the full rules the hash follows the whole path: ko hashes are taken from it
+  rootBoardLoad(d, g, lane, bd, true);   // the hash follows the whole path: ko hashes are taken from it
   const bool rootBlack = d.rootBlackToMove[g] != 0;
   black = rootBlack;
-  passes = d.consecPasses[g];
   h0 = d.hist[g * 5 + 0]; h1 = d.hist[g * 5 + 1]; h2 = d.hist[g * 5 + 2]; h3 = d.hist[g * 5 + 3]; h4 = d.hist[g * 5 + 4];
   // boards one and two moves ago (ladder planes 15/16): the root's recent boards, shifted as the descent plays moves.
   // Their laddered stones were computed when those positions were leaves themselves (a node's board is its child's
@@ -880,12 +863,10 @@ __device__ void spSelectWarp0(const SPDev& d, int g, int lane, uint32_t* shB, ui
   lad1 = d.prevLad[g * 32 + lane]; lad2 = d.prevLad[G32 + g * 32 + lane];
   node = 0; depth = 0;
   terminal = false;
-  if(d.histRules) {
-    HL = playoutLists(d, g);
-    hst.passes = passes; hst.finished = false; hst.noResult = false;
-    hst.everOcc = d.gEverOcc[g * 32 + lane]; hst.banned = d.rootBanned[g * 32 + lane];
-    bannedValid = true;
-  }
+  HL = playoutLists(d, g);
+  hst.passes = d.consecPasses[g]; hst.finished = false; hst.noResult = false;
+  hst.everOcc = d.gEverOcc[g * 32 + lane]; hst.banned = d.rootBanned[g * 32 + lane];
+  bannedValid = true;
   bool instant = false;   // this playout ended on an existing edge: back it up here, no leaf
 #ifdef KGB_PROFILE_DESCENT   // build variant for tests/gpu_checks/descent_profile.py: where a descent step spends its cycles
   pfAttempts++;
@@ -1055,20 +1036,12 @@ __device__ void spSelectWarp0(const SPDev& d, int g, int lane, uint32_t* shB, ui
     if(d.subtreeValueBiasFactor != 0.0 && d.childNode[nb + move] < 0 && !isPass && h0 != -1) biasKeyNew = biasEntryKey(bd, d.gX[g], d.gY[g], black, h0, p);
     int child = d.childNode[nb + move];
     const bool newEdge = child < 0;
-    if(d.histRules) {
-      // BoardHistory::makeBoardMoveAssumeLegal along the path: pass situations, ko-hash history, game end by repetition rules
-      histMakeMove(bd, hst, HL, p, black, d.gKoRule[g], d.gMultiSuicide[g] != 0, d.zob, false);
-      bannedValid = false;
-      if(newEdge && d.gKoRule[g] != KGB_KO_SIMPLE) {
-        hst.banned = histSuperKoBanned(bd, HL, hst.everOcc, !black, d.gKoRule[g], d.gMultiSuicide[g] != 0, d.zob);
-        bannedValid = true;
-      }
-      passes = hst.passes;
-    }
-    else {
-    if(newEdge && d.trackPosHash) { bd.h0 = d.nodePosH0[gb + node]; bd.h1 = d.nodePosH1[gb + node]; }
-    boardPlay(bd, p, black, (newEdge && d.trackPosHash) ? d.zob : nullptr);
-    passes = isPass ? passes + 1 : 0;
+    // BoardHistory::makeBoardMoveAssumeLegal along the path: pass situations, ko-hash history, game end by repetition rules
+    histMakeMove(bd, hst, HL, p, black, d.gKoRule[g], d.gMultiSuicide[g] != 0, d.zob, false);
+    bannedValid = false;
+    if(newEdge && d.gKoRule[g] != KGB_KO_SIMPLE) {
+      hst.banned = histSuperKoBanned(bd, HL, hst.everOcc, !black, d.gKoRule[g], d.gMultiSuicide[g] != 0, d.zob);
+      bannedValid = true;
     }
     h4 = h3; h3 = h2; h2 = h1; h1 = h0; h0 = isPass ? -2 : p;
     black = !black;
@@ -1079,10 +1052,8 @@ __device__ void spSelectWarp0(const SPDev& d, int g, int lane, uint32_t* shB, ui
       int tableSlot = -1, found = -1;
       if(d.useGraphSearch) {
         unsigned long long s0, s1;
-        if(d.histRules)
-          stateHashX(bd.h0, bd.h1, black, bd.ko, passes, hst.finished, histPassWouldEndPhase(bd, hst, HL, black, d.gKoRule[g]),
-                     d.gKoRule[g] != KGB_KO_SIMPLE ? pointSetHash(hst.banned) : 0ULL, s0, s1);
-        else stateHash(bd.h0, bd.h1, black, bd.ko, passes, passes >= 2, s0, s1);
+        stateHashX(bd.h0, bd.h1, black, bd.ko, hst.passes, hst.finished, histPassWouldEndPhase(bd, hst, HL, black, d.gKoRule[g]),
+                   d.gKoRule[g] != KGB_KO_SIMPLE ? pointSetHash(hst.banned) : 0ULL, s0, s1);
         graphHashOfChild(d.nodeGH0[gb + node], d.nodeGH1[gb + node], s0, s1, simpleRepetitionBoundGt(bd, p, d.graphSearchRepBound), cg0, cg1);
         found = nodeTableFind(d, g, cg0, cg1, tableSlot);
       }
@@ -1098,10 +1069,10 @@ __device__ void spSelectWarp0(const SPDev& d, int g, int lane, uint32_t* shB, ui
         d.nodeNumChildren[gb + node] = nc + 1;
         if(found < 0) {
           d.nodeCount[g] = child + 1;
-          nodeStatsReset(d, gb + child, d.histRules ? hst.finished : passes >= 2);
-          if(d.histRules && hst.noResult) d.nodeTerminal[gb + child] = 2;
+          nodeStatsReset(d, gb + child, hst.finished);
+          if(hst.noResult) d.nodeTerminal[gb + child] = 2;
           if(biasKeyNew != 0) d.nodeBiasEntry[gb + child] = biasFindOrInsert(d, g, biasKeyNew);
-          if(d.trackPosHash) { d.nodePosH0[gb + child] = bd.h0; d.nodePosH1[gb + child] = bd.h1; }
+          d.nodePosH0[gb + child] = bd.h0; d.nodePosH1[gb + child] = bd.h1;
           if(d.useGraphSearch) {
             const size_t ts = (size_t)g * d.nodeTableSize + tableSlot;
             d.nodeTableKey0[ts] = cg0; d.nodeTableKey1[ts] = cg1; d.nodeTableNode[ts] = child;
@@ -1142,10 +1113,8 @@ __device__ void spSelectWarp0(const SPDev& d, int g, int lane, uint32_t* shB, ui
   if(d.cacheSize > 0 && d.nodeTerminal[gb + node] == 0 && d.nodeVisits[gb + node] == 0 && !(node == 0 && rootSyms(d, g) > 1)) {
     // NNEvaluator::evaluate's cache lookup (nneval.cpp:861-905): the key is the situation, not the history behind it
     unsigned long long k0, k1;
-    if(d.histRules)
-      stateHashX(d.nodePosH0[gb + node], d.nodePosH1[gb + node], black, bd.ko, passes >= 1 ? 1 : 0, false, histPassWouldEndPhase(bd, hst, HL, black, d.gKoRule[g]),
-                 (d.gKoRule[g] != KGB_KO_SIMPLE && bannedValid) ? pointSetHash(hst.banned) : 0ULL, k0, k1);
-    else stateHash(d.nodePosH0[gb + node], d.nodePosH1[gb + node], black, bd.ko, passes >= 1 ? 1 : 0, false, k0, k1);
+    stateHashX(d.nodePosH0[gb + node], d.nodePosH1[gb + node], black, bd.ko, hst.passes >= 1 ? 1 : 0, false, histPassWouldEndPhase(bd, hst, HL, black, d.gKoRule[g]),
+               (d.gKoRule[g] != KGB_KO_SIMPLE && bannedValid) ? pointSetHash(hst.banned) : 0ULL, k0, k1);
     {
       // NNInputs::getHash (nninputs.cpp:869-943) = situation + rules + the mover's komi (boardhistory.cpp:1268-1274) + evaluation
       // options.  Komi varies from game to game inside one loop, so it is part of the key; scoring / tax rules, policy optimism and
@@ -1187,7 +1156,7 @@ __device__ void spSelectWarp0(const SPDev& d, int g, int lane, uint32_t* shB, ui
   uint32_t lib1, lib2, lib3;
   boardLibertyClasses(bd, lib1, lib2, lib3);
   uint32_t superKo = 0;
-  if(d.histRules && d.gKoRule[g] != KGB_KO_SIMPLE) {
+  if(d.gKoRule[g] != KGB_KO_SIMPLE) {
     if(!bannedValid) { hst.banned = histSuperKoBanned(bd, HL, hst.everOcc, black, d.gKoRule[g], d.gMultiSuicide[g] != 0, d.zob); bannedValid = true; }
     superKo = hst.banned;
   }
@@ -1239,7 +1208,7 @@ __device__ void spSelectWarp0(const SPDev& d, int g, int lane, uint32_t* shB, ui
     }
   }
   __syncwarp();
-  const bool passEndsLeaf = d.histRules ? histPassWouldEndPhase(bd, hst, HL, black, d.gKoRule[g]) : passes >= 1;
+  const bool passEndsLeaf = histPassWouldEndPhase(bd, hst, HL, black, d.gKoRule[g]);
   if(lane == 0) {
     if(bd.ko >= 0) row[(size_t)posOf(bd.ko, d.X) * 22 + 6] = 1.0f;
     // history planes 9..13: the move k plies ago must have been made by the right colour, which alternation guarantees
@@ -2215,7 +2184,7 @@ __global__ void spRandomOpeningsKernel(const SPDev d, int maxLen) {
   for(unsigned m = 0; m < len; m++) {
     uint32_t l1, l2, l3;
     boardLibertyClasses(rp.bd, l1, l2, l3);
-    const uint32_t legal = boardLegalMask(rp.bd, rp.black, d.gMultiSuicide[g] != 0, l1) & ~(d.histRules ? d.rootBanned[g * 32 + lane] : 0u);
+    const uint32_t legal = boardLegalMask(rp.bd, rp.black, d.gMultiSuicide[g] != 0, l1) & ~d.rootBanned[g * 32 + lane];
     const int n = warpCount(legal);
     if(n == 0) break;
     unsigned r = 0;
@@ -2348,7 +2317,7 @@ __global__ void historyReplayKernel(int X, int Y, int koRule, int multiSuicide, 
 // Board size and ko / suicide rules per game (GameInitializer::createGameSharedUnsynchronized, program/play.cpp:330-650: bSizes /
 // bSizeRelProbs, koRules, multiStoneSuicideLegals drawn per game).  setup[numGames][4] = X, Y, ko rule, multi-stone suicide: taken by each slot's
 // NEXT game; with alsoCurrent also by the game in progress, which must not have started (no move played, root not searched) - its history
-// restarts under the new rules.  Ko rules other than the loop's own need full_history_rules (BoardHistory's lists are per game already).
+// restarts under the new rules.
 __global__ void spApplySetupKernel(const SPDev d, int* refused) {
   const int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
@@ -2527,8 +2496,7 @@ static void initLoop(kgb_selfplay* sp, const kgb_selfplay_config& c) {
   d.numGames = c.num_games; d.maxVisits = c.max_visits; d.maxNodes = c.max_visits + 2;
   d.maxDepth = std::min(c.max_visits + 2, 512);
   d.maxMoves = c.max_moves > 0 ? c.max_moves : 2 * X * Y;
-  d.multiSuicide = c.multi_stone_suicide_legal; d.earlyMoves = c.early_temperature_moves;
-  d.komi = c.komi;
+  d.earlyMoves = c.early_temperature_moves;
   {
     std::vector<float> k((size_t)c.num_games, (float)c.komi);
     d.komiG = sp->alloc<float>(c.num_games); d.nextKomi = sp->alloc<float>(c.num_games); d.lastKomi = sp->alloc<float>(c.num_games);
@@ -2601,9 +2569,6 @@ static void initLoop(kgb_selfplay* sp, const kgb_selfplay_config& c) {
   d.nodeUtilSqAvg = sp->alloc<double>(G * N); d.nodeNNUtil = sp->alloc<double>(G * N); d.nodeNumChildren = sp->alloc<int>(G * N);
   d.childOrder = sp->alloc<uint16_t>(G * N * PS);
   d.nodeMoments = sp->alloc<double>(G * N * 5); d.nodeNNMoments = sp->alloc<double>(G * N * 5); d.leafMoments = sp->alloc<double>(G * 5);
-  d.koRule = c.ko_rule;
-  if(d.koRule < 0 || d.koRule > 3) throw std::invalid_argument("selfplay: ko_rule must be 0 (simple), 1 (positional), 2 (situational) or 3 (spight)");
-  d.histRules = (c.full_history_rules || d.koRule != 0) ? 1 : 0;
   d.histCap = (d.maxMoves > 1024 ? d.maxMoves : 1024) + 16;   // also holds openings given by kgb_selfplay_play_moves (up to 1024 moves)
   d.pathCap = d.maxDepth + 8;
   d.gKo = sp->alloc<unsigned long long>(G * d.histCap); d.gPassB = sp->alloc<unsigned long long>(G * d.histCap); d.gPassW = sp->alloc<unsigned long long>(G * d.histCap);
@@ -2649,7 +2614,6 @@ static void initLoop(kgb_selfplay* sp, const kgb_selfplay_config& c) {
     d.cachePolicy = sp->alloc<float>(S * PS); d.cacheVals = sp->alloc<float>(S * 8); d.cacheLad = sp->alloc<uint32_t>(S * 32);
   }
   d.leafKey = sp->alloc<unsigned long long>(G * 2);
-  d.trackPosHash = (c.use_graph_search || d.cacheSize > 0) ? 1 : 0;
   d.useGraphSearch = c.use_graph_search ? 1 : 0; d.graphSearchRepBound = c.graph_search_rep_bound;
   d.nodeTableSize = 64;
   while(d.nodeTableSize < 2 * (int)N) d.nodeTableSize *= 2;
@@ -2928,7 +2892,6 @@ KGB_API int kgb_selfplay_set_game_setup(kgb_selfplay* sp, const int32_t* setup, 
       const int* q = setup + (size_t)g * 4;
       if(q[0] < 2 || q[0] > d.X || q[1] < 2 || q[1] > d.Y) throw std::invalid_argument("selfplay: a game's board must be at least 2x2 and fit the evaluator's frame");
       if(q[2] < 0 || q[2] > 3) throw std::invalid_argument("selfplay: ko_rule must be 0 (simple), 1 (positional), 2 (situational) or 3 (spight)");
-      if(q[2] != d.koRule && !d.histRules) throw std::invalid_argument("selfplay: per-game ko rules need full_history_rules = 1 (or a superko rule) in the loop's configuration");
       if(q[3] != 0 && q[3] != 1) throw std::invalid_argument("selfplay: multi_stone_suicide_legal must be 0 or 1");
     }
     sp->upload(d.nextSetup, setup, (size_t)d.numGames * 4);

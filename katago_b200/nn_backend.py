@@ -62,7 +62,7 @@ class SelfplayConfig(C.Structure):
         ("chosen_move_temperature_early", C.c_double), ("chosen_move_temperature_only_below_prob", C.c_double),
         ("chosen_move_subtract", C.c_double), ("chosen_move_prune", C.c_double),
         ("nn_cache_size_power_of_two", C.c_int32), ("root_num_symmetries_to_sample", C.c_int32),
-        ("ko_rule", C.c_int32), ("full_history_rules", C.c_int32), ("root_ending_bonus_points", C.c_double),
+        ("ko_rule", C.c_int32), ("root_ending_bonus_points", C.c_double),
         ("use_uncertainty", C.c_int32), ("uncertainty_coeff", C.c_double), ("uncertainty_exponent", C.c_double),
         ("uncertainty_max_weight", C.c_double), ("use_noise_pruning", C.c_int32), ("noise_prune_utility_scale", C.c_double),
         ("noise_pruning_cap", C.c_double),
@@ -637,11 +637,15 @@ class SelfPlay:
                  lcb_stdevs: float = 4.0, min_visit_prop_for_lcb: float = 0.05, chosen_move_temperature: float = 0.0,
                  chosen_move_temperature_early: float = 0.0, chosen_move_temperature_only_below_prob: float = 1.0,
                  chosen_move_subtract: float = 0.0, chosen_move_prune: float = 1.0, nn_cache_size_power_of_two: int = 0, root_num_symmetries_to_sample: int = 1,
-                 ko_rule: int = 0, full_history_rules: bool = False, debug_fixed_symmetry: int = -1,
+                 ko_rule: int = 0, full_history_rules: bool = True, debug_fixed_symmetry: int = -1,
                  root_ending_bonus_points: float = 0.0, root_prune_useless_moves: bool = False,
                  use_uncertainty: bool = False, uncertainty_coeff: float = 0.25, uncertainty_exponent: float = 1.0,
                  uncertainty_max_weight: float = 8.0, use_noise_pruning: bool = False, noise_prune_utility_scale: float = 0.15,
                  noise_pruning_cap: float = 1e50):
+        # The loop always plays BoardHistory's game-end rules.  full_history_rules stays a keyword because bench.py passes it;
+        # False is refused rather than silently ignored.
+        if not full_history_rules:
+            raise ValueError("SelfPlay: the loop always plays the full game-end rules; full_history_rules=False is not supported")
         lib = load_library()
         self.handle = handle
         self.cfg = SelfplayConfig(num_games, max_visits, max_moves, int(multi_stone_suicide_legal), early_temperature_moves, komi,
@@ -659,7 +663,7 @@ class SelfPlay:
                                   int(use_play_selection), int(use_lcb_for_selection), int(use_non_buggy_lcb), int(root_prune_useless_moves), lcb_stdevs, min_visit_prop_for_lcb,
                                   chosen_move_temperature, chosen_move_temperature_early, chosen_move_temperature_only_below_prob,
                                   chosen_move_subtract, chosen_move_prune, int(nn_cache_size_power_of_two), int(root_num_symmetries_to_sample),
-                                  int(ko_rule), int(full_history_rules), float(root_ending_bonus_points),
+                                  int(ko_rule), float(root_ending_bonus_points),
                                   int(use_uncertainty), float(uncertainty_coeff), float(uncertainty_exponent), float(uncertainty_max_weight),
                                   int(use_noise_pruning), float(noise_prune_utility_scale), float(noise_pruning_cap))
         self._p = C.c_void_p()

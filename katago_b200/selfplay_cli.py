@@ -150,7 +150,6 @@ def selfplay_kwargs_from_cfg(cfg, strict=False):
     # configuration carries the first listed ko / suicide rule as its default
     kos = [_KO_RULES[v.upper()] for v in _supported_values(cfg, "koRules", set(_KO_RULES), report, "SIMPLE")]
     kw["ko_rule"] = kos[0]
-    kw["full_history_rules"] = True
     _supported_values(cfg, "scoringRules", {"AREA"}, report, "AREA")
     _supported_values(cfg, "taxRules", {"NONE"}, report, "NONE")
     _supported_values(cfg, "hasButtons", {"false"}, report, "false")

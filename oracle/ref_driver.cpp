@@ -1050,7 +1050,7 @@ static int cmdParamsMap(int argc, char** argv) {
   FD(root_policy_temperature); FD(root_policy_temperature_early); FD(chosen_move_temperature_halflife); FI(use_play_selection); FI(use_lcb_for_selection);
   FI(use_non_buggy_lcb); FD(lcb_stdevs); FD(min_visit_prop_for_lcb); FD(chosen_move_temperature); FD(chosen_move_temperature_early);
   FD(chosen_move_temperature_only_below_prob); FD(chosen_move_subtract); FD(chosen_move_prune); FI(nn_cache_size_power_of_two);
-  FI(root_num_symmetries_to_sample); FI(ko_rule); FI(full_history_rules); FD(root_ending_bonus_points); FI(root_prune_useless_moves);
+  FI(root_num_symmetries_to_sample); FI(ko_rule); FD(root_ending_bonus_points); FI(root_prune_useless_moves);
 #undef FI
 #undef FD
   cout << "\"unsupported\":[";

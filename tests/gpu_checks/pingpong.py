@@ -18,7 +18,7 @@ KW = dict(komi=7.5, cpuct_exploration=1.05, cpuct_exploration_log=0.28, fpu_redu
           use_play_selection=True, use_lcb_for_selection=True, use_non_buggy_lcb=True, lcb_stdevs=5.0, min_visit_prop_for_lcb=0.15,
           chosen_move_temperature=0.15, chosen_move_temperature_early=0.75, static_score_utility_factor=0.05, dynamic_score_utility_factor=0.3,
           dynamic_score_center_zero_weight=0.25, dynamic_score_center_scale=0.5, ladder_nodes_per_wave=256, root_num_symmetries_to_sample=4,
-          full_history_rules=True, root_ending_bonus_points=0.5, root_prune_useless_moves=True)
+          root_ending_bonus_points=0.5, root_prune_useless_moves=True)
 
 
 def measure(pops, games_each):

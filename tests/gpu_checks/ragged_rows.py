@@ -101,7 +101,7 @@ def main():
             for ragged in (True, False):
                 h = handles[ragged][2]
                 loop = SelfPlay(h, N, 200, komi=7.5, seed=1 + run, use_graph_search=True, nn_cache_size_power_of_two=16,
-                                root_num_symmetries_to_sample=4, root_noise_enabled=True, full_history_rules=True)
+                                root_num_symmetries_to_sample=4, root_noise_enabled=True)
                 loop.set_game_setup(setups, also_current_games=True)
                 loop.set_game_setup(nxt)
                 loop.run(20)

@@ -18,7 +18,7 @@ SEARCH = dict(komi=7.5, cpuct_exploration=1.05, cpuct_exploration_log=0.28, root
               fpu_parent_weight_by_visited_policy=True, fpu_parent_weight_by_visited_policy_pow=2.0, root_desired_per_child_visits_coeff=2.0,
               subtree_value_bias_factor=0.30, subtree_value_bias_weight_exponent=0.8, use_graph_search=True, root_noise_enabled=True,
               root_dirichlet_noise_total_concentration=10.83, root_dirichlet_noise_weight=0.25, root_policy_temperature=1.1, root_policy_temperature_early=1.5,
-              root_num_symmetries_to_sample=4, nn_cache_size_power_of_two=20, full_history_rules=True, use_play_selection=True, use_lcb_for_selection=True,
+              root_num_symmetries_to_sample=4, nn_cache_size_power_of_two=20, use_play_selection=True, use_lcb_for_selection=True,
               use_non_buggy_lcb=True, lcb_stdevs=5.0, min_visit_prop_for_lcb=0.15, chosen_move_temperature=0.15, chosen_move_temperature_early=0.75,
               static_score_utility_factor=0.05, dynamic_score_utility_factor=0.30, dynamic_score_center_zero_weight=0.25, dynamic_score_center_scale=0.50)
 path = modelgen.write_model(os.path.join(tempfile.mkdtemp(), cfg + ".bin"), cfg, seed=0)

@@ -17,8 +17,7 @@ sp = SelfPlay(h, 256, 600, komi=7.5, seed=1234, cpuct_exploration=1.05, cpuct_ex
               root_noise_enabled=True, root_policy_temperature=1.1, root_policy_temperature_early=1.5, nn_cache_size_power_of_two=20,
               use_play_selection=True, use_lcb_for_selection=True, use_non_buggy_lcb=True, lcb_stdevs=5.0, min_visit_prop_for_lcb=0.15,
               chosen_move_temperature=0.15, chosen_move_temperature_early=0.75, static_score_utility_factor=0.05, dynamic_score_utility_factor=0.3,
-              dynamic_score_center_zero_weight=0.25, dynamic_score_center_scale=0.5, ladder_nodes_per_wave=cap, root_num_symmetries_to_sample=4,
-              full_history_rules=True)
+              dynamic_score_center_zero_weight=0.25, dynamic_score_center_scale=0.5, ladder_nodes_per_wave=cap, root_num_symmetries_to_sample=4)
 sp.random_openings(150)
 sp.run(700); h.sync()
 sp.debug_cycles(True)

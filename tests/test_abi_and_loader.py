@@ -104,6 +104,12 @@ def test_context_argument_checks(tmp_models):
         NeuralNet.createComputeContext([0], 19, 50, True, lm)
 
 
+def test_selfplay_refuses_the_two_pass_end_alone():
+    """The loop always plays BoardHistory's game-end rules: asking for the two-pass end alone is an error, not ignored."""
+    with pytest.raises(ValueError, match="full_history_rules"):
+        nn_backend.SelfPlay(None, 1, 2, full_history_rules=False)
+
+
 def test_synthetic_file_roundtrip_weights(tmp_models):
     """modelgen -> file -> oracle loader keeps the weights (format check incl. the @BIN@ blocks)."""
     a = orc.load_model(tmp_models["tiny_nbt"], apply_transform=False)

@@ -534,7 +534,7 @@ def test_cpp_recorder_against_python_recorder_on_scripted_slots(tmp_path, size, 
     G, V, NUM = 3, 20, 5
     c = SelfplayConfig()
     c.num_games, c.max_visits, c.max_moves, c.multi_stone_suicide_legal, c.komi, c.seed = G, V, max_moves, 1, komi, 5 + size
-    c.debug_hold_at_max_visits, c.draw_equivalent_wins_for_white, c.ko_rule, c.full_history_rules = 1, 0.5, ko_rule, 1
+    c.debug_hold_at_max_visits, c.draw_equivalent_wins_for_white, c.ko_rule = 1, 0.5, ko_rule
     (tmp_path / "cfg.bin").write_bytes(ctypes.string_at(ctypes.addressof(c), ctypes.sizeof(c)))
     (tmp_path / "model.bin").write_bytes(b"unused")
     log = tmp_path / "log.jsonl"
@@ -642,7 +642,7 @@ def test_recorder_turns_device_games_into_training_rows(tmp_path, tmp_models, ko
                   dynamic_score_center_zero_weight=0.25, dynamic_score_center_scale=0.5, use_play_selection=True, use_lcb_for_selection=True,
                   use_non_buggy_lcb=True, lcb_stdevs=5.0, min_visit_prop_for_lcb=0.15, chosen_move_temperature=0.15,
                   chosen_move_temperature_early=0.75, root_noise_enabled=True, root_dirichlet_noise_total_concentration=10.83,
-                  root_dirichlet_noise_weight=0.25, ko_rule=ko_rule, full_history_rules=True,
+                  root_dirichlet_noise_weight=0.25, ko_rule=ko_rule,
                   ladder_nodes_per_wave=(6 if mode == "pump" else 0))
     games = []
     writer = W.TrainingDataWriter(str(tmp_path), 4096, 1.0, L, "recorder-test")    # one file: rows stay in write order
@@ -755,7 +755,7 @@ def test_recorded_games_through_the_reference_writer(tmp_path, tmp_models, ko_ru
                   dynamic_score_center_zero_weight=0.25, dynamic_score_center_scale=0.5, use_play_selection=True, use_lcb_for_selection=True,
                   use_non_buggy_lcb=True, lcb_stdevs=5.0, min_visit_prop_for_lcb=0.15, chosen_move_temperature=0.15,
                   chosen_move_temperature_early=0.75, root_noise_enabled=True, root_dirichlet_noise_total_concentration=10.83,
-                  root_dirichlet_noise_weight=0.25, ko_rule=ko_rule, full_history_rules=True)
+                  root_dirichlet_noise_weight=0.25, ko_rule=ko_rule)
     cfg_path = tmp_path / "config.bin"
     cfg_path.write_bytes(ctypes.string_at(ctypes.addressof(sp.cfg), ctypes.sizeof(sp.cfg)))
     out_path = tmp_path / "reference_rows.txt"

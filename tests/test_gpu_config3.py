@@ -116,7 +116,7 @@ def test_search_1024_games_1600_visits_matches_reference(fixture_1600, tmp_model
     ctx = NeuralNet.createComputeContext([0], 19, 19, True, lm)
     h = NeuralNet.createComputeHandle(ctx, lm, GAMES, False, True, 0)
     sp = SelfPlay(h, GAMES, VISITS, komi=7.5, multi_stone_suicide_legal=True, early_temperature_moves=0, seed=1, debug_fake_nn=True,
-                  debug_hold_at_max_visits=True, full_history_rules=True, nn_cache_size_power_of_two=20, ladder_nodes_per_wave=256,
+                  debug_hold_at_max_visits=True, nn_cache_size_power_of_two=20, ladder_nodes_per_wave=256,
                   **_kwargs(json.loads(str(d["params"]))))
     _place(sp, d, {s: d[f"c{i}_moves"] for i, s in enumerate(FIXTURE_SLOTS)})
     slots = np.array(FIXTURE_SLOTS)
@@ -171,7 +171,7 @@ def _loop_record(handle, num_games, placed, fx, symmetry=0):
                   root_noise_enabled=True, root_dirichlet_noise_total_concentration=10.83, root_dirichlet_noise_weight=0.25,
                   root_policy_temperature=1.1, root_policy_temperature_early=1.5, chosen_move_temperature_halflife=19.0,
                   nn_cache_size_power_of_two=0, root_num_symmetries_to_sample=4, root_ending_bonus_points=0.5, root_prune_useless_moves=True,
-                  ko_rule=0, full_history_rules=True, use_play_selection=True, use_lcb_for_selection=True, use_non_buggy_lcb=True, lcb_stdevs=5.0,
+                  ko_rule=0, use_play_selection=True, use_lcb_for_selection=True, use_non_buggy_lcb=True, lcb_stdevs=5.0,
                   min_visit_prop_for_lcb=0.15, chosen_move_temperature=0.15, chosen_move_temperature_early=0.75, chosen_move_subtract=0.0,
                   chosen_move_prune=1.0, seed=1234, ladder_nodes_per_wave=256, static_score_utility_factor=0.05,
                   dynamic_score_utility_factor=0.30, dynamic_score_center_zero_weight=0.25, dynamic_score_center_scale=0.50,

@@ -161,7 +161,7 @@ def test_device_post_processing_matches_float64_and_the_reference(rows, tmp_path
         # max_visits 2 (the least the loop takes) and one wave: the wave evaluates each unvisited root once, like the reference's
         # 1-visit search
         sp = SelfPlay(h, len(grp), 2, komi=7.5, multi_stone_suicide_legal=True, early_temperature_moves=0, seed=1, debug_fake_nn=3,
-                      debug_hold_at_max_visits=True, full_history_rules=True, **kw)
+                      debug_hold_at_max_visits=True, **kw)
         sp.set_game_setup(np.array([[r["X"], r["Y"], r["ko"], 1] for r in grp], np.int32), also_current_games=True)
         for g, r in enumerate(grp):
             sp.play_moves_game(g, [None if m is None else tuple(m) for m in r["moves"]])
@@ -242,7 +242,7 @@ def test_wide_hash_net_searches_match_the_reference(tmp_models, case):
     ctx = NeuralNet.createComputeContext([0], frame or X, frame or Y, True, lm)
     h = NeuralNet.createComputeHandle(ctx, lm, 4, False, True, 0)
     sp = SelfPlay(h, 3, visits, komi=7.5, multi_stone_suicide_legal=True, early_temperature_moves=0, seed=1, debug_fake_nn=4,
-                  debug_hold_at_max_visits=True, full_history_rules=True, **kw)
+                  debug_hold_at_max_visits=True, **kw)
     if frame:
         sp.set_game_setup(np.array([[X, Y, params.get("koRule", 0), 1]] * 3, np.int32), also_current_games=True)
     sp.play_moves([None if m[0] < 0 else (int(m[0]), int(m[1])) for m in d[f"c{case}_moves"]])

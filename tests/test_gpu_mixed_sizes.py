@@ -41,7 +41,7 @@ def test_games_of_different_sizes_and_ko_rules_search_like_the_reference(golden_
     ctx = NeuralNet.createComputeContext([0], frame, frame, True, lm)
     h = NeuralNet.createComputeHandle(ctx, lm, 8, False, True, 0)
     sp = SelfPlay(h, n, visits, komi=7.5, multi_stone_suicide_legal=True, early_temperature_moves=0, seed=1, debug_fake_nn=True,
-                  debug_hold_at_max_visits=True, full_history_rules=True, **_kwargs(json.loads(str(d["params"]))))
+                  debug_hold_at_max_visits=True, **_kwargs(json.loads(str(d["params"]))))
     setups = np.stack([d[f"g{g}_setup"] for g in range(n)])
     sp.set_game_setup(setups, also_current_games=True)
     cur, _ = sp.game_setups()
@@ -113,7 +113,7 @@ def test_mixed_size_self_play_runs_games_to_the_end_and_takes_the_next_setup(tmp
     h = NeuralNet.createComputeHandle(ctx, lm, 8, False, True, 0)
     n = 6
     sp = SelfPlay(h, n, 12, komi=7.5, max_moves=60, seed=5, use_graph_search=True, value_weight_exponent=0.5, nn_cache_size_power_of_two=12,
-                  root_num_symmetries_to_sample=2, full_history_rules=True, debug_hold_at_max_visits=True)
+                  root_num_symmetries_to_sample=2, debug_hold_at_max_visits=True)
     first = np.array([[5, 5, 0, 1], [7, 7, 1, 0], [9, 9, 2, 1], [13, 13, 0, 1], [9, 5, 0, 0], [13, 7, 3, 1]], np.int32)
     nxt = np.array([[13, 13, 1, 0], [5, 5, 0, 1], [7, 9, 0, 1], [9, 9, 0, 0], [13, 13, 2, 1], [6, 6, 0, 1]], np.int32)
     komi1 = np.array([5.5, 6.0, 7.0, 7.5, -3.5, 0.5], np.float32)
@@ -162,7 +162,7 @@ def test_games_of_different_sizes_never_share_an_evaluation_cache_entry(tmp_mode
     lm = NeuralNet.loadModelFile(tmp_models["tiny_reg"])
     ctx = NeuralNet.createComputeContext([0], 13, 13, True, lm)
     h = NeuralNet.createComputeHandle(ctx, lm, 4, False, True, 0)
-    sp = SelfPlay(h, 4, 8, komi=7.5, seed=3, nn_cache_size_power_of_two=10, full_history_rules=True, debug_fixed_symmetry=0)
+    sp = SelfPlay(h, 4, 8, komi=7.5, seed=3, nn_cache_size_power_of_two=10, debug_fixed_symmetry=0)
     sp.set_game_setup(np.array([[9, 9, 0, 1], [13, 13, 0, 1], [9, 9, 1, 1], [9, 9, 0, 1]], np.int32), also_current_games=True)
     sp.play_moves([(2, 2), (3, 3)])
     sp.run(1)
@@ -181,7 +181,7 @@ def test_policy_initialised_openings(tmp_models, golden_dir):
     h = NeuralNet.createComputeHandle(ctx, lm, 64, False, True, 0)
     want = np.array([0, 3, 10, 5, 0, 7, 1, 12], np.int32)
     sp = SelfPlay(h, 8, 16, komi=7.5, seed=11, debug_hold_at_max_visits=True, nn_cache_size_power_of_two=10, root_num_symmetries_to_sample=2, root_noise_enabled=True,
-                  use_play_selection=True, full_history_rules=True)
+                  use_play_selection=True)
     sizes = np.array([[9, 9, 0, 1]] * 6 + [[7, 7, 0, 1], [9, 5, 0, 1]], np.int32)
     sp.set_game_setup(sizes, also_current_games=True)
     sp.set_policy_init(want, 1.0, also_current_games=True)

@@ -261,7 +261,7 @@ def run_loops(path, n, visits, iterations, max_moves, layouts=(True, False), cac
         eh = EnvHandle(path, n, {"KGB_RAGGED_ROWS": None if ragged else "0"})
         sp = SelfPlay(eh.h, n, visits, komi=7.5, max_moves=max_moves, seed=21, use_graph_search=True, nn_cache_size_power_of_two=cache,
                       root_num_symmetries_to_sample=4, root_noise_enabled=True, use_play_selection=True, chosen_move_temperature_early=0.75,
-                      chosen_move_temperature=0.15, full_history_rules=True, debug_hold_at_max_visits=True)
+                      chosen_move_temperature=0.15, debug_hold_at_max_visits=True)
         sp.set_game_setup(first, also_current_games=True)
         sp.set_game_setup(nxt)
         loops.append(sp); handles.append(eh)

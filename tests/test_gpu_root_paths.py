@@ -61,7 +61,7 @@ def _random_opening_lists(n, games, max_len, superko):
 
 
 def _loop(h, games, superko):
-    kw = dict(ko_rule=KO_POSITIONAL, full_history_rules=True) if superko else {}
+    kw = dict(ko_rule=KO_POSITIONAL) if superko else {}
     return SelfPlay(h, games, 8, komi=7.5, seed=SEED, debug_fake_nn=True, **kw)
 
 

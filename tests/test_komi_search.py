@@ -175,7 +175,7 @@ def test_lead_of_a_position_equals_the_reference_computeLead(golden_dir, stream,
     ctx = NeuralNet.createComputeContext([0], size, size, False, lm)
     h = NeuralNet.createComputeHandle(ctx, lm, 4, False, True, 0)
     kw = KomiSearcher.noiseless_kwargs(dict(cpuct_exploration=1.0, cpuct_exploration_log=0.45, cpuct_exploration_base=500.0, fpu_reduction_max=0.2, root_fpu_reduction_max=0.1))
-    sp = SelfPlay(h, 4, visits, komi=7.5, multi_stone_suicide_legal=True, seed=1, debug_hold_at_max_visits=True, debug_fixed_symmetry=0, full_history_rules=True, **kw)
+    sp = SelfPlay(h, 4, visits, komi=7.5, multi_stone_suicide_legal=True, seed=1, debug_hold_at_max_visits=True, debug_fixed_symmetry=0, **kw)
     ks = KomiSearcher(sp)
     got = []
     ks.submit(compute_lead(komi, size, size), (size, size, 0, 1), moves, got.append)

@@ -234,7 +234,7 @@ def test_two_loops_play_the_same_games_move_for_move(tmp_models):
         ctx = NeuralNet.createComputeContext([0], 9, 9, True, lm)
         h = NeuralNet.createComputeHandle(ctx, lm, 8, False, True, 0)
         owned += [h, ctx]
-        loops.append(SelfPlay(h, 6, 12 + 4 * i, komi=7.5, max_moves=40, seed=3 + i, use_graph_search=True, value_weight_exponent=0.5, full_history_rules=True,
+        loops.append(SelfPlay(h, 6, 12 + 4 * i, komi=7.5, max_moves=40, seed=3 + i, use_graph_search=True, value_weight_exponent=0.5,
                               debug_hold_at_max_visits=True, use_play_selection=True, chosen_move_temperature=0.2, chosen_move_temperature_early=0.5))
     init = GameInitializer([(5, 5), (7, 7), (9, 9), (9, 7)], [1, 1, 1, 1], ko_rules=(0, 1), multi_stone_suicide_legals=(False, True), komi_mean=6.5, komi_stdev=1.0, seed=4)
     games = []

@@ -48,7 +48,7 @@ def test_stock_training_config_maps_onto_the_loop(stock_cfg):
     assert kw["root_fpu_reduction_max"] == 0.0 and kw["value_weight_exponent"] == 0.5 and kw["use_graph_search"] is True
     assert kw["subtree_value_bias_factor"] == 0.30 and kw["root_num_symmetries_to_sample"] == 4 and kw["use_lcb_for_selection"] is True
     assert kw["root_policy_temperature_early"] == 1.5 and kw["chosen_move_temperature_halflife"] == 19.0 and kw["nn_cache_size_power_of_two"] == 24
-    assert kw["max_moves"] == 1600 and kw["ko_rule"] == 0 and kw["full_history_rules"] is True and kw["multi_stone_suicide_legal"] is False
+    assert kw["max_moves"] == 1600 and kw["ko_rule"] == 0 and kw["multi_stone_suicide_legal"] is False
     gi = data.pop("game_init")
     ks = data.pop("komi_search")
     fk = data.pop("forks")
