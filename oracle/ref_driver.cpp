@@ -11,6 +11,8 @@
 //   kgref_driver featstream X Y MULTISUICIDE KOMI "x,y x,y pass ..." EVERY OUT.bin
 //       NNInputs::fillRowV7 (neuralnet/nninputs.cpp:2288-2731) rows along a game played through BoardHistory with the rule
 //       subset of the device loop (area scoring, simple ko, no tax): after every EVERY-th move writes the NHWC row + globals.
+//   kgref_driver ladderrows IN.txt OUT.bin
+//       fillRowV7 rows of many positions (one per line of IN.txt) and the time of each position's slowest ladder search.
 //   kgref_driver boardstream X Y NMOVES SEED MULTISUICIDE OUT.bin
 //       random legal move stream on a reference Board (game/board.h): after every move records the board, ko, capture
 //       counters, pos_hash, per-stone liberty counts, the legality mask of the player to move next and the Benson pass-alive /
@@ -36,6 +38,7 @@
 #include "core/config_parser.h"
 #include "integration/b200params.h"
 #include "core/logger.h"
+#include "core/timer.h"
 
 #include <cstdint>
 #include <cstdio>
@@ -1328,6 +1331,80 @@ static int cmdFeatStream(int argc, char** argv) {
   return 0;
 }
 
+// ladderrows IN.txt OUT.bin: the fillRowV7 row of many positions in one process (tests/golden/make_ladder_fixtures.py).  Each line of
+// IN.txt is "X Y NX NY KORULE MULTISUICIDE move move ..." (moves "x,y" or "pass"), replayed through BoardHistory with the rules of
+// featstream (area scoring, no tax, komi 7.5); the row is written for an NX x NY frame with the board in its corner.  Per position OUT.bin
+// holds: int32 status (0, or 1 = a move was illegal), float32 microseconds of the slowest single ladder search of the final position (the
+// public Board::searchIsLadderCaptured / searchIsLadderCapturedAttackerFirst2Libs on a fresh copy, best of 3 runs: a search that
+// reaches the 25 000-node budget takes orders of magnitude longer than the rest, and the reference offers no other view of its node
+// count), int32 x, y of a stone of that chain, then the NX*NY*22 spatial values as uint8 (every V7 plane is 0/1) and 19 float32 globals.
+static int cmdLadderRows(int argc, char** argv) {
+  if(argc != 4) { cerr << "usage: ladderrows IN.txt OUT.bin" << endl; return 1; }
+  Board::initHash();
+  ScoreValue::initTables();
+  ifstream in(argv[2]);
+  ofstream out(argv[3], ios::binary);
+  string line;
+  int count = 0;
+  while(getline(in, line)) {
+    std::istringstream ls(line);
+    int X, Y, NX, NY, koRule, multi;
+    if(!(ls >> X >> Y >> NX >> NY >> koRule >> multi)) continue;
+    if(NX < X || NY < Y) { cerr << "frame smaller than the board: " << line << endl; return 1; }
+    Rules rules;
+    rules.koRule = koRule == 1 ? Rules::KO_POSITIONAL : koRule == 2 ? Rules::KO_SITUATIONAL : koRule == 3 ? Rules::KO_SPIGHT : Rules::KO_SIMPLE;
+    rules.scoringRule = Rules::SCORING_AREA; rules.taxRule = Rules::TAX_NONE;
+    rules.multiStoneSuicideLegal = multi != 0; rules.hasButton = false; rules.whiteHandicapBonusRule = Rules::WHB_ZERO;
+    rules.friendlyPassOk = false; rules.komi = 7.5f;
+    Board board(X, Y);
+    Player pla = P_BLACK;
+    BoardHistory hist(board, pla, rules, 0, false);
+    int32_t status = 0;
+    string tok;
+    while(ls >> tok) {
+      Loc loc;
+      if(tok == "pass") loc = Board::PASS_LOC;
+      else { int x, y; if(sscanf(tok.c_str(), "%d,%d", &x, &y) != 2) { cerr << "bad move " << tok << endl; return 1; } loc = Location::getLoc(x, y, X); }
+      if(hist.isGameFinished || !hist.isLegal(board, loc, pla)) { status = 1; break; }
+      hist.makeBoardMoveAssumeLegal(board, loc, pla, NULL);
+      pla = getOpp(pla);
+    }
+    float slowest = 0.0f;
+    int32_t sx = -1, sy = -1;
+    vector<Loc> buf, working;
+    for(int y = 0; y < Y && status == 0; y++)
+      for(int x = 0; x < X; x++) {
+        const Loc loc = Location::getLoc(x, y, X);
+        if(board.colors[loc] != P_BLACK && board.colors[loc] != P_WHITE) continue;
+        const int libs = board.getNumLiberties(loc);
+        if(libs != 1 && libs != 2) continue;
+        if(board.chain_head[loc] != loc) continue;   // one search per chain
+        double best = 1e30;
+        for(int rep = 0; rep < 3; rep++) {
+          Board copy(board);
+          ClockTimer timer;
+          if(libs == 1) copy.searchIsLadderCaptured(loc, true, buf);
+          else copy.searchIsLadderCapturedAttackerFirst2Libs(loc, buf, working);
+          best = std::min(best, timer.getSeconds());
+        }
+        if(best * 1e6 > slowest) { slowest = (float)(best * 1e6); sx = x; sy = y; }
+      }
+    vector<float> sp((size_t)NNInputs::NUM_FEATURES_SPATIAL_V7 * NX * NY), gl(NNInputs::NUM_FEATURES_GLOBAL_V7);
+    if(status == 0) {
+      MiscNNInputParams params;
+      NNInputs::fillRowV7(board, hist, pla, params, NX, NY, true, sp.data(), gl.data());
+    }
+    vector<uint8_t> bits(sp.size());
+    for(size_t i = 0; i < sp.size(); i++) bits[i] = sp[i] != 0.0f ? 1 : 0;
+    put<int32_t>(out, status); put<float>(out, slowest); put<int32_t>(out, sx); put<int32_t>(out, sy);
+    out.write((const char*)bits.data(), bits.size());
+    out.write((const char*)gl.data(), gl.size() * sizeof(float));
+    count++;
+  }
+  cerr << "wrote " << count << " rows" << endl;
+  return 0;
+}
+
 // computelead MODELFILE X Y VISITS KOMI MOVES: PlayUtils::computeLead (program/playutils.cpp:612-660) of the position after MOVES at KOMI, one bot,
 // the driver's default search parameters (as in searchfake), no evaluation cache, symmetry 0 - the komi-bisection searches that
 // katago_b200/komi_search.py restates as jobs on a side loop.  Prints "lead <value>" and, for the same position,
@@ -1479,6 +1556,7 @@ int main(int argc, char** argv) {
   if(cmd == "rungame") return cmdRunGame(argc, argv);
   if(cmd == "tinyfeatures") return cmdTinyFeatures(argc, argv);
   if(cmd == "featstream") return cmdFeatStream(argc, argv);
+  if(cmd == "ladderrows") return cmdLadderRows(argc, argv);
   if(cmd == "computelead") return cmdComputeLead(argc, argv);
   if(cmd == "komitable") return cmdKomiTable(argc, argv);
   if(cmd == "gameinit") return cmdGameInit(argc, argv);
