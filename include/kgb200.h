@@ -108,6 +108,14 @@ KGB_API int kgb_forward(kgb_handle* handle, int n, const float* spatial, const f
 KGB_API int kgb_forward_device(kgb_handle* handle, int n, const float* d_spatial, const float* d_global, const int32_t* d_symmetry,
                        const float* d_policy_optimism, float* d_policy, float* d_value, float* d_score_value,
                        float* d_ownership);
+/* Test hook: kgb_forward_device's ops one at a time, without the forward's graph, with a stream synchronise after each, so that no
+ * convolution launch overlaps the one before it.  Synchronous.  The chained forward must give bit-identical outputs. */
+KGB_API int kgb_test_forward_serial(kgb_handle* handle, int n, const float* d_spatial, const float* d_global, const int32_t* d_symmetry,
+                                    const float* d_policy_optimism, float* d_policy, float* d_value, float* d_score_value,
+                                    float* d_ownership);
+/* *out = 1 once a chained convolution launch of this process gave up waiting for the launch before it (a sticky word: every
+ * synchronising call reports it as KGB_ERR_CUDA from then on), else 0. */
+KGB_API int kgb_conv_chain_error(int* out);
 /* The same two entry points for an SGF-metadata (human SL) net (kgb_model_info.num_input_meta_channels = 192), with one more input:
  *   meta           [n][192]   NNResultBuf::rowMetaBuf (SGFMetadata::fillMetadataRow output)
  * The net's metadata encoder (three fully connected layers) turns each row into a per-image bias of the initial convolution, added
@@ -123,6 +131,8 @@ KGB_API int kgb_handle_sync(kgb_handle* handle);
 KGB_API uint64_t kgb_handle_stream(kgb_handle* handle);
 /* Number of kernel launches one kgb_forward of batch n issues (for bench.py's gpu_launches accounting); a metadata net's encoder adds 3. */
 KGB_API int kgb_handle_launches_per_forward(const kgb_handle* handle);
+/* Of those, the convolution launches that follow another convolution launch directly and start while it still runs (chained). */
+KGB_API int kgb_handle_chained_launches_per_forward(const kgb_handle* handle);
 /* The row layout the last forward or self-play wave on the handle used (waits for the handle's stream): the rows and 128-row
  * tiles every convolution ran over, and the number of segments (board widths).  Each image takes (h+pad)*(w+pad) rows for the
  * bounding box w x h of its mask, so a batch of small boards takes fewer rows than n*(nnYLen+pad)*(nnXLen+pad).  All zero

@@ -123,6 +123,31 @@ struct Builder {
   int actMul;  // 2 in split mode ([hi | lo])
   Builder(kgb_handle& hh) : h(hh), m(*hh.model), Mmax(hh.planRows(hh.maxBatch)), actMul(hh.split ? 2 : 1) {}
 
+  // Chaining (kgb_conv.cuh, launchConvWG): in a forward (build), a convolution op that directly follows another convolution op is
+  // launched as a programmatic dependent of it, with the previous op's flag slot as its predecessor.  The single-layer hooks emit
+  // ops that run one at a time, without a predecessor; nothing reads their flags, so these are never zeroed.
+  bool chain = false;
+  int lastConvOp = -1, lastConvSlot = -1, lastConvParts = 0;
+  // The flag slot of the next convolution op, and the slot and flag target of its predecessor (-1: none)
+  struct ChainLink {
+    int slot, pred, predParts;
+  };
+  ChainLink nextLink() {
+    const bool linked = chain && lastConvOp >= 0 && (size_t)lastConvOp + 1 == h.ops.size();
+    h.chainedLaunches += linked ? 1 : 0;
+    return ChainLink{h.chainSlots++, linked ? lastConvSlot : -1, linked ? lastConvParts : 0};
+  }
+  void linkConvOp(const ChainLink& l, int parts) {
+    lastConvOp = (int)h.ops.size() - 1;
+    lastConvSlot = l.slot;
+    lastConvParts = parts;
+  }
+  static void applyLink(const kgb_handle& hh, const ChainLink& l, ConvParams& p) {
+    p.tile_flags = hh.chainFlags(l.slot);
+    p.pred_flags = l.pred >= 0 ? hh.chainFlags(l.pred) : nullptr;
+    p.pred_parts = l.predParts;
+  }
+
   struct Level {
     int C = 0, cp = 0;
     bool fp32 = false;
@@ -247,9 +272,11 @@ struct Builder {
                           convParams(h, h.maxBatch, wpre, nullptr, false, nullptr, innerS, innerFp32, innerAOut, bn2)))
       return false;
     kgb_handle* hp = &h;
+    const ChainLink link = nextLink();
     h.ops.push_back([=](int n, cudaStream_t s) {
-      const ConvParams p1 = convParams(*hp, n, wpost, S, sFp32, nullptr, S, sFp32, nullptr, bn1);
+      ConvParams p1 = convParams(*hp, n, wpost, S, sFp32, nullptr, S, sFp32, nullptr, bn1);
       const ConvParams p2 = convParams(*hp, n, wpre, nullptr, false, nullptr, innerS, innerFp32, innerAOut, bn2);
+      applyLink(*hp, link, p1);
       ConvPairTmaps tm;
       memset(&tm, 0, sizeof(tm));
       tm.A = makeTmap2D(innerA, (uint64_t)p1.M, (uint64_t)wpost.cin_p, (uint32_t)convABoxRows(1, 1, p1.Wp));
@@ -260,6 +287,7 @@ struct Builder {
       tm.act2 = makeTmapSlices(innerAOut, (uint64_t)p1.M, (uint64_t)wpre.cout_p, false);
       CK(launchConvPair(tm, p1, p2, s));
     });
+    linkConvOp(link, kConvPairParts);
     h.launchesPerForward++;
     return true;
   }
@@ -275,8 +303,10 @@ struct Builder {
       throw std::logic_error("emitConv: the residual and the raw output differ in dtype");
     kgb_handle* hp = &h;
     const int actMulL = actMul;
+    const ChainLink link = nextLink();
     h.ops.push_back([=](int n, cudaStream_t s) {
-      const ConvParams p = convParams(*hp, n, cw, residual, residualFp32, ncbias, rawOut, rawFp32, actOut, bn);
+      ConvParams p = convParams(*hp, n, cw, residual, residualFp32, ncbias, rawOut, rawFp32, actOut, bn);
+      applyLink(*hp, link, p);
       ConvTmaps tm;
       memset(&tm, 0, sizeof(tm));
       tm.A = makeTmap2D(A, (uint64_t)p.M, (uint64_t)cw.cin_p * actMulL, (uint32_t)convABoxRows(cw.ky, cw.kx, p.Wp));
@@ -286,6 +316,7 @@ struct Builder {
       if(actOut != nullptr) tm.act = makeTmapSlices(actOut, (uint64_t)p.M, (uint64_t)cw.cout_p * actMulL, false);
       CK(launchConvWG(tm, p, s));
     });
+    linkConvOp(link, 2 * cw.num_n_tiles);
     h.launchesPerForward++;
   }
 
@@ -377,7 +408,9 @@ struct Builder {
     __half* inAct = h.dalloc<__half>(Mmax * cinP * actMul);
     kgb_handle* hp = &h;
     const int C = m.numInputChannels, split = h.split;
+    chain = true;
     h.ops.push_back([=](int n, cudaStream_t s) {
+      CK(cudaMemsetAsync(hp->chain, 0, (size_t)hp->chainSlots * hp->chainStride() * sizeof(int), s));
       CK(launchPlanRows(hp->dSpatial, n, C, hp->nhwc, hp->dSymmetry, hp->L, hp->plan, s));
       CK(launchPackInput(hp->dSpatial, n, C, hp->nhwc, hp->dSymmetry, hp->L, hp->plan, hp->planRows(n), inAct, cinP, split, hp->dMask,
                          hp->dMaskSum, s));
@@ -468,6 +501,7 @@ struct Builder {
                         hp->dValue, hp->dScore, s));
     });
     h.launchesPerForward += (version >= 15 ? 11 : 10);
+    h.allocChain();
     // constants the ops above captured by value, and the post-processing constants callers read from the model: a staged model
     // (kgb_handle_stage_weights) must agree on all of them
     char buf[512];
@@ -479,7 +513,16 @@ struct Builder {
   }
 };
 
-void runOps(kgb_handle* h, int n) {
+// serial: the ops one at a time, outside a graph, each followed by a stream synchronise - the reference the chained graph is
+// tested against (kgb_test_forward_serial)
+void runOps(kgb_handle* h, int n, bool serial = false) {
+  if(serial) {
+    for(auto& op : h->ops) {
+      op(n, h->stream);
+      CK(cudaStreamSynchronize(h->stream));
+    }
+    return;
+  }
   auto it = h->graphs.find(n);
   if(it == h->graphs.end())
     it = h->graphs.emplace(n, captureGraph(h->stream, [&] { for(auto& op : h->ops) op(n, h->stream); })).first;
@@ -855,6 +898,7 @@ KGB_API int kgb_handle_broadcast_staged_weights(kgb_handle* handle, int root, fl
 KGB_API int kgb_handle_is_fp16(const kgb_handle* handle) { return handle && !handle->split ? 1 : 0; }
 KGB_API uint64_t kgb_handle_stream(kgb_handle* handle) { return handle ? (uint64_t)(uintptr_t)handle->stream : 0; }
 KGB_API int kgb_handle_launches_per_forward(const kgb_handle* handle) { return handle ? handle->launchesPerForward : 0; }
+KGB_API int kgb_handle_chained_launches_per_forward(const kgb_handle* handle) { return handle ? handle->chainedLaunches : 0; }
 
 KGB_API int kgb_handle_get_layout_stats(kgb_handle* handle, int64_t* rows, int64_t* m_tiles, int64_t* segments) {
   return guarded([&] {
@@ -872,6 +916,7 @@ KGB_API int kgb_handle_sync(kgb_handle* handle) {
     if(!handle) throw std::invalid_argument("kgb_handle_sync: NULL handle");
     CK(cudaSetDevice(handle->device));
     CK(cudaStreamSynchronize(handle->stream));
+    CK(convChainStatus());
   });
 }
 
@@ -917,6 +962,7 @@ static void forwardHost(kgb_handle* h, int n, const float* spatial, const float*
   CK(cudaMemcpyAsync(h->hScore, h->dScore, (size_t)n * 6 * sizeof(float), cudaMemcpyDeviceToHost, s));
   if(ownership) CK(cudaMemcpyAsync(h->hOwnership, h->dOwnership, (size_t)n * XY * sizeof(float), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
+  CK(convChainStatus());
   memcpy(policy, h->hPolicy, (size_t)n * (XY + 1) * sizeof(float));
   memcpy(value, h->hValue, (size_t)n * 3 * sizeof(float));
   memcpy(score_value, h->hScore, (size_t)n * 6 * sizeof(float));
@@ -924,7 +970,8 @@ static void forwardHost(kgb_handle* h, int n, const float* spatial, const float*
 }
 
 static void forwardDevice(kgb_handle* h, int n, const float* d_spatial, const float* d_global, const float* d_meta, const int32_t* d_symmetry,
-                          const float* d_policy_optimism, float* d_policy, float* d_value, float* d_score_value, float* d_ownership) {
+                          const float* d_policy_optimism, float* d_policy, float* d_value, float* d_score_value, float* d_ownership,
+                          bool serial = false) {
   CK(cudaSetDevice(h->device));
   const ModelDesc& m = *h->model;
   const int XY = h->L.X * h->L.Y;
@@ -939,7 +986,7 @@ static void forwardDevice(kgb_handle* h, int n, const float* d_spatial, const fl
   else CK(cudaMemsetAsync(h->dSymmetry, 0, n * sizeof(int), s));
   if(d_policy_optimism) CK(cudaMemcpyAsync(h->dOptimism, d_policy_optimism, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
   else CK(cudaMemsetAsync(h->dOptimism, 0, n * sizeof(float), s));
-  runOps(h, n);
+  runOps(h, n, serial);
   CK(cudaMemcpyAsync(d_policy, h->dPolicy, (size_t)n * (XY + 1) * sizeof(float), cudaMemcpyDeviceToDevice, s));
   CK(cudaMemcpyAsync(d_value, h->dValue, (size_t)n * 3 * sizeof(float), cudaMemcpyDeviceToDevice, s));
   CK(cudaMemcpyAsync(d_score_value, h->dScore, (size_t)n * 6 * sizeof(float), cudaMemcpyDeviceToDevice, s));
@@ -970,6 +1017,23 @@ KGB_API int kgb_forward_device(kgb_handle* h, int n, const float* d_spatial, con
     checkForwardArgs(h, n, d_spatial, d_global, d_policy, d_value, d_score_value);
     checkMetaArgs(h, nullptr, "kgb_forward_device");
     forwardDevice(h, n, d_spatial, d_global, nullptr, d_symmetry, d_policy_optimism, d_policy, d_value, d_score_value, d_ownership);
+  });
+}
+
+KGB_API int kgb_test_forward_serial(kgb_handle* h, int n, const float* d_spatial, const float* d_global, const int32_t* d_symmetry,
+                                    const float* d_policy_optimism, float* d_policy, float* d_value, float* d_score_value, float* d_ownership) {
+  return guarded([&] {
+    checkForwardArgs(h, n, d_spatial, d_global, d_policy, d_value, d_score_value);
+    checkMetaArgs(h, nullptr, "kgb_test_forward_serial");
+    forwardDevice(h, n, d_spatial, d_global, nullptr, d_symmetry, d_policy_optimism, d_policy, d_value, d_score_value, d_ownership, true);
+    CK(cudaStreamSynchronize(h->stream));
+  });
+}
+
+KGB_API int kgb_conv_chain_error(int* out) {
+  return guarded([&] {
+    if(!out) throw std::invalid_argument("kgb_conv_chain_error: NULL argument");
+    *out = convChainStatus() == cudaSuccess ? 0 : 1;
   });
 }
 
@@ -1176,6 +1240,7 @@ struct SingleConv {
       if(raw) raws.push_back(raw);
       b.emitConv(cw, A, kind == 2 || kind == 4 ? raw : nullptr, rawF32, ncbias, raw, rawF32, act, kind == 0 ? Builder::BNDev() : dev);
     }
+    h.allocChain();
   }
   ~SingleConv() {
     for(void* p : h.allocs) cudaFree(p);
@@ -1326,6 +1391,7 @@ struct BoundaryConv {
         b.emitConv(wpre, s.trunkA, nullptr, false, nullptr, s.innerS, innerF32, s.innerA, bn2);
       }
     }
+    h.allocChain();
     CK(cudaStreamSynchronize(h.stream));
   }
   ~BoundaryConv() {

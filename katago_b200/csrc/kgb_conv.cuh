@@ -46,6 +46,10 @@ struct ConvParams {
   const float* bn_bias;   // [cout_p]
   int act;                // kgb::Activation
   const float* mask;      // [M] 1.0 on-board, 0.0 pad/off-board
+  // chaining (launchConvWG / launchConvPair)
+  int* tile_flags;        // [num_m_tiles] this launch's tile flags, zero before the launch when a chained launch reads them
+  const int* pred_flags;  // the previous launch's tile_flags when this launch is chained to it, else null
+  int pred_parts;         // the value a tile flag of the previous launch has once the tile is written (convChainParts)
 };
 
 // fp32 activation functions of the small kernels, and of the convolution epilogue except its mish, which epilogue_store
@@ -78,7 +82,20 @@ struct ConvTmaps {
 // same dtype: the raw output is written back over the residual slice in shared memory.  The residual may alias raw_out (each
 // element is read and written by the CTA of its own tile); A must alias neither raw_out nor act_out, since a tile's halo rows
 // belong to the neighbouring tiles.
+//
+// Chaining.  Every launch adds 1 to p.tile_flags[m] per (n-group, consumer warpgroup) once that part's TMA stores of 128-row tile m
+// are complete, so a tile is written when its flag reaches convChainParts(p) if the flags were zero before the launch.  With
+// p.pred_flags set, the launch is a programmatic dependent launch of the previous kernel on the stream, which must be a
+// convolution launch whose tile_flags these are, with pred_parts = convChainParts of it.  Its CTAs may then start while that
+// kernel's last tiles still run: before a tile loads its operand rows or its residual it waits until the previous launch's tiles
+// m-1, m and m+1 are written.  A CTA does not exit before the previous launch has completed, so a launch that follows a chained
+// one in the ordinary way still sees every launch of the chain complete.  Data written inside a chain is read through TMA only.
+// A flag wait that lasts longer than ~4 s gives up and sets the sticky word that convChainStatus reports.  The word is one for the
+// process (mapped host memory, shared by every device and handle) and is never reset: after one wait has given up, the outputs of
+// that forward are wrong and every later synchronising call of every handle reports the error.
 cudaError_t launchConvWG(const ConvTmaps& tm, const ConvParams& p, cudaStream_t stream);
+inline int convChainParts(const ConvParams& p) { return 2 * p.num_n_tiles; }
+cudaError_t convChainStatus();  // cudaErrorLaunchTimeout once a flag wait of this process has given up
 inline int convABoxRows(int ky, int kx, int Wp) { return 128 + 2 * ((ky / 2) * Wp + (kx / 2)); }  // TMA box rows of the A halo tile
 inline int convSliceBoxRows() { return 64; }  // TMA box rows of the epilogue's slices: one consumer warpgroup's half of a tile
 cudaError_t convWGInit();  // per device, before the first launch (sets the kernels' shared-memory limit, reads the SM count)
@@ -90,11 +107,13 @@ cudaError_t convWGInit();  // per device, before the first launch (sets the kern
 // so the results are bit-identical.  p2.act_out may be the same buffer as p1's A (a tile reads all of its rows of A before its
 // epilogue writes them, and there is no halo).  Tensor maps: A = p1's operand, box {64, 128}; W1 = the exit's packed weights, box
 // {64, 64}; W2 = the entry's, box {64, p2.n_tile}; stream1 = p1's residual and raw stream, stream2 = p2.raw_out, act2 = p2.act_out
-// (slice boxes as in ConvTmaps).
+// (slice boxes as in ConvTmaps).  Chaining as launchConvWG, with p1's chain fields; a tile is written (all of p1's and p2's outputs)
+// when its flag reaches kConvPairParts.
 struct ConvPairTmaps {
   CUtensorMap A, W1, W2, stream1, stream2, act2;
 };
 static constexpr int kConvPairChunk = 64;   // box rows of W1
+static constexpr int kConvPairParts = 2;    // one per consumer warpgroup
 // Whether launchConvPair takes these launches: fp16 operands, mish at both ends, 1x1 filters, (inner, trunk) widths the kernel is
 // compiled for, and rings that fit in shared memory.
 bool convPairSupported(const ConvParams& p1, const ConvParams& p2);

@@ -102,6 +102,68 @@ __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.comm
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
+// ------------------------------------------------------------------------------------------------------------
+// Chained launches (kgb_conv.cuh, launchConvWG).  The ordering argument, in terms of the PTX memory consistency model
+// (PTX ISA, "Memory Consistency Model"):
+//   writer  the leader thread that issued a tile part's TMA stores waits for their completion (cp.async.bulk.wait_group 0: the
+//           writes are performed), then fence.proxy.async orders those async-proxy writes before its later generic-proxy
+//           operations ("Proxies", "Proxy fences"), and red.release.gpu adds to the tile's flag: a release pattern at gpu scope.
+//   reader  the producer / residual lane reads the flags with ld.acquire.gpu.  An acquire that observes the value of the writers'
+//           releases synchronizes with them ("Release and acquire patterns", "Causality order"), so the stores are visible to
+//           the reader's later operations; fence.proxy.async then extends that to the TMA loads it issues next, which run in the
+//           async proxy.  What the consumers do with the loaded rows follows the loads through the mbarriers.
+// Both RAW (a tile's operand and residual rows) and WAR (a launch overwriting rows that an earlier launch still reads through its
+// halo, in place or in a buffer that levels share) are covered by waiting on the previous launch's tiles m-1..m+1 only: that
+// launch's tile m' was written after it had waited on tiles m'-1..m'+1 of the launch before it, so by induction a launch k steps
+// back has finished every tile within k tiles of m.  A halo is at most 64 rows (BLOCK_M + 2 * halo <= 256), so every reader of
+// tile m's rows is one of tiles m-1..m+1 of its launch.  1x1 launches wait on the same three tiles, so that the induction does
+// not depend on which launches have a halo.
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+__device__ __forceinline__ int ld_acquire_gpu(const int* p) {
+  int v;
+  asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void red_release_gpu_add(int* p, int v) {
+  asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint64_t globaltimer_ns() {
+  uint64_t t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+__device__ int* g_chainError;   // host-mapped sticky word (convWGInit), set when a flag wait gives up
+
+// Leader of a consumer warpgroup: its TMA stores of tile m_tile are all issued; publish them.  Out of line, so that it adds nothing
+// to the register pressure of the consumers' accumulators.
+__device__ __noinline__ void chain_publish(int* flags, int m_tile) {
+  bulk_wait0();
+  fence_proxy_async_global();
+  red_release_gpu_add(flags + m_tile, 1);
+}
+
+// Producer lanes, before a tile's loads: the previous launch's tiles m_tile-1..m_tile+1 (of the plan's m_tiles) are written.  The
+// wait sleeps between polls, so that a waiter sharing an SM with the previous launch's CTA does not take its issue slots.
+__device__ __noinline__ void chain_wait(const int* pred, int parts, int m_tile, int m_tiles) {
+  if(pred == nullptr) return;
+  for(int t = max(m_tile - 1, 0); t <= min(m_tile + 1, m_tiles - 1); t++) {
+    if(ld_acquire_gpu(pred + t) >= parts) continue;
+    const uint64_t t0 = globaltimer_ns();
+    uint32_t ns = 64;
+    while(ld_acquire_gpu(pred + t) < parts) {
+      __nanosleep(ns);
+      if(ns < 2048) ns *= 2;
+      if(globaltimer_ns() - t0 > 4000000000ull) {   // never in a correct chain: record it and go on rather than hang the device
+        atomicExch_system(g_chainError, 1);
+        break;
+      }
+    }
+  }
+  fence_proxy_async_global();
+}
+
 // wgmma shared-memory descriptor, K-major, 128B swizzle:
 //   [0,14) start>>4 | [16,30) LBO>>4 (1, unused for swizzled K-major) | [32,46) SBO>>4 (1024 B = 8 rows x 128 B) | [62,64) 1 = 128B swizzle
 // Weight tiles start 1024-aligned, so the base offset [49,52) is 0; +32 bytes (+2 units) steps 16 fp16 along K inside the row.
@@ -298,6 +360,7 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
   const int parts = p.split ? 3 : 1;
   const int phases = (p.cin_p / BLOCK_K) * parts;             // one A halo tile per (k-block, split part)
 
+  pdl_launch_dependents();   // the next launch's CTAs take the SMs this grid leaves (they need all of shared memory)
   if(threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapB) : "memory");
@@ -330,6 +393,7 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
       for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
         const int m0 = (tile / p.num_n_tiles) * BLOCK_M;
         const int wp = __ldg(p.tile_wp + m0 / BLOCK_M);       // loaded here, ahead of the consumers, who read it from the A slot
+        chain_wait(p.pred_flags, p.pred_parts, m0 / BLOCK_M, tiles / p.num_n_tiles);
         for(int ph = 0; ph < phases; ph++, ac++) {
           const int kb = ph / parts, part = ph - kb * parts;
           const int colA = kb * BLOCK_K + (part == 1 ? p.cin_p : 0);
@@ -356,6 +420,7 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
       uint32_t rphase = 0;
       for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
         const int m0 = (tile / p.num_n_tiles) * BLOCK_M;
+        chain_wait(p.pred_flags, p.pred_parts, m0 / BLOCK_M, tiles / p.num_n_tiles);
         for(int s = 0; s < slices; s++) {
           mbar_wait(smem_u32(&bars->r_empty[rs]), rphase ^ 1);
           const uint32_t rfull = smem_u32(&bars->r_full[rs]), dst = smem_r + rs * r_slot_bytes;
@@ -391,6 +456,7 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
   uint32_t rphase = 0;
   uint8_t* const ring = smem + (smem_r - smem_base);
   uint8_t* const act_ring = smem + (smem_act - smem_base);
+  int pending = -1;   // the m-tile whose stores this warpgroup issued last and has not published yet
   for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
     const int m0 = (tile / p.num_n_tiles) * BLOCK_M;
     int wp = 0;                                               // the tile's row pitch, from the A slot
@@ -451,6 +517,8 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
     fence_acc(acc);
     __syncwarp();
     if(lane == 0) mbar_arrive(smem_u32(&bars->empty[prev_stage]));   // the tile's last stage: the producer is already on the next tile
+    // the previous tile's stores were issued a whole main loop ago
+    if(leader && pending >= 0) chain_publish(p.tile_flags, pending);
 
     // ===================== epilogue: one 32-column slice at a time, into shared memory, out by TMA stores =====================
 #pragma unroll
@@ -479,12 +547,20 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
       if(++rs >= r_slots) { rs = 0; rphase ^= 1; }   // r_slots is 0 when there is no stream
       as ^= 1;
     }
+    pending = m0 / BLOCK_M;
   }
+  if(leader && pending >= 0) chain_publish(p.tile_flags, pending);
   if(leader) bulk_wait0();
+  pdl_wait();   // this grid completes after the previous one
 }
 
 static int g_smCount[64];   // per device ordinal, read by convWGInit
+static int* g_chainErrorHost;   // the sticky word chain_wait sets, in mapped host memory shared by every device
 static cudaError_t convPairInit();
+
+cudaError_t convChainStatus() {
+  return g_chainErrorHost != nullptr && *(volatile int*)g_chainErrorHost != 0 ? cudaErrorLaunchTimeout : cudaSuccess;
+}
 
 cudaError_t convWGInit() {
   int dev = 0;
@@ -492,6 +568,19 @@ cudaError_t convWGInit() {
   if(e0 != cudaSuccess) return e0;
   if(dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
   e0 = cudaDeviceGetAttribute(&g_smCount[dev], cudaDevAttrMultiProcessorCount, dev);
+  if(e0 != cudaSuccess) return e0;
+  static int* word = [] {
+    int* w = nullptr;
+    if(cudaHostAlloc((void**)&w, sizeof(int), cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess) return (int*)nullptr;
+    *w = 0;
+    return w;
+  }();
+  if(word == nullptr) return cudaErrorMemoryAllocation;
+  g_chainErrorHost = word;
+  int* devWord = nullptr;
+  e0 = cudaHostGetDevicePointer((void**)&devWord, word, 0);
+  if(e0 != cudaSuccess) return e0;
+  e0 = cudaMemcpyToSymbol(g_chainError, &devWord, sizeof(devWord));
   if(e0 != cudaSuccess) return e0;
   for(cudaError_t e : {cudaFuncSetAttribute(kgb_conv_wg_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
                        cudaFuncSetAttribute(kgb_conv_wg_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
@@ -506,10 +595,25 @@ cudaError_t convWGInit() {
   return cudaSuccess;
 }
 
+// A chained launch (p.pred_flags set) may start while the previous kernel on the stream still runs
+template <class... Args>
+static cudaError_t launchChained(void (*kernel)(Args...), const ConvParams& p, int grid, int smem, cudaStream_t stream, Args... args) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(THREADS);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = p.pred_flags != nullptr ? 1 : 0;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  return cudaLaunchKernelEx(&cfg, kernel, args...);
+}
+
 template <int N>
 static cudaError_t launchN(const ConvTmaps& tm, const ConvParams& p, int grid, int stages, int smem, cudaStream_t stream) {
-  kgb_conv_wg_kernel<N><<<grid, THREADS, smem, stream>>>(tm.A, tm.B, tm.residual, tm.raw, tm.act, p, stages);
-  return cudaGetLastError();
+  return launchChained(kgb_conv_wg_kernel<N>, p, grid, smem, stream, tm.A, tm.B, tm.residual, tm.raw, tm.act, p, stages);
 }
 
 cudaError_t launchConvWG(const ConvTmaps& tm, const ConvParams& p, cudaStream_t stream) {
@@ -518,6 +622,7 @@ cudaError_t launchConvWG(const ConvTmaps& tm, const ConvParams& p, cudaStream_t 
   if(p.n_tile % RES_COLS != 0) return cudaErrorInvalidValue;
   // the raw output is written over the residual slice it was read from
   if(p.residual != nullptr && p.raw_out != nullptr && (p.residual_fp32 != 0) != (p.raw_fp32 != 0)) return cudaErrorInvalidValue;
+  if(p.tile_flags == nullptr) return cudaErrorInvalidValue;
   int dev = 0;
   const cudaError_t e = cudaGetDevice(&dev);
   if(e != cudaSuccess) return e;
@@ -636,6 +741,7 @@ kgb_conv_pair_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_con
   const int lane = threadIdx.x & 31;
   const int tiles = __ldg(p1.m_tiles);
 
+  pdl_launch_dependents();
   if(threadIdx.x == 0) {
     for(const CUtensorMap* m : {&tmapA, &tmapW1, &tmapW2, &tmapS1, &tmapS2, &tmapA2})
       asm volatile("prefetch.tensormap [%0];" ::"l"(m) : "memory");
@@ -672,14 +778,19 @@ kgb_conv_pair_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_con
         }
         if(++stage == stages) { stage = 0; phase ^= 1; }
       };
+      // the first tile's first exit chunk goes out before its chain wait (weights do not depend on the previous launch)
+      bool pre = (int)blockIdx.x < tiles;
+      if(pre) loadW(false, 0);
       for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
         const int m0 = tile * BLOCK_M;
+        chain_wait(p1.pred_flags, p1.pred_parts, tile, tiles);
         mbar_wait(smem_u32(&bars->a_empty), aphase ^ 1);
         const uint32_t afull = smem_u32(&bars->a_full);
         mbar_arrive_expect_tx(afull, (uint32_t)A_BYTES);
         for(int kb = 0; kb < K1 / BLOCK_K; kb++) tma_load_2d(smem_base + kb * BLOCK_M * 128, &tmapA, afull, kb * BLOCK_K, m0);
         aphase ^= 1;
-        loadW(false, 0);
+        if(!pre) loadW(false, 0);
+        pre = false;
         for(int c = 0; c < chunks; c++) {
           if(c + 1 < chunks) loadW(false, c + 1);
           loadW(true, c);
@@ -692,6 +803,7 @@ kgb_conv_pair_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_con
       uint32_t rphase = 0;
       for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
         const int m0 = tile * BLOCK_M;
+        chain_wait(p1.pred_flags, p1.pred_parts, tile, tiles);
         for(int s = 0; s < N1 / RES_COLS; s++) {
           mbar_wait(smem_u32(&bars->r_empty[rs]), rphase ^ 1);
           const uint32_t rfull = smem_u32(&bars->r_full[rs]), dst = smem_r + rs * R1_BYTES;
@@ -720,6 +832,7 @@ kgb_conv_pair_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_con
   uint8_t* const t_ring = smem + (smem_t - smem_base);
   uint8_t* const stg_ring = smem + (smem_stg - smem_base);
   uint8_t* const act_ring = smem + (smem_act - smem_base);
+  int pending = -1;   // as in kgb_conv_wg_kernel
   auto take = [&]() {
     const int st = stage;
     mbar_wait(smem_u32(&bars->full[st]), phase);
@@ -773,6 +886,7 @@ kgb_conv_pair_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_con
     fence_acc(acc1);
     release(smem_u32(&bars->empty[st1]));
     if(chunks == 1) release(smem_u32(&bars->a_empty));
+    if(leader && pending >= 0) chain_publish(p1.tile_flags, pending);
 #pragma unroll
     for(int c = 0; c < chunks; c++) {
       // ---- the exit's epilogue of chunk c: residual in, raw stream out, activated operand into T slot c & 1 ----
@@ -843,8 +957,11 @@ kgb_conv_pair_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_con
       ps ^= 1;
       as ^= 1;
     }
+    pending = tile;
   }
+  if(leader && pending >= 0) chain_publish(p1.tile_flags, pending);
   if(leader) bulk_wait0();
+  pdl_wait();
 }
 
 template <int N2, int N1>
@@ -888,12 +1005,11 @@ static cudaError_t launchPairN(const ConvPairTmaps& tm, const ConvParams& p1, co
                                cudaStream_t stream) {
   auto k = p1.raw_fp32 ? (p2.raw_fp32 ? kgb_conv_pair_kernel<N2, N1, true, true> : kgb_conv_pair_kernel<N2, N1, true, false>)
                        : kgb_conv_pair_kernel<N2, N1, false, false>;
-  k<<<grid, THREADS, l.smem, stream>>>(tm.A, tm.W1, tm.W2, tm.stream1, tm.stream2, tm.act2, p1, p2, l.stages, l.r_slots);
-  return cudaGetLastError();
+  return launchChained(k, p1, grid, l.smem, stream, tm.A, tm.W1, tm.W2, tm.stream1, tm.stream2, tm.act2, p1, p2, l.stages, l.r_slots);
 }
 
 cudaError_t launchConvPair(const ConvPairTmaps& tm, const ConvParams& p1, const ConvParams& p2, cudaStream_t stream) {
-  if(!convPairSupported(p1, p2)) return cudaErrorInvalidValue;
+  if(!convPairSupported(p1, p2) || p1.tile_flags == nullptr) return cudaErrorInvalidValue;
   int dev = 0;
   const cudaError_t e = cudaGetDevice(&dev);
   if(e != cudaSuccess) return e;

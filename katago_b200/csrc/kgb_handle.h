@@ -77,6 +77,14 @@ struct kgb_handle {
   size_t planRows(int n) const { return fixedPlan ? (size_t)n * L.P : kgb::planRowCapacity(L, n); }   // rows the row buffers hold
   std::vector<std::function<void(int, cudaStream_t)>> ops;
   int launchesPerForward = 0;
+  // Tile flags of the convolution launches (kgb_conv.cuh, launchConvWG): one slot of chainStride() ints per launch, allocated
+  // once the ops are emitted.  A forward zeroes them all at its head.
+  int* chain = nullptr;
+  int chainSlots = 0;
+  int chainedLaunches = 0;   // convolution launches per forward that are programmatic dependents of the one before
+  size_t chainStride() const { return (planRows(maxBatch) + 127) / 128; }
+  int* chainFlags(int slot) const { return chain + (size_t)slot * chainStride(); }
+  void allocChain() { chain = dalloc<int>((size_t)std::max(chainSlots, 1) * chainStride()); }
   std::map<int, cudaGraphExec_t> graphs;
 
   // Weights live in ONE arena: a net of the same architecture is swapped in between two waves by one device copy

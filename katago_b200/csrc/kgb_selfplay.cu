@@ -36,6 +36,7 @@
 
 #include "../../include/kgb200.h"
 #include "kgb_board.cuh"
+#include "kgb_conv.cuh"
 #include "kgb_devrand.cuh"
 #include "kgb_handle.h"
 #include "kgb_history.cuh"
@@ -2416,7 +2417,10 @@ struct kgb_selfplay {
     sync();
   }
   template <class T> void fill(T* dst, int byte, size_t count) { CK(cudaMemsetAsync(dst, byte, count * sizeof(T), h->stream)); }
-  void sync() { CK(cudaStreamSynchronize(h->stream)); }
+  void sync() {
+    CK(cudaStreamSynchronize(h->stream));
+    CK(convChainStatus());
+  }
   // What every entry point does first: make the loop's device current and, with `drain`, wait for the waves queued on its stream
   void enter(bool drain = true) {
     CK(cudaSetDevice(h->device));
