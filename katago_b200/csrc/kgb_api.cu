@@ -258,6 +258,7 @@ struct Builder {
     p.act_out = actOut;
     p.bn_scale = bn.scale; p.bn_bias = bn.bias; p.act = bn.act;
     p.mask = hh.dMask;
+    p.epi_wg = hh.epilogueWG ? 1 : 0;
     return p;
   }
 
@@ -318,6 +319,7 @@ struct Builder {
     });
     linkConvOp(link, 2 * cw.num_n_tiles);
     h.launchesPerForward++;
+    h.epilogueWGLaunches += convEpilogueWG(convParams(h, h.maxBatch, cw, residual, residualFp32, ncbias, rawOut, rawFp32, actOut, bn)) ? 1 : 0;
   }
 
   // blocks operate on stream lv.S, with lv.A = act(preBN_0(S)) on entry and = act(finalBN(S_out)) on exit.
@@ -670,11 +672,18 @@ static void ncclCheck(ncclResult_t r, const char* what) {
   if(r != ncclSuccess) throw CudaFailure(std::string(what) + ": " + ncclApi().getErrorString(r));
 }
 
+// KGB_EPILOGUE_WG=0 keeps every convolution on kgb_conv_wg_kernel (same-build A/B runs and tests; the results are the same).  Read
+// where a handle is made: kgb_handle_create and the single-layer test hooks.
+static bool epilogueWGFromEnv() {
+  const char* e = getenv("KGB_EPILOGUE_WG");
+  return !(e && std::string(e) == "0");
+}
+
 // The settings that decide how the graph builder lays the weights out
 static void copyBuildSettings(kgb_handle& dst, const kgb_handle& src) {
   dst.device = src.device; dst.model = src.model; dst.L = src.L; dst.maxBatch = src.maxBatch; dst.split = src.split;
   dst.nhwc = src.nhwc; dst.streamTrunkFp32 = src.streamTrunkFp32; dst.streamInnerFp32 = src.streamInnerFp32;
-  dst.fuseBoundaries = src.fuseBoundaries;
+  dst.fuseBoundaries = src.fuseBoundaries; dst.epilogueWG = src.epilogueWG;
 }
 
 // Makes device `dev` (-1: the current device) current, after checking that it exists and is the sm_90a device the kernels are
@@ -760,6 +769,7 @@ KGB_API int kgb_handle_create(kgb_context* ctx, const kgb_model* model, int max_
     // results are the same)
     const char* ragged = getenv("KGB_RAGGED_ROWS");
     h.plan.ragged = !(ragged && std::string(ragged) == "0");
+    h.epilogueWG = epilogueWGFromEnv();
     CK(cudaStreamCreateWithFlags(&h.stream, cudaStreamNonBlocking));
     CK(convWGInit());
     CK(cudaStreamCreateWithFlags(&h.copyStream, cudaStreamNonBlocking));
@@ -899,6 +909,7 @@ KGB_API int kgb_handle_is_fp16(const kgb_handle* handle) { return handle && !han
 KGB_API uint64_t kgb_handle_stream(kgb_handle* handle) { return handle ? (uint64_t)(uintptr_t)handle->stream : 0; }
 KGB_API int kgb_handle_launches_per_forward(const kgb_handle* handle) { return handle ? handle->launchesPerForward : 0; }
 KGB_API int kgb_handle_chained_launches_per_forward(const kgb_handle* handle) { return handle ? handle->chainedLaunches : 0; }
+KGB_API int kgb_handle_epilogue_wg_launches_per_forward(const kgb_handle* handle) { return handle ? handle->epilogueWGLaunches : 0; }
 
 KGB_API int kgb_handle_get_layout_stats(kgb_handle* handle, int64_t* rows, int64_t* m_tiles, int64_t* segments) {
   return guarded([&] {
@@ -1200,6 +1211,7 @@ struct SingleConv {
     h.model = &dummy;
     h.maxBatch = n;
     h.split = use_fp16 ? 0 : 1;
+    h.epilogueWG = epilogueWGFromEnv();
     h.L = boardLayout(X, Y, std::max(1, std::max(ky / 2, kx / 2)));
     h.streamTrunkFp32 = h.streamInnerFp32 = h.split != 0;
     CK(cudaStreamCreateWithFlags(&h.stream, cudaStreamNonBlocking));

@@ -50,6 +50,7 @@ struct ConvParams {
   int* tile_flags;        // [num_m_tiles] this launch's tile flags, zero before the launch when a chained launch reads them
   const int* pred_flags;  // the previous launch's tile_flags when this launch is chained to it, else null
   int pred_parts;         // the value a tile flag of the previous launch has once the tile is written (convChainParts)
+  int epi_wg;             // launchConvWG may take the epilogue-warpgroup kernel (convEpilogueWG); 0 keeps kgb_conv_wg_kernel
 };
 
 // fp32 activation functions of the small kernels, and of the convolution epilogue except its mish, which epilogue_store
@@ -84,7 +85,8 @@ struct ConvTmaps {
 // belong to the neighbouring tiles.
 //
 // Chaining.  Every launch adds 1 to p.tile_flags[m] per (n-group, consumer warpgroup) once that part's TMA stores of 128-row tile m
-// are complete, so a tile is written when its flag reaches convChainParts(p) if the flags were zero before the launch.  With
+// are complete (2 per n-group at once from the epilogue warpgroup of kgb_conv_wg_epi_kernel), so a tile is written when its flag
+// reaches convChainParts(p) if the flags were zero before the launch.  With
 // p.pred_flags set, the launch is a programmatic dependent launch of the previous kernel on the stream, which must be a
 // convolution launch whose tile_flags these are, with pred_parts = convChainParts of it.  Its CTAs may then start while that
 // kernel's last tiles still run: before a tile loads its operand rows or its residual it waits until the previous launch's tiles
@@ -94,6 +96,11 @@ struct ConvTmaps {
 // process (mapped host memory, shared by every device and handle) and is never reset: after one wait has given up, the outputs of
 // that forward are wrong and every later synchronising call of every handle reports the error.
 cudaError_t launchConvWG(const ConvTmaps& tm, const ConvParams& p, cudaStream_t stream);
+// Whether launchConvWG runs these parameters with kgb_conv_wg_epi_kernel (a dedicated epilogue warpgroup fed through a shared-memory
+// accumulator tile, so the MMAs of the next tile run under each tile's epilogue) rather than kgb_conv_wg_kernel: p.epi_wg set, fp16
+// operands, a filter wider than 1x1, n_tile 96 to 192, an fp16 stream or none (or only a raw fp32 output), and rings that fit.
+// Both kernels give the same bits.
+bool convEpilogueWG(const ConvParams& p);
 inline int convChainParts(const ConvParams& p) { return 2 * p.num_n_tiles; }
 cudaError_t convChainStatus();  // cudaErrorLaunchTimeout once a flag wait of this process has given up
 inline int convABoxRows(int ky, int kx, int Wp) { return 128 + 2 * ((ky / 2) * Wp + (kx / 2)); }  // TMA box rows of the A halo tile

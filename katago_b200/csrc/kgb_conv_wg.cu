@@ -554,6 +554,341 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
   pdl_wait();   // this grid completes after the previous one
 }
 
+// ------------------------------------------------------------------------------------------------------------
+// Epilogue warpgroup (kgb_conv_wg_epi_kernel, launchConvWG when convEpilogueWG)
+// ------------------------------------------------------------------------------------------------------------
+// In kgb_conv_wg_kernel both consumer warpgroups leave the main loop together and run the epilogue arithmetic with the tensor
+// pipe idle.  Here a fourth warpgroup runs it, 512 threads:
+//   warpgroup 0     TMA producers as above (one residual slot instead of a ring of four).
+//   warpgroups 1-2  the same main loop, so every accumulator holds the same bits.  At the end of a tile they wait until the
+//                   accumulator tile in shared memory is empty, write their fp32 accumulators into it (N/32 slices of 128 x 32 in
+//                   slice_offset's fp32 layout), arrive on t_full and start the next tile at once.
+//   warpgroup 3     the epilogue, one thread per tile row: slice by slice it reads its row's 32 accumulators (and the residual),
+//                   applies epilogue_store<F> to each column pair exactly as the other kernel does, and writes the raw output
+//                   and the activated operand back into the slice it read (raw fp16 in the first 8 KB, the operand in the
+//                   second; a raw fp32 output over the whole slice), out by TMA stores.  Once the last stores have read shared
+//                   memory it arrives on t_empty, and once they are complete it publishes the tile for the chain.
+// Shared memory for N = 192 at the 19x19 pitch: 2 x 22 KB A halo tiles, 96 KB accumulator tile, 8 KB residual slot, 3 x 24 KB
+// weight stages.  Registers after setmaxnreg: producers 40, consumers 184 (96 accumulators, 2 x 16 fragments), epilogue 104.
+static constexpr int EPI_WG_THREADS = 512;
+static constexpr int EPI_WG_MIN_STAGES = 3;
+static constexpr int ACC_SLICE_BYTES = BLOCK_M * RES_COLS * 4;
+
+// The epilogues it has a copy of: fp16 mode's 3x3 layers (kgb_conv_wg_kernel's epiDispatch without fp32 streams or split mode),
+// and the gpool unit's raw fp32 output, which is written over the accumulator slice it came from.
+#define KGB_EPI_WG_FLAGS(X) X(EPI_RAW | EPI_FP32) X(EPI_MISH) X(EPI_RES | EPI_RAW | EPI_MISH) X(EPI_RES | EPI_MISH) \
+  X(EPI_RAW | EPI_MISH) X(EPI_RAW | EPI_MISH | EPI_NCBIAS)
+// The widths it is compiled for: b28's 256-column tiles would need 128 KB of accumulator tile, and the 64-column copy spills
+#define KGB_EPI_WG_SHAPES(X) X(96) X(128) X(160) X(192)
+
+struct __align__(8) EpiBars {
+  uint64_t full[MAX_STAGES];    // weight tile landed
+  uint64_t empty[MAX_STAGES];   // weight tile consumed by every consumer warp
+  uint64_t a_full[2];           // A halo tile landed
+  uint64_t a_empty[2];          // A halo tile consumed by all of its taps
+  uint64_t r_full, r_empty;     // residual slice landed / read by the epilogue warpgroup
+  uint64_t t_full, t_empty;     // accumulator tile written by every consumer warp / read, and its stores' reads done
+  int a_wp[2];                  // row pitch of the tile whose A halo tile is in the slot
+};
+
+// Epilogue warpgroup: tile m_tile's stores are all issued; publish it for both halves of the parts count (convChainParts).
+__device__ __noinline__ void chain_publish_tile(int* flags, int m_tile) {
+  bulk_wait0();
+  fence_proxy_async_global();
+  red_release_gpu_add(flags + m_tile, 2);
+}
+// The epilogue warpgroup.  bar.sync is .aligned: a warp reaches it converged, so after an mbarrier wait loop (which its lanes may
+// leave in different iterations) the epilogue brings the warp together with __syncwarp.
+__device__ __forceinline__ void epi_wg_sync() { asm volatile("bar.sync 4, 128;" ::: "memory"); }
+
+// One row's part of slice s: its 16 column pairs through epilogue_store<F>, the outputs gathered in registers and written into
+// the slice `region` it was read from as 16-byte chunks (every row of the slice has been read by then).
+template <int F>
+__device__ __forceinline__ void epilogue_row(const ConvParams& p, int row, int rl, int col0, const float (&v)[RES_COLS],
+                                             const uint32_t (&res)[RES_COLS / 2], float maskv, const float* sc, const float* bi,
+                                             uint8_t* region) {
+  constexpr bool raw32 = (F & EPI_FP32) != 0;
+  float2 rawf[RES_COLS / 2];
+  uint32_t rawh[RES_COLS / 2], act[RES_COLS / 2];
+#pragma unroll
+  for(int k = 0; k < RES_COLS / 2; k++) {
+    const float2 r = (F & EPI_RES) ? __half22float2(*reinterpret_cast<const __half2*>(&res[k])) : make_float2(0.0f, 0.0f);
+    epilogue_store<F>(p, row, col0 + 2 * k, v[2 * k], v[2 * k + 1], maskv, r, sc + 2 * k, bi + 2 * k,
+                      raw32 ? reinterpret_cast<uint8_t*>(&rawf[k]) : reinterpret_cast<uint8_t*>(&rawh[k]),
+                      reinterpret_cast<uint8_t*>(&act[k]), nullptr);
+  }
+  if(F & EPI_RAW) {
+    if(raw32) {
+#pragma unroll
+      for(int k = 0; k < RES_COLS / 4; k++)
+        *reinterpret_cast<float4*>(region + slice_offset(rl, 4 * k, true)) =
+          make_float4(rawf[2 * k].x, rawf[2 * k].y, rawf[2 * k + 1].x, rawf[2 * k + 1].y);
+    }
+    else {
+#pragma unroll
+      for(int k = 0; k < RES_COLS / 8; k++)
+        *reinterpret_cast<uint4*>(region + slice_offset(rl, 8 * k, false)) = make_uint4(rawh[4 * k], rawh[4 * k + 1], rawh[4 * k + 2], rawh[4 * k + 3]);
+    }
+  }
+  if(F & EPI_MISH) {
+#pragma unroll
+    for(int k = 0; k < RES_COLS / 8; k++)
+      *reinterpret_cast<uint4*>(region + ACT_SLICE_BYTES + slice_offset(rl, 8 * k, false)) =
+        make_uint4(act[4 * k], act[4 * k + 1], act[4 * k + 2], act[4 * k + 3]);
+  }
+}
+
+template <int N>
+__global__ void __launch_bounds__(EPI_WG_THREADS, 1)
+kgb_conv_wg_epi_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapB,
+                       const __grid_constant__ CUtensorMap tmapR, const __grid_constant__ CUtensorMap tmapRaw,
+                       const __grid_constant__ CUtensorMap tmapAct, const __grid_constant__ ConvParams p, int stages) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  constexpr int b_tile_bytes = N * BLOCK_K * 2;
+  constexpr int slices = N / RES_COLS;
+  const int halo = (p.ky / 2) * p.Wp + (p.kx / 2);
+  const int a_tx_bytes = (BLOCK_M + 2 * halo) * BLOCK_K * 2;
+  const int a_buf_bytes = (a_tx_bytes + 1023) / 1024 * 1024;
+  const int flags = epiFlags(p);
+  // [<=1023 B slack][2 x A halo tile][accumulator tile: slices x 16 KB][residual slot, 8 KB][stages x weight tile][EpiBars][BN]
+  const uint32_t smem_acc = smem_base + 2 * a_buf_bytes;
+  const uint32_t smem_r = smem_acc + slices * ACC_SLICE_BYTES;
+  const uint32_t smem_b = smem_r + (p.residual != nullptr ? ACT_SLICE_BYTES : 0);
+  uint8_t* const smem = smem_raw + (smem_base - smem_u32(smem_raw));
+  EpiBars* bars = reinterpret_cast<EpiBars*>(smem + (smem_b - smem_base) + (size_t)stages * b_tile_bytes);
+  float* const s_scale = reinterpret_cast<float*>(bars + 1);
+  float* const s_bias = s_scale + N;
+  uint8_t* const acc_tile = smem + (smem_acc - smem_base);
+
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  const int tiles = __ldg(p.m_tiles) * p.num_n_tiles;
+  const int n0 = (blockIdx.x % p.num_n_tiles) * N;
+  const int taps = p.ky * p.kx;
+  const int phases = p.cin_p / BLOCK_K;                       // one A halo tile per k-block (no split mode here)
+
+  pdl_launch_dependents();
+  if(threadIdx.x == 0) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapA) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapB) : "memory");
+    if(p.residual != nullptr) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapR) : "memory");
+    if(p.raw_out != nullptr) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapRaw) : "memory");
+    if(p.act_out != nullptr) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapAct) : "memory");
+    for(int s = 0; s < stages; s++) {
+      mbar_init(smem_u32(&bars->full[s]), 1);
+      mbar_init(smem_u32(&bars->empty[s]), CONSUMER_WARPS);
+    }
+    for(int s = 0; s < 2; s++) {
+      mbar_init(smem_u32(&bars->a_full[s]), 1);
+      mbar_init(smem_u32(&bars->a_empty[s]), CONSUMER_WARPS);
+    }
+    mbar_init(smem_u32(&bars->r_full), 1);
+    mbar_init(smem_u32(&bars->r_empty), 1);
+    mbar_init(smem_u32(&bars->t_full), CONSUMER_WARPS);
+    mbar_init(smem_u32(&bars->t_empty), 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if(warp < 4) {
+    // ===================== TMA producers =====================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if(warp == 0 && lane == 0) {
+      int stage = 0, ac = 0;
+      uint32_t phase = 0;
+      for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        const int m0 = (tile / p.num_n_tiles) * BLOCK_M;
+        const int wp = __ldg(p.tile_wp + m0 / BLOCK_M);
+        chain_wait(p.pred_flags, p.pred_parts, m0 / BLOCK_M, tiles / p.num_n_tiles);
+        for(int kb = 0; kb < phases; kb++, ac++) {
+          const int abuf = ac & 1;
+          mbar_wait(smem_u32(&bars->a_empty[abuf]), ((ac >> 1) & 1) ^ 1);
+          const uint32_t afull = smem_u32(&bars->a_full[abuf]);
+          bars->a_wp[abuf] = wp;
+          mbar_arrive_expect_tx(afull, (uint32_t)a_tx_bytes);
+          tma_load_2d(smem_base + abuf * a_buf_bytes, &tmapA, afull, kb * BLOCK_K, m0 - halo);
+          for(int t = 0; t < taps; t++) {
+            mbar_wait(smem_u32(&bars->empty[stage]), phase ^ 1);
+            const uint32_t full = smem_u32(&bars->full[stage]);
+            mbar_arrive_expect_tx(full, (uint32_t)b_tile_bytes);
+            tma_load_2d(smem_b + stage * b_tile_bytes, &tmapB, full, kb * BLOCK_K, t * p.cout_p + n0);
+            if(++stage == stages) { stage = 0; phase ^= 1; }
+          }
+        }
+      }
+    }
+    else if(warp == 1 && lane == 0 && p.residual != nullptr) {
+      // fp16 residual slices into the one slot, each as soon as the epilogue warpgroup has read the one before
+      uint32_t rphase = 0;
+      for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        const int m0 = (tile / p.num_n_tiles) * BLOCK_M;
+        chain_wait(p.pred_flags, p.pred_parts, m0 / BLOCK_M, tiles / p.num_n_tiles);
+        for(int s = 0; s < slices; s++) {
+          mbar_wait(smem_u32(&bars->r_empty), rphase ^ 1);
+          const uint32_t rfull = smem_u32(&bars->r_full);
+          mbar_arrive_expect_tx(rfull, (uint32_t)ACT_SLICE_BYTES);
+          tma_load_2d(smem_r, &tmapR, rfull, n0 + s * RES_COLS, m0);
+          tma_load_2d(smem_r + ACT_SLICE_BYTES / 2, &tmapR, rfull, n0 + s * RES_COLS, m0 + BLOCK_M / 2);
+          rphase ^= 1;
+        }
+      }
+    }
+    return;
+  }
+
+  if(warp >= 12) {
+    // ===================== epilogue warpgroup: thread rl finishes row rl of every tile =====================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 104;");
+    const int rl = threadIdx.x - 384;
+    const bool leader = rl == 0;    // issues the TMA stores and publishes the tiles
+    if(p.act_out != nullptr)
+      for(int i = rl; i < N; i += 128) { s_scale[i] = __ldg(p.bn_scale + n0 + i); s_bias[i] = __ldg(p.bn_bias + n0 + i); }
+    epi_wg_sync();
+    uint32_t tphase = 0, rphase = 0;
+    for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+      const int m0 = (tile / p.num_n_tiles) * BLOCK_M, row = m0 + rl;
+      const float maskv = row < p.M ? __ldg(p.mask + row) : 0.0f;
+      mbar_wait(smem_u32(&bars->t_full), tphase);
+      __syncwarp();
+#pragma unroll 1
+      for(int s = 0; s < slices; s++) {
+        uint8_t* const region = acc_tile + s * ACC_SLICE_BYTES;
+        float v[RES_COLS];
+#pragma unroll
+        for(int k = 0; k < RES_COLS / 4; k++) {
+          const float4 f = *reinterpret_cast<const float4*>(region + slice_offset(rl, 4 * k, true));
+          v[4 * k] = f.x; v[4 * k + 1] = f.y; v[4 * k + 2] = f.z; v[4 * k + 3] = f.w;
+        }
+        uint32_t res[RES_COLS / 2];
+        if(p.residual != nullptr) {
+          mbar_wait(smem_u32(&bars->r_full), rphase);
+          __syncwarp();
+          rphase ^= 1;
+#pragma unroll
+          for(int k = 0; k < RES_COLS / 8; k++) {
+            const uint4 u = *reinterpret_cast<const uint4*>(smem + (smem_r - smem_base) + slice_offset(rl, 8 * k, false));
+            res[4 * k] = u.x; res[4 * k + 1] = u.y; res[4 * k + 2] = u.z; res[4 * k + 3] = u.w;
+          }
+          // the slot's next TMA load (async proxy) follows these reads through the barrier below and r_empty: without the proxy
+          // fence it may land before a read has returned its value
+          fence_proxy_async();
+        }
+        else {
+#pragma unroll
+          for(int k = 0; k < RES_COLS / 2; k++) res[k] = 0;
+        }
+        epi_wg_sync();   // every row of the slice and the residual slot are read: the slot refills, the slice takes the outputs
+        if(leader && p.residual != nullptr) mbar_arrive(smem_u32(&bars->r_empty));
+        if(row < p.M) {   // no ncbias entry for rows past the batch; the TMA stores clip them
+          const int lc = s * RES_COLS;
+          switch(flags) {
+#define KGB_EPI_ROW(F) case (F): epilogue_row<(F)>(p, row, rl, n0 + lc, v, res, maskv, s_scale + lc, s_bias + lc, region); break;
+            KGB_EPI_WG_FLAGS(KGB_EPI_ROW)
+#undef KGB_EPI_ROW
+            default: break;   // launchConvWG launches no other
+          }
+        }
+        fence_proxy_async();
+        epi_wg_sync();
+        if(leader) {
+          const int c0 = n0 + s * RES_COLS;
+          const bool raw32 = (flags & EPI_FP32) != 0;
+          for(int h = 0; h < 2; h++) {
+            const int r0 = m0 + h * (BLOCK_M / 2);
+            if(p.raw_out != nullptr) tma_store_2d(&tmapRaw, smem_u32(region + h * (raw32 ? ACC_SLICE_BYTES : ACT_SLICE_BYTES) / 2), c0, r0);
+            if(p.act_out != nullptr) tma_store_2d(&tmapAct, smem_u32(region + ACT_SLICE_BYTES + h * (ACT_SLICE_BYTES / 2)), c0, r0);
+          }
+          bulk_commit();
+        }
+      }
+      tphase ^= 1;
+      if(leader) {
+        bulk_wait_read0();   // the stores have read the tile: the consumers may write the next one
+        mbar_arrive(smem_u32(&bars->t_empty));
+        chain_publish_tile(p.tile_flags, m0 / BLOCK_M);
+      }
+    }
+    pdl_wait();
+    return;
+  }
+
+  // ===================== consumers: warpgroup g owns tile rows 64g..64g+63, warp q of it rows 16q..16q+15 =====================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 184;");
+  const int g = (warp - 4) >> 2, q = warp & 3;
+  const int ry = p.ky / 2, rx = p.kx / 2;
+  const int lrow = g * 64 + q * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
+  const uint32_t lchunk = (uint32_t)(lane >> 4);
+  // acc[4j + 2h + e]: row 16q + lane/4 + 8h of the warpgroup's 64, column 8j + 2*(lane%4) + e
+  const int rloc = g * 64 + q * 16 + (lane >> 2);
+  int stage = 0, ph = 0;
+  uint32_t phase = 0, tphase = 0;
+  for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    int wp = 0;
+    float acc[N / 2];
+#pragma unroll
+    for(int i = 0; i < N / 2; i++) acc[i] = 0.0f;
+    fence_acc(acc);
+    // the main loop of kgb_conv_wg_kernel (one k-block = one A halo tile here)
+    int prev_stage = -1, dy = -ry, dx = -rx;
+    auto step = [&](uint32_t (&af)[4][4]) {
+      const int abuf = ph & 1;
+      if(dy == -ry && dx == -rx) {
+        mbar_wait(smem_u32(&bars->a_full[abuf]), (ph >> 1) & 1);
+        wp = bars->a_wp[abuf];
+      }
+      const uint32_t a_base = smem_base + abuf * a_buf_bytes;
+      const uint32_t r = (uint32_t)(lrow + halo + dy * wp + dx);
+#pragma unroll
+      for(int k = 0; k < 4; k++) ldmatrix_x4(a_base + r * 128u + (((2u * k + lchunk) ^ (r & 7u)) << 4), af[k]);
+      mbar_wait(smem_u32(&bars->full[stage]), phase);
+      const uint64_t db = make_smem_desc(smem_b + stage * b_tile_bytes);
+      wgmma_fence();
+#pragma unroll
+      for(int k = 0; k < 4; k++) Wgmma<N>::mma(acc, af[k], db + 2 * k);
+      wgmma_commit();
+      if(dy == ry && dx == rx) {
+        __syncwarp();
+        if(lane == 0) mbar_arrive(smem_u32(&bars->a_empty[abuf]));
+      }
+      wgmma_wait1();
+      if(prev_stage >= 0) {
+        __syncwarp();
+        if(lane == 0) mbar_arrive(smem_u32(&bars->empty[prev_stage]));
+      }
+      prev_stage = stage;
+      if(++stage == stages) { stage = 0; phase ^= 1; }
+      if(++dx > rx) {
+        dx = -rx;
+        if(++dy > ry) { dy = -ry; ph++; }
+      }
+    };
+    const int steps = phases * taps;
+    uint32_t af0[4][4], af1[4][4];
+    for(int i = 0; i + 1 < steps; i += 2) {
+      step(af0);
+      step(af1);
+    }
+    if(steps & 1) step(af0);
+    wgmma_wait0();
+    fence_acc(acc);
+    __syncwarp();
+    if(lane == 0) mbar_arrive(smem_u32(&bars->empty[prev_stage]));
+    // hand the accumulators to the epilogue warpgroup once it has read the previous tile out of the accumulator tile
+    mbar_wait(smem_u32(&bars->t_empty), tphase ^ 1);
+    tphase ^= 1;
+#pragma unroll
+    for(int j = 0; j < N / 8; j++)
+#pragma unroll
+      for(int h = 0; h < 2; h++)
+        *reinterpret_cast<float2*>(acc_tile + (j / 4) * ACC_SLICE_BYTES + slice_offset(rloc + 8 * h, 8 * (j % 4) + 2 * (lane & 3), true)) =
+          make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+    __syncwarp();
+    if(lane == 0) mbar_arrive(smem_u32(&bars->t_full));
+  }
+  pdl_wait();
+}
+
 static int g_smCount[64];   // per device ordinal, read by convWGInit
 static int* g_chainErrorHost;   // the sticky word chain_wait sets, in mapped host memory shared by every device
 static cudaError_t convPairInit();
@@ -590,6 +925,9 @@ cudaError_t convWGInit() {
                        cudaFuncSetAttribute(kgb_conv_wg_kernel<192>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
                        cudaFuncSetAttribute(kgb_conv_wg_kernel<224>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
                        cudaFuncSetAttribute(kgb_conv_wg_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
+#define KGB_EPI_WG_ATTR(N) cudaFuncSetAttribute(kgb_conv_wg_epi_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
+                       KGB_EPI_WG_SHAPES(KGB_EPI_WG_ATTR)
+#undef KGB_EPI_WG_ATTR
                        convPairInit()})
     if(e != cudaSuccess) return e;
   return cudaSuccess;
@@ -597,10 +935,11 @@ cudaError_t convWGInit() {
 
 // A chained launch (p.pred_flags set) may start while the previous kernel on the stream still runs
 template <class... Args>
-static cudaError_t launchChained(void (*kernel)(Args...), const ConvParams& p, int grid, int smem, cudaStream_t stream, Args... args) {
+static cudaError_t launchChained(void (*kernel)(Args...), const ConvParams& p, int grid, int threads, int smem, cudaStream_t stream,
+                                 Args... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(THREADS);
+  cfg.blockDim = dim3(threads);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
@@ -613,7 +952,34 @@ static cudaError_t launchChained(void (*kernel)(Args...), const ConvParams& p, i
 
 template <int N>
 static cudaError_t launchN(const ConvTmaps& tm, const ConvParams& p, int grid, int stages, int smem, cudaStream_t stream) {
-  return launchChained(kgb_conv_wg_kernel<N>, p, grid, smem, stream, tm.A, tm.B, tm.residual, tm.raw, tm.act, p, stages);
+  return launchChained(kgb_conv_wg_kernel<N>, p, grid, THREADS, smem, stream, tm.A, tm.B, tm.residual, tm.raw, tm.act, p, stages);
+}
+
+// Shared memory of kgb_conv_wg_epi_kernel: the accumulator tile and the residual slot come first, the weight ring gets what is left
+struct EpiLayout {
+  int stages = 0, smem = 0;
+};
+static EpiLayout epiLayout(const ConvParams& p) {
+  EpiLayout l;
+  const int halo = (p.ky / 2) * p.Wp + (p.kx / 2);
+  const int fixed = 1024 + 2 * aBufBytes(BLOCK_M + 2 * halo) + p.n_tile / RES_COLS * ACC_SLICE_BYTES + (p.residual != nullptr ? ACT_SLICE_BYTES : 0) +
+                    (int)sizeof(EpiBars) + 2 * p.n_tile * (int)sizeof(float);
+  l.stages = std::min(MAX_STAGES, (SMEM_LIMIT - fixed) / (p.n_tile * BLOCK_K * 2));
+  l.smem = fixed + l.stages * p.n_tile * BLOCK_K * 2;
+  return l;
+}
+
+bool convEpilogueWG(const ConvParams& p) {
+  if(!p.epi_wg || p.split || p.ky * p.kx == 1) return false;
+  const int f = epiFlags(p), halo = (p.ky / 2) * p.Wp + (p.kx / 2);
+  bool shape = false, epi = false;
+#define KGB_EPI_WG_IS(N) shape = shape || p.n_tile == N;
+  KGB_EPI_WG_SHAPES(KGB_EPI_WG_IS)
+#undef KGB_EPI_WG_IS
+#define KGB_EPI_WG_IS(F) epi = epi || f == (F);
+  KGB_EPI_WG_FLAGS(KGB_EPI_WG_IS)
+#undef KGB_EPI_WG_IS
+  return shape && epi && BLOCK_M + 2 * halo <= 256 && epiLayout(p).stages >= EPI_WG_MIN_STAGES;
 }
 
 cudaError_t launchConvWG(const ConvTmaps& tm, const ConvParams& p, cudaStream_t stream) {
@@ -627,6 +993,18 @@ cudaError_t launchConvWG(const ConvTmaps& tm, const ConvParams& p, cudaStream_t 
   const cudaError_t e = cudaGetDevice(&dev);
   if(e != cudaSuccess) return e;
   if(dev < 0 || dev >= 64 || g_smCount[dev] < 1) return cudaErrorInitializationError;   // convWGInit not run on this device
+  // persistent grid: at most one CTA per SM (the rings take all of shared memory), a multiple of num_n_tiles
+  const int tiles = p.num_m_tiles * p.num_n_tiles;
+  int grid = std::min(tiles, g_smCount[dev]) / p.num_n_tiles * p.num_n_tiles;
+  if(grid < p.num_n_tiles) grid = p.num_n_tiles;
+  if(convEpilogueWG(p)) {
+    const EpiLayout l = epiLayout(p);
+#define KGB_EPI_WG_LAUNCH(N) \
+    if(p.n_tile == N)        \
+      return launchChained(kgb_conv_wg_epi_kernel<N>, p, grid, EPI_WG_THREADS, l.smem, stream, tm.A, tm.B, tm.residual, tm.raw, tm.act, p, l.stages);
+    KGB_EPI_WG_SHAPES(KGB_EPI_WG_LAUNCH)
+#undef KGB_EPI_WG_LAUNCH
+  }
   const int bTile = p.n_tile * BLOCK_K * 2;
   // the stream and act rings and the BN copies come first; the weight ring gets what is left
   const int fixed = 1024 + 2 * aBufBytes(BLOCK_M + 2 * halo) + streamSlots(p) * streamSlotBytes(p) + ACT_SLOTS * actSlotBytes(p) +
@@ -635,10 +1013,6 @@ cudaError_t launchConvWG(const ConvTmaps& tm, const ConvParams& p, cudaStream_t 
   if(stages > MAX_STAGES) stages = MAX_STAGES;
   if(stages < 2) return cudaErrorInvalidValue;
   const int smem = fixed + stages * bTile;
-  // persistent grid: at most one CTA per SM (the rings take all of shared memory), a multiple of num_n_tiles
-  const int tiles = p.num_m_tiles * p.num_n_tiles;
-  int grid = std::min(tiles, g_smCount[dev]) / p.num_n_tiles * p.num_n_tiles;
-  if(grid < p.num_n_tiles) grid = p.num_n_tiles;
   switch(p.n_tile) {
     case 32: return launchN<32>(tm, p, grid, stages, smem, stream);
     case 64: return launchN<64>(tm, p, grid, stages, smem, stream);
@@ -1005,7 +1379,7 @@ static cudaError_t launchPairN(const ConvPairTmaps& tm, const ConvParams& p1, co
                                cudaStream_t stream) {
   auto k = p1.raw_fp32 ? (p2.raw_fp32 ? kgb_conv_pair_kernel<N2, N1, true, true> : kgb_conv_pair_kernel<N2, N1, true, false>)
                        : kgb_conv_pair_kernel<N2, N1, false, false>;
-  return launchChained(k, p1, grid, l.smem, stream, tm.A, tm.W1, tm.W2, tm.stream1, tm.stream2, tm.act2, p1, p2, l.stages, l.r_slots);
+  return launchChained(k, p1, grid, THREADS, l.smem, stream, tm.A, tm.W1, tm.W2, tm.stream1, tm.stream2, tm.act2, p1, p2, l.stages, l.r_slots);
 }
 
 cudaError_t launchConvPair(const ConvPairTmaps& tm, const ConvParams& p1, const ConvParams& p2, cudaStream_t stream) {

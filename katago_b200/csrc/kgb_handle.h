@@ -59,6 +59,7 @@ struct kgb_handle {
   bool nhwc = true;
   bool streamTrunkFp32 = true, streamInnerFp32 = false;
   bool fuseBoundaries = false;   // consecutive nested blocks' exit + entry 1x1 as one launch (launchConvPair)
+  bool epilogueWG = true;        // launchConvWG may take the epilogue-warpgroup kernel (convEpilogueWG); KGB_EPILOGUE_WG=0 keeps the other
   std::vector<void*> allocs;
   // inputs / outputs (device, fixed addresses so graphs can be replayed)
   float *dSpatial = nullptr, *dGlobal = nullptr, *dMeta = nullptr, *dOptimism = nullptr;   // dMeta: SGF-metadata nets only
@@ -82,6 +83,7 @@ struct kgb_handle {
   int* chain = nullptr;
   int chainSlots = 0;
   int chainedLaunches = 0;   // convolution launches per forward that are programmatic dependents of the one before
+  int epilogueWGLaunches = 0;   // convolution launches per forward that run with the epilogue warpgroup (convEpilogueWG)
   size_t chainStride() const { return (planRows(maxBatch) + 127) / 128; }
   int* chainFlags(int slot) const { return chain + (size_t)slot * chainStride(); }
   void allocChain() { chain = dalloc<int>((size_t)std::max(chainSlots, 1) * chainStride()); }
