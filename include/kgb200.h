@@ -136,6 +136,9 @@ KGB_API int kgb_handle_chained_launches_per_forward(const kgb_handle* handle);
 /* Of those, the convolution launches that run with a dedicated epilogue warpgroup (the 3x3 layers in fp16 mode; KGB_EPILOGUE_WG=0 at
  * handle creation turns it off). */
 KGB_API int kgb_handle_epilogue_wg_launches_per_forward(const kgb_handle* handle);
+/* Of the fused block boundaries, those that run with the exit's epilogue in a warpgroup of its own (b18c384nbt's in fp16 mode with
+ * fp16 streams; KGB_PAIR_EPILOGUE_WG=0 at handle creation keeps the other kernel, with the same results). */
+KGB_API int kgb_handle_pair_epilogue_wg_launches_per_forward(const kgb_handle* handle);
 /* The row layout the last forward or self-play wave on the handle used (waits for the handle's stream): the rows and 128-row
  * tiles every convolution ran over, and the number of segments (board widths).  Each image takes (h+pad)*(w+pad) rows for the
  * bounding box w x h of its mask, so a batch of small boards takes fewer rows than n*(nnYLen+pad)*(nnXLen+pad).  All zero

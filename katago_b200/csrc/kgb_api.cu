@@ -67,6 +67,21 @@ static CUtensorMap makeTmap2D(const void* ptr, uint64_t rows, uint64_t cols, uin
   return m;
 }
 
+// 2-D fp16 row-major tensor [rows][cols], box {32 cols, boxRows}, 64B swizzle, zero OOB fill: one 32-column k-chunk of a packed
+// weight matrix, K-major, for kgb_conv_pair_epi_kernel's entry MMAs.
+static CUtensorMap makeTmapK32(const void* ptr, uint64_t rows, uint64_t cols, uint32_t boxRows) {
+  CUtensorMap m;
+  cuuint64_t gdim[2] = {cols, rows};
+  cuuint64_t gstride[1] = {cols * sizeof(__half)};
+  cuuint32_t box[2] = {(cuuint32_t)kConvPairEpiChunk, boxRows};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = getEncodeTiled()(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
+                                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if(r != CUDA_SUCCESS) throw CudaFailure("cuTensorMapEncodeTiled (k32) failed with CUresult " + std::to_string((int)r));
+  return m;
+}
+
 // Epilogue slices of a stream or operand [rows][cols], fp32 or fp16, box {32 cols, convSliceBoxRows() rows}: the residual the
 // convolution's epilogue reads into shared memory and the raw and activated outputs it stores from there, 128B-swizzled for fp32
 // (128 B rows) and 64B-swizzled for fp16 (64 B rows), zero OOB fill (rows past the end are clipped on store).
@@ -259,6 +274,7 @@ struct Builder {
     p.bn_scale = bn.scale; p.bn_bias = bn.bias; p.act = bn.act;
     p.mask = hh.dMask;
     p.epi_wg = hh.epilogueWG ? 1 : 0;
+    p.pair_epi_wg = hh.pairEpilogueWG ? 1 : 0;
     return p;
   }
 
@@ -269,9 +285,11 @@ struct Builder {
   // Returns false, emitting nothing, when the kernel does not take these shapes or epilogues.
   bool emitConvPair(const ConvWeights& wpost, const __half* innerA, void* S, bool sFp32, BNDev bn1, const ConvWeights& wpre, void* innerS,
                     bool innerFp32, __half* innerAOut, BNDev bn2) {
-    if(!convPairSupported(convParams(h, h.maxBatch, wpost, S, sFp32, nullptr, S, sFp32, nullptr, bn1),
-                          convParams(h, h.maxBatch, wpre, nullptr, false, nullptr, innerS, innerFp32, innerAOut, bn2)))
-      return false;
+    const ConvParams q1 = convParams(h, h.maxBatch, wpost, S, sFp32, nullptr, S, sFp32, nullptr, bn1);
+    const ConvParams q2 = convParams(h, h.maxBatch, wpre, nullptr, false, nullptr, innerS, innerFp32, innerAOut, bn2);
+    if(!convPairSupported(q1, q2)) return false;
+    // the kernel choice depends on the shapes and streams only, which do not change with the batch
+    const bool epi = convPairEpilogueWG(q1, q2);
     kgb_handle* hp = &h;
     const ChainLink link = nextLink();
     h.ops.push_back([=](int n, cudaStream_t s) {
@@ -281,15 +299,16 @@ struct Builder {
       ConvPairTmaps tm;
       memset(&tm, 0, sizeof(tm));
       tm.A = makeTmap2D(innerA, (uint64_t)p1.M, (uint64_t)wpost.cin_p, (uint32_t)convABoxRows(1, 1, p1.Wp));
-      tm.W1 = makeTmap2D(wpost.w, (uint64_t)wpost.cout_p, (uint64_t)wpost.cin_p, (uint32_t)kConvPairChunk);
-      tm.W2 = wpre.tmapB;
+      tm.W1 = makeTmap2D(wpost.w, (uint64_t)wpost.cout_p, (uint64_t)wpost.cin_p, (uint32_t)(epi ? kConvPairEpiChunk : kConvPairChunk));
+      tm.W2 = epi ? makeTmapK32(wpre.w, (uint64_t)wpre.cout_p, (uint64_t)wpre.cin_p, (uint32_t)wpre.n_tile) : wpre.tmapB;
       tm.stream1 = makeTmapSlices(S, (uint64_t)p1.M, (uint64_t)wpost.cout_p, sFp32);
       tm.stream2 = makeTmapSlices(innerS, (uint64_t)p1.M, (uint64_t)wpre.cout_p, innerFp32);
       tm.act2 = makeTmapSlices(innerAOut, (uint64_t)p1.M, (uint64_t)wpre.cout_p, false);
       CK(launchConvPair(tm, p1, p2, s));
     });
-    linkConvOp(link, kConvPairParts);
+    linkConvOp(link, convPairChainParts(q1, q2));
     h.launchesPerForward++;
+    h.pairEpilogueWGLaunches += epi ? 1 : 0;
     return true;
   }
 
@@ -678,12 +697,18 @@ static bool epilogueWGFromEnv() {
   const char* e = getenv("KGB_EPILOGUE_WG");
   return !(e && std::string(e) == "0");
 }
+// KGB_PAIR_EPILOGUE_WG=0 keeps every fused block boundary on kgb_conv_pair_kernel, in the same way
+static bool pairEpilogueWGFromEnv() {
+  const char* e = getenv("KGB_PAIR_EPILOGUE_WG");
+  return !(e && std::string(e) == "0");
+}
 
 // The settings that decide how the graph builder lays the weights out
 static void copyBuildSettings(kgb_handle& dst, const kgb_handle& src) {
   dst.device = src.device; dst.model = src.model; dst.L = src.L; dst.maxBatch = src.maxBatch; dst.split = src.split;
   dst.nhwc = src.nhwc; dst.streamTrunkFp32 = src.streamTrunkFp32; dst.streamInnerFp32 = src.streamInnerFp32;
   dst.fuseBoundaries = src.fuseBoundaries; dst.epilogueWG = src.epilogueWG;
+  dst.pairEpilogueWG = src.pairEpilogueWG;
 }
 
 // Makes device `dev` (-1: the current device) current, after checking that it exists and is the sm_90a device the kernels are
@@ -770,6 +795,7 @@ KGB_API int kgb_handle_create(kgb_context* ctx, const kgb_model* model, int max_
     const char* ragged = getenv("KGB_RAGGED_ROWS");
     h.plan.ragged = !(ragged && std::string(ragged) == "0");
     h.epilogueWG = epilogueWGFromEnv();
+    h.pairEpilogueWG = pairEpilogueWGFromEnv();
     CK(cudaStreamCreateWithFlags(&h.stream, cudaStreamNonBlocking));
     CK(convWGInit());
     CK(cudaStreamCreateWithFlags(&h.copyStream, cudaStreamNonBlocking));
@@ -910,6 +936,7 @@ KGB_API uint64_t kgb_handle_stream(kgb_handle* handle) { return handle ? (uint64
 KGB_API int kgb_handle_launches_per_forward(const kgb_handle* handle) { return handle ? handle->launchesPerForward : 0; }
 KGB_API int kgb_handle_chained_launches_per_forward(const kgb_handle* handle) { return handle ? handle->chainedLaunches : 0; }
 KGB_API int kgb_handle_epilogue_wg_launches_per_forward(const kgb_handle* handle) { return handle ? handle->epilogueWGLaunches : 0; }
+KGB_API int kgb_handle_pair_epilogue_wg_launches_per_forward(const kgb_handle* handle) { return handle ? handle->pairEpilogueWGLaunches : 0; }
 
 KGB_API int kgb_handle_get_layout_stats(kgb_handle* handle, int64_t* rows, int64_t* m_tiles, int64_t* segments) {
   return guarded([&] {
@@ -1319,6 +1346,7 @@ struct BoundaryConv {
     h.device = selectDevice(-1);
     h.model = &dummy;
     h.maxBatch = n;
+    h.pairEpilogueWG = pairEpilogueWGFromEnv();
     h.L = boardLayout(X, Y, 1);
     CK(cudaStreamCreateWithFlags(&h.stream, cudaStreamNonBlocking));
     CK(convWGInit());

@@ -51,6 +51,7 @@ struct ConvParams {
   const int* pred_flags;  // the previous launch's tile_flags when this launch is chained to it, else null
   int pred_parts;         // the value a tile flag of the previous launch has once the tile is written (convChainParts)
   int epi_wg;             // launchConvWG may take the epilogue-warpgroup kernel (convEpilogueWG); 0 keeps kgb_conv_wg_kernel
+  int pair_epi_wg;        // launchConvPair may take the exit-epilogue-warpgroup kernel (convPairEpilogueWG); 0 keeps kgb_conv_pair_kernel
 };
 
 // fp32 activation functions of the small kernels, and of the convolution epilogue except its mish, which epilogue_store
@@ -115,15 +116,25 @@ cudaError_t convWGInit();  // per device, before the first launch (sets the kern
 // epilogue writes them, and there is no halo).  Tensor maps: A = p1's operand, box {64, 128}; W1 = the exit's packed weights, box
 // {64, 64}; W2 = the entry's, box {64, p2.n_tile}; stream1 = p1's residual and raw stream, stream2 = p2.raw_out, act2 = p2.act_out
 // (slice boxes as in ConvTmaps).  Chaining as launchConvWG, with p1's chain fields; a tile is written (all of p1's and p2's outputs)
-// when its flag reaches kConvPairParts.
+// when its flag reaches convPairChainParts.
+// When convPairEpilogueWG(p1, p2), the exit is made in chunks of kConvPairEpiChunk columns instead: W1 has box {64,
+// kConvPairEpiChunk}, and W2 box {kConvPairEpiChunk, p2.n_tile} with the 64B swizzle (makeTmapK32 in kgb_api.cu).
 struct ConvPairTmaps {
   CUtensorMap A, W1, W2, stream1, stream2, act2;
 };
-static constexpr int kConvPairChunk = 64;   // box rows of W1
-static constexpr int kConvPairParts = 2;    // one per consumer warpgroup
+static constexpr int kConvPairChunk = 64;      // box rows of W1
+static constexpr int kConvPairEpiChunk = 32;   // box rows of W1 and box columns of W2 for kgb_conv_pair_epi_kernel
+static constexpr int kConvPairParts = 2;       // one per consumer warpgroup
 // Whether launchConvPair takes these launches: fp16 operands, mish at both ends, 1x1 filters, (inner, trunk) widths the kernel is
 // compiled for, and rings that fit in shared memory.
 bool convPairSupported(const ConvParams& p1, const ConvParams& p2);
+// Whether launchConvPair runs them with kgb_conv_pair_epi_kernel (the exit's epilogue in a warpgroup of its own, fed through
+// shared-memory accumulator slots) rather than kgb_conv_pair_kernel: p1.pair_epi_wg set, fp16 streams, (inner, trunk) = (192, 384).
+// Both kernels give the same bits.
+bool convPairEpilogueWG(const ConvParams& p1, const ConvParams& p2);
+// The value a tile flag of the launch reaches once the tile is written: kConvPairParts, or 3 with the exit-epilogue warpgroup
+// (each MMA warpgroup publishes its half of the entry's outputs, the epilogue warpgroup the exit's).
+int convPairChainParts(const ConvParams& p1, const ConvParams& p2);
 cudaError_t launchConvPair(const ConvPairTmaps& tm, const ConvParams& p1, const ConvParams& p2, cudaStream_t stream);
 
 }  // namespace kgb

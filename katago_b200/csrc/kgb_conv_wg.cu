@@ -100,6 +100,7 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t sr
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -140,6 +141,13 @@ __device__ int* g_chainError;   // host-mapped sticky word (convWGInit), set whe
 // to the register pressure of the consumers' accumulators.
 __device__ __noinline__ void chain_publish(int* flags, int m_tile) {
   bulk_wait0();
+  fence_proxy_async_global();
+  red_release_gpu_add(flags + m_tile, 1);
+}
+
+// The same for the tile whose stores are all but the last 4 bulk groups the thread has committed
+__device__ __noinline__ void chain_publish_before4(int* flags, int m_tile) {
+  asm volatile("cp.async.bulk.wait_group 4;" ::: "memory");
   fence_proxy_async_global();
   red_release_gpu_add(flags + m_tile, 1);
 }
@@ -601,12 +609,13 @@ __device__ __noinline__ void chain_publish_tile(int* flags, int m_tile) {
 // leave in different iterations) the epilogue brings the warp together with __syncwarp.
 __device__ __forceinline__ void epi_wg_sync() { asm volatile("bar.sync 4, 128;" ::: "memory"); }
 
-// One row's part of slice s: its 16 column pairs through epilogue_store<F>, the outputs gathered in registers and written into
-// the slice `region` it was read from as 16-byte chunks (every row of the slice has been read by then).
+// One row's part of slice s: its 16 column pairs through epilogue_store<F>, the outputs gathered in registers and written as
+// 16-byte chunks, the raw output into `region` (the slice it was read from: every row of the slice has been read by then) and
+// the activated operand into `act_region`.
 template <int F>
 __device__ __forceinline__ void epilogue_row(const ConvParams& p, int row, int rl, int col0, const float (&v)[RES_COLS],
                                              const uint32_t (&res)[RES_COLS / 2], float maskv, const float* sc, const float* bi,
-                                             uint8_t* region) {
+                                             uint8_t* region, uint8_t* act_region) {
   constexpr bool raw32 = (F & EPI_FP32) != 0;
   float2 rawf[RES_COLS / 2];
   uint32_t rawh[RES_COLS / 2], act[RES_COLS / 2];
@@ -633,7 +642,7 @@ __device__ __forceinline__ void epilogue_row(const ConvParams& p, int row, int r
   if(F & EPI_MISH) {
 #pragma unroll
     for(int k = 0; k < RES_COLS / 8; k++)
-      *reinterpret_cast<uint4*>(region + ACT_SLICE_BYTES + slice_offset(rl, 8 * k, false)) =
+      *reinterpret_cast<uint4*>(act_region + slice_offset(rl, 8 * k, false)) =
         make_uint4(act[4 * k], act[4 * k + 1], act[4 * k + 2], act[4 * k + 3]);
   }
 }
@@ -783,7 +792,7 @@ kgb_conv_wg_epi_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_c
         if(row < p.M) {   // no ncbias entry for rows past the batch; the TMA stores clip them
           const int lc = s * RES_COLS;
           switch(flags) {
-#define KGB_EPI_ROW(F) case (F): epilogue_row<(F)>(p, row, rl, n0 + lc, v, res, maskv, s_scale + lc, s_bias + lc, region); break;
+#define KGB_EPI_ROW(F) case (F): epilogue_row<(F)>(p, row, rl, n0 + lc, v, res, maskv, s_scale + lc, s_bias + lc, region, region + ACT_SLICE_BYTES); break;
             KGB_EPI_WG_FLAGS(KGB_EPI_ROW)
 #undef KGB_EPI_ROW
             default: break;   // launchConvWG launches no other
@@ -1338,6 +1347,372 @@ kgb_conv_pair_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_con
   pdl_wait();
 }
 
+// ------------------------------------------------------------------------------------------------------------
+// Fused block boundary with an exit-epilogue warpgroup (kgb_conv_pair_epi_kernel, launchConvPair when convPairEpilogueWG)
+// ------------------------------------------------------------------------------------------------------------
+// In kgb_conv_pair_kernel the two consumer warpgroups run each exit chunk's epilogue themselves, so only one chunk of entry MMAs
+// overlaps it and the loads and stores in flight wait on their arithmetic.  Here a fourth warpgroup runs the exit's epilogue,
+// 512 threads, with exit chunks of PAIR_EPI_NC = 32 columns:
+//   warpgroup 0     TMA producers: the inner operand tile, the weight chunks in consumption order (W1(0), then W1(c+1), W2(c)),
+//                   the exit's residual slices into a ring.
+//   warpgroups 1-2  MMA, 64 rows each.  Step c issues P1(c) (acc1 = A x W1 chunk c), writes acc1 as fp32 into accumulator slot
+//                   c & 1 (slice_offset's fp32 layout) and arrives on acc_full, then issues P2(c-1) (acc2 += T x W2 chunk c-1) once
+//                   T slot (c-1) & 1 is full: P1(c+1) is handed over while the epilogue warpgroup works on chunk c.  After the
+//                   tile's last P2 they hand over the next tile's chunk 0, then run the entry's epilogue from acc2 as
+//                   kgb_conv_pair_kernel does, and publish their halves of it 3 chunks into the next tile.
+//   warpgroup 3     the exit's epilogue, one thread per row: for chunk c it reads its row of accumulator slot c & 1 and of the
+//                   residual slice, applies epilogue_store<F1> (epilogue_row), writes the raw trunk stream back over the residual
+//                   slice for its TMA store and the activated operand into T slot c & 1, and arrives on t_full.  It publishes the
+//                   tile's exit part once its stores are complete, 3 chunks into the next tile, so a tile is written when its flag
+//                   reaches 3 (convPairChainParts).
+// Every exit column is still summed over K1 in k-block, k16 order and every entry output over the trunk channels in k16 order (12
+// chunks of 2 k16 steps instead of 6 of 4): the same bits as kgb_conv_pair_kernel and the two launches.
+// Shared memory for (192, 384) with fp16 streams: A tile 48 KB, 2 accumulator slots of 16 KB, 2 T slots of 8 KB, a 4-slot residual
+// ring of 8 KB, entry staging 2 x 8 KB raw + 2 x 8 KB act, 5 weight stages of 12 KB (W1 chunk: K1/64 boxes {64, 32}, 128B swizzle;
+// W2 chunk: one box {32, N2}, 64B swizzle), PairEpiBars and the BN constants: 231,184 B of the 232,448.  A 64-column chunk would need
+// 32 KB accumulator slots and 24 KB weight stages, 64 KB more than fits.  Registers after setmaxnreg: producers 40, MMA 184 (acc2 96,
+// acc1 16), epilogue 104.
+static constexpr int PAIR_EPI_NC = RES_COLS;
+static constexpr int PAIR_EPI_THREADS = 512;
+
+struct __align__(8) PairEpiBars {
+  uint64_t full[MAX_STAGES];
+  uint64_t empty[MAX_STAGES];
+  uint64_t a_full, a_empty;     // the inner operand tile of the current tile
+  uint64_t r_full[RES_SLOTS];   // residual slice landed
+  uint64_t r_empty[RES_SLOTS];  // residual slice read and the raw stream written over it stored
+  uint64_t acc_full[2];         // accumulator slot written by every MMA warp
+  uint64_t acc_empty[2];        // accumulator slot read by every epilogue warp
+  uint64_t t_full[2];           // T slot written by the epilogue warpgroup
+  uint64_t t_empty[2];          // T slot read by every MMA warp's P2
+};
+
+// dynamic smem: [<=1023 B slack][A tile][2 x accumulator slot][2 x T slot][residual ring][2 x raw staging][2 x act slice]
+//               [stages x weights][PairEpiBars][BN scale / bias: exit N1, entry N2]
+static PairLayout pairEpiLayout(const ConvParams& p1, const ConvParams& p2) {
+  PairLayout l;
+  const int n2 = p2.cout_p, n1 = p1.cout_p;
+  const int wBytes = n2 * PAIR_EPI_NC * 2;
+  const int fixed = 1024 + BLOCK_M * n2 * 2 + 2 * ACC_SLICE_BYTES + 2 * ACT_SLICE_BYTES + RES_SLOTS * ACT_SLICE_BYTES +
+                    STAGE_SLOTS * ACT_SLICE_BYTES + ACT_SLOTS * ACT_SLICE_BYTES + (int)sizeof(PairEpiBars) + 2 * (n1 + n2) * (int)sizeof(float);
+  l.r_slots = RES_SLOTS;
+  l.stages = std::min(MAX_STAGES, (SMEM_LIMIT - fixed) / wBytes);
+  l.smem = fixed + l.stages * wBytes;
+  return l;
+}
+
+template <int N2, int N1>
+__global__ void __launch_bounds__(PAIR_EPI_THREADS, 1)
+kgb_conv_pair_epi_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapW1,
+                         const __grid_constant__ CUtensorMap tmapW2, const __grid_constant__ CUtensorMap tmapS1,
+                         const __grid_constant__ CUtensorMap tmapS2, const __grid_constant__ CUtensorMap tmapA2,
+                         const __grid_constant__ ConvParams p1, const __grid_constant__ ConvParams p2, int stages) {
+  constexpr int F1 = EPI_RES | EPI_RAW | EPI_MISH;
+  constexpr int F2 = EPI_RAW | EPI_MISH;
+  constexpr int NC = PAIR_EPI_NC;
+  constexpr int K1 = N2;
+  constexpr int A_BYTES = BLOCK_M * K1 * 2;
+  constexpr int W_BYTES = N2 * NC * 2;
+  constexpr int chunks = N1 / NC;
+  static_assert(chunks >= 4, "the MMA loop keeps the P2 of two chunks in flight; tiles are published 3 chunks into the next");
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t smem_acc = smem_base + A_BYTES;
+  const uint32_t smem_t = smem_acc + 2 * ACC_SLICE_BYTES;
+  const uint32_t smem_r = smem_t + 2 * ACT_SLICE_BYTES;
+  const uint32_t smem_stg = smem_r + RES_SLOTS * ACT_SLICE_BYTES;
+  const uint32_t smem_act = smem_stg + STAGE_SLOTS * ACT_SLICE_BYTES;
+  const uint32_t smem_w = smem_act + ACT_SLOTS * ACT_SLICE_BYTES;
+  uint8_t* const smem = smem_raw + (smem_base - smem_u32(smem_raw));
+  PairEpiBars* bars = reinterpret_cast<PairEpiBars*>(smem + (smem_w - smem_base) + (size_t)stages * W_BYTES);
+  float* const s_scale1 = reinterpret_cast<float*>(bars + 1);
+  float* const s_bias1 = s_scale1 + N1;
+  float* const s_scale2 = s_bias1 + N1;
+  float* const s_bias2 = s_scale2 + N2;
+
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  const int tiles = __ldg(p1.m_tiles);
+
+  pdl_launch_dependents();
+  if(threadIdx.x == 0) {
+    for(const CUtensorMap* m : {&tmapA, &tmapW1, &tmapW2, &tmapS1, &tmapS2, &tmapA2})
+      asm volatile("prefetch.tensormap [%0];" ::"l"(m) : "memory");
+    for(int s = 0; s < stages; s++) {
+      mbar_init(smem_u32(&bars->full[s]), 1);
+      mbar_init(smem_u32(&bars->empty[s]), CONSUMER_WARPS);
+    }
+    mbar_init(smem_u32(&bars->a_full), 1);
+    mbar_init(smem_u32(&bars->a_empty), CONSUMER_WARPS);
+    for(int s = 0; s < RES_SLOTS; s++) {
+      mbar_init(smem_u32(&bars->r_full[s]), 1);
+      mbar_init(smem_u32(&bars->r_empty[s]), 1);
+    }
+    for(int s = 0; s < 2; s++) {
+      mbar_init(smem_u32(&bars->acc_full[s]), CONSUMER_WARPS);
+      mbar_init(smem_u32(&bars->acc_empty[s]), 4);
+      mbar_init(smem_u32(&bars->t_full[s]), 1);
+      mbar_init(smem_u32(&bars->t_empty[s]), CONSUMER_WARPS);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if(warp < 4) {
+    // ===================== TMA producers =====================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if(warp == 0 && lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0, aphase = 0;
+      auto loadW = [&](bool entry, int c) {
+        mbar_wait(smem_u32(&bars->empty[stage]), phase ^ 1);
+        const uint32_t full = smem_u32(&bars->full[stage]), dst = smem_w + stage * W_BYTES;
+        mbar_arrive_expect_tx(full, (uint32_t)W_BYTES);
+        if(entry) tma_load_2d(dst, &tmapW2, full, c * NC, 0);
+        else
+          for(int kb = 0; kb < K1 / BLOCK_K; kb++) tma_load_2d(dst + kb * NC * 128, &tmapW1, full, kb * BLOCK_K, c * NC);
+        if(++stage == stages) { stage = 0; phase ^= 1; }
+      };
+      bool pre = (int)blockIdx.x < tiles;
+      if(pre) loadW(false, 0);
+      for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        const int m0 = tile * BLOCK_M;
+        chain_wait(p1.pred_flags, p1.pred_parts, tile, tiles);
+        mbar_wait(smem_u32(&bars->a_empty), aphase ^ 1);
+        const uint32_t afull = smem_u32(&bars->a_full);
+        mbar_arrive_expect_tx(afull, (uint32_t)A_BYTES);
+        for(int kb = 0; kb < K1 / BLOCK_K; kb++) tma_load_2d(smem_base + kb * BLOCK_M * 128, &tmapA, afull, kb * BLOCK_K, m0);
+        aphase ^= 1;
+        if(!pre) loadW(false, 0);
+        pre = false;
+        for(int c = 0; c < chunks; c++) {
+          if(c + 1 < chunks) loadW(false, c + 1);
+          loadW(true, c);
+        }
+      }
+    }
+    else if(warp == 1 && lane == 0) {
+      int rs = 0;
+      uint32_t rphase = 0;
+      for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        const int m0 = tile * BLOCK_M;
+        chain_wait(p1.pred_flags, p1.pred_parts, tile, tiles);
+        for(int s = 0; s < chunks; s++) {
+          mbar_wait(smem_u32(&bars->r_empty[rs]), rphase ^ 1);
+          const uint32_t rfull = smem_u32(&bars->r_full[rs]), dst = smem_r + rs * ACT_SLICE_BYTES;
+          mbar_arrive_expect_tx(rfull, (uint32_t)ACT_SLICE_BYTES);
+          tma_load_2d(dst, &tmapS1, rfull, s * RES_COLS, m0);
+          tma_load_2d(dst + ACT_SLICE_BYTES / 2, &tmapS1, rfull, s * RES_COLS, m0 + BLOCK_M / 2);
+          if(++rs == RES_SLOTS) { rs = 0; rphase ^= 1; }
+        }
+      }
+    }
+    return;
+  }
+
+  if(warp >= 12) {
+    // ===================== exit epilogue: thread rl finishes row rl of every chunk =====================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 104;");
+    const int rl = threadIdx.x - 384;
+    const bool leader = rl == 0;    // issues the TMA stores and publishes the tiles' exit part
+    for(int i = rl; i < N1; i += 128) { s_scale1[i] = __ldg(p1.bn_scale + i); s_bias1[i] = __ldg(p1.bn_bias + i); }
+    epi_wg_sync();
+    int rs = 0, prev_rs = -1, k = 0;   // k: chunks finished by this CTA, whose parity picks the accumulator and T slot
+    uint32_t rphase = 0;
+    int pending = -1;   // the tile whose exit stores were issued last and are not published yet
+    for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+      const int m0 = tile * BLOCK_M, row = m0 + rl;
+      const float maskv = row < p1.M ? __ldg(p1.mask + row) : 0.0f;
+#pragma unroll 1
+      for(int c = 0; c < chunks; c++, k++) {
+        const int slot = k & 1;
+        const uint32_t par = (k >> 1) & 1;
+        uint8_t* const rslot = smem + (smem_r - smem_base) + rs * ACT_SLICE_BYTES;
+        mbar_wait(smem_u32(&bars->acc_full[slot]), par);
+        __syncwarp();
+        const uint8_t* const aslot = smem + (smem_acc - smem_base) + slot * ACC_SLICE_BYTES;
+        float v[RES_COLS];
+#pragma unroll
+        for(int j = 0; j < RES_COLS / 4; j++) {
+          const float4 f = *reinterpret_cast<const float4*>(aslot + slice_offset(rl, 4 * j, true));
+          v[4 * j] = f.x; v[4 * j + 1] = f.y; v[4 * j + 2] = f.z; v[4 * j + 3] = f.w;
+        }
+        mbar_wait(smem_u32(&bars->r_full[rs]), rphase);
+        __syncwarp();
+        uint32_t res[RES_COLS / 2];
+#pragma unroll
+        for(int j = 0; j < RES_COLS / 8; j++) {
+          const uint4 u = *reinterpret_cast<const uint4*>(rslot + slice_offset(rl, 8 * j, false));
+          res[4 * j] = u.x; res[4 * j + 1] = u.y; res[4 * j + 2] = u.z; res[4 * j + 3] = u.w;
+        }
+        // the warp's rows of the accumulator slot are read: the MMA warpgroups may write chunk k + 2 into it
+        __syncwarp();
+        if(lane == 0) mbar_arrive(smem_u32(&bars->acc_empty[slot]));
+        mbar_wait(smem_u32(&bars->t_empty[slot]), par ^ 1);   // P2 of chunk k - 2 has read the T slot
+        __syncwarp();
+        uint8_t* const tslot = smem + (smem_t - smem_base) + slot * ACT_SLICE_BYTES;
+        if(row < p1.M) epilogue_row<F1>(p1, row, rl, c * NC, v, res, maskv, s_scale1 + c * NC, s_bias1 + c * NC, rslot, tslot);
+        fence_proxy_async();   // the raw slice for its TMA store, the T slot for the wgmma that reads it
+        epi_wg_sync();
+        if(leader) {
+          mbar_arrive(smem_u32(&bars->t_full[slot]));
+          for(int h = 0; h < 2; h++)
+            tma_store_2d(&tmapS1, smem_u32(rslot + h * (ACT_SLICE_BYTES / 2)), c * NC, m0 + h * (BLOCK_M / 2));
+          bulk_commit();
+          // the previous chunk's store has read its residual slot: the slot may be refilled (only warp 0 waits for that)
+          bulk_wait_read1();
+          if(prev_rs >= 0) mbar_arrive(smem_u32(&bars->r_empty[prev_rs]));
+          // the previous tile's exit part, once the stores of this tile's first 4 chunks are the only ones that may be in flight:
+          // publishing at the end of a tile would hold the warpgroup until its last stores are complete
+          if(c == 3 && pending >= 0) chain_publish_before4(p1.tile_flags, pending);
+        }
+        prev_rs = rs;
+        if(++rs == RES_SLOTS) { rs = 0; rphase ^= 1; }
+      }
+      pending = tile;
+    }
+    if(leader && pending >= 0) chain_publish(p1.tile_flags, pending);
+    if(leader) bulk_wait0();
+    pdl_wait();
+    return;
+  }
+
+  // ===================== MMA warpgroups: warpgroup g owns tile rows 64g..64g+63 =====================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 184;");
+  const int g = (warp - 4) >> 2, q = warp & 3;
+  const bool leader = q == 0 && lane == 0;
+  const int rloc = g * 64 + q * 16 + (lane >> 2);
+  for(int i = threadIdx.x - 128; i < N2; i += 32 * CONSUMER_WARPS) { s_scale2[i] = __ldg(p2.bn_scale + i); s_bias2[i] = __ldg(p2.bn_bias + i); }
+  consumer_sync();
+
+  int stage = 0, ps = 0, as = 0, k = 0;   // k: as the epilogue warpgroup's
+  uint32_t phase = 0, aphase = 0;
+  uint8_t* const acc_ring = smem + (smem_acc - smem_base);
+  uint8_t* const stg_ring = smem + (smem_stg - smem_base);
+  uint8_t* const act_ring = smem + (smem_act - smem_base);
+  int pending = -1;   // as in kgb_conv_wg_kernel
+  auto take = [&]() {
+    const int st = stage;
+    mbar_wait(smem_u32(&bars->full[st]), phase);
+    if(++stage == stages) { stage = 0; phase ^= 1; }
+    return st;
+  };
+  auto release = [&](uint32_t bar) {
+    __syncwarp();
+    if(lane == 0) mbar_arrive(bar);
+  };
+  float acc1[NC / 2];
+  // P1 of the chunk with index kc (acc1 = A rows 64g.. x the W1 chunk of the next weight stage, K1 / 64 k-blocks of 4 k16 steps, as
+  // the exit's launch sums them), handed to the epilogue warpgroup through accumulator slot kc & 1 once it has read chunk kc - 2
+  // out of it.  The wait for P1 also completes every P2 issued before it.
+  auto handChunk = [&](int kc, bool last) {
+#pragma unroll
+    for(int i = 0; i < NC / 2; i++) acc1[i] = 0.0f;
+    fence_acc(acc1);
+    wgmma_fence();
+    const int st1 = take();
+    const uint32_t w = smem_w + st1 * W_BYTES, a = smem_base + g * 64 * 128;
+#pragma unroll
+    for(int kb = 0; kb < K1 / BLOCK_K; kb++)
+#pragma unroll
+      for(int j = 0; j < 4; j++)
+        WgmmaSS<NC>::mma(acc1, make_smem_desc(a + kb * BLOCK_M * 128) + 2 * j, make_smem_desc(w + kb * NC * 128) + 2 * j);
+    wgmma_commit();
+    wgmma_wait0();
+    fence_acc(acc1);
+    release(smem_u32(&bars->empty[st1]));
+    if(last) release(smem_u32(&bars->a_empty));   // the tile's last P1: the next tile's A may land
+    const int slot = kc & 1;
+    mbar_wait(smem_u32(&bars->acc_empty[slot]), ((kc >> 1) & 1) ^ 1);
+    uint8_t* const dst = acc_ring + slot * ACC_SLICE_BYTES;
+#pragma unroll
+    for(int j = 0; j < NC / 8; j++)
+#pragma unroll
+      for(int h = 0; h < 2; h++)
+        *reinterpret_cast<float2*>(dst + slice_offset(rloc + 8 * h, 8 * j + 2 * (lane & 3), true)) =
+          make_float2(acc1[4 * j + 2 * h], acc1[4 * j + 2 * h + 1]);
+    release(smem_u32(&bars->acc_full[slot]));
+  };
+  bool have0 = false;   // the tile's chunk 0 was handed over before the previous tile's entry epilogue
+  for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int m0 = tile * BLOCK_M;
+    const float mask0 = m0 + rloc < p1.M ? __ldg(p1.mask + m0 + rloc) : 0.0f;
+    const float mask1 = m0 + rloc + 8 < p1.M ? __ldg(p1.mask + m0 + rloc + 8) : 0.0f;
+    float acc2[N2 / 2];
+#pragma unroll
+    for(int i = 0; i < N2 / 2; i++) acc2[i] = 0.0f;
+    fence_acc(acc2);   // no access to acc2 from here to the tile's last wait: P2(c - 1) runs on while P1(c) is handed off
+    if(!have0) {
+      mbar_wait(smem_u32(&bars->a_full), aphase);
+      aphase ^= 1;
+    }
+    // P2(c): acc2 += T slot rows 64g.. x W2 chunk c (its k16 steps in order), once the epilogue warpgroup has filled the slot;
+    // returns the weight stage, released with the T slot once the MMAs are complete (releaseP2)
+    auto issueP2 = [&](int c) {
+      const int tslot = (k + c) & 1;
+      mbar_wait(smem_u32(&bars->t_full[tslot]), ((k + c) >> 1) & 1);
+      const int st = take();
+      const uint32_t w = smem_w + st * W_BYTES, t = smem_t + tslot * ACT_SLICE_BYTES + g * 64 * 64;
+#pragma unroll
+      for(int j = 0; j < NC / 16; j++) WgmmaSS<N2>::mma(acc2, make_smem_desc_sw64(t) + 2 * j, make_smem_desc_sw64(w) + 2 * j);
+      wgmma_commit();
+      return st;
+    };
+    auto releaseP2 = [&](int c, int st) {
+      release(smem_u32(&bars->empty[st]));
+      release(smem_u32(&bars->t_empty[(k + c) & 1]));
+    };
+    // Chunk c: P1(c), handed to the epilogue warpgroup as soon as it is complete; then P2(c - 1) once the epilogue warpgroup has
+    // made T slot (c - 1) & 1 out of chunk c - 1.  So the epilogue warpgroup finds chunk c ready when it finishes chunk c - 1, and
+    // runs it while the MMA warpgroups issue P2(c - 1) and P1(c + 1).
+    int st2 = -1;   // the weight stage of the P2 in flight
+#pragma unroll 1
+    for(int c = have0 ? 1 : 0; c < chunks; c++) {
+      handChunk(k + c, c + 1 == chunks);   // P1(c) and P2(c - 2) are complete
+      if(st2 >= 0) releaseP2(c - 2, st2);
+      // the previous tile's entry stores were issued 3 chunks ago
+      if(c == 3 && leader && pending >= 0) chain_publish(p1.tile_flags, pending);
+      st2 = c > 0 ? issueP2(c - 1) : -1;
+    }
+    const int st2_last = issueP2(chunks - 1);
+    wgmma_wait0();
+    fence_acc(acc2);
+    releaseP2(chunks - 2, st2);
+    releaseP2(chunks - 1, st2_last);
+    k += chunks;
+    // the next tile's chunk 0 goes to the epilogue warpgroup now, so that it does not idle through this tile's entry epilogue
+    have0 = tile + (int)gridDim.x < tiles;
+    if(have0) {
+      mbar_wait(smem_u32(&bars->a_full), aphase);
+      aphase ^= 1;
+      handChunk(k, false);
+    }
+
+    // ---- the entry's epilogue: raw inner stream and activated inner operand, one 32-column slice at a time ----
+#pragma unroll
+    for(int s = 0; s < N2 / RES_COLS; s++) {
+      uint8_t* const slot = stg_ring + ps * ACT_SLICE_BYTES;
+      uint8_t* const aslot = act_ring + as * ACT_SLICE_BYTES;
+      epilogue_slice<F2, N2>(p2, acc2, s, m0, 0, rloc, lane, mask0, mask1, s_scale2, s_bias2, slot, aslot);
+      fence_proxy_async();
+      if(leader) bulk_wait_read0();
+      warpgroup_sync(g);
+      if(leader) {
+        const int c0 = s * RES_COLS, r0 = m0 + g * (BLOCK_M / 2);
+        tma_store_2d(&tmapS2, smem_u32(slot + g * (ACT_SLICE_BYTES / 2)), c0, r0);
+        tma_store_2d(&tmapA2, smem_u32(aslot + g * (ACT_SLICE_BYTES / 2)), c0, r0);
+        bulk_commit();
+      }
+      ps ^= 1;
+      as ^= 1;
+    }
+    pending = tile;
+  }
+  if(leader && pending >= 0) chain_publish(p1.tile_flags, pending);
+  if(leader) bulk_wait0();
+  pdl_wait();
+}
+
 template <int N2, int N1>
 static cudaError_t pairFuncAttrs() {
   for(cudaError_t e : {cudaFuncSetAttribute(kgb_conv_pair_kernel<N2, N1, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
@@ -1351,10 +1726,15 @@ static cudaError_t pairFuncAttrs() {
 // streams (256-column acc2 next to acc1), so its boundaries keep two launches.
 #define KGB_PAIR_SHAPES(X) X(64, 64) X(64, 128) X(192, 384)
 
+// The (inner, trunk) widths kgb_conv_pair_epi_kernel is compiled for: b18c384nbt's
+#define KGB_PAIR_EPI_SHAPES(X) X(192, 384)
+
 static cudaError_t convPairInit() {
 #define KGB_PAIR_ATTR(N2, N1) pairFuncAttrs<N2, N1>(),
-  for(cudaError_t e : {KGB_PAIR_SHAPES(KGB_PAIR_ATTR)})
+#define KGB_PAIR_EPI_ATTR(N2, N1) cudaFuncSetAttribute(kgb_conv_pair_epi_kernel<N2, N1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
+  for(cudaError_t e : {KGB_PAIR_SHAPES(KGB_PAIR_ATTR) KGB_PAIR_EPI_SHAPES(KGB_PAIR_EPI_ATTR)})
     if(e != cudaSuccess) return e;
+#undef KGB_PAIR_EPI_ATTR
 #undef KGB_PAIR_ATTR
   return cudaSuccess;
 }
@@ -1374,6 +1754,17 @@ bool convPairSupported(const ConvParams& p1, const ConvParams& p2) {
          (p1.residual_fp32 != 0) == (p1.raw_fp32 != 0) && !(p2.raw_fp32 && !p1.raw_fp32) && pairLayout(p1, p2).stages >= 2;
 }
 
+bool convPairEpilogueWG(const ConvParams& p1, const ConvParams& p2) {
+  if(!p1.pair_epi_wg || p1.residual_fp32 || p1.raw_fp32 || p2.raw_fp32 || !convPairSupported(p1, p2)) return false;
+  bool shape = false;
+#define KGB_PAIR_EPI_IS(N2, N1) shape = shape || (p2.cout_p == N2 && p1.cout_p == N1);
+  KGB_PAIR_EPI_SHAPES(KGB_PAIR_EPI_IS)
+#undef KGB_PAIR_EPI_IS
+  return shape && pairEpiLayout(p1, p2).stages >= 4;
+}
+
+int convPairChainParts(const ConvParams& p1, const ConvParams& p2) { return convPairEpilogueWG(p1, p2) ? 3 : kConvPairParts; }
+
 template <int N2, int N1>
 static cudaError_t launchPairN(const ConvPairTmaps& tm, const ConvParams& p1, const ConvParams& p2, int grid, const PairLayout& l,
                                cudaStream_t stream) {
@@ -1388,8 +1779,17 @@ cudaError_t launchConvPair(const ConvPairTmaps& tm, const ConvParams& p1, const 
   const cudaError_t e = cudaGetDevice(&dev);
   if(e != cudaSuccess) return e;
   if(dev < 0 || dev >= 64 || g_smCount[dev] < 1) return cudaErrorInitializationError;
-  const PairLayout l = pairLayout(p1, p2);
   const int grid = std::min(p1.num_m_tiles, g_smCount[dev]);
+  if(convPairEpilogueWG(p1, p2)) {
+    const PairLayout l = pairEpiLayout(p1, p2);
+#define KGB_PAIR_EPI_LAUNCH(N2, N1)                                                                                                         \
+    if(p2.cout_p == N2 && p1.cout_p == N1)                                                                                                   \
+      return launchChained(kgb_conv_pair_epi_kernel<N2, N1>, p1, grid, PAIR_EPI_THREADS, l.smem, stream, tm.A, tm.W1, tm.W2, tm.stream1, \
+                           tm.stream2, tm.act2, p1, p2, l.stages);
+    KGB_PAIR_EPI_SHAPES(KGB_PAIR_EPI_LAUNCH)
+#undef KGB_PAIR_EPI_LAUNCH
+  }
+  const PairLayout l = pairLayout(p1, p2);
 #define KGB_PAIR_LAUNCH(N2, N1) if(p2.cout_p == N2 && p1.cout_p == N1) return launchPairN<N2, N1>(tm, p1, p2, grid, l, stream);
   KGB_PAIR_SHAPES(KGB_PAIR_LAUNCH)
 #undef KGB_PAIR_LAUNCH

@@ -60,6 +60,7 @@ struct kgb_handle {
   bool streamTrunkFp32 = true, streamInnerFp32 = false;
   bool fuseBoundaries = false;   // consecutive nested blocks' exit + entry 1x1 as one launch (launchConvPair)
   bool epilogueWG = true;        // launchConvWG may take the epilogue-warpgroup kernel (convEpilogueWG); KGB_EPILOGUE_WG=0 keeps the other
+  bool pairEpilogueWG = true;    // launchConvPair may take the exit-epilogue-warpgroup kernel (convPairEpilogueWG); KGB_PAIR_EPILOGUE_WG=0 keeps the other
   std::vector<void*> allocs;
   // inputs / outputs (device, fixed addresses so graphs can be replayed)
   float *dSpatial = nullptr, *dGlobal = nullptr, *dMeta = nullptr, *dOptimism = nullptr;   // dMeta: SGF-metadata nets only
@@ -84,6 +85,7 @@ struct kgb_handle {
   int chainSlots = 0;
   int chainedLaunches = 0;   // convolution launches per forward that are programmatic dependents of the one before
   int epilogueWGLaunches = 0;   // convolution launches per forward that run with the epilogue warpgroup (convEpilogueWG)
+  int pairEpilogueWGLaunches = 0;   // fused block boundaries per forward that run with the exit-epilogue warpgroup (convPairEpilogueWG)
   size_t chainStride() const { return (planRows(maxBatch) + 127) / 128; }
   int* chainFlags(int slot) const { return chain + (size_t)slot * chainStride(); }
   void allocChain() { chain = dalloc<int>((size_t)std::max(chainSlots, 1) * chainStride()); }

@@ -80,7 +80,7 @@ ABI_SYMBOLS = [
     "kgb_global_init", "kgb_global_cleanup", "kgb_last_error", "kgb_device_count", "kgb_device_name",
     "kgb_model_load_file", "kgb_model_free", "kgb_model_get_info", "kgb_context_create", "kgb_context_free",
     "kgb_handle_create", "kgb_handle_free", "kgb_handle_is_fp16", "kgb_forward", "kgb_forward_device", "kgb_test_forward_serial", "kgb_conv_chain_error", "kgb_forward_meta", "kgb_forward_device_meta", "kgb_handle_sync",
-    "kgb_handle_stream", "kgb_handle_launches_per_forward", "kgb_handle_chained_launches_per_forward", "kgb_handle_epilogue_wg_launches_per_forward", "kgb_handle_get_layout_stats", "kgb_test_conv", "kgb_bench_conv_ex", "kgb_test_conv_epilogue",
+    "kgb_handle_stream", "kgb_handle_launches_per_forward", "kgb_handle_chained_launches_per_forward", "kgb_handle_epilogue_wg_launches_per_forward", "kgb_handle_pair_epilogue_wg_launches_per_forward", "kgb_handle_get_layout_stats", "kgb_test_conv", "kgb_bench_conv_ex", "kgb_test_conv_epilogue",
     "kgb_test_conv_ex", "kgb_test_conv_boundary", "kgb_bench_conv_boundary", "kgb_test_conv_plan", "kgb_test_conv_boundary_plan",
     "kgb_test_head_kernel",
     "kgb_selfplay_create", "kgb_selfplay_free", "kgb_selfplay_run", "kgb_selfplay_get_stats", "kgb_selfplay_get_game",
@@ -158,6 +158,7 @@ def load_library():
     lib.kgb_handle_launches_per_forward.argtypes = [P]
     lib.kgb_handle_chained_launches_per_forward.argtypes = [P]
     lib.kgb_handle_epilogue_wg_launches_per_forward.argtypes = [P]
+    lib.kgb_handle_pair_epilogue_wg_launches_per_forward.argtypes = [P]
     lib.kgb_handle_get_layout_stats.argtypes = [P, P, P, P]
     lib.kgb_test_conv.argtypes = [I, I, I, I, P, I, I, I, I, P, P]
     lib.kgb_bench_conv_ex.argtypes = [I, I, I, I, I, I, I, I, I, I, I, I, F]
