@@ -184,19 +184,179 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
   return d;
 }
 
-struct __align__(8) Bars {
+// The operand rings of kgb_conv_wg_kernel and kgb_conv_wg_epi_kernel
+struct __align__(8) RingBars {
   uint64_t full[MAX_STAGES];    // weight tile landed
   uint64_t empty[MAX_STAGES];   // weight tile consumed by every consumer warp
   uint64_t a_full[2];           // A halo tile landed
   uint64_t a_empty[2];          // A halo tile consumed by all of its taps
-  uint64_t r_full[RES_SLOTS];   // residual slice landed
-  uint64_t r_empty[RES_SLOTS];  // residual slice read, and the raw stream written over it stored, by both consumer warpgroups
   int a_wp[2];                  // row pitch of the tile whose A halo tile is in the slot (written before the slot's a_full arrive)
 };
 
+struct __align__(8) Bars {
+  RingBars ring;
+  uint64_t r_full[RES_SLOTS];   // residual slice landed
+  uint64_t r_empty[RES_SLOTS];  // residual slice read, and the raw stream written over it stored, by both consumer warpgroups
+};
+
+// Rows of A above / below the tile that the widest pitch's taps reach
+__host__ __device__ inline int convHalo(const ConvParams& p) { return (p.ky / 2) * p.Wp + (p.kx / 2); }
 // dynamic smem: [<=1023 B slack][2 x A halo tile][stream ring][ACT_SLOTS x act slice (x 2 split)][stages x weight tile][Bars]
 //               [BN scale N][BN bias N]
-static inline int aBufBytes(int a_box_rows) { return (a_box_rows * BLOCK_K * 2 + 1023) / 1024 * 1024; }
+__host__ __device__ inline int aBufBytes(int a_box_rows) { return (a_box_rows * BLOCK_K * 2 + 1023) / 1024 * 1024; }
+
+__device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) { asm volatile("prefetch.tensormap [%0];" ::"l"(m) : "memory"); }
+
+// A weight ring of `stages` stages, each filled by one TMA transaction count and emptied by every consumer warp
+__device__ __forceinline__ void init_weight_ring(uint64_t* full, uint64_t* empty, int stages) {
+  for(int s = 0; s < stages; s++) {
+    mbar_init(smem_u32(&full[s]), 1);
+    mbar_init(smem_u32(&empty[s]), CONSUMER_WARPS);
+  }
+}
+
+// Thread 0 of kgb_conv_wg_kernel and kgb_conv_wg_epi_kernel: the tensor maps the launch uses, and the operand rings' barriers
+__device__ __forceinline__ void init_operand_rings(RingBars& b, int stages, const ConvParams& p, const CUtensorMap& tmapA,
+                                                   const CUtensorMap& tmapB, const CUtensorMap& tmapR, const CUtensorMap& tmapRaw,
+                                                   const CUtensorMap& tmapAct) {
+  prefetch_tmap(&tmapA);
+  prefetch_tmap(&tmapB);
+  if(p.residual != nullptr) prefetch_tmap(&tmapR);
+  if(p.raw_out != nullptr) prefetch_tmap(&tmapRaw);
+  if(p.act_out != nullptr) prefetch_tmap(&tmapAct);
+  init_weight_ring(b.full, b.empty, stages);
+  for(int s = 0; s < 2; s++) {
+    mbar_init(smem_u32(&b.a_full[s]), 1);
+    mbar_init(smem_u32(&b.a_empty[s]), CONSUMER_WARPS);
+  }
+}
+
+// One arrival of the warp on `bar`, once all of its lanes are done with what the barrier guards
+__device__ __forceinline__ void warp_arrive(uint32_t bar, int lane) {
+  __syncwarp();
+  if(lane == 0) mbar_arrive(bar);
+}
+
+// Lane 0 of warp 0 of kgb_conv_wg_kernel and kgb_conv_wg_epi_kernel: the A halo tiles into a 2-deep ring at smem_a and one weight
+// tile per tap into a ring of `stages` at smem_b, running ahead across tiles as far as the two rings allow.  One A halo tile per
+// (k-block, split part): `parts` is 3 in split mode, whose part 1 reads A's lo half and part 2 W's (columns cin_p on), else 1.
+template <int N>
+__device__ __forceinline__ void produce_operands(const ConvParams& p, RingBars& bars, const CUtensorMap& tmapA, const CUtensorMap& tmapB,
+                                                 uint32_t smem_a, uint32_t smem_b, int stages, int tiles, int n0, int parts) {
+  constexpr int b_tile_bytes = N * BLOCK_K * 2;   // one tap's weight tile
+  const int halo = convHalo(p), taps = p.ky * p.kx, phases = (p.cin_p / BLOCK_K) * parts;
+  const int a_tx_bytes = (BLOCK_M + 2 * halo) * BLOCK_K * 2, a_buf_bytes = aBufBytes(BLOCK_M + 2 * halo);
+  int stage = 0, ac = 0;
+  uint32_t phase = 0;
+  for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int m0 = (tile / p.num_n_tiles) * BLOCK_M;
+    const int wp = __ldg(p.tile_wp + m0 / BLOCK_M);       // loaded here, ahead of the consumers, who read it from the A slot
+    chain_wait(p.pred_flags, p.pred_parts, m0 / BLOCK_M, tiles / p.num_n_tiles);
+    for(int ph = 0; ph < phases; ph++, ac++) {
+      const int kb = ph / parts, part = ph - kb * parts;
+      const int colA = kb * BLOCK_K + (part == 1 ? p.cin_p : 0);
+      const int colB = kb * BLOCK_K + (part == 2 ? p.cin_p : 0);
+      const int abuf = ac & 1;
+      mbar_wait(smem_u32(&bars.a_empty[abuf]), ((ac >> 1) & 1) ^ 1);
+      const uint32_t afull = smem_u32(&bars.a_full[abuf]);
+      bars.a_wp[abuf] = wp;
+      mbar_arrive_expect_tx(afull, (uint32_t)a_tx_bytes);
+      tma_load_2d(smem_a + abuf * a_buf_bytes, &tmapA, afull, colA, m0 - halo);
+      for(int t = 0; t < taps; t++) {
+        mbar_wait(smem_u32(&bars.empty[stage]), phase ^ 1);
+        const uint32_t full = smem_u32(&bars.full[stage]);
+        mbar_arrive_expect_tx(full, (uint32_t)b_tile_bytes);
+        tma_load_2d(smem_b + stage * b_tile_bytes, &tmapB, full, colB, t * p.cout_p + n0);
+        if(++stage == stages) { stage = 0; phase ^= 1; }
+      }
+    }
+  }
+}
+
+// Lane 0 of warp 1: the residual stream's slices, `slices` of RES_COLS columns per tile from column col0, into a ring of `slots`
+// slots of `slot_bytes` at smem_r, each slice as two TMA boxes of 64 rows.  In a lane of its own, so that one waiting on a slot
+// does not hold up the next tile's operands.  The tiles are m-major, `n_tiles` per 128-row m-tile.
+__device__ __forceinline__ void produce_residual(const ConvParams& p, uint64_t* r_full, uint64_t* r_empty, const CUtensorMap& tmapR,
+                                                 uint32_t smem_r, int slots, int slot_bytes, int col0, int slices, int tiles, int n_tiles) {
+  int rs = 0;
+  uint32_t rphase = 0;
+  for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int m0 = (tile / n_tiles) * BLOCK_M;
+    chain_wait(p.pred_flags, p.pred_parts, m0 / BLOCK_M, tiles / n_tiles);
+    for(int s = 0; s < slices; s++) {
+      mbar_wait(smem_u32(&r_empty[rs]), rphase ^ 1);
+      const uint32_t rfull = smem_u32(&r_full[rs]), dst = smem_r + rs * slot_bytes;
+      mbar_arrive_expect_tx(rfull, (uint32_t)slot_bytes);
+      tma_load_2d(dst, &tmapR, rfull, col0 + s * RES_COLS, m0);
+      tma_load_2d(dst + slot_bytes / 2, &tmapR, rfull, col0 + s * RES_COLS, m0 + BLOCK_M / 2);
+      if(++rs == slots) { rs = 0; rphase ^= 1; }
+    }
+  }
+}
+
+// A consumer warp's positions in the operand rings, carried across tiles like the producer's
+struct RingPos {
+  int stage = 0;        // the weight stage of the next step
+  uint32_t phase = 0;   // its parity
+  int ph = 0;           // A halo tiles taken: the next one is in slot ph & 1 with parity (ph >> 1) & 1
+};
+
+// The main loop of one 128-row x N tile for a consumer warp: acc = the sum over the tile's `phases` A halo tiles and the taps.
+// ldmatrix.x4 lane roles: matrix j = lane / 8 supplies (rows +0 / +8) x (k 0-7 / 8-15) of a 16 x 16 A fragment, lrow being this
+// lane's row of the tile.  One step = one (k-block, tap): ldmatrix the tap's A fragments into `af` and issue its 4 wgmma as one
+// group.  Steps alternate between two fragment buffers; wait_group 1 after issuing step i means step i-1's group has finished, so
+// its weight stage can be released and its fragment buffer is free for step i+1.  The MMAs reach the accumulators in k-block,
+// tap, k16 order.  Returns with the MMAs complete and every stage of the tile released.
+template <int N>
+__device__ __forceinline__ void conv_main_loop(float (&acc)[N / 2], RingPos& rp, RingBars& bars, const ConvParams& p, uint32_t smem_a,
+                                               uint32_t smem_b, int stages, int phases, int lrow, int lane, int halo, int a_buf_bytes) {
+  constexpr int b_tile_bytes = N * BLOCK_K * 2;
+  const int ry = p.ky / 2, rx = p.kx / 2;
+  const uint32_t lchunk = (uint32_t)(lane >> 4);
+#pragma unroll
+  for(int i = 0; i < N / 2; i++) acc[i] = 0.0f;
+  fence_acc(acc);
+  // the tap is (dy, dx); the k-block's first tap is (-ry, -rx), its last (ry, rx)
+  int wp = 0, prev_stage = -1, dy = -ry, dx = -rx;
+  auto step = [&](uint32_t (&af)[4][4]) {
+    const int abuf = rp.ph & 1;
+    if(dy == -ry && dx == -rx) {
+      mbar_wait(smem_u32(&bars.a_full[abuf]), (rp.ph >> 1) & 1);
+      wp = bars.a_wp[abuf];
+    }
+    const uint32_t a_base = smem_a + abuf * a_buf_bytes;
+    // tap (dy,dx) = the tile's rows shifted by `halo + dy*wp + dx`; the 128B swizzle puts 16-byte chunk c of row r at c ^ (r & 7)
+    const uint32_t r = (uint32_t)(lrow + halo + dy * wp + dx);
+#pragma unroll
+    for(int k = 0; k < 4; k++) ldmatrix_x4(a_base + r * 128u + (((2u * k + lchunk) ^ (r & 7u)) << 4), af[k]);
+    mbar_wait(smem_u32(&bars.full[rp.stage]), rp.phase);
+    const uint64_t db = make_smem_desc(smem_b + rp.stage * b_tile_bytes);
+    wgmma_fence();
+#pragma unroll
+    for(int k = 0; k < 4; k++) Wgmma<N>::mma(acc, af[k], db + 2 * k);
+    wgmma_commit();
+    // the wgmma issue above consumed the fragments of the k-block's last tap, so its A halo tile may be refilled
+    if(dy == ry && dx == rx) warp_arrive(smem_u32(&bars.a_empty[abuf]), lane);
+    wgmma_wait1();
+    if(prev_stage >= 0) warp_arrive(smem_u32(&bars.empty[prev_stage]), lane);
+    prev_stage = rp.stage;
+    if(++rp.stage == stages) { rp.stage = 0; rp.phase ^= 1; }
+    if(++dx > rx) {
+      dx = -rx;
+      if(++dy > ry) { dy = -ry; rp.ph++; }
+    }
+  };
+  const int steps = phases * (p.ky * p.kx);
+  uint32_t af0[4][4], af1[4][4];
+  for(int i = 0; i + 1 < steps; i += 2) {
+    step(af0);
+    step(af1);
+  }
+  if(steps & 1) step(af0);
+  wgmma_wait0();
+  fence_acc(acc);
+  warp_arrive(smem_u32(&bars.empty[prev_stage]), lane);   // the tile's last stage: the producer is already on the next tile
+}
 // The stream ring holds the residual, and the raw output written back over it; without a residual it only stages the raw output.
 // When both exist they have the same dtype (the launcher checks it).
 __host__ __device__ inline bool streamFp32(const ConvParams& p) { return p.residual != nullptr ? p.residual_fp32 != 0 : p.raw_fp32 != 0; }
@@ -344,14 +504,12 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
                    const __grid_constant__ CUtensorMap tmapAct, const __grid_constant__ ConvParams p, int stages) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  constexpr int b_tile_bytes = N * BLOCK_K * 2;               // one tap's weight tile
-  const int halo = (p.ky / 2) * p.Wp + (p.kx / 2);            // rows of A above / below the tile that the widest pitch's taps reach
-  const int a_tx_bytes = (BLOCK_M + 2 * halo) * BLOCK_K * 2;
-  const int a_buf_bytes = (a_tx_bytes + 1023) / 1024 * 1024;
+  constexpr int b_tile_bytes = N * BLOCK_K * 2;
   constexpr int slices = N / RES_COLS;
   const int r_slots = streamSlots(p), r_slot_bytes = streamSlotBytes(p), act_slot_bytes = actSlotBytes(p);
   const bool s_fp32 = streamFp32(p);
   const int flags = epiFlags(p);
+  const int halo = convHalo(p), a_buf_bytes = aBufBytes(BLOCK_M + 2 * halo);
   const uint32_t smem_r = smem_base + 2 * a_buf_bytes;
   const uint32_t smem_act = smem_r + r_slots * r_slot_bytes;
   const uint32_t smem_b = smem_act + ACT_SLOTS * act_slot_bytes;
@@ -364,25 +522,11 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
   const int lane = threadIdx.x & 31;
   const int tiles = __ldg(p.m_tiles) * p.num_n_tiles;        // the plan's tiles; a CTA past them has nothing to do
   const int n0 = (blockIdx.x % p.num_n_tiles) * N;            // gridDim.x is a multiple of num_n_tiles: one n0 per CTA
-  const int taps = p.ky * p.kx;
   const int parts = p.split ? 3 : 1;
-  const int phases = (p.cin_p / BLOCK_K) * parts;             // one A halo tile per (k-block, split part)
 
   pdl_launch_dependents();   // the next launch's CTAs take the SMs this grid leaves (they need all of shared memory)
   if(threadIdx.x == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapA) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapB) : "memory");
-    if(p.residual != nullptr) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapR) : "memory");
-    if(p.raw_out != nullptr) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapRaw) : "memory");
-    if(p.act_out != nullptr) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapAct) : "memory");
-    for(int s = 0; s < stages; s++) {
-      mbar_init(smem_u32(&bars->full[s]), 1);
-      mbar_init(smem_u32(&bars->empty[s]), CONSUMER_WARPS);
-    }
-    for(int s = 0; s < 2; s++) {
-      mbar_init(smem_u32(&bars->a_full[s]), 1);
-      mbar_init(smem_u32(&bars->a_empty[s]), CONSUMER_WARPS);
-    }
+    init_operand_rings(bars->ring, stages, p, tmapA, tmapB, tmapR, tmapRaw, tmapAct);
     for(int s = 0; s < RES_SLOTS; s++) {
       mbar_init(smem_u32(&bars->r_full[s]), 1);
       mbar_init(smem_u32(&bars->r_empty[s]), 2);
@@ -394,51 +538,9 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
   if(warp < 4) {
     // ===================== TMA producers =====================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-    if(warp == 0 && lane == 0) {
-      // A halo tiles and weight tiles, running ahead across tiles as far as the two rings allow
-      int stage = 0, ac = 0;
-      uint32_t phase = 0;
-      for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-        const int m0 = (tile / p.num_n_tiles) * BLOCK_M;
-        const int wp = __ldg(p.tile_wp + m0 / BLOCK_M);       // loaded here, ahead of the consumers, who read it from the A slot
-        chain_wait(p.pred_flags, p.pred_parts, m0 / BLOCK_M, tiles / p.num_n_tiles);
-        for(int ph = 0; ph < phases; ph++, ac++) {
-          const int kb = ph / parts, part = ph - kb * parts;
-          const int colA = kb * BLOCK_K + (part == 1 ? p.cin_p : 0);
-          const int colB = kb * BLOCK_K + (part == 2 ? p.cin_p : 0);
-          const int abuf = ac & 1;
-          mbar_wait(smem_u32(&bars->a_empty[abuf]), ((ac >> 1) & 1) ^ 1);
-          const uint32_t afull = smem_u32(&bars->a_full[abuf]);
-          bars->a_wp[abuf] = wp;
-          mbar_arrive_expect_tx(afull, (uint32_t)a_tx_bytes);
-          tma_load_2d(smem_base + abuf * a_buf_bytes, &tmapA, afull, colA, m0 - halo);
-          for(int t = 0; t < taps; t++) {
-            mbar_wait(smem_u32(&bars->empty[stage]), phase ^ 1);
-            const uint32_t full = smem_u32(&bars->full[stage]);
-            mbar_arrive_expect_tx(full, (uint32_t)b_tile_bytes);
-            tma_load_2d(smem_b + stage * b_tile_bytes, &tmapB, full, colB, t * p.cout_p + n0);
-            if(++stage == stages) { stage = 0; phase ^= 1; }
-          }
-        }
-      }
-    }
-    else if(warp == 1 && lane == 0 && p.residual != nullptr) {
-      // residual slices, in their own lane so that one waiting on a slot does not hold up the next tile's A
-      int rs = 0;
-      uint32_t rphase = 0;
-      for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-        const int m0 = (tile / p.num_n_tiles) * BLOCK_M;
-        chain_wait(p.pred_flags, p.pred_parts, m0 / BLOCK_M, tiles / p.num_n_tiles);
-        for(int s = 0; s < slices; s++) {
-          mbar_wait(smem_u32(&bars->r_empty[rs]), rphase ^ 1);
-          const uint32_t rfull = smem_u32(&bars->r_full[rs]), dst = smem_r + rs * r_slot_bytes;
-          mbar_arrive_expect_tx(rfull, (uint32_t)r_slot_bytes);
-          tma_load_2d(dst, &tmapR, rfull, n0 + s * RES_COLS, m0);
-          tma_load_2d(dst + r_slot_bytes / 2, &tmapR, rfull, n0 + s * RES_COLS, m0 + BLOCK_M / 2);
-          if(++rs == RES_SLOTS) { rs = 0; rphase ^= 1; }
-        }
-      }
-    }
+    if(warp == 0 && lane == 0) produce_operands<N>(p, bars->ring, tmapA, tmapB, smem_base, smem_b, stages, tiles, n0, parts);
+    else if(warp == 1 && lane == 0 && p.residual != nullptr)
+      produce_residual(p, bars->r_full, bars->r_empty, tmapR, smem_r, RES_SLOTS, r_slot_bytes, n0, slices, tiles, p.num_n_tiles);
     return;
   }
 
@@ -446,10 +548,7 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
   const int g = (warp - 4) >> 2, q = warp & 3;
   const bool leader = q == 0 && lane == 0;    // issues the warpgroup's TMA stores
-  const int ry = p.ky / 2, rx = p.kx / 2;
-  // ldmatrix.x4 lane roles: matrix j = lane / 8 supplies (rows +0 / +8) x (k 0-7 / 8-15) of a 16 x 16 A fragment
   const int lrow = g * 64 + q * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
-  const uint32_t lchunk = (uint32_t)(lane >> 4);
   // acc[4j + 2h + e]: row 16q + lane/4 + 8h of the warpgroup's 64, column 8j + 2*(lane%4) + e
   const int rloc = g * 64 + q * 16 + (lane >> 2);
   // the CTA's BN constants into shared memory, once: every tile of the CTA has the same n0
@@ -457,9 +556,7 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
     for(int i = threadIdx.x - 128; i < N; i += 32 * CONSUMER_WARPS) { s_scale[i] = __ldg(p.bn_scale + n0 + i); s_bias[i] = __ldg(p.bn_bias + n0 + i); }
   consumer_sync();
 
-  // ring positions, carried across tiles like the producers'
-  int stage = 0, ph = 0;
-  uint32_t phase = 0;
+  RingPos rp;
   int rs = 0, prev_rs = -1, as = 0;
   uint32_t rphase = 0;
   uint8_t* const ring = smem + (smem_r - smem_base);
@@ -467,64 +564,11 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
   int pending = -1;   // the m-tile whose stores this warpgroup issued last and has not published yet
   for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
     const int m0 = (tile / p.num_n_tiles) * BLOCK_M;
-    int wp = 0;                                               // the tile's row pitch, from the A slot
     // this thread's two epilogue rows' mask values; the loads complete during the main loop
     const float mask0 = m0 + rloc < p.M ? __ldg(p.mask + m0 + rloc) : 0.0f;
     const float mask1 = m0 + rloc + 8 < p.M ? __ldg(p.mask + m0 + rloc + 8) : 0.0f;
     float acc[N / 2];
-#pragma unroll
-    for(int i = 0; i < N / 2; i++) acc[i] = 0.0f;
-    fence_acc(acc);
-    // One step = one (k-block, tap): ldmatrix the tap's A fragments into `af` and issue its 4 wgmma as one group.  Steps alternate
-    // between two fragment buffers; wait_group 1 after issuing step i means step i-1's group has finished, so its weight stage can
-    // be released and its fragment buffer is free for step i+1.  The MMAs reach the accumulators in k-block, tap, k16 order.
-    // the tap is (dy, dx); the k-block's first tap is (-ry, -rx), its last (ry, rx)
-    int prev_stage = -1, dy = -ry, dx = -rx;
-    auto step = [&](uint32_t (&af)[4][4]) {
-      const int abuf = ph & 1;
-      if(dy == -ry && dx == -rx) {
-        mbar_wait(smem_u32(&bars->a_full[abuf]), (ph >> 1) & 1);
-        wp = bars->a_wp[abuf];
-      }
-      const uint32_t a_base = smem_base + abuf * a_buf_bytes;
-      // tap (dy,dx) = the tile's rows shifted by `halo + dy*wp + dx`; the 128B swizzle puts 16-byte chunk c of row r at c ^ (r & 7)
-      const uint32_t r = (uint32_t)(lrow + halo + dy * wp + dx);
-#pragma unroll
-      for(int k = 0; k < 4; k++) ldmatrix_x4(a_base + r * 128u + (((2u * k + lchunk) ^ (r & 7u)) << 4), af[k]);
-      mbar_wait(smem_u32(&bars->full[stage]), phase);
-      const uint64_t db = make_smem_desc(smem_b + stage * b_tile_bytes);
-      wgmma_fence();
-#pragma unroll
-      for(int k = 0; k < 4; k++) Wgmma<N>::mma(acc, af[k], db + 2 * k);
-      wgmma_commit();
-      // the wgmma issue above consumed the fragments of the k-block's last tap, so its A halo tile may be refilled
-      if(dy == ry && dx == rx) {
-        __syncwarp();
-        if(lane == 0) mbar_arrive(smem_u32(&bars->a_empty[abuf]));
-      }
-      wgmma_wait1();
-      if(prev_stage >= 0) {
-        __syncwarp();
-        if(lane == 0) mbar_arrive(smem_u32(&bars->empty[prev_stage]));
-      }
-      prev_stage = stage;
-      if(++stage == stages) { stage = 0; phase ^= 1; }
-      if(++dx > rx) {
-        dx = -rx;
-        if(++dy > ry) { dy = -ry; ph++; }
-      }
-    };
-    const int steps = phases * taps;
-    uint32_t af0[4][4], af1[4][4];
-    for(int i = 0; i + 1 < steps; i += 2) {
-      step(af0);
-      step(af1);
-    }
-    if(steps & 1) step(af0);
-    wgmma_wait0();
-    fence_acc(acc);
-    __syncwarp();
-    if(lane == 0) mbar_arrive(smem_u32(&bars->empty[prev_stage]));   // the tile's last stage: the producer is already on the next tile
+    conv_main_loop<N>(acc, rp, bars->ring, p, smem_base, smem_b, stages, (p.cin_p / BLOCK_K) * parts, lrow, lane, halo, a_buf_bytes);
     // the previous tile's stores were issued a whole main loop ago
     if(leader && pending >= 0) chain_publish(p.tile_flags, pending);
 
@@ -562,13 +606,16 @@ kgb_conv_wg_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_const
   pdl_wait();   // this grid completes after the previous one
 }
 
+// The widths it is compiled for
+#define KGB_WG_SHAPES(X) X(32) X(64) X(96) X(128) X(160) X(192) X(224) X(256)
+
 // ------------------------------------------------------------------------------------------------------------
 // Epilogue warpgroup (kgb_conv_wg_epi_kernel, launchConvWG when convEpilogueWG)
 // ------------------------------------------------------------------------------------------------------------
 // In kgb_conv_wg_kernel both consumer warpgroups leave the main loop together and run the epilogue arithmetic with the tensor
 // pipe idle.  Here a fourth warpgroup runs it, 512 threads:
-//   warpgroup 0     TMA producers as above (one residual slot instead of a ring of four).
-//   warpgroups 1-2  the same main loop, so every accumulator holds the same bits.  At the end of a tile they wait until the
+//   warpgroup 0     produce_operands and produce_residual, with one residual slot instead of a ring of four.
+//   warpgroups 1-2  conv_main_loop, so every accumulator holds the same bits.  At the end of a tile they wait until the
 //                   accumulator tile in shared memory is empty, write their fp32 accumulators into it (N/32 slices of 128 x 32 in
 //                   slice_offset's fp32 layout), arrive on t_full and start the next tile at once.
 //   warpgroup 3     the epilogue, one thread per tile row: slice by slice it reads its row's 32 accumulators (and the residual),
@@ -590,13 +637,9 @@ static constexpr int ACC_SLICE_BYTES = BLOCK_M * RES_COLS * 4;
 #define KGB_EPI_WG_SHAPES(X) X(96) X(128) X(160) X(192)
 
 struct __align__(8) EpiBars {
-  uint64_t full[MAX_STAGES];    // weight tile landed
-  uint64_t empty[MAX_STAGES];   // weight tile consumed by every consumer warp
-  uint64_t a_full[2];           // A halo tile landed
-  uint64_t a_empty[2];          // A halo tile consumed by all of its taps
+  RingBars ring;
   uint64_t r_full, r_empty;     // residual slice landed / read by the epilogue warpgroup
   uint64_t t_full, t_empty;     // accumulator tile written by every consumer warp / read, and its stores' reads done
-  int a_wp[2];                  // row pitch of the tile whose A halo tile is in the slot
 };
 
 // Epilogue warpgroup: tile m_tile's stores are all issued; publish it for both halves of the parts count (convChainParts).
@@ -608,6 +651,34 @@ __device__ __noinline__ void chain_publish_tile(int* flags, int m_tile) {
 // The epilogue warpgroup.  bar.sync is .aligned: a warp reaches it converged, so after an mbarrier wait loop (which its lanes may
 // leave in different iterations) the epilogue brings the warp together with __syncwarp.
 __device__ __forceinline__ void epi_wg_sync() { asm volatile("bar.sync 4, 128;" ::: "memory"); }
+
+// Epilogue warpgroups: row rl of an fp32 accumulator slice (slice_offset's fp32 layout)
+__device__ __forceinline__ void load_acc_row(const uint8_t* slice, int rl, float (&v)[RES_COLS]) {
+#pragma unroll
+  for(int k = 0; k < RES_COLS / 4; k++) {
+    const float4 f = *reinterpret_cast<const float4*>(slice + slice_offset(rl, 4 * k, true));
+    v[4 * k] = f.x; v[4 * k + 1] = f.y; v[4 * k + 2] = f.z; v[4 * k + 3] = f.w;
+  }
+}
+// Row rl of an fp16 stream slice, as half2
+__device__ __forceinline__ void load_half_row(const uint8_t* slice, int rl, uint32_t (&res)[RES_COLS / 2]) {
+#pragma unroll
+  for(int k = 0; k < RES_COLS / 8; k++) {
+    const uint4 u = *reinterpret_cast<const uint4*>(slice + slice_offset(rl, 8 * k, false));
+    res[4 * k] = u.x; res[4 * k + 1] = u.y; res[4 * k + 2] = u.z; res[4 * k + 3] = u.w;
+  }
+}
+// Consumer warps: the accumulator fragments of N columns (rows rloc and rloc + 8, as in epilogue_slice) into N / 32 fp32 slices
+// from `dst`, for an epilogue warpgroup to read by rows
+template <int N>
+__device__ __forceinline__ void store_acc_slices(uint8_t* dst, const float (&acc)[N / 2], int rloc, int lane) {
+#pragma unroll
+  for(int j = 0; j < N / 8; j++)
+#pragma unroll
+    for(int h = 0; h < 2; h++)
+      *reinterpret_cast<float2*>(dst + (j / 4) * ACC_SLICE_BYTES + slice_offset(rloc + 8 * h, 8 * (j % 4) + 2 * (lane & 3), true)) =
+        make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+}
 
 // One row's part of slice s: its 16 column pairs through epilogue_store<F>, the outputs gathered in registers and written as
 // 16-byte chunks, the raw output into `region` (the slice it was read from: every row of the slice has been read by then) and
@@ -656,11 +727,9 @@ kgb_conv_wg_epi_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_c
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr int b_tile_bytes = N * BLOCK_K * 2;
   constexpr int slices = N / RES_COLS;
-  const int halo = (p.ky / 2) * p.Wp + (p.kx / 2);
-  const int a_tx_bytes = (BLOCK_M + 2 * halo) * BLOCK_K * 2;
-  const int a_buf_bytes = (a_tx_bytes + 1023) / 1024 * 1024;
   const int flags = epiFlags(p);
   // [<=1023 B slack][2 x A halo tile][accumulator tile: slices x 16 KB][residual slot, 8 KB][stages x weight tile][EpiBars][BN]
+  const int halo = convHalo(p), a_buf_bytes = aBufBytes(BLOCK_M + 2 * halo);
   const uint32_t smem_acc = smem_base + 2 * a_buf_bytes;
   const uint32_t smem_r = smem_acc + slices * ACC_SLICE_BYTES;
   const uint32_t smem_b = smem_r + (p.residual != nullptr ? ACT_SLICE_BYTES : 0);
@@ -674,24 +743,10 @@ kgb_conv_wg_epi_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_c
   const int lane = threadIdx.x & 31;
   const int tiles = __ldg(p.m_tiles) * p.num_n_tiles;
   const int n0 = (blockIdx.x % p.num_n_tiles) * N;
-  const int taps = p.ky * p.kx;
-  const int phases = p.cin_p / BLOCK_K;                       // one A halo tile per k-block (no split mode here)
 
   pdl_launch_dependents();
   if(threadIdx.x == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapA) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapB) : "memory");
-    if(p.residual != nullptr) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapR) : "memory");
-    if(p.raw_out != nullptr) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapRaw) : "memory");
-    if(p.act_out != nullptr) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmapAct) : "memory");
-    for(int s = 0; s < stages; s++) {
-      mbar_init(smem_u32(&bars->full[s]), 1);
-      mbar_init(smem_u32(&bars->empty[s]), CONSUMER_WARPS);
-    }
-    for(int s = 0; s < 2; s++) {
-      mbar_init(smem_u32(&bars->a_full[s]), 1);
-      mbar_init(smem_u32(&bars->a_empty[s]), CONSUMER_WARPS);
-    }
+    init_operand_rings(bars->ring, stages, p, tmapA, tmapB, tmapR, tmapRaw, tmapAct);
     mbar_init(smem_u32(&bars->r_full), 1);
     mbar_init(smem_u32(&bars->r_empty), 1);
     mbar_init(smem_u32(&bars->t_full), CONSUMER_WARPS);
@@ -703,46 +758,10 @@ kgb_conv_wg_epi_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_c
   if(warp < 4) {
     // ===================== TMA producers =====================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-    if(warp == 0 && lane == 0) {
-      int stage = 0, ac = 0;
-      uint32_t phase = 0;
-      for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-        const int m0 = (tile / p.num_n_tiles) * BLOCK_M;
-        const int wp = __ldg(p.tile_wp + m0 / BLOCK_M);
-        chain_wait(p.pred_flags, p.pred_parts, m0 / BLOCK_M, tiles / p.num_n_tiles);
-        for(int kb = 0; kb < phases; kb++, ac++) {
-          const int abuf = ac & 1;
-          mbar_wait(smem_u32(&bars->a_empty[abuf]), ((ac >> 1) & 1) ^ 1);
-          const uint32_t afull = smem_u32(&bars->a_full[abuf]);
-          bars->a_wp[abuf] = wp;
-          mbar_arrive_expect_tx(afull, (uint32_t)a_tx_bytes);
-          tma_load_2d(smem_base + abuf * a_buf_bytes, &tmapA, afull, kb * BLOCK_K, m0 - halo);
-          for(int t = 0; t < taps; t++) {
-            mbar_wait(smem_u32(&bars->empty[stage]), phase ^ 1);
-            const uint32_t full = smem_u32(&bars->full[stage]);
-            mbar_arrive_expect_tx(full, (uint32_t)b_tile_bytes);
-            tma_load_2d(smem_b + stage * b_tile_bytes, &tmapB, full, kb * BLOCK_K, t * p.cout_p + n0);
-            if(++stage == stages) { stage = 0; phase ^= 1; }
-          }
-        }
-      }
-    }
-    else if(warp == 1 && lane == 0 && p.residual != nullptr) {
-      // fp16 residual slices into the one slot, each as soon as the epilogue warpgroup has read the one before
-      uint32_t rphase = 0;
-      for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-        const int m0 = (tile / p.num_n_tiles) * BLOCK_M;
-        chain_wait(p.pred_flags, p.pred_parts, m0 / BLOCK_M, tiles / p.num_n_tiles);
-        for(int s = 0; s < slices; s++) {
-          mbar_wait(smem_u32(&bars->r_empty), rphase ^ 1);
-          const uint32_t rfull = smem_u32(&bars->r_full);
-          mbar_arrive_expect_tx(rfull, (uint32_t)ACT_SLICE_BYTES);
-          tma_load_2d(smem_r, &tmapR, rfull, n0 + s * RES_COLS, m0);
-          tma_load_2d(smem_r + ACT_SLICE_BYTES / 2, &tmapR, rfull, n0 + s * RES_COLS, m0 + BLOCK_M / 2);
-          rphase ^= 1;
-        }
-      }
-    }
+    // no split mode here: one A halo tile per k-block
+    if(warp == 0 && lane == 0) produce_operands<N>(p, bars->ring, tmapA, tmapB, smem_base, smem_b, stages, tiles, n0, 1);
+    else if(warp == 1 && lane == 0 && p.residual != nullptr)   // each slice as soon as the epilogue warpgroup has read the one before
+      produce_residual(p, &bars->r_full, &bars->r_empty, tmapR, smem_r, 1, ACT_SLICE_BYTES, n0, slices, tiles, p.num_n_tiles);
     return;
   }
 
@@ -764,21 +783,13 @@ kgb_conv_wg_epi_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_c
       for(int s = 0; s < slices; s++) {
         uint8_t* const region = acc_tile + s * ACC_SLICE_BYTES;
         float v[RES_COLS];
-#pragma unroll
-        for(int k = 0; k < RES_COLS / 4; k++) {
-          const float4 f = *reinterpret_cast<const float4*>(region + slice_offset(rl, 4 * k, true));
-          v[4 * k] = f.x; v[4 * k + 1] = f.y; v[4 * k + 2] = f.z; v[4 * k + 3] = f.w;
-        }
+        load_acc_row(region, rl, v);
         uint32_t res[RES_COLS / 2];
         if(p.residual != nullptr) {
           mbar_wait(smem_u32(&bars->r_full), rphase);
           __syncwarp();
           rphase ^= 1;
-#pragma unroll
-          for(int k = 0; k < RES_COLS / 8; k++) {
-            const uint4 u = *reinterpret_cast<const uint4*>(smem + (smem_r - smem_base) + slice_offset(rl, 8 * k, false));
-            res[4 * k] = u.x; res[4 * k + 1] = u.y; res[4 * k + 2] = u.z; res[4 * k + 3] = u.w;
-          }
+          load_half_row(smem + (smem_r - smem_base), rl, res);
           // the slot's next TMA load (async proxy) follows these reads through the barrier below and r_empty: without the proxy
           // fence it may land before a read has returned its value
           fence_proxy_async();
@@ -825,75 +836,19 @@ kgb_conv_wg_epi_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_c
   // ===================== consumers: warpgroup g owns tile rows 64g..64g+63, warp q of it rows 16q..16q+15 =====================
   asm volatile("setmaxnreg.inc.sync.aligned.u32 184;");
   const int g = (warp - 4) >> 2, q = warp & 3;
-  const int ry = p.ky / 2, rx = p.kx / 2;
   const int lrow = g * 64 + q * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
-  const uint32_t lchunk = (uint32_t)(lane >> 4);
   // acc[4j + 2h + e]: row 16q + lane/4 + 8h of the warpgroup's 64, column 8j + 2*(lane%4) + e
   const int rloc = g * 64 + q * 16 + (lane >> 2);
-  int stage = 0, ph = 0;
-  uint32_t phase = 0, tphase = 0;
+  RingPos rp;
+  uint32_t tphase = 0;
   for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-    int wp = 0;
     float acc[N / 2];
-#pragma unroll
-    for(int i = 0; i < N / 2; i++) acc[i] = 0.0f;
-    fence_acc(acc);
-    // the main loop of kgb_conv_wg_kernel (one k-block = one A halo tile here)
-    int prev_stage = -1, dy = -ry, dx = -rx;
-    auto step = [&](uint32_t (&af)[4][4]) {
-      const int abuf = ph & 1;
-      if(dy == -ry && dx == -rx) {
-        mbar_wait(smem_u32(&bars->a_full[abuf]), (ph >> 1) & 1);
-        wp = bars->a_wp[abuf];
-      }
-      const uint32_t a_base = smem_base + abuf * a_buf_bytes;
-      const uint32_t r = (uint32_t)(lrow + halo + dy * wp + dx);
-#pragma unroll
-      for(int k = 0; k < 4; k++) ldmatrix_x4(a_base + r * 128u + (((2u * k + lchunk) ^ (r & 7u)) << 4), af[k]);
-      mbar_wait(smem_u32(&bars->full[stage]), phase);
-      const uint64_t db = make_smem_desc(smem_b + stage * b_tile_bytes);
-      wgmma_fence();
-#pragma unroll
-      for(int k = 0; k < 4; k++) Wgmma<N>::mma(acc, af[k], db + 2 * k);
-      wgmma_commit();
-      if(dy == ry && dx == rx) {
-        __syncwarp();
-        if(lane == 0) mbar_arrive(smem_u32(&bars->a_empty[abuf]));
-      }
-      wgmma_wait1();
-      if(prev_stage >= 0) {
-        __syncwarp();
-        if(lane == 0) mbar_arrive(smem_u32(&bars->empty[prev_stage]));
-      }
-      prev_stage = stage;
-      if(++stage == stages) { stage = 0; phase ^= 1; }
-      if(++dx > rx) {
-        dx = -rx;
-        if(++dy > ry) { dy = -ry; ph++; }
-      }
-    };
-    const int steps = phases * taps;
-    uint32_t af0[4][4], af1[4][4];
-    for(int i = 0; i + 1 < steps; i += 2) {
-      step(af0);
-      step(af1);
-    }
-    if(steps & 1) step(af0);
-    wgmma_wait0();
-    fence_acc(acc);
-    __syncwarp();
-    if(lane == 0) mbar_arrive(smem_u32(&bars->empty[prev_stage]));
+    conv_main_loop<N>(acc, rp, bars->ring, p, smem_base, smem_b, stages, p.cin_p / BLOCK_K, lrow, lane, halo, a_buf_bytes);
     // hand the accumulators to the epilogue warpgroup once it has read the previous tile out of the accumulator tile
     mbar_wait(smem_u32(&bars->t_empty), tphase ^ 1);
     tphase ^= 1;
-#pragma unroll
-    for(int j = 0; j < N / 8; j++)
-#pragma unroll
-      for(int h = 0; h < 2; h++)
-        *reinterpret_cast<float2*>(acc_tile + (j / 4) * ACC_SLICE_BYTES + slice_offset(rloc + 8 * h, 8 * (j % 4) + 2 * (lane & 3), true)) =
-          make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-    __syncwarp();
-    if(lane == 0) mbar_arrive(smem_u32(&bars->t_full));
+    store_acc_slices<N>(acc_tile, acc, rloc, lane);
+    warp_arrive(smem_u32(&bars->t_full), lane);
   }
   pdl_wait();
 }
@@ -926,19 +881,22 @@ cudaError_t convWGInit() {
   if(e0 != cudaSuccess) return e0;
   e0 = cudaMemcpyToSymbol(g_chainError, &devWord, sizeof(devWord));
   if(e0 != cudaSuccess) return e0;
-  for(cudaError_t e : {cudaFuncSetAttribute(kgb_conv_wg_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
-                       cudaFuncSetAttribute(kgb_conv_wg_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
-                       cudaFuncSetAttribute(kgb_conv_wg_kernel<96>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
-                       cudaFuncSetAttribute(kgb_conv_wg_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
-                       cudaFuncSetAttribute(kgb_conv_wg_kernel<160>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
-                       cudaFuncSetAttribute(kgb_conv_wg_kernel<192>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
-                       cudaFuncSetAttribute(kgb_conv_wg_kernel<224>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
-                       cudaFuncSetAttribute(kgb_conv_wg_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
+#define KGB_WG_ATTR(N) cudaFuncSetAttribute(kgb_conv_wg_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
 #define KGB_EPI_WG_ATTR(N) cudaFuncSetAttribute(kgb_conv_wg_epi_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT),
-                       KGB_EPI_WG_SHAPES(KGB_EPI_WG_ATTR)
-#undef KGB_EPI_WG_ATTR
-                       convPairInit()})
+  for(cudaError_t e : {KGB_WG_SHAPES(KGB_WG_ATTR) KGB_EPI_WG_SHAPES(KGB_EPI_WG_ATTR) convPairInit()})
     if(e != cudaSuccess) return e;
+#undef KGB_EPI_WG_ATTR
+#undef KGB_WG_ATTR
+  return cudaSuccess;
+}
+
+// The SM count convWGInit recorded for the current device: the persistent grids' CTA limit
+static cudaError_t smCount(int* n) {
+  int dev = 0;
+  const cudaError_t e = cudaGetDevice(&dev);
+  if(e != cudaSuccess) return e;
+  if(dev < 0 || dev >= 64 || g_smCount[dev] < 1) return cudaErrorInitializationError;   // convWGInit not run on this device
+  *n = g_smCount[dev];
   return cudaSuccess;
 }
 
@@ -959,28 +917,35 @@ static cudaError_t launchChained(void (*kernel)(Args...), const ConvParams& p, i
   return cudaLaunchKernelEx(&cfg, kernel, args...);
 }
 
-template <int N>
-static cudaError_t launchN(const ConvTmaps& tm, const ConvParams& p, int grid, int stages, int smem, cudaStream_t stream) {
-  return launchChained(kgb_conv_wg_kernel<N>, p, grid, THREADS, smem, stream, tm.A, tm.B, tm.residual, tm.raw, tm.act, p, stages);
+// A kernel's shared memory: its fixed bytes first, then as many weight stages as fit
+struct SmemLayout {
+  int stages = 0, smem = 0;
+  int r_slots = 0;   // the fused boundary's residual ring
+};
+static SmemLayout fitStages(int fixed, int stage_bytes, int r_slots = 0) {
+  SmemLayout l;
+  l.stages = std::min(MAX_STAGES, (SMEM_LIMIT - fixed) / stage_bytes);
+  l.smem = fixed + l.stages * stage_bytes;
+  l.r_slots = r_slots;
+  return l;
 }
 
-// Shared memory of kgb_conv_wg_epi_kernel: the accumulator tile and the residual slot come first, the weight ring gets what is left
-struct EpiLayout {
-  int stages = 0, smem = 0;
-};
-static EpiLayout epiLayout(const ConvParams& p) {
-  EpiLayout l;
-  const int halo = (p.ky / 2) * p.Wp + (p.kx / 2);
-  const int fixed = 1024 + 2 * aBufBytes(BLOCK_M + 2 * halo) + p.n_tile / RES_COLS * ACC_SLICE_BYTES + (p.residual != nullptr ? ACT_SLICE_BYTES : 0) +
-                    (int)sizeof(EpiBars) + 2 * p.n_tile * (int)sizeof(float);
-  l.stages = std::min(MAX_STAGES, (SMEM_LIMIT - fixed) / (p.n_tile * BLOCK_K * 2));
-  l.smem = fixed + l.stages * p.n_tile * BLOCK_K * 2;
-  return l;
+// kgb_conv_wg_kernel: the stream and act rings and the BN copies are fixed
+static SmemLayout wgLayout(const ConvParams& p) {
+  return fitStages(1024 + 2 * aBufBytes(BLOCK_M + 2 * convHalo(p)) + streamSlots(p) * streamSlotBytes(p) + ACT_SLOTS * actSlotBytes(p) +
+                   (int)sizeof(Bars) + 2 * p.n_tile * (int)sizeof(float), p.n_tile * BLOCK_K * 2);
+}
+
+// kgb_conv_wg_epi_kernel: the accumulator tile, the residual slot and the BN copies are fixed
+static SmemLayout epiLayout(const ConvParams& p) {
+  return fitStages(1024 + 2 * aBufBytes(BLOCK_M + 2 * convHalo(p)) + p.n_tile / RES_COLS * ACC_SLICE_BYTES +
+                   (p.residual != nullptr ? ACT_SLICE_BYTES : 0) + (int)sizeof(EpiBars) + 2 * p.n_tile * (int)sizeof(float),
+                   p.n_tile * BLOCK_K * 2);
 }
 
 bool convEpilogueWG(const ConvParams& p) {
   if(!p.epi_wg || p.split || p.ky * p.kx == 1) return false;
-  const int f = epiFlags(p), halo = (p.ky / 2) * p.Wp + (p.kx / 2);
+  const int f = epiFlags(p), halo = convHalo(p);
   bool shape = false, epi = false;
 #define KGB_EPI_WG_IS(N) shape = shape || p.n_tile == N;
   KGB_EPI_WG_SHAPES(KGB_EPI_WG_IS)
@@ -992,47 +957,34 @@ bool convEpilogueWG(const ConvParams& p) {
 }
 
 cudaError_t launchConvWG(const ConvTmaps& tm, const ConvParams& p, cudaStream_t stream) {
-  const int halo = (p.ky / 2) * p.Wp + (p.kx / 2);
-  if(BLOCK_M + 2 * halo > 256) return cudaErrorInvalidValue;  // TMA box limit
+  if(BLOCK_M + 2 * convHalo(p) > 256) return cudaErrorInvalidValue;  // TMA box limit
   if(p.n_tile % RES_COLS != 0) return cudaErrorInvalidValue;
   // the raw output is written over the residual slice it was read from
   if(p.residual != nullptr && p.raw_out != nullptr && (p.residual_fp32 != 0) != (p.raw_fp32 != 0)) return cudaErrorInvalidValue;
   if(p.tile_flags == nullptr) return cudaErrorInvalidValue;
-  int dev = 0;
-  const cudaError_t e = cudaGetDevice(&dev);
+  int sms = 0;
+  const cudaError_t e = smCount(&sms);
   if(e != cudaSuccess) return e;
-  if(dev < 0 || dev >= 64 || g_smCount[dev] < 1) return cudaErrorInitializationError;   // convWGInit not run on this device
   // persistent grid: at most one CTA per SM (the rings take all of shared memory), a multiple of num_n_tiles
   const int tiles = p.num_m_tiles * p.num_n_tiles;
-  int grid = std::min(tiles, g_smCount[dev]) / p.num_n_tiles * p.num_n_tiles;
+  int grid = std::min(tiles, sms) / p.num_n_tiles * p.num_n_tiles;
   if(grid < p.num_n_tiles) grid = p.num_n_tiles;
   if(convEpilogueWG(p)) {
-    const EpiLayout l = epiLayout(p);
+    const SmemLayout l = epiLayout(p);
 #define KGB_EPI_WG_LAUNCH(N) \
     if(p.n_tile == N)        \
       return launchChained(kgb_conv_wg_epi_kernel<N>, p, grid, EPI_WG_THREADS, l.smem, stream, tm.A, tm.B, tm.residual, tm.raw, tm.act, p, l.stages);
     KGB_EPI_WG_SHAPES(KGB_EPI_WG_LAUNCH)
 #undef KGB_EPI_WG_LAUNCH
   }
-  const int bTile = p.n_tile * BLOCK_K * 2;
-  // the stream and act rings and the BN copies come first; the weight ring gets what is left
-  const int fixed = 1024 + 2 * aBufBytes(BLOCK_M + 2 * halo) + streamSlots(p) * streamSlotBytes(p) + ACT_SLOTS * actSlotBytes(p) +
-                    (int)sizeof(Bars) + 2 * p.n_tile * (int)sizeof(float);
-  int stages = (SMEM_LIMIT - fixed) / bTile;
-  if(stages > MAX_STAGES) stages = MAX_STAGES;
-  if(stages < 2) return cudaErrorInvalidValue;
-  const int smem = fixed + stages * bTile;
-  switch(p.n_tile) {
-    case 32: return launchN<32>(tm, p, grid, stages, smem, stream);
-    case 64: return launchN<64>(tm, p, grid, stages, smem, stream);
-    case 96: return launchN<96>(tm, p, grid, stages, smem, stream);
-    case 128: return launchN<128>(tm, p, grid, stages, smem, stream);
-    case 160: return launchN<160>(tm, p, grid, stages, smem, stream);
-    case 192: return launchN<192>(tm, p, grid, stages, smem, stream);
-    case 224: return launchN<224>(tm, p, grid, stages, smem, stream);
-    case 256: return launchN<256>(tm, p, grid, stages, smem, stream);
-    default: return cudaErrorInvalidValue;
-  }
+  const SmemLayout l = wgLayout(p);
+  if(l.stages < 2) return cudaErrorInvalidValue;
+#define KGB_WG_LAUNCH(N) \
+  if(p.n_tile == N)      \
+    return launchChained(kgb_conv_wg_kernel<N>, p, grid, THREADS, l.smem, stream, tm.A, tm.B, tm.residual, tm.raw, tm.act, p, l.stages);
+  KGB_WG_SHAPES(KGB_WG_LAUNCH)
+#undef KGB_WG_LAUNCH
+  return cudaErrorInvalidValue;
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1070,27 +1022,98 @@ __device__ __forceinline__ uint64_t make_smem_desc_sw64(uint32_t smem_addr) {
   return d;
 }
 
-// dynamic smem: [<=1023 B slack][A tile: K1/64 x 16 KB][2 x T slot][residual ring][2 x raw staging][2 x act slice][stages x weights]
-//               [PairBars][BN scale / bias: exit N1, entry N2]
-struct PairLayout {
-  int r_slots = 0, stages = 0, smem = 0;
-};
-static PairLayout pairLayout(const ConvParams& p1, const ConvParams& p2) {
-  PairLayout l;
-  const int n2 = p2.cout_p, n1 = p1.cout_p;
-  const int r1 = BLOCK_M * RES_COLS * (p1.residual_fp32 ? 4 : 2), r2 = BLOCK_M * RES_COLS * (p2.raw_fp32 ? 4 : 2);
-  const int wBytes = n2 * PAIR_NC * 2;
-  // a full residual ring when it leaves room for three weight stages, else half of one
-  for(int rs : {RES_SLOTS, 2}) {
-    const int fixed = 1024 + BLOCK_M * n2 * 2 + 2 * PAIR_T_BYTES + rs * r1 + STAGE_SLOTS * r2 + ACT_SLOTS * ACT_SLICE_BYTES +
-                      (int)sizeof(PairBars) + 2 * (n1 + n2) * (int)sizeof(float);
-    const int stages = std::min(MAX_STAGES, (SMEM_LIMIT - fixed) / wBytes);
-    if(stages >= 3 || (rs == 2 && stages >= 2)) {
-      l.r_slots = rs; l.stages = stages; l.smem = fixed + stages * wBytes;
-      return l;
+// Lane 0 of warp 0 of the fused boundary: the inner operand tile (K1/64 boxes {64, 128}), then the weight chunks of NC columns in the
+// order the consumers take them: W1(0), then W1(c+1), W2(c) for each chunk c.  A W1 chunk is K1/64 boxes {64, NC} and a W2 chunk
+// NC/64 boxes {64, N2} or one box {32, N2}, either way one stage of N2 * NC * 2 bytes.
+template <int N2, int N1, int NC, class PB>
+__device__ __forceinline__ void produce_pair_operands(const ConvParams& p1, PB& bars, const CUtensorMap& tmapA, const CUtensorMap& tmapW1,
+                                                      const CUtensorMap& tmapW2, uint32_t smem_a, uint32_t smem_w, int stages, int tiles) {
+  constexpr int K1 = N2, A_BYTES = BLOCK_M * K1 * 2, W_BYTES = N2 * NC * 2, chunks = N1 / NC;
+  int stage = 0;
+  uint32_t phase = 0, aphase = 0;
+  auto loadW = [&](bool entry, int c) {
+    mbar_wait(smem_u32(&bars.empty[stage]), phase ^ 1);
+    const uint32_t full = smem_u32(&bars.full[stage]), dst = smem_w + stage * W_BYTES;
+    mbar_arrive_expect_tx(full, (uint32_t)W_BYTES);
+    if(entry) {
+      for(int j = 0; j < (NC + BLOCK_K - 1) / BLOCK_K; j++) tma_load_2d(dst + j * N2 * 128, &tmapW2, full, c * NC + j * BLOCK_K, 0);
+    }
+    else {
+      for(int kb = 0; kb < K1 / BLOCK_K; kb++) tma_load_2d(dst + kb * NC * 128, &tmapW1, full, kb * BLOCK_K, c * NC);
+    }
+    if(++stage == stages) { stage = 0; phase ^= 1; }
+  };
+  // the first tile's first exit chunk goes out before its chain wait (weights do not depend on the previous launch)
+  bool pre = (int)blockIdx.x < tiles;
+  if(pre) loadW(false, 0);
+  for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int m0 = tile * BLOCK_M;
+    chain_wait(p1.pred_flags, p1.pred_parts, tile, tiles);
+    mbar_wait(smem_u32(&bars.a_empty), aphase ^ 1);
+    const uint32_t afull = smem_u32(&bars.a_full);
+    mbar_arrive_expect_tx(afull, (uint32_t)A_BYTES);
+    for(int kb = 0; kb < K1 / BLOCK_K; kb++) tma_load_2d(smem_a + kb * BLOCK_M * 128, &tmapA, afull, kb * BLOCK_K, m0);
+    aphase ^= 1;
+    if(!pre) loadW(false, 0);
+    pre = false;
+    for(int c = 0; c < chunks; c++) {
+      if(c + 1 < chunks) loadW(false, c + 1);
+      loadW(true, c);
     }
   }
-  return l;
+}
+
+// Fused-boundary consumers: wait for the next weight stage and return it
+__device__ __forceinline__ int take_stage(uint64_t* full, int stages, int& stage, uint32_t& phase) {
+  const int st = stage;
+  mbar_wait(smem_u32(&full[st]), phase);
+  if(++stage == stages) { stage = 0; phase ^= 1; }
+  return st;
+}
+
+// The entry's epilogue for consumer warpgroup g: the inner raw stream and the activated inner operand out of acc2, one 32-column
+// slice at a time through the staging ring at stg_ring (slot ps) and the act ring at act_ring (slot as), out by TMA stores.  Once
+// the first slice's bulk_wait_read0 shows that the stores before it have read their slots, the leader also releases the exit's
+// residual slot `release_rs` (-1: none).
+template <int F2, int N2, int R2_BYTES>
+__device__ __forceinline__ void pair_entry_epilogue(const ConvParams& p2, const float (&acc2)[N2 / 2], int m0, int g, int rloc, int lane,
+                                                    bool leader, float mask0, float mask1, const float* s_scale2, const float* s_bias2,
+                                                    uint8_t* stg_ring, uint8_t* act_ring, int& ps, int& as, const CUtensorMap& tmapS2,
+                                                    const CUtensorMap& tmapA2, uint64_t* r_empty, int release_rs) {
+#pragma unroll
+  for(int s = 0; s < N2 / RES_COLS; s++) {
+    uint8_t* const slot = stg_ring + ps * R2_BYTES;
+    uint8_t* const aslot = act_ring + as * ACT_SLICE_BYTES;
+    epilogue_slice<F2, N2>(p2, acc2, s, m0, 0, rloc, lane, mask0, mask1, s_scale2, s_bias2, slot, aslot);
+    fence_proxy_async();
+    if(leader) {
+      bulk_wait_read0();
+      if(s == 0 && release_rs >= 0) mbar_arrive(smem_u32(&r_empty[release_rs]));
+    }
+    warpgroup_sync(g);
+    if(leader) {
+      const int c0 = s * RES_COLS, r0 = m0 + g * (BLOCK_M / 2);
+      tma_store_2d(&tmapS2, smem_u32(slot + g * (R2_BYTES / 2)), c0, r0);
+      tma_store_2d(&tmapA2, smem_u32(aslot + g * (ACT_SLICE_BYTES / 2)), c0, r0);
+      bulk_commit();
+    }
+    ps ^= 1;
+    as ^= 1;
+  }
+}
+
+// dynamic smem: [<=1023 B slack][A tile: K1/64 x 16 KB][2 x T slot][residual ring][2 x raw staging][2 x act slice][stages x weights]
+//               [PairBars][BN scale / bias: exit N1, entry N2]
+static SmemLayout pairLayout(const ConvParams& p1, const ConvParams& p2) {
+  const int n2 = p2.cout_p, n1 = p1.cout_p;
+  const int r1 = BLOCK_M * RES_COLS * (p1.residual_fp32 ? 4 : 2), r2 = BLOCK_M * RES_COLS * (p2.raw_fp32 ? 4 : 2);
+  // a full residual ring when it leaves room for three weight stages, else half of one
+  for(int rs : {RES_SLOTS, 2}) {
+    const SmemLayout l = fitStages(1024 + BLOCK_M * n2 * 2 + 2 * PAIR_T_BYTES + rs * r1 + STAGE_SLOTS * r2 + ACT_SLOTS * ACT_SLICE_BYTES +
+                                   (int)sizeof(PairBars) + 2 * (n1 + n2) * (int)sizeof(float), n2 * PAIR_NC * 2, rs);
+    if(l.stages >= 3 || (rs == 2 && l.stages >= 2)) return l;
+  }
+  return SmemLayout();
 }
 
 template <int N2, int N1, bool S1_FP32, bool S2_FP32>
@@ -1126,12 +1149,8 @@ kgb_conv_pair_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_con
 
   pdl_launch_dependents();
   if(threadIdx.x == 0) {
-    for(const CUtensorMap* m : {&tmapA, &tmapW1, &tmapW2, &tmapS1, &tmapS2, &tmapA2})
-      asm volatile("prefetch.tensormap [%0];" ::"l"(m) : "memory");
-    for(int s = 0; s < stages; s++) {
-      mbar_init(smem_u32(&bars->full[s]), 1);
-      mbar_init(smem_u32(&bars->empty[s]), CONSUMER_WARPS);
-    }
+    for(const CUtensorMap* m : {&tmapA, &tmapW1, &tmapW2, &tmapS1, &tmapS2, &tmapA2}) prefetch_tmap(m);
+    init_weight_ring(bars->full, bars->empty, stages);
     mbar_init(smem_u32(&bars->a_full), 1);
     mbar_init(smem_u32(&bars->a_empty), CONSUMER_WARPS);
     for(int s = 0; s < RES_SLOTS; s++) {
@@ -1145,58 +1164,9 @@ kgb_conv_pair_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_con
   if(warp < 4) {
     // ===================== TMA producers =====================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-    if(warp == 0 && lane == 0) {
-      // the inner operand tile, then the weight chunks in consumption order
-      int stage = 0;
-      uint32_t phase = 0, aphase = 0;
-      auto loadW = [&](bool entry, int c) {
-        mbar_wait(smem_u32(&bars->empty[stage]), phase ^ 1);
-        const uint32_t full = smem_u32(&bars->full[stage]), dst = smem_w + stage * W_BYTES;
-        mbar_arrive_expect_tx(full, (uint32_t)W_BYTES);
-        if(entry) {
-          for(int j = 0; j < PAIR_NC / BLOCK_K; j++) tma_load_2d(dst + j * N2 * 128, &tmapW2, full, c * PAIR_NC + j * BLOCK_K, 0);
-        }
-        else {
-          for(int kb = 0; kb < K1 / BLOCK_K; kb++) tma_load_2d(dst + kb * PAIR_NC * 128, &tmapW1, full, kb * BLOCK_K, c * PAIR_NC);
-        }
-        if(++stage == stages) { stage = 0; phase ^= 1; }
-      };
-      // the first tile's first exit chunk goes out before its chain wait (weights do not depend on the previous launch)
-      bool pre = (int)blockIdx.x < tiles;
-      if(pre) loadW(false, 0);
-      for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-        const int m0 = tile * BLOCK_M;
-        chain_wait(p1.pred_flags, p1.pred_parts, tile, tiles);
-        mbar_wait(smem_u32(&bars->a_empty), aphase ^ 1);
-        const uint32_t afull = smem_u32(&bars->a_full);
-        mbar_arrive_expect_tx(afull, (uint32_t)A_BYTES);
-        for(int kb = 0; kb < K1 / BLOCK_K; kb++) tma_load_2d(smem_base + kb * BLOCK_M * 128, &tmapA, afull, kb * BLOCK_K, m0);
-        aphase ^= 1;
-        if(!pre) loadW(false, 0);
-        pre = false;
-        for(int c = 0; c < chunks; c++) {
-          if(c + 1 < chunks) loadW(false, c + 1);
-          loadW(true, c);
-        }
-      }
-    }
-    else if(warp == 1 && lane == 0) {
-      // the exit's residual slices
-      int rs = 0;
-      uint32_t rphase = 0;
-      for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-        const int m0 = tile * BLOCK_M;
-        chain_wait(p1.pred_flags, p1.pred_parts, tile, tiles);
-        for(int s = 0; s < N1 / RES_COLS; s++) {
-          mbar_wait(smem_u32(&bars->r_empty[rs]), rphase ^ 1);
-          const uint32_t rfull = smem_u32(&bars->r_full[rs]), dst = smem_r + rs * R1_BYTES;
-          mbar_arrive_expect_tx(rfull, (uint32_t)R1_BYTES);
-          tma_load_2d(dst, &tmapS1, rfull, s * RES_COLS, m0);
-          tma_load_2d(dst + R1_BYTES / 2, &tmapS1, rfull, s * RES_COLS, m0 + BLOCK_M / 2);
-          if(++rs == r_slots) { rs = 0; rphase ^= 1; }
-        }
-      }
-    }
+    if(warp == 0 && lane == 0) produce_pair_operands<N2, N1, PAIR_NC>(p1, *bars, tmapA, tmapW1, tmapW2, smem_base, smem_w, stages, tiles);
+    else if(warp == 1 && lane == 0)   // the exit's residual slices
+      produce_residual(p1, bars->r_full, bars->r_empty, tmapS1, smem_r, r_slots, R1_BYTES, 0, N1 / RES_COLS, tiles, 1);
     return;
   }
 
@@ -1215,17 +1185,7 @@ kgb_conv_pair_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_con
   uint8_t* const t_ring = smem + (smem_t - smem_base);
   uint8_t* const stg_ring = smem + (smem_stg - smem_base);
   uint8_t* const act_ring = smem + (smem_act - smem_base);
-  int pending = -1;   // as in kgb_conv_wg_kernel
-  auto take = [&]() {
-    const int st = stage;
-    mbar_wait(smem_u32(&bars->full[st]), phase);
-    if(++stage == stages) { stage = 0; phase ^= 1; }
-    return st;
-  };
-  auto release = [&](uint32_t bar) {
-    __syncwarp();
-    if(lane == 0) mbar_arrive(bar);
-  };
+  int pending = -1;   // the tile whose stores this warpgroup issued last and has not published yet
   for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
     const int m0 = tile * BLOCK_M;
     const float mask0 = m0 + rloc < p1.M ? __ldg(p1.mask + m0 + rloc) : 0.0f;
@@ -1262,13 +1222,13 @@ kgb_conv_pair_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_con
     zeroAcc1();
     fence_acc(acc1);
     fence_acc(acc2);
-    int st1 = take(), st2 = -1;
+    int st1 = take_stage(bars->full, stages, stage, phase), st2 = -1;
     wgmma_fence();
     issueP1(st1);
     wgmma_wait0();
     fence_acc(acc1);
-    release(smem_u32(&bars->empty[st1]));
-    if(chunks == 1) release(smem_u32(&bars->a_empty));
+    warp_arrive(smem_u32(&bars->empty[st1]), lane);
+    if(chunks == 1) warp_arrive(smem_u32(&bars->a_empty), lane);
     if(leader && pending >= 0) chain_publish(p1.tile_flags, pending);
 #pragma unroll
     for(int c = 0; c < chunks; c++) {
@@ -1295,51 +1255,32 @@ kgb_conv_pair_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_con
       // P2(c - 1) has read T slot (c - 1) & 1 and its weight stage
       if(c > 0) {
         wgmma_wait0();
-        release(smem_u32(&bars->empty[st2]));
+        warp_arrive(smem_u32(&bars->empty[st2]), lane);
       }
       zeroAcc1();
       fence_acc(acc1);
       fence_acc(acc2);
       wgmma_fence();
       if(c + 1 < chunks) {
-        st1 = take();
+        st1 = take_stage(bars->full, stages, stage, phase);
         issueP1(st1);
       }
-      st2 = take();
+      st2 = take_stage(bars->full, stages, stage, phase);
       issueP2(st2, c & 1);
       if(c + 1 < chunks) {
         wgmma_wait1();   // P1(c + 1) done, P2(c) may still run under the next chunk's epilogue
         fence_acc(acc1);
-        release(smem_u32(&bars->empty[st1]));
-        if(c + 2 == chunks) release(smem_u32(&bars->a_empty));   // the tile's last P1: the next tile's A may land
+        warp_arrive(smem_u32(&bars->empty[st1]), lane);
+        if(c + 2 == chunks) warp_arrive(smem_u32(&bars->a_empty), lane);   // the tile's last P1: the next tile's A may land
       }
     }
     wgmma_wait0();
     fence_acc(acc2);
-    release(smem_u32(&bars->empty[st2]));
+    warp_arrive(smem_u32(&bars->empty[st2]), lane);
 
-    // ---- the entry's epilogue: raw inner stream and activated inner operand, one 32-column slice at a time ----
-#pragma unroll
-    for(int s = 0; s < N2 / RES_COLS; s++) {
-      uint8_t* const slot = stg_ring + ps * R2_BYTES;
-      uint8_t* const aslot = act_ring + as * ACT_SLICE_BYTES;
-      epilogue_slice<F2, N2>(p2, acc2, s, m0, 0, rloc, lane, mask0, mask1, s_scale2, s_bias2, slot, aslot);
-      fence_proxy_async();
-      if(leader) {
-        bulk_wait_read0();
-        if(prev_rs >= 0) mbar_arrive(smem_u32(&bars->r_empty[prev_rs]));
-      }
-      prev_rs = -1;
-      warpgroup_sync(g);
-      if(leader) {
-        const int c0 = s * RES_COLS, r0 = m0 + g * (BLOCK_M / 2);
-        tma_store_2d(&tmapS2, smem_u32(slot + g * (R2_BYTES / 2)), c0, r0);
-        tma_store_2d(&tmapA2, smem_u32(aslot + g * (ACT_SLICE_BYTES / 2)), c0, r0);
-        bulk_commit();
-      }
-      ps ^= 1;
-      as ^= 1;
-    }
+    pair_entry_epilogue<F2, N2, R2_BYTES>(p2, acc2, m0, g, rloc, lane, leader, mask0, mask1, s_scale2, s_bias2, stg_ring, act_ring, ps, as,
+                                          tmapS2, tmapA2, bars->r_empty, prev_rs);
+    prev_rs = -1;
     pending = tile;
   }
   if(leader && pending >= 0) chain_publish(p1.tile_flags, pending);
@@ -1389,16 +1330,11 @@ struct __align__(8) PairEpiBars {
 
 // dynamic smem: [<=1023 B slack][A tile][2 x accumulator slot][2 x T slot][residual ring][2 x raw staging][2 x act slice]
 //               [stages x weights][PairEpiBars][BN scale / bias: exit N1, entry N2]
-static PairLayout pairEpiLayout(const ConvParams& p1, const ConvParams& p2) {
-  PairLayout l;
+static SmemLayout pairEpiLayout(const ConvParams& p1, const ConvParams& p2) {
   const int n2 = p2.cout_p, n1 = p1.cout_p;
-  const int wBytes = n2 * PAIR_EPI_NC * 2;
-  const int fixed = 1024 + BLOCK_M * n2 * 2 + 2 * ACC_SLICE_BYTES + 2 * ACT_SLICE_BYTES + RES_SLOTS * ACT_SLICE_BYTES +
-                    STAGE_SLOTS * ACT_SLICE_BYTES + ACT_SLOTS * ACT_SLICE_BYTES + (int)sizeof(PairEpiBars) + 2 * (n1 + n2) * (int)sizeof(float);
-  l.r_slots = RES_SLOTS;
-  l.stages = std::min(MAX_STAGES, (SMEM_LIMIT - fixed) / wBytes);
-  l.smem = fixed + l.stages * wBytes;
-  return l;
+  return fitStages(1024 + BLOCK_M * n2 * 2 + 2 * ACC_SLICE_BYTES + 2 * ACT_SLICE_BYTES + RES_SLOTS * ACT_SLICE_BYTES +
+                   STAGE_SLOTS * ACT_SLICE_BYTES + ACT_SLOTS * ACT_SLICE_BYTES + (int)sizeof(PairEpiBars) + 2 * (n1 + n2) * (int)sizeof(float),
+                   n2 * PAIR_EPI_NC * 2, RES_SLOTS);
 }
 
 template <int N2, int N1>
@@ -1436,12 +1372,8 @@ kgb_conv_pair_epi_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid
 
   pdl_launch_dependents();
   if(threadIdx.x == 0) {
-    for(const CUtensorMap* m : {&tmapA, &tmapW1, &tmapW2, &tmapS1, &tmapS2, &tmapA2})
-      asm volatile("prefetch.tensormap [%0];" ::"l"(m) : "memory");
-    for(int s = 0; s < stages; s++) {
-      mbar_init(smem_u32(&bars->full[s]), 1);
-      mbar_init(smem_u32(&bars->empty[s]), CONSUMER_WARPS);
-    }
+    for(const CUtensorMap* m : {&tmapA, &tmapW1, &tmapW2, &tmapS1, &tmapS2, &tmapA2}) prefetch_tmap(m);
+    init_weight_ring(bars->full, bars->empty, stages);
     mbar_init(smem_u32(&bars->a_full), 1);
     mbar_init(smem_u32(&bars->a_empty), CONSUMER_WARPS);
     for(int s = 0; s < RES_SLOTS; s++) {
@@ -1461,52 +1393,9 @@ kgb_conv_pair_epi_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid
   if(warp < 4) {
     // ===================== TMA producers =====================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-    if(warp == 0 && lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0, aphase = 0;
-      auto loadW = [&](bool entry, int c) {
-        mbar_wait(smem_u32(&bars->empty[stage]), phase ^ 1);
-        const uint32_t full = smem_u32(&bars->full[stage]), dst = smem_w + stage * W_BYTES;
-        mbar_arrive_expect_tx(full, (uint32_t)W_BYTES);
-        if(entry) tma_load_2d(dst, &tmapW2, full, c * NC, 0);
-        else
-          for(int kb = 0; kb < K1 / BLOCK_K; kb++) tma_load_2d(dst + kb * NC * 128, &tmapW1, full, kb * BLOCK_K, c * NC);
-        if(++stage == stages) { stage = 0; phase ^= 1; }
-      };
-      bool pre = (int)blockIdx.x < tiles;
-      if(pre) loadW(false, 0);
-      for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-        const int m0 = tile * BLOCK_M;
-        chain_wait(p1.pred_flags, p1.pred_parts, tile, tiles);
-        mbar_wait(smem_u32(&bars->a_empty), aphase ^ 1);
-        const uint32_t afull = smem_u32(&bars->a_full);
-        mbar_arrive_expect_tx(afull, (uint32_t)A_BYTES);
-        for(int kb = 0; kb < K1 / BLOCK_K; kb++) tma_load_2d(smem_base + kb * BLOCK_M * 128, &tmapA, afull, kb * BLOCK_K, m0);
-        aphase ^= 1;
-        if(!pre) loadW(false, 0);
-        pre = false;
-        for(int c = 0; c < chunks; c++) {
-          if(c + 1 < chunks) loadW(false, c + 1);
-          loadW(true, c);
-        }
-      }
-    }
-    else if(warp == 1 && lane == 0) {
-      int rs = 0;
-      uint32_t rphase = 0;
-      for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-        const int m0 = tile * BLOCK_M;
-        chain_wait(p1.pred_flags, p1.pred_parts, tile, tiles);
-        for(int s = 0; s < chunks; s++) {
-          mbar_wait(smem_u32(&bars->r_empty[rs]), rphase ^ 1);
-          const uint32_t rfull = smem_u32(&bars->r_full[rs]), dst = smem_r + rs * ACT_SLICE_BYTES;
-          mbar_arrive_expect_tx(rfull, (uint32_t)ACT_SLICE_BYTES);
-          tma_load_2d(dst, &tmapS1, rfull, s * RES_COLS, m0);
-          tma_load_2d(dst + ACT_SLICE_BYTES / 2, &tmapS1, rfull, s * RES_COLS, m0 + BLOCK_M / 2);
-          if(++rs == RES_SLOTS) { rs = 0; rphase ^= 1; }
-        }
-      }
-    }
+    if(warp == 0 && lane == 0) produce_pair_operands<N2, N1, NC>(p1, *bars, tmapA, tmapW1, tmapW2, smem_base, smem_w, stages, tiles);
+    else if(warp == 1 && lane == 0)
+      produce_residual(p1, bars->r_full, bars->r_empty, tmapS1, smem_r, RES_SLOTS, ACT_SLICE_BYTES, 0, chunks, tiles, 1);
     return;
   }
 
@@ -1530,24 +1419,14 @@ kgb_conv_pair_epi_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid
         uint8_t* const rslot = smem + (smem_r - smem_base) + rs * ACT_SLICE_BYTES;
         mbar_wait(smem_u32(&bars->acc_full[slot]), par);
         __syncwarp();
-        const uint8_t* const aslot = smem + (smem_acc - smem_base) + slot * ACC_SLICE_BYTES;
         float v[RES_COLS];
-#pragma unroll
-        for(int j = 0; j < RES_COLS / 4; j++) {
-          const float4 f = *reinterpret_cast<const float4*>(aslot + slice_offset(rl, 4 * j, true));
-          v[4 * j] = f.x; v[4 * j + 1] = f.y; v[4 * j + 2] = f.z; v[4 * j + 3] = f.w;
-        }
+        load_acc_row(smem + (smem_acc - smem_base) + slot * ACC_SLICE_BYTES, rl, v);
         mbar_wait(smem_u32(&bars->r_full[rs]), rphase);
         __syncwarp();
         uint32_t res[RES_COLS / 2];
-#pragma unroll
-        for(int j = 0; j < RES_COLS / 8; j++) {
-          const uint4 u = *reinterpret_cast<const uint4*>(rslot + slice_offset(rl, 8 * j, false));
-          res[4 * j] = u.x; res[4 * j + 1] = u.y; res[4 * j + 2] = u.z; res[4 * j + 3] = u.w;
-        }
+        load_half_row(rslot, rl, res);
         // the warp's rows of the accumulator slot are read: the MMA warpgroups may write chunk k + 2 into it
-        __syncwarp();
-        if(lane == 0) mbar_arrive(smem_u32(&bars->acc_empty[slot]));
+        warp_arrive(smem_u32(&bars->acc_empty[slot]), lane);
         mbar_wait(smem_u32(&bars->t_empty[slot]), par ^ 1);   // P2 of chunk k - 2 has read the T slot
         __syncwarp();
         uint8_t* const tslot = smem + (smem_t - smem_base) + slot * ACT_SLICE_BYTES;
@@ -1590,17 +1469,7 @@ kgb_conv_pair_epi_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid
   uint8_t* const acc_ring = smem + (smem_acc - smem_base);
   uint8_t* const stg_ring = smem + (smem_stg - smem_base);
   uint8_t* const act_ring = smem + (smem_act - smem_base);
-  int pending = -1;   // as in kgb_conv_wg_kernel
-  auto take = [&]() {
-    const int st = stage;
-    mbar_wait(smem_u32(&bars->full[st]), phase);
-    if(++stage == stages) { stage = 0; phase ^= 1; }
-    return st;
-  };
-  auto release = [&](uint32_t bar) {
-    __syncwarp();
-    if(lane == 0) mbar_arrive(bar);
-  };
+  int pending = -1;   // the tile whose stores this warpgroup issued last and has not published yet
   float acc1[NC / 2];
   // P1 of the chunk with index kc (acc1 = A rows 64g.. x the W1 chunk of the next weight stage, K1 / 64 k-blocks of 4 k16 steps, as
   // the exit's launch sums them), handed to the epilogue warpgroup through accumulator slot kc & 1 once it has read chunk kc - 2
@@ -1610,7 +1479,7 @@ kgb_conv_pair_epi_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid
     for(int i = 0; i < NC / 2; i++) acc1[i] = 0.0f;
     fence_acc(acc1);
     wgmma_fence();
-    const int st1 = take();
+    const int st1 = take_stage(bars->full, stages, stage, phase);
     const uint32_t w = smem_w + st1 * W_BYTES, a = smem_base + g * 64 * 128;
 #pragma unroll
     for(int kb = 0; kb < K1 / BLOCK_K; kb++)
@@ -1620,18 +1489,12 @@ kgb_conv_pair_epi_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid
     wgmma_commit();
     wgmma_wait0();
     fence_acc(acc1);
-    release(smem_u32(&bars->empty[st1]));
-    if(last) release(smem_u32(&bars->a_empty));   // the tile's last P1: the next tile's A may land
+    warp_arrive(smem_u32(&bars->empty[st1]), lane);
+    if(last) warp_arrive(smem_u32(&bars->a_empty), lane);   // the tile's last P1: the next tile's A may land
     const int slot = kc & 1;
     mbar_wait(smem_u32(&bars->acc_empty[slot]), ((kc >> 1) & 1) ^ 1);
-    uint8_t* const dst = acc_ring + slot * ACC_SLICE_BYTES;
-#pragma unroll
-    for(int j = 0; j < NC / 8; j++)
-#pragma unroll
-      for(int h = 0; h < 2; h++)
-        *reinterpret_cast<float2*>(dst + slice_offset(rloc + 8 * h, 8 * j + 2 * (lane & 3), true)) =
-          make_float2(acc1[4 * j + 2 * h], acc1[4 * j + 2 * h + 1]);
-    release(smem_u32(&bars->acc_full[slot]));
+    store_acc_slices<NC>(acc_ring + slot * ACC_SLICE_BYTES, acc1, rloc, lane);
+    warp_arrive(smem_u32(&bars->acc_full[slot]), lane);
   };
   bool have0 = false;   // the tile's chunk 0 was handed over before the previous tile's entry epilogue
   for(int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
@@ -1651,7 +1514,7 @@ kgb_conv_pair_epi_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid
     auto issueP2 = [&](int c) {
       const int tslot = (k + c) & 1;
       mbar_wait(smem_u32(&bars->t_full[tslot]), ((k + c) >> 1) & 1);
-      const int st = take();
+      const int st = take_stage(bars->full, stages, stage, phase);
       const uint32_t w = smem_w + st * W_BYTES, t = smem_t + tslot * ACT_SLICE_BYTES + g * 64 * 64;
 #pragma unroll
       for(int j = 0; j < NC / 16; j++) WgmmaSS<N2>::mma(acc2, make_smem_desc_sw64(t) + 2 * j, make_smem_desc_sw64(w) + 2 * j);
@@ -1659,8 +1522,8 @@ kgb_conv_pair_epi_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid
       return st;
     };
     auto releaseP2 = [&](int c, int st) {
-      release(smem_u32(&bars->empty[st]));
-      release(smem_u32(&bars->t_empty[(k + c) & 1]));
+      warp_arrive(smem_u32(&bars->empty[st]), lane);
+      warp_arrive(smem_u32(&bars->t_empty[(k + c) & 1]), lane);
     };
     // Chunk c: P1(c), handed to the epilogue warpgroup as soon as it is complete; then P2(c - 1) once the epilogue warpgroup has
     // made T slot (c - 1) & 1 out of chunk c - 1.  So the epilogue warpgroup finds chunk c ready when it finishes chunk c - 1, and
@@ -1688,24 +1551,8 @@ kgb_conv_pair_epi_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid
       handChunk(k, false);
     }
 
-    // ---- the entry's epilogue: raw inner stream and activated inner operand, one 32-column slice at a time ----
-#pragma unroll
-    for(int s = 0; s < N2 / RES_COLS; s++) {
-      uint8_t* const slot = stg_ring + ps * ACT_SLICE_BYTES;
-      uint8_t* const aslot = act_ring + as * ACT_SLICE_BYTES;
-      epilogue_slice<F2, N2>(p2, acc2, s, m0, 0, rloc, lane, mask0, mask1, s_scale2, s_bias2, slot, aslot);
-      fence_proxy_async();
-      if(leader) bulk_wait_read0();
-      warpgroup_sync(g);
-      if(leader) {
-        const int c0 = s * RES_COLS, r0 = m0 + g * (BLOCK_M / 2);
-        tma_store_2d(&tmapS2, smem_u32(slot + g * (ACT_SLICE_BYTES / 2)), c0, r0);
-        tma_store_2d(&tmapA2, smem_u32(aslot + g * (ACT_SLICE_BYTES / 2)), c0, r0);
-        bulk_commit();
-      }
-      ps ^= 1;
-      as ^= 1;
-    }
+    pair_entry_epilogue<F2, N2, ACT_SLICE_BYTES>(p2, acc2, m0, g, rloc, lane, leader, mask0, mask1, s_scale2, s_bias2, stg_ring, act_ring,
+                                                 ps, as, tmapS2, tmapA2, bars->r_empty, -1);
     pending = tile;
   }
   if(leader && pending >= 0) chain_publish(p1.tile_flags, pending);
@@ -1766,7 +1613,7 @@ bool convPairEpilogueWG(const ConvParams& p1, const ConvParams& p2) {
 int convPairChainParts(const ConvParams& p1, const ConvParams& p2) { return convPairEpilogueWG(p1, p2) ? 3 : kConvPairParts; }
 
 template <int N2, int N1>
-static cudaError_t launchPairN(const ConvPairTmaps& tm, const ConvParams& p1, const ConvParams& p2, int grid, const PairLayout& l,
+static cudaError_t launchPairN(const ConvPairTmaps& tm, const ConvParams& p1, const ConvParams& p2, int grid, const SmemLayout& l,
                                cudaStream_t stream) {
   auto k = p1.raw_fp32 ? (p2.raw_fp32 ? kgb_conv_pair_kernel<N2, N1, true, true> : kgb_conv_pair_kernel<N2, N1, true, false>)
                        : kgb_conv_pair_kernel<N2, N1, false, false>;
@@ -1775,13 +1622,12 @@ static cudaError_t launchPairN(const ConvPairTmaps& tm, const ConvParams& p1, co
 
 cudaError_t launchConvPair(const ConvPairTmaps& tm, const ConvParams& p1, const ConvParams& p2, cudaStream_t stream) {
   if(!convPairSupported(p1, p2) || p1.tile_flags == nullptr) return cudaErrorInvalidValue;
-  int dev = 0;
-  const cudaError_t e = cudaGetDevice(&dev);
+  int sms = 0;
+  const cudaError_t e = smCount(&sms);
   if(e != cudaSuccess) return e;
-  if(dev < 0 || dev >= 64 || g_smCount[dev] < 1) return cudaErrorInitializationError;
-  const int grid = std::min(p1.num_m_tiles, g_smCount[dev]);
+  const int grid = std::min(p1.num_m_tiles, sms);
   if(convPairEpilogueWG(p1, p2)) {
-    const PairLayout l = pairEpiLayout(p1, p2);
+    const SmemLayout l = pairEpiLayout(p1, p2);
 #define KGB_PAIR_EPI_LAUNCH(N2, N1)                                                                                                         \
     if(p2.cout_p == N2 && p1.cout_p == N1)                                                                                                   \
       return launchChained(kgb_conv_pair_epi_kernel<N2, N1>, p1, grid, PAIR_EPI_THREADS, l.smem, stream, tm.A, tm.W1, tm.W2, tm.stream1, \
@@ -1789,7 +1635,7 @@ cudaError_t launchConvPair(const ConvPairTmaps& tm, const ConvParams& p1, const 
     KGB_PAIR_EPI_SHAPES(KGB_PAIR_EPI_LAUNCH)
 #undef KGB_PAIR_EPI_LAUNCH
   }
-  const PairLayout l = pairLayout(p1, p2);
+  const SmemLayout l = pairLayout(p1, p2);
 #define KGB_PAIR_LAUNCH(N2, N1) if(p2.cout_p == N2 && p1.cout_p == N1) return launchPairN<N2, N1>(tm, p1, p2, grid, l, stream);
   KGB_PAIR_SHAPES(KGB_PAIR_LAUNCH)
 #undef KGB_PAIR_LAUNCH
