@@ -496,16 +496,17 @@ KGB_API int kgb_bench_conv_ex(int ky, int kx, int in_c, int out_c, int n, int nn
 KGB_API int kgb_test_conv_epilogue(int ky, int kx, int in_c, int out_c, const float* weights, int n, int nn_x_len, int nn_y_len, int use_fp16,
                            int epilogue_kind, const float* input, const float* residual_in, const float* bn_scale, const float* bn_bias,
                            int activation, float* raw_out, float* act_out);
-/* Test hook that reaches every input of the fused epilogue (kinds 0-4 above; kgb_test_conv and kgb_test_conv_epilogue are its
- * narrower forms).  Beyond kgb_test_conv_epilogue's arguments:
+/* Test hook that reaches every input of the fused epilogue (kinds 0-4 above, and 5 and 6 = kinds 2 and 4 without the raw output: the
+ * residual is read and the stream is left as it was, as the last block of a level runs; kgb_test_conv and kgb_test_conv_epilogue are
+ * its narrower forms).  Beyond kgb_test_conv_epilogue's arguments:
  *   board_xy [n][2] {X_i, Y_i}, or NULL for the whole frame: the mask is 1 on image i's top-left X_i x Y_i board and 0 elsewhere, as
  *     the self-play loop places smaller boards.  The input may be nonzero off the board; only the mask zeroes those outputs.
  *   ncbias [n][out_c] or NULL: a per-image bias added before the residual, as the initial conv adds the global-input bias.  The
  *     kernel applies it in every kind; tests/test_gpu_conv_fp64.py checks it in kind 3, the initial conv's, only.
  *   residual_in is fp32; an fp16 stream holds it rounded to nearest.  activation 0 identity, 1 relu, 2 mish, 3 silu.
- * Outputs, NHWC [n][y][x][out_c] as floats: raw_out (kind 0 and kinds 2-4), act_hi_out (kinds 1-4) and, in split mode, act_lo_out
- * (kinds 1-4), the activated operand's two fp16 halves as the next layer reads them.  The hook fails if any output is nonzero in a
- * row the mask zeroes, or in the padded channels out_c..cout_p of any row. */
+ * Outputs, NHWC [n][y][x][out_c] as floats: raw_out (kind 0 and kinds 2-4), act_hi_out (kinds 1-6) and, in split mode, act_lo_out
+ * (kinds 1-6), the activated operand's two fp16 halves as the next layer reads them.  The hook fails if any output is nonzero in a
+ * row the mask zeroes, or in the padded channels out_c..cout_p of any row, or if kind 5 or 6 changed the stream. */
 KGB_API int kgb_test_conv_ex(int ky, int kx, int in_c, int out_c, const float* weights, int n, int nn_x_len, int nn_y_len, int use_fp16,
                              int epilogue_kind, const float* input, const int32_t* board_xy, const float* ncbias, const float* residual_in,
                              const float* bn_scale, const float* bn_bias, int activation, float* raw_out, float* act_hi_out,
@@ -537,6 +538,22 @@ KGB_API int kgb_test_conv_plan(int ky, int kx, int in_c, int out_c, const float*
 KGB_API int kgb_test_conv_boundary_plan(int inner_c, int trunk_c, int n, int nn_x_len, int nn_y_len, const int32_t* board_xy,
                                         const int32_t* symmetry, int ragged, int trunk_fp32, int inner_fp32, uint32_t seed, int64_t* out,
                                         int64_t* layout_stats);
+/* The same boundary on the caller's data, run one way: fused != 0 as one fused launch, 0 as the two launches.  inner_a [n][y][x][inner_c]
+ * is the inner operand (rounded to fp16), trunk_s [n][y][x][trunk_c] the trunk stream (rounded to fp16 unless trunk_fp32); exit_w
+ * [inner_c][trunk_c] with trunk_scale / trunk_bias [trunk_c], entry_w [trunk_c][inner_c] with inner_scale / inner_bias [inner_c]; mish at
+ * both ends.  ragged -1 is the frame layout (board_xy as in kgb_test_conv_ex, symmetry NULL), 0 or 1 plan mode as in kgb_test_conv_plan
+ * (layout_stats [3] or NULL); every array is NHWC in the coordinates after the symmetry, and only board positions are read.  Returns the
+ * trunk stream, the inner stream and the inner operand after the launch, NHWC as floats (0 off the board).  Fails if an output is
+ * nonzero in a row the mask zeroes or in a padded channel, or, in plan mode, was written at or past the plan's end. */
+KGB_API int kgb_test_conv_boundary_ex(int inner_c, int trunk_c, int n, int nn_x_len, int nn_y_len, const float* inner_a, const float* exit_w,
+                                      const float* trunk_s, const float* trunk_scale, const float* trunk_bias, const float* entry_w,
+                                      const float* inner_scale, const float* inner_bias, const int32_t* board_xy, const int32_t* symmetry,
+                                      int ragged, int trunk_fp32, int inner_fp32, int fused, float* trunk_s_out, float* inner_s_out,
+                                      float* inner_a_out, int64_t* layout_stats);
+/* The kernel the last convolution test hook (kgb_test_conv*, kgb_test_conv_boundary*) launched, as the launchers choose it: 0
+ * kgb_conv_wg_kernel, 1 kgb_conv_wg_epi_kernel, 2 kgb_conv_pair_kernel, 3 kgb_conv_pair_epi_kernel (the seeded boundary hooks report
+ * their fused launch).  Fails if no hook has launched, or the last one failed before its launch. */
+KGB_API int kgb_test_last_conv_kernel(int* out);
 /* Test hook of the evaluator's fp32 kernels: one launch of kernel `which` on caller-given fp32 tensors, in a frame of
  * nn_x_len x nn_y_len with `pad` (1 or 2).  Kernels that read rows run under a plan made as for kgb_test_conv_plan (board_xy,
  * symmetry, ragged; layout_stats and plan_out as there); their row inputs are NHWC [n][y][x][C] after the symmetry and are placed

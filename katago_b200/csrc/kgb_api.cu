@@ -1212,6 +1212,11 @@ size_t countTouchedTail(const std::vector<uint8_t>& v, size_t rowBytes, size_t f
   return k;
 }
 
+// The kernel the last convolution test hook launched (kgb_test_last_conv_kernel), as convEpilogueWG and convPairEpilogueWG chose
+// it; -1 until a hook has run, and after one that failed before its launch
+enum { TEST_KERNEL_WG = 0, TEST_KERNEL_WG_EPI = 1, TEST_KERNEL_PAIR = 2, TEST_KERNEL_PAIR_EPI = 3 };
+int g_lastConvKernel = -1;
+
 struct SingleConv {
   kgb_handle h;
   ModelDesc dummy;
@@ -1223,13 +1228,14 @@ struct SingleConv {
   std::vector<void*> raws;
   float* ncbias = nullptr;   // [n][cout_p], the initial conv's per-image bias, when asked for
   std::vector<float> mask;   // [M], as setInput uploaded it
-  bool rawF32 = true;   // the raw output of kind 0 is fp32; the stream of kinds 2-4 is fp32 for kind 4 and in fp32-equivalent mode
+  bool rawF32 = true;   // the raw output of kind 0 is fp32; the stream of kinds 2-6 is fp32 for kinds 4 and 6 and in fp32-equivalent mode
   int rotate, next = 0;
   // kind: 0 = fp32 raw output only; 1 = the first conv of a residual unit (BN + mish + mask -> fp16 operand of the next conv);
   // 2 = the second conv of a unit (+ fp16 residual stream, updated in place, and the next unit's BN + mish operand); 3 = a nested
   // block's pre conv (fp16 raw stream + activated operand); 4 = kind 2 with an fp32 residual stream, as the trunk runs in fp16 mode
-  // with KGB_STREAM_FP32=trunk.  In fp32-equivalent mode every stream is fp32.  `rotate` independent buffer sets are cycled through
-  // by run() so that a timing loop does not live in L2.
+  // with KGB_STREAM_FP32=trunk; 5 and 6 = kinds 2 and 4 without the raw output (the residual is read, the stream is not written),
+  // as the last block of a level runs.  In fp32-equivalent mode every stream is fp32.  `rotate` independent buffer sets are cycled
+  // through by run() so that a timing loop does not live in L2.
   SingleConv(int ky, int kx, int in_c, int out_c, const float* weights, int n_, int X_, int Y_, int use_fp16, int kind, int rotate_ = 1,
              const float* bnScale = nullptr, const float* bnBias = nullptr, int actKind = ACT_MISH, bool withNcbias = false,
              int ragged = -1)
@@ -1268,7 +1274,8 @@ struct SingleConv {
       h.dMask = h.dalloc<float>(M + 128);
       h.dMaskSum = h.dalloc<float>(n);
     }
-    rawF32 = kind == 0 || kind == 4 || h.split != 0;
+    rawF32 = kind == 0 || kind == 4 || kind == 6 || h.split != 0;
+    const bool residual = kind == 2 || kind == 4 || kind == 5 || kind == 6, rawOut = kind != 1 && kind != 5 && kind != 6;
     if(withNcbias) ncbias = h.dalloc<float>((size_t)n * cw.cout_p);
     for(int r = 0; r < rotate; r++) {
       __half* A = h.dalloc<__half>(M * cw.cin_p * b.actMul);
@@ -1277,7 +1284,7 @@ struct SingleConv {
       As.push_back(A);
       if(act) acts.push_back(act);
       if(raw) raws.push_back(raw);
-      b.emitConv(cw, A, kind == 2 || kind == 4 ? raw : nullptr, rawF32, ncbias, raw, rawF32, act, kind == 0 ? Builder::BNDev() : dev);
+      b.emitConv(cw, A, residual ? raw : nullptr, rawF32, ncbias, rawOut ? raw : nullptr, rawF32, act, kind == 0 ? Builder::BNDev() : dev);
     }
     h.allocChain();
   }
@@ -1321,16 +1328,38 @@ struct SingleConv {
   void run() { h.ops[next](n, h.stream); next = (next + 1) % rotate; }
 };
 
-// A nested-block boundary on its own: the exit 1x1 (inner_c -> trunk_c, + the trunk stream) of one block and the entry 1x1
-// (trunk_c -> inner_c) of the next, with seeded random weights, BN constants and inputs.  Buffer set 2r runs it as one fused launch
-// (launchConvPair), set 2r + 1 as the two launches of the unfused path, on the same inputs; `rotate` pairs of sets are cycled
-// through by run() so that a timing loop does not live in L2.
+// The seeded boundary's host arrays, from one generator: the exit's and the entry's weights, the trunk's and the inner BN
+// constants, then (BoundaryConv::seedInputs) the inputs of every board row in row order
+struct BoundarySeed {
+  uint32_t st;
+  explicit BoundarySeed(uint32_t seed) : st(seed * 2654435761u + 12345u) {}
+  float uni() { st = st * 1664525u + 1013904223u; return (st >> 8) * (1.0f / 16777216.0f); }
+  ConvDesc conv(int cin, int cout) {
+    ConvDesc c;
+    c.ky = c.kx = 1; c.cin = cin; c.cout = cout;
+    c.w.resize((size_t)cin * cout);
+    for(auto& v : c.w) v = (uni() - 0.5f) * 4.0f / std::sqrt((float)cin);
+    return c;
+  }
+  BNDesc bn(int c) {
+    BNDesc b;
+    b.c = c;
+    for(int i = 0; i < c; i++) { b.scale.push_back(0.5f + uni()); b.bias.push_back(uni() - 0.5f); }
+    return b;
+  }
+};
+
+// A nested-block boundary on its own: the exit 1x1 `post` (inner_c -> trunk_c, + the trunk stream, then the trunk BN and mish) of
+// one block and the entry 1x1 `pre` (trunk_c -> inner_c, then the inner BN and mish) of the next.  Buffer set 2r runs it as one fused
+// launch (launchConvPair), set 2r + 1 as the two launches of the unfused path, on the same inputs (setInputs); `rotate` pairs of sets
+// are cycled through by run() so that a timing loop does not live in L2.
 struct BoundaryConv {
   kgb_handle h;
   ModelDesc dummy;
   ConvWeights wpost, wpre;
-  int n, innerCp = 0, trunkCp = 0, rotate, next = 0;
-  bool trunkF32, innerF32;
+  int n, innerC, trunkC, innerCp = 0, trunkCp = 0, rotate, next = 0;
+  int fusedKernel = TEST_KERNEL_PAIR;   // the kernel of the fused op, as emitConvPair counted convPairEpilogueWG's choice
+  bool trunkF32, innerF32, planned;
   size_t M;
   struct Set {
     __half *innerA = nullptr, *trunkA = nullptr;
@@ -1340,9 +1369,10 @@ struct BoundaryConv {
   std::vector<float> mask;
   HostPlan hp;   // plan mode: the plan; every buffer's rows from hp.stats[0] on hold all-ones bytes before the launches
   // ragged < 0: the fixed frame layout; else plan mode, boards moved by `symmetry` (planBoards)
-  BoundaryConv(int inner_c, int trunk_c, int n_, int X, int Y, const int32_t* boardXY, bool trunkFp32, bool innerFp32, uint32_t seed, int rotate_,
-               const int32_t* symmetry = nullptr, int ragged = -1)
-      : n(n_), rotate(rotate_ < 1 ? 1 : rotate_), trunkF32(trunkFp32), innerF32(innerFp32) {
+  BoundaryConv(int inner_c, int trunk_c, int n_, int X, int Y, const int32_t* boardXY, bool trunkFp32, bool innerFp32, const ConvDesc& post,
+               const ConvDesc& pre, const BNDesc& bnTrunk, const BNDesc& bnInner, int rotate_, const int32_t* symmetry = nullptr, int ragged = -1)
+      : n(n_), innerC(inner_c), trunkC(trunk_c), rotate(rotate_ < 1 ? 1 : rotate_), trunkF32(trunkFp32), innerF32(innerFp32),
+        planned(ragged >= 0) {
     h.device = selectDevice(-1);
     h.model = &dummy;
     h.maxBatch = n;
@@ -1356,22 +1386,6 @@ struct BoundaryConv {
       allocPlan(h);
       hp = finishPlan(h, n, planBoards(h, n, boardXY, symmetry));
     }
-    uint32_t st = seed * 2654435761u + 12345u;
-    auto uni = [&]() { st = st * 1664525u + 1013904223u; return (st >> 8) * (1.0f / 16777216.0f); };
-    ConvDesc post, pre;
-    post.ky = post.kx = pre.ky = pre.kx = 1;
-    post.cin = pre.cout = inner_c; post.cout = pre.cin = trunk_c;
-    for(ConvDesc* c : {&post, &pre}) {
-      c->w.resize((size_t)c->cin * c->cout);
-      for(auto& v : c->w) v = (uni() - 0.5f) * 4.0f / std::sqrt((float)c->cin);
-    }
-    auto randBN = [&](int c) {
-      BNDesc bn;
-      bn.c = c;
-      for(int i = 0; i < c; i++) { bn.scale.push_back(0.5f + uni()); bn.bias.push_back(uni() - 0.5f); }
-      return bn;
-    };
-    const BNDesc bnTrunk = randBN(trunk_c), bnInner = randBN(inner_c);
     Builder::BNDev bn1, bn2;
     buildWeights(h, [&](kgb_handle& hh) {
       Builder b(hh);
@@ -1393,16 +1407,6 @@ struct BoundaryConv {
       CK(cudaMemcpyAsync(h.dMask, mask.data(), M * sizeof(float), cudaMemcpyHostToDevice, h.stream));
     }
     else mask = hp.mask;
-    // inputs as the previous layers leave them: zero in masked rows and padded channels
-    std::vector<__half> hA(M * innerCp, __float2half(0.0f));
-    std::vector<float> hS(M * trunkCp, 0.0f);
-    for(size_t r = 0; r < M; r++) {
-      if(mask[r] == 0.0f) continue;
-      for(int c = 0; c < inner_c; c++) hA[r * innerCp + c] = __float2half_rn(uni() * 2.0f);
-      for(int c = 0; c < trunk_c; c++) hS[r * trunkCp + c] = (uni() - 0.5f) * 8.0f;
-    }
-    std::vector<__half> hS16(hS.size());
-    for(size_t k = 0; k < hS.size(); k++) hS16[k] = __float2half_rn(hS[k]);
     Builder b(h);
     for(int k = 0; k < 2 * rotate; k++) {
       Set s;
@@ -1410,15 +1414,6 @@ struct BoundaryConv {
       s.trunkA = h.dalloc<__half>(M * trunkCp);
       s.trunkS = trunkF32 ? (void*)h.dalloc<float>(M * trunkCp) : (void*)h.dalloc<__half>(M * trunkCp);
       s.innerS = innerF32 ? (void*)h.dalloc<float>(M * innerCp) : (void*)h.dalloc<__half>(M * innerCp);
-      CK(cudaMemcpyAsync(s.innerA, hA.data(), hA.size() * sizeof(__half), cudaMemcpyHostToDevice, h.stream));
-      if(trunkF32) CK(cudaMemcpyAsync(s.trunkS, hS.data(), hS.size() * sizeof(float), cudaMemcpyHostToDevice, h.stream));
-      else CK(cudaMemcpyAsync(s.trunkS, hS16.data(), hS16.size() * sizeof(__half), cudaMemcpyHostToDevice, h.stream));
-      if(ragged >= 0) {   // 1x1 convolutions: no tap reaches past a tile's own rows, so every buffer can hold NaN there
-        poisonTail(h, s.innerA, (size_t)innerCp * 2, hp.stats[0], M);
-        poisonTail(h, s.trunkA, (size_t)trunkCp * 2, hp.stats[0], M);
-        poisonTail(h, s.trunkS, (size_t)trunkCp * (trunkF32 ? 4 : 2), hp.stats[0], M);
-        poisonTail(h, s.innerS, (size_t)innerCp * (innerF32 ? 4 : 2), hp.stats[0], M);
-      }
       sets.push_back(s);
       if(k % 2 == 0) {
         if(!b.emitConvPair(wpost, s.innerA, s.trunkS, trunkF32, bn1, wpre, s.innerS, innerF32, s.innerA, bn2))
@@ -1431,6 +1426,7 @@ struct BoundaryConv {
         b.emitConv(wpre, s.trunkA, nullptr, false, nullptr, s.innerS, innerF32, s.innerA, bn2);
       }
     }
+    fusedKernel = h.pairEpilogueWGLaunches > 0 ? TEST_KERNEL_PAIR_EPI : TEST_KERNEL_PAIR;
     h.allocChain();
     CK(cudaStreamSynchronize(h.stream));
   }
@@ -1438,6 +1434,34 @@ struct BoundaryConv {
     for(void* p : h.allocs) cudaFree(p);
     if(h.wHost) cudaFreeHost(h.wHost);
     if(h.stream) cudaStreamDestroy(h.stream);
+  }
+  // The inputs of every set, as the previous layers leave them: the inner operand hA [M][innerCp] and the trunk stream hS
+  // [M][trunkCp], zero in masked rows and padded channels
+  void setInputs(const std::vector<__half>& hA, const std::vector<float>& hS) {
+    std::vector<__half> hS16(hS.size());
+    for(size_t k = 0; k < hS.size(); k++) hS16[k] = __float2half_rn(hS[k]);
+    for(const Set& s : sets) {
+      CK(cudaMemcpyAsync(s.innerA, hA.data(), hA.size() * sizeof(__half), cudaMemcpyHostToDevice, h.stream));
+      if(trunkF32) CK(cudaMemcpyAsync(s.trunkS, hS.data(), hS.size() * sizeof(float), cudaMemcpyHostToDevice, h.stream));
+      else CK(cudaMemcpyAsync(s.trunkS, hS16.data(), hS16.size() * sizeof(__half), cudaMemcpyHostToDevice, h.stream));
+      if(planned) {   // 1x1 convolutions: no tap reaches past a tile's own rows, so every buffer can hold NaN there
+        poisonTail(h, s.innerA, (size_t)innerCp * 2, hp.stats[0], M);
+        poisonTail(h, s.trunkA, (size_t)trunkCp * 2, hp.stats[0], M);
+        poisonTail(h, s.trunkS, (size_t)trunkCp * (trunkF32 ? 4 : 2), hp.stats[0], M);
+        poisonTail(h, s.innerS, (size_t)innerCp * (innerF32 ? 4 : 2), hp.stats[0], M);
+      }
+    }
+    CK(cudaStreamSynchronize(h.stream));
+  }
+  void seedInputs(BoundarySeed& g) {
+    std::vector<__half> hA(M * innerCp, __float2half(0.0f));
+    std::vector<float> hS(M * trunkCp, 0.0f);
+    for(size_t r = 0; r < M; r++) {
+      if(mask[r] == 0.0f) continue;
+      for(int c = 0; c < innerC; c++) hA[r * innerCp + c] = __float2half_rn(g.uni() * 2.0f);
+      for(int c = 0; c < trunkC; c++) hS[r * trunkCp + c] = (g.uni() - 0.5f) * 8.0f;
+    }
+    setInputs(hA, hS);
   }
   // ops: set 2r's fused op is op 3r, set 2r + 1's two launches ops 3r + 1 and 3r + 2
   void run(bool fused) {
@@ -1457,16 +1481,20 @@ void testConv(const char* fn, int ky, int kx, int in_c, int out_c, const float* 
               const float* input, const int32_t* board_xy, const float* ncbias, const float* residual_in, const float* bn_scale,
               const float* bn_bias, int activation, float* raw_out, float* act_hi_out, float* act_lo_out, const int32_t* symmetry = nullptr,
               int ragged = -1, int64_t* stats_out = nullptr, int32_t* plan_out = nullptr) {
-  const bool hasResidual = kind == 2 || kind == 4;
+  const bool hasResidual = kind == 2 || kind == 4 || kind == 5 || kind == 6;
+  const bool hasRaw = kind == 0 || (kind >= 2 && kind <= 4);
   const bool planned = ragged >= 0;
-  if(!weights || !input || n < 1 || kind < 0 || kind > 4 || activation < ACT_IDENTITY || activation > ACT_SILU ||
+  g_lastConvKernel = -1;
+  if(!weights || !input || n < 1 || kind < 0 || kind > 6 || activation < ACT_IDENTITY || activation > ACT_SILU ||
      (kind == 0 ? !raw_out : !act_hi_out))
     throw std::invalid_argument(std::string(fn) + ": bad argument");
-  if(hasResidual && !residual_in) throw std::invalid_argument(std::string(fn) + ": kinds 2 and 4 need residual_in");
-  if(kind >= 2 && !raw_out) throw std::invalid_argument(std::string(fn) + ": kinds 2 to 4 need raw_out");
+  if(hasResidual && !residual_in) throw std::invalid_argument(std::string(fn) + ": kinds 2, 4, 5 and 6 need residual_in");
+  if(kind >= 2 && kind <= 4 && !raw_out) throw std::invalid_argument(std::string(fn) + ": kinds 2 to 4 need raw_out");
   checkBoards(fn, n, nn_x_len, nn_y_len, board_xy, symmetry, planned);
   SingleConv sc(ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16, kind, 1, bn_scale, bn_bias, activation, ncbias != nullptr,
                 planned ? (ragged != 0) : -1);
+  // emitConv counted convEpilogueWG's choice for the op, as launchConvWG makes it
+  const int kernel = sc.h.epilogueWGLaunches > 0 ? TEST_KERNEL_WG_EPI : TEST_KERNEL_WG;
   HostPlan hp;
   if(planned) {
     hp = sc.setInputPlanned(input, board_xy, symmetry);
@@ -1487,6 +1515,9 @@ void testConv(const char* fn, int ky, int kx, int in_c, int out_c, const float* 
     for(int i = 0; i < n; i++) for(int c = 0; c < out_c; c++) hb[(size_t)i * cp + c] = ncbias[(size_t)i * out_c + c];
     CK(cudaMemcpyAsync(sc.ncbias, hb.data(), hb.size() * sizeof(float), cudaMemcpyHostToDevice, s));
   }
+  const int am = split ? 2 : 1;
+  const size_t rawRowBytes = (size_t)cp * (f32 ? 4 : 2), actRowBytes = (size_t)cp * am * 2;
+  std::vector<uint8_t> streamIn;   // the stream's bytes as uploaded
   if(hasResidual) {
     // given as fp32; an fp16 stream holds it rounded to nearest
     std::vector<float> hf(sc.M * cp, 0.0f);
@@ -1495,20 +1526,21 @@ void testConv(const char* fn, int ky, int kx, int in_c, int out_c, const float* 
       if(row < 0) continue;
       for(int c = 0; c < out_c; c++) hf[row * cp + c] = residual_in[(((size_t)i * nn_y_len + y) * nn_x_len + x) * out_c + c];
     }
-    if(f32) CK(cudaMemcpyAsync(sc.raws[0], hf.data(), hf.size() * sizeof(float), cudaMemcpyHostToDevice, s));
-    else {
-      std::vector<__half> hh(hf.size());
-      for(size_t k = 0; k < hf.size(); k++) hh[k] = __float2half_rn(hf[k]);
-      CK(cudaMemcpyAsync(sc.raws[0], hh.data(), hh.size() * sizeof(__half), cudaMemcpyHostToDevice, s));
-    }
+    streamIn.resize(sc.M * rawRowBytes);
+    if(f32) memcpy(streamIn.data(), hf.data(), streamIn.size());
+    else
+      for(size_t k = 0; k < hf.size(); k++) {
+        const __half v = __float2half_rn(hf[k]);
+        memcpy(&streamIn[2 * k], &v, 2);
+      }
+    CK(cudaMemcpyAsync(sc.raws[0], streamIn.data(), streamIn.size(), cudaMemcpyHostToDevice, s));
   }
-  const int am = split ? 2 : 1;
-  const size_t rawRowBytes = (size_t)cp * (f32 ? 4 : 2), actRowBytes = (size_t)cp * am * 2;
   if(planned) {
     if(!sc.raws.empty()) poisonTail(sc.h, sc.raws[0], rawRowBytes, used, sc.M);
     if(!sc.acts.empty()) poisonTail(sc.h, sc.acts[0], actRowBytes, used, sc.M);
   }
   sc.run();
+  g_lastConvKernel = kernel;
   auto download = [&](void* dst, const void* src, size_t bytes) {
     CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
@@ -1518,8 +1550,18 @@ void testConv(const char* fn, int ky, int kx, int in_c, int out_c, const float* 
     ha.resize(sc.M * cp * am);
     download(ha.data(), sc.acts[0], ha.size() * sizeof(__half));
   }
+  if(hasResidual && !hasRaw) {
+    // kinds 5 and 6 read the stream and must leave it as it was (rows past the plan's end are checked below with the others)
+    std::vector<uint8_t> v(streamIn.size());
+    download(v.data(), sc.raws[0], v.size());
+    if(memcmp(v.data(), streamIn.data(), used * rawRowBytes) != 0) throw std::runtime_error(std::string(fn) + ": the residual stream was written");
+    if(planned) {
+      if(const size_t k = countTouchedTail(v, rawRowBytes, used))
+        throw std::runtime_error(std::string(fn) + ": the residual stream was written past the plan's end (" + std::to_string(k) + " bytes)");
+    }
+  }
   std::vector<float> hr;
-  if(!sc.raws.empty()) {
+  if(hasRaw) {
     hr.resize(sc.M * cp);
     if(f32) download(hr.data(), sc.raws[0], hr.size() * sizeof(float));
     else {
@@ -1537,8 +1579,8 @@ void testConv(const char* fn, int ky, int kx, int in_c, int out_c, const float* 
         throw std::runtime_error(std::string(fn) + ": " + what + " was written past the plan's " + std::to_string(used) + " rows (" +
                                  std::to_string(k) + " bytes)");
     };
-    if(!sc.raws.empty() && f32) tail("the raw output", hr.data(), rawRowBytes);
-    if(!sc.raws.empty() && !f32) {
+    if(hasRaw && f32) tail("the raw output", hr.data(), rawRowBytes);
+    if(hasRaw && !f32) {
       std::vector<__half> hh(sc.M * cp);
       download(hh.data(), sc.raws[0], hh.size() * sizeof(__half));
       tail("the raw output", hh.data(), rawRowBytes);
@@ -1586,14 +1628,21 @@ void testConv(const char* fn, int ky, int kx, int in_c, int out_c, const float* 
 void testBoundary(const char* fn, int inner_c, int trunk_c, int n, int nn_x_len, int nn_y_len, const int32_t* board_xy, const int32_t* symmetry,
                   int ragged, int trunk_fp32, int inner_fp32, uint32_t seed, int64_t* out, int64_t* stats_out) {
   const bool planned = ragged >= 0;
+  g_lastConvKernel = -1;
   if(!out || n < 1 || inner_c < 1 || trunk_c < 1 || nn_x_len < 2 || nn_y_len < 2 || (inner_fp32 && !trunk_fp32))
     throw std::invalid_argument(std::string(fn) + ": bad argument");
   checkBoards(fn, n, nn_x_len, nn_y_len, board_xy, symmetry, planned);
-  BoundaryConv bc(inner_c, trunk_c, n, nn_x_len, nn_y_len, board_xy, trunk_fp32 != 0, inner_fp32 != 0, seed, 1, symmetry, planned ? (ragged != 0) : -1);
+  BoundarySeed g(seed);
+  const ConvDesc post = g.conv(inner_c, trunk_c), pre = g.conv(trunk_c, inner_c);
+  const BNDesc bnTrunk = g.bn(trunk_c), bnInner = g.bn(inner_c);
+  BoundaryConv bc(inner_c, trunk_c, n, nn_x_len, nn_y_len, board_xy, trunk_fp32 != 0, inner_fp32 != 0, post, pre, bnTrunk, bnInner, 1, symmetry,
+                  planned ? (ragged != 0) : -1);
+  bc.seedInputs(g);
   if(planned) bc.hp.copyOut(n, stats_out, nullptr);
   const size_t used = planned ? (size_t)bc.hp.stats[0] : bc.M;
   bc.run(true);
   bc.run(false);
+  g_lastConvKernel = bc.fusedKernel;
   const cudaStream_t s = bc.h.stream;
   auto download = [&](const void* src, size_t bytes) {
     std::vector<uint8_t> v(bytes);
@@ -1626,6 +1675,88 @@ void testBoundary(const char* fn, int inner_c, int trunk_c, int n, int nn_x_len,
     if(planned) {
       out[6 + k] = nan;
       out[9 + k] = (int64_t)(countTouchedTail(f, (size_t)o.cp * o.esize, used) + countTouchedTail(u, (size_t)o.cp * o.esize, used));
+    }
+  }
+}
+
+// kgb_test_conv_boundary_ex: the boundary on the caller's operand, stream, weights and BN constants, one path (fused or the two
+// launches).  Inputs and outputs are NHWC in the coordinates after the symmetry; only board positions are read.
+void testBoundaryEx(int inner_c, int trunk_c, int n, int nn_x_len, int nn_y_len, const float* inner_a, const float* exit_w, const float* trunk_s,
+                    const float* trunk_scale, const float* trunk_bias, const float* entry_w, const float* inner_scale, const float* inner_bias,
+                    const int32_t* board_xy, const int32_t* symmetry, int ragged, int trunk_fp32, int inner_fp32, int fused, float* trunk_s_out,
+                    float* inner_s_out, float* inner_a_out, int64_t* stats_out) {
+  const char* fn = "kgb_test_conv_boundary_ex";
+  const bool planned = ragged >= 0;
+  g_lastConvKernel = -1;
+  if(n < 1 || inner_c < 1 || trunk_c < 1 || nn_x_len < 2 || nn_y_len < 2 || (inner_fp32 && !trunk_fp32) || (symmetry && !planned) ||
+     !inner_a || !exit_w || !trunk_s || !trunk_scale || !trunk_bias || !entry_w || !inner_scale || !inner_bias || !trunk_s_out ||
+     !inner_s_out || !inner_a_out)
+    throw std::invalid_argument(std::string(fn) + ": bad argument");
+  checkBoards(fn, n, nn_x_len, nn_y_len, board_xy, symmetry, planned);
+  auto conv = [](int cin, int cout, const float* w) {
+    ConvDesc c;
+    c.ky = c.kx = 1; c.cin = cin; c.cout = cout;
+    c.w.assign(w, w + (size_t)cin * cout);
+    return c;
+  };
+  auto bn = [](int c, const float* scale, const float* bias) {
+    BNDesc b;
+    b.c = c; b.scale.assign(scale, scale + c); b.bias.assign(bias, bias + c);
+    return b;
+  };
+  BoundaryConv bc(inner_c, trunk_c, n, nn_x_len, nn_y_len, board_xy, trunk_fp32 != 0, inner_fp32 != 0, conv(inner_c, trunk_c, exit_w),
+                  conv(trunk_c, inner_c, entry_w), bn(trunk_c, trunk_scale, trunk_bias), bn(inner_c, inner_scale, inner_bias), 1, symmetry,
+                  planned ? (ragged != 0) : -1);
+  if(planned) bc.hp.copyOut(n, stats_out, nullptr);
+  const size_t used = planned ? (size_t)bc.hp.stats[0] : bc.M;
+  const Layout& L = bc.h.L;
+  auto rowOf = [&](int i, int y, int x) -> long {
+    const long r = planned ? bc.hp.row(L, i, y, x) : (long)((size_t)i * L.P + (size_t)(y + L.pad) * L.Wp + x);
+    return r >= 0 && bc.mask[r] != 0.0f ? r : -1;
+  };
+  std::vector<__half> hA(bc.M * bc.innerCp, __float2half(0.0f));
+  std::vector<float> hS(bc.M * bc.trunkCp, 0.0f);
+  for(int i = 0; i < n; i++) for(int y = 0; y < nn_y_len; y++) for(int x = 0; x < nn_x_len; x++) {
+    const long r = rowOf(i, y, x);
+    if(r < 0) continue;
+    const size_t o = ((size_t)i * nn_y_len + y) * nn_x_len + x;
+    for(int c = 0; c < inner_c; c++) hA[r * bc.innerCp + c] = __float2half_rn(inner_a[o * inner_c + c]);
+    for(int c = 0; c < trunk_c; c++) hS[r * bc.trunkCp + c] = trunk_s[o * trunk_c + c];
+  }
+  bc.setInputs(hA, hS);
+  bc.run(fused != 0);
+  g_lastConvKernel = fused ? bc.fusedKernel : bc.h.epilogueWGLaunches > 0 ? TEST_KERNEL_WG_EPI : TEST_KERNEL_WG;
+  // the set the path ran on: its outputs, with exact zeros in every row the mask zeroes and every padded channel, and in plan mode
+  // nothing written at or past the plan's end
+  const BoundaryConv::Set& st = bc.sets[fused ? 0 : 1];
+  struct Out { const void* p; int cp, c, esize; float* dst; const char* what; };
+  const Out outs[3] = {{st.trunkS, bc.trunkCp, trunk_c, trunk_fp32 ? 4 : 2, trunk_s_out, "the trunk stream"},
+                       {st.innerS, bc.innerCp, inner_c, inner_fp32 ? 4 : 2, inner_s_out, "the inner stream"},
+                       {st.innerA, bc.innerCp, inner_c, 2, inner_a_out, "the inner operand"}};
+  for(const Out& o : outs) {
+    std::vector<uint8_t> v(bc.M * o.cp * o.esize);
+    CK(cudaMemcpyAsync(v.data(), o.p, v.size(), cudaMemcpyDeviceToHost, bc.h.stream));
+    CK(cudaStreamSynchronize(bc.h.stream));
+    auto value = [&](size_t e) {
+      float f;
+      if(o.esize == 4) memcpy(&f, &v[e * 4], 4);
+      else { __half hv; memcpy(&hv, &v[e * 2], 2); f = __half2float(hv); }
+      return f;
+    };
+    for(size_t r = 0; r < used; r++) {
+      const bool off = bc.mask[r] == 0.0f;
+      for(int c = off ? 0 : o.c; c < o.cp; c++)
+        if(value(r * o.cp + c) != 0.0f)
+          throw std::runtime_error(std::string(fn) + ": " + o.what + " is not zero at row " + std::to_string(r) + (off ? " (masked)" : "") +
+                                   ", channel " + std::to_string(c));
+    }
+    if(planned)
+      if(const size_t k = countTouchedTail(v, (size_t)o.cp * o.esize, used))
+        throw std::runtime_error(std::string(fn) + ": " + o.what + " was written past the plan's end (" + std::to_string(k) + " bytes)");
+    for(int i = 0; i < n; i++) for(int y = 0; y < nn_y_len; y++) for(int x = 0; x < nn_x_len; x++) {
+      const long r = rowOf(i, y, x);
+      const size_t q = ((size_t)i * nn_y_len + y) * nn_x_len + x;
+      for(int c = 0; c < o.c; c++) o.dst[q * o.c + c] = r < 0 ? 0.0f : value(r * o.cp + c);
     }
   }
 }
@@ -1897,6 +2028,25 @@ KGB_API int kgb_test_conv_boundary_plan(int inner_c, int trunk_c, int n, int nn_
   });
 }
 
+KGB_API int kgb_test_conv_boundary_ex(int inner_c, int trunk_c, int n, int nn_x_len, int nn_y_len, const float* inner_a, const float* exit_w,
+                                      const float* trunk_s, const float* trunk_scale, const float* trunk_bias, const float* entry_w,
+                                      const float* inner_scale, const float* inner_bias, const int32_t* board_xy, const int32_t* symmetry,
+                                      int ragged, int trunk_fp32, int inner_fp32, int fused, float* trunk_s_out, float* inner_s_out,
+                                      float* inner_a_out, int64_t* layout_stats) {
+  return guarded([&] {
+    testBoundaryEx(inner_c, trunk_c, n, nn_x_len, nn_y_len, inner_a, exit_w, trunk_s, trunk_scale, trunk_bias, entry_w, inner_scale, inner_bias,
+                   board_xy, symmetry, ragged, trunk_fp32, inner_fp32, fused, trunk_s_out, inner_s_out, inner_a_out, layout_stats);
+  });
+}
+
+KGB_API int kgb_test_last_conv_kernel(int* out) {
+  return guarded([&] {
+    if(!out) throw std::invalid_argument("kgb_test_last_conv_kernel: bad argument");
+    if(g_lastConvKernel < 0) throw std::runtime_error("kgb_test_last_conv_kernel: no convolution test hook has launched since the last failure");
+    *out = g_lastConvKernel;
+  });
+}
+
 KGB_API int kgb_test_head_kernel(int which, int n, int nn_x_len, int nn_y_len, int pad, const int32_t* board_xy, const int32_t* symmetry,
                                  int ragged, const int32_t* iparams, int num_iparams, const float* const* inputs, int num_inputs,
                                  float* const* outputs, int num_outputs, int64_t* layout_stats, int32_t* plan_out) {
@@ -1910,7 +2060,11 @@ KGB_API int kgb_bench_conv_boundary(int inner_c, int trunk_c, int n, int nn_x_le
                                     int rotate, int warmup, int iters, float* ms_per_boundary) {
   return guarded([&] {
     if(!ms_per_boundary || n < 1 || iters < 1 || (inner_fp32 && !trunk_fp32)) throw std::invalid_argument("kgb_bench_conv_boundary: bad argument");
-    BoundaryConv bc(inner_c, trunk_c, n, nn_x_len, nn_y_len, nullptr, trunk_fp32 != 0, inner_fp32 != 0, 1, rotate);
+    BoundarySeed g(1);
+    const ConvDesc post = g.conv(inner_c, trunk_c), pre = g.conv(trunk_c, inner_c);
+    const BNDesc bnTrunk = g.bn(trunk_c), bnInner = g.bn(inner_c);
+    BoundaryConv bc(inner_c, trunk_c, n, nn_x_len, nn_y_len, nullptr, trunk_fp32 != 0, inner_fp32 != 0, post, pre, bnTrunk, bnInner, rotate);
+    bc.seedInputs(g);
     for(int i = 0; i < warmup; i++) bc.run(fused != 0);
     cudaEvent_t e0, e1;
     CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));

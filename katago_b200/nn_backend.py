@@ -82,7 +82,7 @@ ABI_SYMBOLS = [
     "kgb_handle_create", "kgb_handle_free", "kgb_handle_is_fp16", "kgb_forward", "kgb_forward_device", "kgb_test_forward_serial", "kgb_conv_chain_error", "kgb_forward_meta", "kgb_forward_device_meta", "kgb_handle_sync",
     "kgb_handle_stream", "kgb_handle_launches_per_forward", "kgb_handle_chained_launches_per_forward", "kgb_handle_epilogue_wg_launches_per_forward", "kgb_handle_pair_epilogue_wg_launches_per_forward", "kgb_handle_get_layout_stats", "kgb_test_conv", "kgb_bench_conv_ex", "kgb_test_conv_epilogue",
     "kgb_test_conv_ex", "kgb_test_conv_boundary", "kgb_bench_conv_boundary", "kgb_test_conv_plan", "kgb_test_conv_boundary_plan",
-    "kgb_test_head_kernel",
+    "kgb_test_conv_boundary_ex", "kgb_test_last_conv_kernel", "kgb_test_head_kernel",
     "kgb_selfplay_create", "kgb_selfplay_free", "kgb_selfplay_run", "kgb_selfplay_get_stats", "kgb_selfplay_get_game",
     "kgb_selfplay_get_root_children", "kgb_selfplay_launches_per_step", "kgb_selfplay_play_moves", "kgb_selfplay_time_tree_kernels", "kgb_zobrist_tables", "kgb_selfplay_get_nn_row", "kgb_selfplay_get_root_row", "kgb_test_board_replay", "kgb_selfplay_get_leaf_path", "kgb_expected_white_score_value", "kgb_value_weight_cdf_table", "kgb_rand_uint32_stream", "kgb_test_root_policy_noise", "kgb_test_history_replay", "kgb_test_repetition_bound", "kgb_selfplay_get_play_selection_values", "kgb_selfplay_random_openings", "kgb_selfplay_set_search_rand", "kgb_selfplay_get_root_value_stats", "kgb_test_choose_index_with_temperature",
     "kgb_handle_weights_bytes", "kgb_handle_stage_weights", "kgb_handle_commit_weights", "kgb_handle_wait_staged", "kgb_nccl_unique_id", "kgb_handle_comm_init",
@@ -166,6 +166,8 @@ def load_library():
     lib.kgb_test_conv_ex.argtypes = [I, I, I, I, P, I, I, I, I, I, P, P, P, P, P, P, I, P, P, P]
     lib.kgb_test_conv_plan.argtypes = [I, I, I, I, P, I, I, I, I, I, P, P, P, I, P, P, P, P, I, P, P, P, P, P]
     lib.kgb_test_conv_boundary_plan.argtypes = [I, I, I, I, I, P, P, I, I, I, C.c_uint32, P, P]
+    lib.kgb_test_conv_boundary_ex.argtypes = [I, I, I, I, I, P, P, P, P, P, P, P, P, P, P, I, I, I, I, P, P, P, P]
+    lib.kgb_test_last_conv_kernel.argtypes = [C.POINTER(I)]
     lib.kgb_test_head_kernel.argtypes = [I, I, I, I, I, P, P, I, P, I, P, I, P, I, P, P]
     lib.kgb_selfplay_create.argtypes = [P, C.POINTER(SelfplayConfig), C.POINTER(P)]
     lib.kgb_selfplay_free.argtypes = [P]
@@ -456,15 +458,16 @@ def test_conv_epilogue(ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_
 
 def test_conv_ex(ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16, kind, x, board_xy=None, ncbias=None, residual=None,
                  bn_scale=None, bn_bias=None, activation=2):
-    """One convolution launch with every epilogue input (include/kgb200.h kgb_test_conv_ex): kinds 0-4 as in test_conv_epilogue,
-    board_xy [n][2] = (X_i, Y_i) boards in the top-left of the frame (None = the whole frame), ncbias [n][out_c], residual in fp32,
-    activation 0-3.  Returns (raw or None, act hi or None, act lo or None), NHWC; lo only in split mode."""
-    if kind not in (0, 1, 2, 3, 4):
-        raise ValueError(f"test_conv_ex: epilogue kind {kind} is not 0-4")
+    """One convolution launch with every epilogue input (include/kgb200.h kgb_test_conv_ex): kinds 0-4 as in test_conv_epilogue, 5 and
+    6 = kinds 2 and 4 without the raw output; board_xy [n][2] = (X_i, Y_i) boards in the top-left of the frame (None = the whole frame),
+    ncbias [n][out_c], residual in fp32, activation 0-3.  Returns (raw or None, act hi or None, act lo or None), NHWC; lo only in split
+    mode."""
+    if kind not in (0, 1, 2, 3, 4, 5, 6):
+        raise ValueError(f"test_conv_ex: epilogue kind {kind} is not 0-6")
     lib = load_library()
     shape = (n, nn_y_len, nn_x_len, out_c)
     w, xx = _f32(weights), _f32(x)
-    raw = np.zeros(shape, np.float32) if kind != 1 else None
+    raw = np.zeros(shape, np.float32) if kind in (0, 2, 3, 4) else None
     hi = np.zeros(shape, np.float32) if kind != 0 else None
     lo = np.zeros(shape, np.float32) if kind != 0 and not use_fp16 else None
     bxy = np.ascontiguousarray(board_xy, dtype=np.int32) if board_xy is not None else None
@@ -483,7 +486,7 @@ def test_conv_plan(ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16
     lib = load_library()
     shape = (n, nn_y_len, nn_x_len, out_c)
     w, xx = _f32(weights), _f32(x)
-    raw = np.zeros(shape, np.float32) if kind != 1 else None
+    raw = np.zeros(shape, np.float32) if kind in (0, 2, 3, 4) else None
     hi = np.zeros(shape, np.float32) if kind != 0 else None
     lo = np.zeros(shape, np.float32) if kind != 0 and not use_fp16 else None
     bxy = np.ascontiguousarray(board_xy, dtype=np.int32)
@@ -496,6 +499,39 @@ def test_conv_plan(ky, kx, in_c, out_c, weights, n, nn_x_len, nn_y_len, use_fp16
                                   bxy.ctypes.data, sym.ctypes.data, int(bool(ragged)), *[ptr(a) for a in opt], activation, ptr(raw), ptr(hi),
                                   ptr(lo), stats.ctypes.data, plan.ctypes.data))
     return raw, hi, lo, dict(rows=int(stats[0]), m_tiles=int(stats[1]), segments=int(stats[2])), plan
+
+
+def test_conv_boundary_ex(inner_c, trunk_c, n, nn_x_len, nn_y_len, inner_a, exit_w, trunk_s, trunk_scale, trunk_bias, entry_w, inner_scale,
+                          inner_bias, board_xy=None, symmetry=None, ragged=None, trunk_fp32=False, inner_fp32=False, fused=True):
+    """The fused block boundary on caller data (include/kgb200.h kgb_test_conv_boundary_ex): inner_a [n][y][x][inner_c], exit_w
+    [inner_c][trunk_c], trunk_s [n][y][x][trunk_c], entry_w [trunk_c][inner_c], BN constants per channel.  ragged None is the frame
+    layout, else plan mode with board_xy moved by symmetry.  Returns (trunk stream, inner stream, inner operand), NHWC float32, and
+    the layout stats dict in plan mode (else None)."""
+    lib = load_library()
+    arrs = [_f32(a) for a in (inner_a, exit_w, trunk_s, trunk_scale, trunk_bias, entry_w, inner_scale, inner_bias)]
+    s_out = np.zeros((n, nn_y_len, nn_x_len, trunk_c), np.float32)
+    i_out = np.zeros((n, nn_y_len, nn_x_len, inner_c), np.float32)
+    a_out = np.zeros((n, nn_y_len, nn_x_len, inner_c), np.float32)
+    bxy = np.ascontiguousarray(board_xy, dtype=np.int32) if board_xy is not None else None
+    sym = np.ascontiguousarray(symmetry, dtype=np.int32) if symmetry is not None else None
+    stats = np.zeros(3, np.int64)
+    ptr = lambda a: a.ctypes.data if a is not None else None
+    _check(lib.kgb_test_conv_boundary_ex(inner_c, trunk_c, n, nn_x_len, nn_y_len, *[a.ctypes.data for a in arrs], ptr(bxy), ptr(sym),
+                                         -1 if ragged is None else int(bool(ragged)), int(bool(trunk_fp32)), int(bool(inner_fp32)),
+                                         int(bool(fused)), s_out.ctypes.data, i_out.ctypes.data, a_out.ctypes.data, stats.ctypes.data))
+    layout = None if ragged is None else dict(rows=int(stats[0]), m_tiles=int(stats[1]), segments=int(stats[2]))
+    return s_out, i_out, a_out, layout
+
+
+CONV_KERNELS = ("kgb_conv_wg_kernel", "kgb_conv_wg_epi_kernel", "kgb_conv_pair_kernel", "kgb_conv_pair_epi_kernel")
+
+
+def test_last_conv_kernel():
+    """The kernel the last convolution test hook launched (include/kgb200.h kgb_test_last_conv_kernel), by name (CONV_KERNELS)."""
+    lib = load_library()
+    k = C.c_int(-1)
+    _check(lib.kgb_test_last_conv_kernel(C.byref(k)))
+    return CONV_KERNELS[k.value]
 
 
 HEAD_KERNELS = {"pack": 0, "gpool": 1, "bias_act": 2, "matmul": 3, "policy": 4, "ownership": 5, "finalize": 6}

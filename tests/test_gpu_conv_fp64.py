@@ -45,11 +45,16 @@ Bounds (every output; a row or channel the mask zeroes must be exactly zero):
 Every check allows the rounding to the stored dtype in full and reports the rest of the error over the computation's bound: a
 correctly rounded output may sit anywhere up to half an ulp from the exact value, so that rounding has no margin to give.
 
+Epilogue kinds (kgb_test_conv_ex): 0 raw fp32 only, 1 act only, 2 residual + raw stream + act, 3 raw stream + act, 4 kind 2 with an
+fp32 stream in fp16 mode, 5 and 6 kinds 2 and 4 without the raw output (residual in, act out: the last block of a level).  Each case
+names the kernel the launcher must take (kgb_conv_wg_kernel or kgb_conv_wg_epi_kernel) and the GPU test asserts it, so that a change
+to a stage count or a flag list cannot move a case to the other kernel unnoticed.
+
 test_bounds_separate_correct_from_broken (no GPU) rehearses every case of the GPU matrix.  The emulation of the correct kernel
 (accumulate() followed by the epilogue in fp32) must stay within a quarter of every bound.  Each emulated mutant must exceed a bound
 at least 8x, unless the case cannot show that mutant (named in _exempt).  The mutants are: a dropped split term, a dropped lo half,
-an fp32 residual rounded through fp16, the neighbouring image's ncbias, and an off-board position left unmasked.  Cases of more than
-24 images are rehearsed on their first 24.
+an fp32 residual rounded through fp16, the residual read from the neighbouring 32-column slice, the neighbouring image's ncbias, and
+an off-board position left unmasked.  Cases of more than 24 images are rehearsed on their first 24.
 """
 import numpy as np
 import pytest
@@ -62,24 +67,29 @@ Z_ROUND = 2.0 ** -22   # the fma's rounding of z is at most 2^-24 |z|: 4x, so th
 REHEARSAL_MAX_N = 24
 
 
-def _case(cid, ky, cin, cout, n, X, Y, kind, fp16, act, boards=None, ncbias=False, bias=1.0, check_images=None):
+WG, WG_EPI = "kgb_conv_wg_kernel", "kgb_conv_wg_epi_kernel"
+
+
+def _case(cid, ky, cin, cout, n, X, Y, kind, fp16, act, boards=None, ncbias=False, bias=1.0, check_images=None, kernel=WG, env=None):
+    """kernel: the kernel the launcher must choose (split mode and 1x1 layers always take kgb_conv_wg_kernel); env: variables set
+    for the launch."""
     return pytest.param(dict(ky=ky, cin=cin, cout=cout, n=n, X=X, Y=Y, kind=kind, fp16=fp16, act=act, boards=boards, ncbias=ncbias,
-                             bias=bias, check_images=check_images), id=cid)
+                             bias=bias, check_images=check_images, kernel=kernel, env=env or {}), id=cid)
 
 
 MIXED = ((19, 19), (9, 9), (13, 13), (7, 11))   # repeated over the batch
 CASES = [
     # the b18 3x3 192 -> 192 in every epilogue kind, both modes
     _case("3x3-192-k1-split-mish", 3, 192, 192, 6, 19, 19, 1, False, 2, bias=12.0),
-    _case("3x3-192-k1-fp16-mish-mixed", 3, 192, 192, 8, 19, 19, 1, True, 2, boards=MIXED, bias=12.0),
+    _case("3x3-192-k1-fp16-mish-mixed", 3, 192, 192, 8, 19, 19, 1, True, 2, boards=MIXED, bias=12.0, kernel=WG_EPI),
     _case("3x3-192-k2-split-identity", 3, 192, 192, 6, 19, 19, 2, False, 0),
     _case("3x3-192-k2-fp16-relu-mixed", 3, 192, 192, 8, 19, 19, 2, True, 1, boards=MIXED),
     _case("3x3-192-k3-split-silu", 3, 192, 192, 6, 19, 19, 3, False, 3, bias=12.0),
-    _case("3x3-192-k3-fp16-mish-13x7", 3, 192, 192, 10, 19, 19, 3, True, 2, boards=((13, 7),)),
+    _case("3x3-192-k3-fp16-mish-13x7", 3, 192, 192, 10, 19, 19, 3, True, 2, boards=((13, 7),), kernel=WG_EPI),
     _case("3x3-192-k4-split-silu", 3, 192, 192, 6, 19, 19, 4, False, 3, bias=12.0),
     _case("3x3-192-k4-fp16-silu", 3, 192, 192, 6, 19, 19, 4, True, 3, bias=12.0),
     _case("3x3-192-k0-split-mixed", 3, 192, 192, 8, 19, 19, 0, False, 0, boards=MIXED),
-    _case("3x3-192-k0-fp16-9x9", 3, 192, 192, 8, 9, 9, 0, True, 0, boards=((7, 5),)),
+    _case("3x3-192-k0-fp16-9x9", 3, 192, 192, 8, 9, 9, 0, True, 0, boards=((7, 5),), kernel=WG_EPI),
     # every tile width: cout 32, 64, 128, 256 and two n-tiles of 160, 224 and 192
     _case("1x1-cout32-k2-split-mish-13x7", 1, 192, 32, 20, 13, 7, 2, False, 2, bias=12.0),
     _case("3x3-cout64-k1-fp16-silu-9x9", 3, 64, 64, 24, 9, 9, 1, True, 3, boards=((9, 9), (5, 7)), bias=12.0),
@@ -91,7 +101,7 @@ CASES = [
     _case("1x1-cout384-k3-split-identity", 1, 192, 384, 6, 19, 19, 3, False, 0),
     # the initial conv: 5x5, 22 input channels, per-image global bias, kind 3, as the evaluator emits it
     _case("5x5-initial-k3-split-mish-mixed", 5, 22, 192, 8, 19, 19, 3, False, 2, boards=MIXED, ncbias=True, bias=12.0),
-    _case("5x5-initial-k3-fp16-mish", 5, 22, 192, 8, 19, 19, 3, True, 2, ncbias=True, bias=12.0),
+    _case("5x5-initial-k3-fp16-mish", 5, 22, 192, 8, 19, 19, 3, True, 2, ncbias=True, bias=12.0, kernel=WG_EPI),
     _case("5x5-initial-k3-split-relu-9x9", 5, 22, 96, 16, 9, 9, 3, False, 1, ncbias=True),
     # frames with fewer than 128 rows in all: one partial tile
     _case("2x2-frame-k2-split-mish", 3, 64, 64, 8, 2, 2, 2, False, 2, bias=12.0),
@@ -113,7 +123,7 @@ CASES = [
     _case("b28-initial3x3-512-k3-split-mish-mixed", 3, 22, 512, 16, 19, 19, 3, False, 2, boards=MIXED, ncbias=True, bias=12.0),
     _case("b28-initial3x3-512-k3-fp16-mish-mixed", 3, 22, 512, 16, 19, 19, 3, True, 2, boards=MIXED, ncbias=True, bias=12.0),
     _case("b28-gpool3x3-256-320-k0-split-mixed", 3, 256, 320, 24, 19, 19, 0, False, 0, boards=MIXED),
-    _case("b28-gpool3x3-256-320-k0-fp16-mixed", 3, 256, 320, 24, 19, 19, 0, True, 0, boards=MIXED),
+    _case("b28-gpool3x3-256-320-k0-fp16-mixed", 3, 256, 320, 24, 19, 19, 0, True, 0, boards=MIXED, kernel=WG_EPI),
     # b28's batch: 1024 images of 400 rows are 3200 whole 128-row tiles, about 24 per CTA; at 1021 image 1020 holds the partial last tile.
     # Checked on the first images, both sides of 511 / 512 and the last ones (the padding rows between images are zero, so they are
     # independent)
@@ -121,6 +131,29 @@ CASES = [
           check_images=(0, 1, 510, 511, 512, 513, 1022, 1023)),
     _case("b28-3x3-256-k2-split-silu-b1021", 3, 256, 256, 1021, 19, 19, 2, False, 3, bias=12.0,
           check_images=(0, 1, 510, 511, 512, 513, 1019, 1020)),
+    # kgb_conv_wg_epi_kernel (fp16 mode, mish, 3x3 and 5x5 tiles of 128, 160 and 192 columns) where its CTAs take more than one tile:
+    # the accumulator tile's t_full / t_empty phases, the one residual slot's reuse and the operand ring carried across tiles.  A
+    # 19x19 image is 400 rows, 3.125 tiles; the H100 has 132 SMs.  b18's commonest 3x3 epilogue at 800 tiles, all of them checked,
+    # and the same case on kgb_conv_wg_kernel as the float64 anchor of the bit-identity tests between the two
+    _case("3x3-192-k2-fp16-mish-b256", 3, 192, 192, 256, 19, 19, 2, True, 2, bias=12.0, kernel=WG_EPI),
+    _case("3x3-192-k2-fp16-mish-b256-no-epilogue-wg", 3, 192, 192, 256, 19, 19, 2, True, 2, bias=12.0, env={"KGB_EPILOGUE_WG": "0"}),
+    _case("3x3-192-k2-fp16-mish-b1021", 3, 192, 192, 1021, 19, 19, 2, True, 2, bias=12.0, kernel=WG_EPI,
+          check_images=(0, 1, 330, 331, 660, 661, 1019, 1020)),
+    _case("3x3-192-k2-fp16-mish-b43-mixed", 3, 192, 192, 43, 19, 19, 2, True, 2, boards=MIXED, bias=12.0, kernel=WG_EPI),
+    _case("3x3-192-k0-fp16-b43-mixed", 3, 192, 192, 43, 19, 19, 0, True, 0, boards=MIXED, kernel=WG_EPI),
+    # cout is padded to 64 channels: 96 runs at 128 columns with 32 padded ones, and 160 columns are two n-tiles of 320
+    _case("3x3-96-k2-fp16-mish-b48", 3, 96, 96, 48, 19, 19, 2, True, 2, bias=12.0, kernel=WG_EPI),
+    _case("3x3-128-k1-fp16-mish-b48-mixed", 3, 128, 128, 48, 19, 19, 1, True, 2, boards=MIXED, bias=12.0, kernel=WG_EPI),
+    _case("3x3-160-320-k3-fp16-mish-b48-mixed", 3, 160, 320, 48, 19, 19, 3, True, 2, boards=MIXED, bias=12.0, kernel=WG_EPI),
+    _case("5x5-initial-22-96-k3-fp16-mish-b48-mixed", 5, 22, 96, 48, 19, 19, 3, True, 2, boards=MIXED, ncbias=True, bias=12.0,
+          kernel=WG_EPI),
+    # kinds 5 and 6: the residual in, no raw output, as the last block of every level runs (b18: the second conv of each nested
+    # block's last inner block, and the trunk's last exit 1x1).  fp16 mode on the epilogue-warpgroup kernel; split mode, the fp32
+    # stream and the 1x1 on kgb_conv_wg_kernel's EPI_RES | EPI_MISH copies
+    _case("3x3-192-k5-fp16-mish-b48-mixed", 3, 192, 192, 48, 19, 19, 5, True, 2, boards=MIXED, bias=12.0, kernel=WG_EPI),
+    _case("3x3-192-k5-split-mish", 3, 192, 192, 6, 19, 19, 5, False, 2, bias=12.0),
+    _case("3x3-192-k6-fp16-mish-mixed", 3, 192, 192, 8, 19, 19, 6, True, 2, boards=MIXED, bias=12.0),
+    _case("exit1x1-192-384-k5-fp16-mish-b24", 1, 192, 384, 24, 19, 19, 5, True, 2, bias=12.0),
 ]
 
 
@@ -139,7 +172,7 @@ def make_data(c, n=None):
     ky, cin, cout, X, Y = c["ky"], c["cin"], c["cout"], c["X"], c["Y"]
     d = dict(w=(rng.standard_normal((ky, ky, cin, cout)) / np.sqrt(ky * ky * cin)).astype(F32),
              x=rng.standard_normal((c["n"], Y, X, cin)).astype(F32)[:n])
-    d["res"] = (4.0 * rng.standard_normal((c["n"], Y, X, cout))).astype(F32)[:n] if c["kind"] in (2, 4) else None
+    d["res"] = (4.0 * rng.standard_normal((c["n"], Y, X, cout))).astype(F32)[:n] if has_residual(c) else None
     d["ncb"] = rng.standard_normal((c["n"], cout)).astype(F32)[:n] if c["ncbias"] else None
     # BN: scales of both signs; biases in three widths so that some channels sit near zero and others deep in the activation's tails
     d["sc"] = (rng.uniform(0.25, 1.5, cout) * rng.choice([-1.0, 1.0], cout, p=[0.25, 0.75])).astype(F32)
@@ -197,11 +230,20 @@ def operands(c, d):
     return split_halves(d["x"]) + split_halves(d["w"])
 
 
+def has_residual(c):
+    return c["kind"] in (2, 4, 5, 6)
+
+
+def has_raw(c):
+    """Kinds 5 and 6 read the residual and write no raw output (kinds 2 and 4 without it)."""
+    return c["kind"] in (0, 2, 3, 4)
+
+
 def stream_residual(c, d):
-    """The residual as the stream holds it: fp32 for kind 4 and in split mode, fp16 otherwise."""
+    """The residual as the stream holds it: fp32 for kinds 4 and 6 and in split mode, fp16 otherwise."""
     if d["res"] is None:
         return 0.0
-    return d["res"].astype(F64) if c["kind"] == 4 or not c["fp16"] else _h(d["res"])
+    return d["res"].astype(F64) if stream_fp32(c) else _h(d["res"])
 
 
 def reference(c, d):
@@ -243,8 +285,14 @@ def accumulator_updates(c):
     return -(-c["cin"] // 16) * c["ky"] * c["ky"] * (1 if c["fp16"] else 3)
 
 
+def stream_fp32(c):
+    """Whether the raw output or the stream is fp32: kind 0's raw output, the fp32 stream of kinds 4 and 6, split mode; a case's "raw32"
+    overrides it (an fp32 stream in fp16 mode, as KGB_STREAM_FP32=all runs the inner streams)."""
+    return c.get("raw32", c["kind"] in (0, 4, 6) or not c["fp16"])
+
+
 def raw_fp32(c):
-    return c["kind"] in (0, 4) or not c["fp16"]
+    return has_raw(c) and stream_fp32(c)
 
 
 def formula_error(z, act):
@@ -265,15 +313,20 @@ def bounds(c, d, ref):
     """(raw bound or None, act bound or None), each a pair (computation, storage): the first bounds the error of the value the
     kernel computes, the second the rounding to the stored dtype.  Both are zero where the mask is zero."""
     m = ref["mask"]
-    e_v = C_ACC * accumulator_updates(c) * 2.0 ** -23 * ref["sigma"] + 2.0 ** -22 * ref["sum_abs"]
+    # An operand computed by an earlier layer inside the same kernel (the fused boundary's entry) brings that layer's error in, carried
+    # through the weights: e_operand from its computation bound, joining this layer's computation term, and s_operand from its
+    # storage rounding, which has no margin to give and joins the storage term in full.  Both are zero for an operand given exactly.
+    s_op = ref.get("s_operand", 0.0)
+    e_v = C_ACC * accumulator_updates(c) * 2.0 ** -23 * ref["sigma"] + 2.0 ** -22 * ref["sum_abs"] + ref.get("e_operand", 0.0)
     V = np.abs(ref["V"])
-    store = 0.5 * (ulp32(V * (1 + 2.0 ** -20) + e_v) if raw_fp32(c) else ulp16(V * (1 + 2.0 ** -9) + e_v))
-    raw_b = (m * e_v, m * store) if c["kind"] != 1 else None
+    store = s_op + 0.5 * (ulp32(V * (1 + 2.0 ** -20) + e_v + s_op) if raw_fp32(c) else ulp16(V * (1 + 2.0 ** -9) + e_v + s_op))
+    raw_b = (m * e_v, m * store) if has_raw(c) else None
     act_b = None
     if c["kind"] != 0:
         z, a = ref["z"], np.abs(act64(ref["z"], c["act"]))
         e_a = ACT_LIPSCHITZ[c["act"]] * (np.abs(d["sc"]).astype(F64) * e_v + Z_ROUND * np.abs(z)) + formula_error(z, c["act"])
-        act_b = (m * e_a, m * store_error((a + e_a) * (1 + 2.0 ** -9), c["fp16"]))
+        s_a = ACT_LIPSCHITZ[c["act"]] * np.abs(d["sc"]).astype(F64) * s_op
+        act_b = (m * e_a, m * (s_a + store_error((a + e_a + s_a) * (1 + 2.0 ** -9), c["fp16"])))
     return raw_b, act_b
 
 
@@ -370,6 +423,8 @@ def emulate(c, d, ref, acc, drop=None):
         R = stream_residual(c, d)
         if drop == "residual-via-fp16":
             R = _h(d["res"])
+        if drop == "residual-neighbour-slice":
+            R = neighbour_slice(R)
         v = (v + R.astype(F32)).astype(F32)
     m = d["mask"][..., None].copy()
     if drop == "unmasked":
@@ -379,7 +434,7 @@ def emulate(c, d, ref, acc, drop=None):
         else:
             m[i, by, 0] = 1.0
     raw = None
-    if c["kind"] != 1:
+    if has_raw(c):
         raw = (v * m.astype(F32)).astype(F32)
         if not raw_fp32(c):
             raw = raw.astype(F16).astype(F32)
@@ -395,7 +450,16 @@ def emulate(c, d, ref, acc, drop=None):
     return raw, hi, lo
 
 
-MUTANTS = ("al*wh", "ah*wl", "act-lo", "residual-via-fp16", "ncbias-neighbour", "unmasked")
+def neighbour_slice(a):
+    """a's channels each read from the neighbouring 32-column slice (slices 2k and 2k + 1 swapped; the padded channels up to the next
+    64 are zero)."""
+    c = a.shape[-1]
+    pad = np.zeros(a.shape[:-1] + (-(-c // 64) * 64,), a.dtype)
+    pad[..., :c] = a
+    return pad[..., np.arange(c) ^ 32]
+
+
+MUTANTS = ("al*wh", "ah*wl", "act-lo", "residual-via-fp16", "residual-neighbour-slice", "ncbias-neighbour", "unmasked")
 
 
 def _exempt(c, mutant):
@@ -405,8 +469,10 @@ def _exempt(c, mutant):
         return "fp16 mode has no lo operands"
     if mutant == "act-lo" and (not split or c["kind"] == 0):
         return "no activated operand in split mode"
-    if mutant == "residual-via-fp16" and not (c["kind"] == 4 or (c["kind"] == 2 and split)):
+    if mutant == "residual-via-fp16" and not (has_residual(c) and stream_fp32(c)):
         return "no fp32 residual stream"
+    if mutant == "residual-neighbour-slice" and not has_residual(c):
+        return "no residual"
     if mutant == "ncbias-neighbour" and not c["ncbias"]:
         return "no ncbias"
     if mutant == "unmasked" and not any(b[0] < c["X"] or b[1] < c["Y"] for b in (c["boards"] or ())):
@@ -421,7 +487,7 @@ def test_bounds_separate_correct_from_broken(c):
     ref = reference(c, d)
     acc = accumulate(c, d)
     r = check(c, d, ref, *emulate(c, d, ref, acc))
-    print("worst error / bound:", {k: f"{v:.3g}" for k, v in r.items()})
+    print("correct emulation, worst error / bound:", {k: f"{v:.3g}" for k, v in r.items()})
     assert r and max(r.values()) <= 0.25, f"the emulated correct kernel uses more than a quarter of a bound: {r}"
     tried = 0
     for mutant in MUTANTS:
@@ -429,19 +495,23 @@ def test_bounds_separate_correct_from_broken(c):
             continue
         tried += 1
         rm = check(c, d, ref, *emulate(c, d, ref, acc, drop=mutant))
+        print(f"mutant {mutant}: worst {max(rm.values()):.3g}x")
         assert max(rm.values()) >= 8.0, f"mutant {mutant} stays within 8x of the bounds: {rm}"
     assert tried > 0, "no mutant can be told apart on this case"
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("c", CASES)
-def test_conv_against_fp64(c):
+def test_conv_against_fp64(c, monkeypatch):
     from katago_b200 import nn_backend
+    for k, v in c["env"].items():
+        monkeypatch.setenv(k, v)
     d = make_data(c)
     raw, hi, lo = nn_backend.test_conv_ex(c["ky"], c["ky"], c["cin"], c["cout"], d["w"], c["n"], c["X"], c["Y"], c["fp16"], c["kind"],
                                           d["x"], board_xy=d["board_xy"], ncbias=d["ncb"], residual=d["res"], bn_scale=d["sc"],
                                           bn_bias=d["bi"], activation=c["act"])
-    assert (hi is None) == (c["kind"] == 0) and (lo is None) == (c["fp16"] or c["kind"] == 0)
+    assert nn_backend.test_last_conv_kernel() == c["kernel"]
+    assert (hi is None) == (c["kind"] == 0) and (lo is None) == (c["fp16"] or c["kind"] == 0) and (raw is None) == (not has_raw(c))
     if c["check_images"] is not None:
         idx = np.array(c["check_images"])
         d = select_images(d, idx)

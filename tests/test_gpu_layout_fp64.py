@@ -188,9 +188,10 @@ def test_plan_places_images_where_the_conv_reference_expects(X, Y, pad, residues
 # ---------------------------------------------------------------------------------------------------------------------------
 # Convolution under ragged plans (GPU)
 # ---------------------------------------------------------------------------------------------------------------------------
-def conv_case(cid, ky, cin, cout, kind, fp16, act, batch, X=19, Y=19, ncbias=False, bias=1.0, check_images=None):
+def conv_case(cid, ky, cin, cout, kind, fp16, act, batch, X=19, Y=19, ncbias=False, bias=1.0, check_images=None, kernel=None):
+    """kernel: the kernel the launcher must take (None: not asserted)."""
     return pytest.param(dict(ky=ky, cin=cin, cout=cout, n=0, X=X, Y=Y, kind=kind, fp16=fp16, act=act, boards=None, ncbias=ncbias, bias=bias,
-                             batch=batch, check_images=check_images), id=cid)
+                             batch=batch, check_images=check_images, kernel=kernel), id=cid)
 
 
 SIZES = [(s, s) for s in range(2, 20)] + [(13, 7), (7, 13), (19, 5)]
@@ -248,6 +249,9 @@ PLAN_CASES = [
     conv_case("b18-3x3-192-k3-fp16-silu-segments", 3, 192, 192, 3, True, 3, "segments", bias=12.0),
     conv_case("b18-3x3-192-k4-split-mish-segments", 3, 192, 192, 4, False, 2, "segments", bias=12.0),
     conv_case("b28-3x3-256-k2-fp16-mish-widths", 3, 256, 256, 2, True, 2, "widths", bias=12.0),
+    # b18's commonest 3x3 epilogue and its last-block form (kind 5: no raw output) on the epilogue-warpgroup kernel
+    conv_case("b18-3x3-192-k2-fp16-mish-widths", 3, 192, 192, 2, True, 2, "widths", bias=12.0, kernel=cf.WG_EPI),
+    conv_case("b18-3x3-192-k5-fp16-mish-widths", 3, 192, 192, 5, True, 2, "widths", bias=12.0, kernel=cf.WG_EPI),
     conv_case("1x1-cout64-k0-split-widths", 1, 128, 64, 0, False, 0, "widths"),
     conv_case("1x1-cout384-k3-fp16-relu-widths", 1, 192, 384, 3, True, 1, "widths"),
     conv_case("5x5-initial-k3-split-mish-ncbias-widths", 5, 22, 192, 3, False, 2, "widths", ncbias=True, bias=12.0),
@@ -295,8 +299,11 @@ def test_plan_cases_rehearse(c):
 @pytest.mark.gpu
 @pytest.mark.parametrize("c", PLAN_CASES)
 def test_conv_under_ragged_plans(c):
+    from katago_b200 import nn_backend
     c, d, sym = plan_data(c)
     raw, hi, lo, stats, plan = _conv_plan(c, d, sym, True)
+    if c["kernel"] is not None:
+        assert nn_backend.test_last_conv_kernel() == c["kernel"]
     pad = max(1, c["ky"] // 2)
     premask = board_masks(d["board_xy"], np.zeros(c["n"], int), c["X"], c["Y"])
     want = restate_plan(premask, sym, pad)
